@@ -1,4 +1,4 @@
-"""autogptq_b200 - a Blackwell-native (sm_100a) drop-in for AutoGPTQ's 4-bit QuantLinear hot path.
+"""autogptq_b200 - an H100-native (sm_90a) drop-in for AutoGPTQ's 4-bit QuantLinear hot path.
 
 Only what the path needs lives here:
   csrc/            hand-written CUDA kernels + the C ABI (include/autogptq_b200.h)

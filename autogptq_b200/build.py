@@ -1,4 +1,4 @@
-"""In-tree build of the C-ABI library (nvcc, sm_100a only).
+"""In-tree build of the C-ABI library (nvcc, sm_90a only).
 
     python -m autogptq_b200.build        # or: python __graft_entry__.py build
 
@@ -21,16 +21,16 @@ LIB_PATH = os.path.join(OUT_DIR, LIB_NAME)
 STAMP = os.path.join(OUT_DIR, "build.stamp")
 
 NVCC_FLAGS = [
-    "-gencode", "arch=compute_100a,code=sm_100a",
+    "-gencode", "arch=compute_90a,code=sm_90a",
     "-O3", "-std=c++17", "-lineinfo",
     "-Xcompiler", "-fPIC",
     "-DAGB200_NO_FAST_MATH",
 ]
-if os.environ.get("AGB200_EXPERIMENTAL", "0") == "1":      # the three decode kernel families AUTO never selects (DESIGN.md 3.6)
+if os.environ.get("AGB200_EXPERIMENTAL", "0") == "1":      # the two decode kernel families AUTO never selects (DESIGN.md 3.6)
     NVCC_FLAGS.append("-DAGB200_EXPERIMENTAL_KERNELS")
 # translation units of the library (compiled in parallel, then linked)
 UNITS = ["abi.cu", "chain.cu"]
-# chain.cu holds only the 576-thread persistent chain kernel: 65536 / 576 = 113 registers per thread at most
+# chain.cu holds only the 448-thread persistent chain kernel (one CTA per SM)
 UNIT_FLAGS = {"chain.cu": ["-maxrregcount=112"]}
 
 
@@ -80,7 +80,7 @@ def build_extension(force: bool = False, verbose: bool = False) -> str:
             raise RuntimeError(f"nvcc failed on {unit} with exit code {proc.returncode}")
         if verbose:
             sys.stderr.write(err)
-    link = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_100a,code=sm_100a", "-o", LIB_PATH, *objs],
+    link = subprocess.run([nvcc, "-shared", "-gencode", "arch=compute_90a,code=sm_90a", "-o", LIB_PATH, *objs],
                           capture_output=True, text=True)
     if link.returncode != 0:
         sys.stderr.write(link.stdout + link.stderr)

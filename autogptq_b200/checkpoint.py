@@ -141,7 +141,7 @@ def build_quant_linear(tensors: Mapping[str, torch.Tensor], settings: QuantSetti
     on rank 0 only and its outputs are PARTIAL sums - wrap it in ``autogptq_b200.tp.RowParallelQuantLinear`` or run it in a
     ``TPDecodeChain``)."""
     if settings.bits != 4:
-        raise NotImplementedError(f"{settings.bits}-bit GPTQ checkpoints are outside the B200 hot path (4-bit only)")
+        raise NotImplementedError(f"{settings.bits}-bit GPTQ checkpoints are outside the H100 hot path (4-bit only)")
     if settings.checkpoint_format != "gptq":
         raise NotImplementedError(f"checkpoint_format={settings.checkpoint_format!r}: only the GPTQ pack layout is read "
                                   "(Marlin / AWQ checkpoints must be converted back, cf. marlin_utils.py:118-198)")

@@ -1,4 +1,4 @@
-// C-ABI of the B200-native GPTQ W4A16 hot path (declared in include/autogptq_b200.h).
+// C-ABI of the H100-native GPTQ W4A16 hot path (declared in include/autogptq_b200.h).
 // Host-side argument checking, kernel selection and launch; no torch, no exceptions across the ABI.
 #include <cuda_runtime.h>
 
@@ -12,17 +12,16 @@
 #include "../../include/autogptq_b200.h"
 #include "internal.h"
 #include "aux_kernels.cuh"
-#include "gemm_tcgen05.cuh"
+#include "gemm_tcgen05.cuh"   // the wgmma GEMM (file name kept from the first target)
 #include "gemv.cuh"
 #include "skinny.cuh"
 #include "decode_imma.cuh"
 #include "decode_imma_persistent.cuh"
-// Three decode kernel families that AUTO never selects (honest negative results of round 1: TMA-staged mma.sync decode,
-// tcgen05 small-N decode, TMA-staged IMMA decode - DESIGN.md 3.6) are only compiled with -DAGB200_EXPERIMENTAL_KERNELS
+// Two decode kernel families that AUTO never selects (negative results: TMA-staged mma.sync decode, TMA-staged IMMA
+// decode - DESIGN.md 3.6) are only compiled with -DAGB200_EXPERIMENTAL_KERNELS
 // (`AGB200_EXPERIMENTAL=1 python -m autogptq_b200.build`); a default build answers AGB200_ENOSUP for them.
 #ifdef AGB200_EXPERIMENTAL_KERNELS
 #include "decode_tma.cuh"
-#include "decode_tc.cuh"
 #include "decode_imma_tma.cuh"
 #endif
 
@@ -88,7 +87,7 @@ int get_device_info(DeviceInfo& out) {
     AGB_CUDA(cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
     int major = 0;
     AGB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 10) return fail(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_100a only", dev, major);
+    if (major != 9) return fail(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
     d.ok = true;
     cache[dev] = d;
     ready[dev].store(true, std::memory_order_release);
@@ -168,16 +167,15 @@ int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, cons
   p.x = x; p.qweight = qweight; p.qzeros = qzeros; p.scales = scales; p.perm = perm; p.bias = bias; p.y = y;
   p.K = K; p.N = N; p.rows = K / 8; p.rows_per_group = group_size / 8;
   p.pf = take_prefetch_hint();
-  // measured on B200 (tools/sweep_gemv.py, profiles/): wide layers (N/32 >= 2 x #SMs) run best as one wave of
-  // 32-column CTAs without split-K at 3 CTAs/SM; narrower ones as 128-column tiles with cluster split-K
+  // wide layers (N/32 >= 2 x #SMs) run as one wave of 32-column CTAs without split-K at 3 CTAs/SM; narrower ones as
+  // 128-column tiles with cluster split-K (tools/sweep_gemv.py sweeps the choices)
   p.occ3 = 0;
   if (ln == 0 && split == 0 && m == 1 && (N + 31) / 32 >= 2 * di.sms) { ln = 8; split = 1; p.occ3 = 1; }
   if (occ_req == 3) p.occ3 = 1;        // tuning knob (flags bits 4-5): force the 3- / 4-CTAs-per-SM instantiation
   if (occ_req == 4) p.occ3 = 2;
   // Everything else of Llama size: 32-column CTAs (128-byte row segments) as well.  Short K (q/k/v/o of a 7B model):
   // no clusters - half of the CTA slots stay free, so sibling layers launched on parallel graph branches overlap
-  // (tools/concurrency_probe.py: a q|k|v trio takes 11.2 us instead of 15.6 us).  Long K: 2-way cluster split-K
-  // (tools/sweep_occ.py: 11008x4096 9.7 us vs 14.8 us unsplit).
+  // (tools/concurrency_probe.py).  Long K: 2-way cluster split-K (tools/sweep_occ.py).  Not re-tuned on H100.
   if (ln == 0 && split == 0 && N >= 1024) {
     const int tiles32 = (N + 31) / 32;
     ln = 8;
@@ -648,12 +646,12 @@ extern "C" {
 int agb200_abi_version(void) { return AGB200_ABI_VERSION; }
 const char* agb200_last_error(void) { return g_err; }
 const char* agb200_build_info(void) {
-  return "autogptq_b200 sm_100a: decode=IMMA.16832.U8.S8 on raw nibbles x block-fixed-point activations (M<=8) + PDL; "
-         "gemv=cuda-core FHFMA (fma.rn.f32.f16) + cluster/DSMEM split-K; "
-         "gemm=tcgen05.mma kind::f16 (A=dequantised W^T in TMEM, B=x via TMA SWIZZLE_128B), fp32 TMEM accumulators; "
+  return "autogptq_b200 sm_90a: decode=IMMA.16832.U8.S8 on raw nibbles x block-fixed-point activations (M<=8) + PDL; "
+         "gemv=cuda-core fp32 FMA on subnormal-unpacked nibbles + cluster/DSMEM split-K; "
+         "gemm=wgmma m64nNk16 (A=dequantised W^T in registers, B=x via TMA SWIZZLE_128B), fp32 register accumulators; "
          "chain=persistent TMA ring + IMMA consumers + tagged-word dependencies"
 #ifdef AGB200_EXPERIMENTAL_KERNELS
-         "; experimental=decode_tma,decode_tc,decode_imma_tma"
+         "; experimental=decode_tma,decode_imma_tma"
 #endif
       ;
 }
@@ -696,20 +694,20 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
   const bool bf16 = dtype == AGB200_BF16;
   if (kernel == AGB200_KERNEL_AUTO) {
     const bool tc_ok = group_size % 32 == 0;            // skinny / tensor-core kernels need whole groups per 32 k
-    // TMA rows of qzeros must be 16-byte multiples; a 64-k pipeline stage of the tcgen05 kernel loads one group row (two
+    // TMA rows of qzeros must be 16-byte multiples; a 64-k pipeline stage of the wgmma kernel loads one group row (two
     // for 32-k groups), so it must not straddle a group boundary: group sizes like 96 / 160 go to the skinny kernel
     const bool gemm_ok = (group_size == 32 || group_size % 64 == 0) && N % 32 == 0 && qweight_tc != nullptr;
     const bool imma_ok = imma_rows_per_block(K, group_size) == 16;      // persistent integer kernel: 128-k flush blocks
-    // measured crossover points (profiles/): one row of x runs best on the FHFMA GEMV; 2..8 rows on the persistent integer
+    // crossover points (tuned on the previous GPU generation): one row of x on the CUDA-core GEMV; 2..8 rows on the integer
     // tensor-core kernel, which is close to HBM-bound for every such M; shapes it cannot take go to the GEMV (M <= 2) or
-    // the warp-MMA skinny kernel; everything above 8 rows to the tcgen05 kernel
+    // the warp-MMA skinny kernel; everything above 8 rows to the wgmma kernel
     // (the integer kernel converts x once per SM: that cost grows with M and makes the skinny kernel the better choice
     //  for 5..8 rows except on very large layers)
     const bool huge = static_cast<double>(K) * N >= 1.0e8;
     if (M == 1 || (!imma_ok && (M <= 2 || !tc_ok))) kernel = AGB200_KERNEL_GEMV;      // GEMV loops over M in passes of 4
     else if (imma_ok && (M <= 4 || (M == 5 && huge))) kernel = AGB200_KERNEL_IMMA;
     else if (!gemm_ok || (M <= AGB200_SKINNY_MAX_M && !huge)) kernel = AGB200_KERNEL_SKINNY;     // passes of 8 rows
-    // (5..8 rows on >= 100 MB layers: the 32-row tcgen05 tile is ahead of the skinny kernel, 65-69 us vs 83-100 us)
+    // (5..8 rows on >= 100 MB layers: the 32-row tensor-core tile)
     else kernel = AGB200_KERNEL_GEMM;
     if (M <= AGB200_SKINNY_MAX_M && tc_ok) {
       static int forced = -1;                                             // measurement aid: AGB200_SMALL_M_KERNEL=1|3|4|6
@@ -732,8 +730,10 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
     }
     return 0;
   }
+  if (kernel == AGB200_KERNEL_TCDECODE)
+    return fail(AGB200_ENOSUP, "kernel %d (tensor-memory decode) needs tcgen05, which sm_90a does not have", kernel);
 #ifndef AGB200_EXPERIMENTAL_KERNELS
-  if (kernel == AGB200_KERNEL_DECODE || kernel == AGB200_KERNEL_TCDECODE)
+  if (kernel == AGB200_KERNEL_DECODE)
     return fail(AGB200_ENOSUP, "kernel %d is an experimental kernel that AUTO never selects: build with AGB200_EXPERIMENTAL=1", kernel);
 #else
   if (kernel == AGB200_KERNEL_DECODE) {
@@ -775,25 +775,6 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
     }
     return 0;
   }
-#ifdef AGB200_EXPERIMENTAL_KERNELS
-  if (kernel == AGB200_KERNEL_TCDECODE) {
-    if (qweight_tc == nullptr)
-      return fail(AGB200_ENOSUP, "the tcgen05 decode kernel needs qweight_tc: run agb200_w4_prepare_tc once at load time");
-    const size_t xs = static_cast<size_t>(K) * 2, ys = static_cast<size_t>(N) * 2;
-    for (int m0 = 0; m0 < M; m0 += agb::kTdMT) {
-      agb::GemmArgs a{};
-      a.x = static_cast<const char*>(x) + m0 * xs; a.qweight = qweight_tc; a.qzeros = qzeros; a.scales = scales; a.perm = perm;
-      a.bias = bias; a.y = static_cast<char*>(y) + m0 * ys;
-      a.M = (M - m0 < agb::kTdMT) ? (M - m0) : agb::kTdMT; a.K = K; a.N = N; a.group_size = group_size; a.bf16 = bf16;
-      a.workspace = workspace; a.workspace_bytes = workspace_bytes;
-      a.split_k = tune1; a.sms = di.sms; a.smem_optin = di.smem_optin;
-      char msg[400] = "";
-      const int rc = agb::launch_w4a16_tcdecode(a, pdl_allowed(), stream, msg, sizeof(msg));
-      if (rc != 0) return fail(rc, "%s", msg);
-    }
-    return 0;
-  }
-#endif
   if (kernel == AGB200_KERNEL_GEMM) {
     if (qweight_tc == nullptr)
       return fail(AGB200_ENOSUP, "the tensor-core path (M=%d > 8) needs qweight_tc: run agb200_w4_prepare_tc once at load time", M);

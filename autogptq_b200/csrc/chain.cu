@@ -168,7 +168,7 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "chain: device index %d out of range", dev);
   int major = 0, sms = 0, smem_optin = 0, coop = 0;
   CH_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 10) return failf(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_100a only", dev, major);
+  if (major != 9) return failf(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
   CH_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
   CH_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
   CH_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
@@ -288,8 +288,8 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
       hs[i].next_x_ll = nx.x_ll; hs[i].next_K = nx.K; hs[i].next_rows = nx.rows;
     }
   }
-  // ring depth: whatever shared memory is left after the digits of the widest x (measured on B200, 7B shapes: 9 slots
-  // 817 us / token, 6 slots 916 us - the ring is what keeps HBM streaming while a stage boundary stalls the arithmetic)
+  // ring depth: whatever shared memory is left after the digits of the widest x (the ring is what keeps HBM streaming
+  // while a stage boundary stalls the arithmetic)
   int smem_cap = smem_optin;
   if (const char* e = getenv("AGB200_CHAIN_SMEM_KB")) { const int v = atoi(e); if (v >= 64 && v * 1024 < smem_optin) smem_cap = v * 1024; }
   const size_t fixed = M == 1 ? agb::ChainSmem<1>::fixed(rows_pad_max, xs_bytes) : agb::ChainSmem<2>::fixed(rows_pad_max, xs_bytes);
@@ -320,7 +320,7 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   c->params.xs_bytes = xs_bytes;
   c->params.inflight = inflight;
   c->params.diag = diag_device_ptr();
-  c->params.poll_backoff = 400;    // measured (7B chain): 0 -> 814 us / token, 400 -> 804, 1200 -> 816
+  c->params.poll_backoff = 400;    // cycles after a failed poll of x (AGB200_CHAIN_POLL_BACKOFF; not tuned on H100)
   if (const char* e = getenv("AGB200_CHAIN_POLL_BACKOFF")) { const int v = atoi(e); if (v >= 0 && v <= 100000) c->params.poll_backoff = v; }
   *handle_out = c;
   return 0;

@@ -1,24 +1,23 @@
 // Whole-token decode chain: ONE persistent launch runs a list of dependent QuantLinear "stages" (each stage = up to four
 // sibling layers that consume the same x: q|k|v, o, gate|up, down, ... of every decoder block), M <= 2 rows of x.
 //
-// Why: a decode token of a 7B model is 128 dependent launches of 4-17 us; each boundary costs ~2 us of launch +
-// dependency + first-byte latency during which HBM idles (profiles/r01_summary.md 4.2: 0.445 of the HBM roofline on the
-// chain although the kernels reach 0.55+ in steady state).  The weights never depend on the previous layer - only x
+// Why: a decode token of a 7B model is 128 dependent launches; each boundary costs launch + dependency + first-byte
+// latency during which HBM idles.  The weights never depend on the previous layer - only x
 // does.  So here the weight stream never stops:
 //   * one CTA per SM (cooperative launch): 12 consumer warps (3 groups of 4), a PRODUCER warp and an EPILOGUE warp - 14
 //     warps, at most 4 per SM sub-partition, so every thread has 128 registers;
 //   * the producer walks over the tile schedule of the WHOLE chain and keeps a deep shared-memory ring (all the shared
-//     memory the digits of x leave: 9 slots of [128 k8-rows x 32 columns] packed weights + the 8 scale rows + 8
-//     zero-word rows they need on 7B shapes, 157 KB per SM, 23 MB over the chip) filled with cp.async.bulk.tensor (TMA)
+//     memory the digits of x leave: slots of [128 k8-rows x 32 columns] packed weights + the 8 scale rows + 8
+//     zero-word rows they need) filled with cp.async.bulk.tensor (TMA)
 //     loads.  It never waits for a layer boundary, only for a free slot, so it runs a stage or more AHEAD of the
-//     arithmetic; the arithmetic is ~2.5x faster than the stream in bursts, so the ring is what keeps HBM busy while a
-//     stage boundary stalls it (measured: 6 slots 916 us / token, 9 slots 812 us);
+//     arithmetic; the arithmetic is faster than the stream in bursts, so the ring is what keeps HBM busy while a
+//     stage boundary stalls it;
 //   * dependencies are DATA FLOW, not barriers: a stage's y is published as 8-byte {two 16-bit values, launch tag} words
 //     (single-copy atomic stores, the "LL" idea of NCCL's low-latency protocol); the consumers of the next stage poll the
 //     very words they need.  No flag, no fence, no atomic, no grid barrier sits between a tile's last MMA and the next
-//     stage's first one - measured on B200 the flag protocol (store, fence, atomic, poll, load: four dependent L2 round
-//     trips of ~1 us each while the TMA stream saturates L2) cost 4 us per stage;
-//   * an L2 round trip under a saturating TMA stream takes 1.5-2 us (the response queues behind the SM's own in-flight
+//     stage's first one - a flag protocol (store, fence, atomic, poll, load) costs four dependent L2 round
+//     trips per stage while the TMA stream saturates L2;
+//   * an L2 round trip under a saturating TMA stream is slow (the response queues behind the SM's own in-flight
 //     weight tiles), so every consumer thread polls its own rows of x at once (384 loads in flight, one round trip), and
 //     the rows of the NEXT stage are prefetched into L1 while the last tile of a stage computes - tags make stale L1 lines
 //     harmless, and x that is complete early (q for o_proj, gate for down_proj) then costs no round trip at all;

@@ -1,4 +1,4 @@
-// Shared device helpers for the sm_100a W4A16 kernels.
+// Shared device helpers for the sm_90a W4A16 kernels.
 #pragma once
 #include <cuda_bf16.h>
 #include <cuda_fp16.h>
@@ -80,10 +80,8 @@ __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepc
 
 // ---------------------------------------------------------------- next-layer L2 prefetch (opt-in, measured NEGATIVE)
 // Idea: while layer i computes, pull the weights of layer i+1 (named by the host, which has seen the call order
-// before) into the 126 MB L2 so that the DRAM stream never pauses at a kernel boundary.  Measured on the Llama-2-7B
-// decode chain (profiles/r01_summary.md): 780 tokens/s with cp.async.bulk.prefetch.L2, 745 with per-line
-// prefetch.global.L2::evict_last, against 862 without - the prefetch traffic delays the demand loads of the running
-// layer more than it saves the next one.  Kept behind autogptq_b200.set_next_layer_prefetch(True) for experiments.
+// before) into the L2 so that the DRAM stream never pauses at a kernel boundary.  It measured slower on the previous
+// GPU generation (the prefetch traffic delays the demand loads of the running layer); not measured on H100.  Kept behind autogptq_b200.set_next_layer_prefetch(True) for experiments.
 constexpr int kMaxPrefetchRanges = 8;
 struct PrefetchHint {
   const char* ptr[kMaxPrefetchRanges];
@@ -116,26 +114,22 @@ __device__ __forceinline__ void l2_prefetch_slices(const PrefetchHint& h, unsign
   }
 }
 
-// ---------------------------------------------------------------- mixed-precision FMA (SASS: FHFMA / FHFMA.BF16)
-// c += a.{lo|hi} * b.{lo|hi} with 16-bit inputs taken from packed registers and an fp32 accumulator.
+// ---------------------------------------------------------------- 16-bit x 16-bit + fp32 FMA
+// c += a.{lo|hi} * b.{lo|hi} with 16-bit inputs taken from packed registers and an fp32 accumulator.  sm_90 has no
+// mixed-precision FMA: both inputs widen exactly to fp32 and their product (<= 22 significant bits) is exact in fp32,
+// so fmaf rounds once - the same result as a fused f32 += f16 * f16.
 template <bool kBf16, bool kHi>
 __device__ __forceinline__ float fma_mixed(uint32_t a2, uint32_t b2, float c) {
+  float a, b;
   if constexpr (!kBf16) {
-    if constexpr (!kHi)
-      asm("{.reg .f16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.f16 %0, al, bl, %0;}"
-          : "+f"(c) : "r"(a2), "r"(b2));
-    else
-      asm("{.reg .f16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.f16 %0, ah, bh, %0;}"
-          : "+f"(c) : "r"(a2), "r"(b2));
+    const __half2 ah = *reinterpret_cast<const __half2*>(&a2), bh = *reinterpret_cast<const __half2*>(&b2);
+    a = kHi ? __high2float(ah) : __low2float(ah);
+    b = kHi ? __high2float(bh) : __low2float(bh);
   } else {
-    if constexpr (!kHi)
-      asm("{.reg .b16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.bf16 %0, al, bl, %0;}"
-          : "+f"(c) : "r"(a2), "r"(b2));
-    else
-      asm("{.reg .b16 al, ah, bl, bh; mov.b32 {al,ah}, %1; mov.b32 {bl,bh}, %2; fma.rn.f32.bf16 %0, ah, bh, %0;}"
-          : "+f"(c) : "r"(a2), "r"(b2));
+    a = __uint_as_float(kHi ? (a2 & 0xffff0000u) : (a2 << 16));
+    b = __uint_as_float(kHi ? (b2 & 0xffff0000u) : (b2 << 16));
   }
-  return c;
+  return fmaf(a, b, c);
 }
 
 // (a & b) | c in one LOP3

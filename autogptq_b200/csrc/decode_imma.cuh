@@ -2,10 +2,9 @@
 //
 // Roofline: HBM.  Algorithmic bytes per launch = K*N/2 + G*N*2 + G*N/2 (+4K) + 2*M*K + 2*M*N (SURVEY.md 8d).
 //
-// Why integers: the FHFMA GEMV (gemv.cuh) spends 13 issue slots per packed word (8 weights) and is issue-bound at
-// ~55% of the HBM roofline (tools/probe/pipe_probe.cu: 16.9 clk per word per SM sub-partition).  Here the CUDA
-// cores only split a word into its even / odd nibbles (3 ops per word: AND, SHF, AND) and the products run on
-// IMMA.16832.U8.S8 - 8 clk per 1024 weights - so one 16-byte load costs ~32 clk instead of ~68.
+// Why integers: the CUDA-core GEMV (gemv.cuh) spends 13+ issue slots per packed word (8 weights) and is issue-bound.
+// Here the CUDA cores only split a word into its even / odd nibbles (3 ops per word: AND, SHF, AND) and the products
+// run on IMMA.16832.U8.S8, so the per-word instruction cost is independent of M.
 //
 //   * A operand = 16 weight columns x 32 k of raw nibbles as u8 (no zero point, no scale);
 //   * B operand = x as block fixed point: per K chunk and per row of x a power-of-two scale 2^p with

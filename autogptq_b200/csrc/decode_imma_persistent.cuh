@@ -1,7 +1,7 @@
 // Persistent form of the integer tensor-core decode kernel (decode_imma.cuh): ONE 512-thread CTA per SM walks over
 // 32-column tiles (round-robin over the SMs, all sibling layers of a grouped launch concatenated).
 //
-// What it changes relative to the tile-per-CTA kernel (ncu, profiles/r01_summary.md): there the fixed work of a CTA -
+// What it changes relative to the tile-per-CTA kernel: there the fixed work of a CTA -
 // ring set-up, turning x into fixed-point digits, the reduction epilogue - was as many issue slots as its main loop,
 // and three CTAs per SM each repeated it.  Here x is converted once per SM, the 16 warps split the K range of every
 // tile at flush-block granularity, the register ring of 16-byte weight loads keeps running ACROSS tile boundaries

@@ -1,12 +1,12 @@
 // TMA-staged form of the integer tensor-core decode kernel (tune0 = 3; AUTO uses the register-ring form of
 // decode_imma_persistent.cuh, which measured equal or faster).  group_size 128 layers, M <= 8.
 //
-// Decode is a chain of 1-10 us HBM-bound layers.  What decides the achieved bandwidth is whether layer i+1's weights
+// Decode is a chain of short HBM-bound layers.  What decides the achieved bandwidth is whether layer i+1's weights
 // are already streaming while layer i finishes - which programmatic dependent launch only delivers when BOTH kernels
 // fit on an SM at the same time.  A register ring (decode_imma_persistent.cuh) needs 128 registers x 512 threads: the
 // whole register file.  Here the bytes in flight live in shared memory instead:
 //   * one persistent CTA per SM: a producer warp + 16 consumer warps, <= 64 registers per thread.  With <= ~110 KB of
-//     shared memory two consecutive layers are co-resident - which measured SLOWER (6.4 us vs 4.8 us at 4096^2) than a
+//     shared memory two consecutive layers are co-resident - which measured SLOWER (previous GPU generation) than a
 //     ring as deep as the SM allows, so the launcher takes all the shared memory it can get;
 //   * the producer issues TMA loads the moment the CTA starts (BEFORE griddepcontrol.wait): per stage one box of
 //     packed weights [128 k8-rows x 32 columns] (16 KB, checkpoint layout, OOB rows / columns zero-filled), the
@@ -20,7 +20,7 @@
 #pragma once
 #include "common.cuh"
 #include "decode_imma.cuh"
-#include "gemm_tcgen05.cuh"   // EncodeTiledFn, get_encode_fn
+#include "tmap.cuh"          // EncodeTiledFn, get_encode_fn
 #include "ptx.cuh"
 
 namespace agb {

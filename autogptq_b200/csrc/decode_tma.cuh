@@ -1,7 +1,7 @@
 // W4A16 decode kernel (M <= 8), TMA-staged, fp16 warp-MMA consumers.  EXPERIMENTAL (AGB200_KERNEL_DECODE): parity-green but
-// slower than the GEMV (9 us vs 4.6 us at 4096^2) - kept as the record of this design; AUTO never selects it.
+// slower than the GEMV where measured - kept as the record of this design; AUTO never selects it.
 //
-// Decode is a chain of ~1-4 us HBM-bound layers; what decides the achieved bandwidth is not the inner loop
+// Decode is a chain of short HBM-bound layers; what decides the achieved bandwidth is not the inner loop
 // but whether layer i+1's weights are already streaming while layer i finishes.  Design rules (DESIGN.md 3.1):
 //   * a CTA uses < 1/2 of an SM (<= 110 KB smem, 288 threads, < 100 regs) and the grid is <= #SMs persistent
 //     CTAs, so two consecutive layers are co-resident under programmatic dependent launch (PDL);

@@ -1,29 +1,15 @@
-// W4A16 GEMM on the 5th-generation tensor cores (sm_100a): y[M,N] = x[M,K] * dequant(W)[K,N].
-//
-// The contraction is issued "swapped":  D[n, m] = sum_k Wt[n, k] * x[m, k]
-//   * A operand = dequantised W^T tile, 128 weight columns (UMMA M = 128) x 64 k per stage, written by the
-//     dequant warps with tcgen05.st straight into TENSOR MEMORY (row n = TMEM lane, two 16-bit k per
-//     32-bit column) - it never touches shared memory, so the int4 -> fp16 expansion costs no smem bandwidth;
-//   * B operand = x tile, kMT rows (UMMA N = kMT in {32,64,128,256}) x 64 k, staged by TMA into shared
-//     memory in the K-major SWIZZLE_128B canonical layout;
-//   * D = fp32 accumulators in TMEM (128 lanes x kMT columns), read back once with tcgen05.ld for the
-//     epilogue (bias, cast, store).
-// Packed weights ([K/8, N] int32, tensor-core nibble order of agb200_w4_prepare_tc) are staged by TMA, 4 KB per
-// stage; thread = one weight column for the whole K loop, so the per-group scale / zero-point are plain registers.
-//
-// Warp roles (384 threads): 0 = TMA producer, 1 = MMA issuer (one elected lane), 2 = TMEM allocator,
-// 3 = spare, 4..11 = dequant warps (TMEM quadrant = warp % 4, two warps per quadrant split the 64 k of a
-// stage) which also run the epilogue.  Pipelines: b_full (TMA -> MMA), a_full (dequant -> MMA),
-// empty (tcgen05.commit -> TMA + dequant), acc_full (last commit -> epilogue).
-// Split-K (small M): the CTAs of a thread-block cluster each take a K range; fp32 partial tiles are reduced
-// through distributed shared memory - no atomics, no global workspace.
-//
-// Roofline: tensor pipe for M >~ 128 (2*M*K*N flop), HBM for small M (algorithmic bytes of SURVEY 8d).
+// W4A16 GEMM on the Hopper warpgroup tensor cores (sm_90a): y[M,N] = x[M,K] * dequant(W)[K,N], issued "swapped" as
+// D[n, m] = sum_k Wt[n, k] * x[m, k].  A = dequantised W^T from REGISTERS (wgmma register-A form: each consumer thread
+// expands exactly the A-fragment elements it owns); B = x tile [kMT rows x 64 k] staged by TMA, K-major SWIZZLE_128B;
+// D = fp32 register accumulators.  Packed weights (tensor-core nibble order of agb200_w4_prepare_tc), scales and zeros
+// arrive by TMA next to the x tile.  384 threads: warpgroup 0 = producers (x after griddepcontrol.wait; weights at once),
+// warpgroups 1, 2 = consumers of weight columns 0..63 / 64..127.  Split-K: thread-block cluster, DSMEM reduction.
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched through the runtime)
 
 #include <cstdio>
+#include <type_traits>
 
 #include "aux_kernels.cuh"
 #include "common.cuh"
@@ -39,32 +25,19 @@ struct GemmArgs {
   int tile_m, split_k, sms, smem_optin;
 };
 
-// dequant warp groups (4 warps each, one per TMEM quadrant) taking pipeline stages round-robin.  Two groups (384-thread
-// CTAs, two per SM for the small-M tiles).  Four groups were tried for the compute-bound tiles: no gain at M = 4096
-// (the limiter is the A-operand feed into TMEM, not the dequant issue rate), M <= 64 twice as slow when applied to the
-// small tiles (one CTA per SM), and one unexplained launch failure in a long benchmark run - not kept.
-__host__ __device__ constexpr int gemm_groups(int /*mt*/) { return 2; }
-__host__ __device__ constexpr int gemm_threads(int mt) { return 128 + gemm_groups(mt) * 128; }
-constexpr int kGemmBN = 128;      // weight columns per CTA  (UMMA M)
-constexpr int kGemmBK = 64;       // k per pipeline stage    (one 128-byte swizzle row of 16-bit x)
-constexpr int kGemmStages = 6;       // x (B operand) shared-memory stages == TMEM A stages (profiles/: 4 left the MMA waiting on x)
-constexpr int kGemmWStages = 6;      // packed-weight ring (own producer warp, not tied to the MMA)
-constexpr int kGemmPF = 4;        // stages of packed weights prefetched into registers
+constexpr int kGemmThreads = 384;
+constexpr int kGemmConsumers = 256;
+constexpr int kGemmBN = 128;      // weight columns per CTA (two wgmma M = 64 slices)
+constexpr int kGemmBK = 64;       // k per pipeline stage   (one 128-byte swizzle row of 16-bit x)
+constexpr int kGemmLd = kGemmBN + 4;   // fp32 staging row pitch: conflict-free fragment stores
+__host__ __device__ constexpr int gemm_stages(int mt) { return mt == 256 ? 5 : 6; }
 
-// K-major SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp SmemDescriptor):
-// start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled K-major) | SBO>>4 [32,46) = 1024 B between 8-row
-// groups | version=1 [46,48) | layout SWIZZLE_128B=2 [61,64)
+// K-major SWIZZLE_128B shared-memory matrix descriptor (wgmma): start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled
+// K-major, 1) | SBO>>4 [32,46) = 1024 B between 8-row groups | layout [62,64) = 1 (128B swizzle)
 __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
-  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-// Instruction descriptor, kind::f16 (InstrDescriptor): D=f32 [4,6)=1 | A fmt [7,10) | B fmt [10,13) |
-// A,B K-major (bits 15,16 = 0) | N>>3 [17,23) | M>>4 [24,29)
-__host__ __device__ constexpr uint32_t make_idesc(bool bf16, int umma_m, int umma_n) {
-  return (1u << 4) | ((bf16 ? 1u : 0u) << 7) | ((bf16 ? 1u : 0u) << 10) | (static_cast<uint32_t>(umma_n >> 3) << 17) |
-         (static_cast<uint32_t>(umma_m >> 4) << 24);
+  return static_cast<uint64_t>((smem_addr >> 4) & 0x3FFFu) | (1ull << 16) | (64ull << 32) | (1ull << 62);
 }
 
-// -------------------------------------------------------------------------------------------- kernel
 struct GemmParams {
   const int32_t* qweight; const int32_t* qzeros; const void* scales; const void* bias; void* y;
   int M, K, N;
@@ -74,134 +47,107 @@ struct GemmParams {
   int num_kb;          // ceil(K / 64)
   int kb_per_split;
   int split;
-  int debug;           // measurement aid: bit0 = MMA does not wait for dequantised A (dequant warps idle), bit1 = no x loads
+  int debug;           // measurement aid: bit0 = no weight loads, bit1 = no x loads
 };
 
 template <int kMT>
 struct GemmSmem {
+  static constexpr int kStages = gemm_stages(kMT);
   static constexpr int kBStage = kMT * 128;                       // bytes of one x stage
-  static constexpr int kBBytes = kBStage * kGemmStages;           // == 128 * kMT * 4: reused as fp32 staging
   static constexpr int kWStage = (kGemmBK / 8) * kGemmBN * 4;     // packed weight tile [8 k8-rows][128 cols] int32 = 4 KB
-  static constexpr int kWOff = kBBytes;
   static constexpr int kSStage = 2 * kGemmBN * 2;                 // scales of up to two groups x 128 columns (16-bit)
   static constexpr int kZStage = 2 * (kGemmBN / 8) * 4;           // packed zero-points of up to two groups
-  static constexpr int kSOff = kWOff + kWStage * kGemmWStages;
-  static constexpr int kZOff = kSOff + kSStage * kGemmWStages;
-  static constexpr int kBarOff = kZOff + kZStage * kGemmWStages;
-  static constexpr int kTotal = kBarOff + 512 + 1024;             // + barriers + alignment slack
+  static constexpr int kWOff = kBStage * kStages;
+  static constexpr int kSOff = kWOff + kWStage * kStages;
+  static constexpr int kZOff = kSOff + kSStage * kStages;
+  static constexpr int kRing = kZOff + kZStage * kStages;
+  static constexpr int kStaging = kMT * kGemmLd * 4;              // fp32 [kMT][kGemmLd], reuses the ring
+  static constexpr int kBarOff = (kRing > kStaging ? kRing : kStaging);
+  static constexpr int kTotal = kBarOff + 256 + 1024;             // + barriers + alignment slack
 };
 
-template <int kMT> __host__ __device__ constexpr int gemm_tmem_cols() {
-  constexpr int need = kMT + kGemmStages * (kGemmBK / 2);
-  return need <= 32 ? 32 : need <= 64 ? 64 : need <= 128 ? 128 : need <= 256 ? 256 : 512;
+// k-pair `pair` of a tensor-core-order word (bits [4p, 4p+4) and [16+4p, 20+4p)) as s * (q - z), rounded once
+template <bool kBf16>
+__device__ __forceinline__ uint32_t dequant_pair(uint32_t w, int pair, uint32_t s2, uint32_t zc) {
+  const uint32_t b = lop3_and_or(w >> (4 * pair), 0x000f000fu, kBf16 ? 0x43004300u : 0x64006400u);
+  uint32_t out;
+  if constexpr (!kBf16) {
+    const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2*>(&b), *reinterpret_cast<const __half2*>(&zc)),
+                              *reinterpret_cast<const __half2*>(&s2));
+    out = *reinterpret_cast<const uint32_t*>(&v);
+  } else {
+    const __nv_bfloat162 v = __hmul2(__hsub2(*reinterpret_cast<const __nv_bfloat162*>(&b), *reinterpret_cast<const __nv_bfloat162*>(&zc)),
+                                     *reinterpret_cast<const __nv_bfloat162*>(&s2));
+    out = *reinterpret_cast<const uint32_t*>(&v);
+  }
+  return out;
 }
 
-// dequantise one word of the tensor-core copy (8 consecutive k of one column, nibble order of
-// agb200_w4_prepare_tc) to 4 registers (k0,k1)(k2,k3)(k4,k5)(k6,k7); value = s * (q - z) rounded once to the
-// 16-bit type (what the reference forms in scales.dtype).  13 ALU ops per word, no byte permutes.
-template <bool kBf16>
-__device__ __forceinline__ void dequant_word(uint32_t w, uint32_t s2, uint32_t zc_lo, uint32_t zc_hi, uint32_t* out) {
-  if constexpr (!kBf16) {
-    const uint32_t t = w >> 8;
-    uint32_t b01 = lop3_and_or(w, 0x000f000fu, 0x64006400u);   // 1024 + q
-    uint32_t b23 = lop3_and_or(w, 0x00f000f0u, 0x64006400u);   // 1024 + 16 q
-    uint32_t b45 = lop3_and_or(t, 0x000f000fu, 0x64006400u);
-    uint32_t b67 = lop3_and_or(t, 0x00f000f0u, 0x64006400u);
-    const __half2 sc = *reinterpret_cast<const __half2*>(&s2);
-    const __half2 zl = *reinterpret_cast<const __half2*>(&zc_lo);   // 1024 + z
-    const __half2 zh = *reinterpret_cast<const __half2*>(&zc_hi);   // -(64 + z)
-    const __half2 k16 = __float2half2_rn(0.0625f);
-    __half2 v01 = __hmul2(__hsub2(*reinterpret_cast<__half2*>(&b01), zl), sc);
-    __half2 v45 = __hmul2(__hsub2(*reinterpret_cast<__half2*>(&b45), zl), sc);
-    __half2 v23 = __hmul2(__hfma2(*reinterpret_cast<__half2*>(&b23), k16, zh), sc);
-    __half2 v67 = __hmul2(__hfma2(*reinterpret_cast<__half2*>(&b67), k16, zh), sc);
-    out[0] = *reinterpret_cast<uint32_t*>(&v01); out[1] = *reinterpret_cast<uint32_t*>(&v23);
-    out[2] = *reinterpret_cast<uint32_t*>(&v45); out[3] = *reinterpret_cast<uint32_t*>(&v67);
-  } else {
-    uint32_t b01 = lop3_and_or(w, 0x000f000fu, 0x43004300u);         // 128 + q
-    uint32_t b23 = lop3_and_or(w >> 4, 0x000f000fu, 0x43004300u);
-    uint32_t b45 = lop3_and_or(w >> 8, 0x000f000fu, 0x43004300u);
-    uint32_t b67 = lop3_and_or(w >> 12, 0x000f000fu, 0x43004300u);
-    const __nv_bfloat162 sc = *reinterpret_cast<const __nv_bfloat162*>(&s2);
-    const __nv_bfloat162 zl = *reinterpret_cast<const __nv_bfloat162*>(&zc_lo);   // 128 + z
-    __nv_bfloat162 v01 = __hmul2(__hsub2(*reinterpret_cast<__nv_bfloat162*>(&b01), zl), sc);
-    __nv_bfloat162 v23 = __hmul2(__hsub2(*reinterpret_cast<__nv_bfloat162*>(&b23), zl), sc);
-    __nv_bfloat162 v45 = __hmul2(__hsub2(*reinterpret_cast<__nv_bfloat162*>(&b45), zl), sc);
-    __nv_bfloat162 v67 = __hmul2(__hsub2(*reinterpret_cast<__nv_bfloat162*>(&b67), zl), sc);
-    out[0] = *reinterpret_cast<uint32_t*>(&v01); out[1] = *reinterpret_cast<uint32_t*>(&v23);
-    out[2] = *reinterpret_cast<uint32_t*>(&v45); out[3] = *reinterpret_cast<uint32_t*>(&v67);
-  }
+template <int kMT, bool kBf16>
+__device__ __forceinline__ void wgmma_tile(float (&d)[kMT / 2], const uint32_t* a, uint64_t b_desc) {
+  if constexpr (kMT == 32) { if constexpr (kBf16) wgmma_m64n32k16_bf16(d, a, b_desc); else wgmma_m64n32k16_f16(d, a, b_desc); }
+  if constexpr (kMT == 64) { if constexpr (kBf16) wgmma_m64n64k16_bf16(d, a, b_desc); else wgmma_m64n64k16_f16(d, a, b_desc); }
+  if constexpr (kMT == 128) { if constexpr (kBf16) wgmma_m64n128k16_bf16(d, a, b_desc); else wgmma_m64n128k16_f16(d, a, b_desc); }
+  if constexpr (kMT == 256) { if constexpr (kBf16) wgmma_m64n256k16_bf16(d, a, b_desc); else wgmma_m64n256k16_f16(d, a, b_desc); }
 }
+
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kGemmConsumers) : "memory"); }
 
 // kMcast: clusters of two CTAs along N (adjacent weight-column tiles, same x rows).  Each CTA fetches HALF of the
-// x tile and TMA-multicasts it into both CTAs' shared memory, halving the L2->SM traffic of the B operand
-// (at MT=256 one SM would otherwise pull 36 KB per 512 MMA cycles = 70 B/clk, above the ~42 B/clk/SM L2 fabric share).
+// x tile and TMA-multicasts it into both CTAs' shared memory, halving the L2->SM traffic of the B operand.
 template <int kMT, bool kBf16, bool kMcast>
-__global__ void __launch_bounds__(gemm_threads(kMT), 1)
+__global__ void __launch_bounds__(kGemmThreads, 1)
 w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                   const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_z) {
   using Smem = GemmSmem<kMT>;
-  constexpr int kTmemCols = gemm_tmem_cols<kMT>();
-  constexpr int kAColBase = kMT;                  // A stages live after the accumulator columns
-  constexpr uint32_t kIdesc = make_idesc(kBf16, kGemmBN, kMT);
+  constexpr int kGemmStages = Smem::kStages;
 
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
   unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
   const uint32_t bar_base = smem_base + Smem::kBarOff;
   auto b_full = [&](int s) { return bar_base + 8u * s; };
-  auto a_full = [&](int s) { return bar_base + 8u * (kGemmStages + s); };
-  auto empty = [&](int s) { return bar_base + 8u * (2 * kGemmStages + s); };
-  const uint32_t acc_full = bar_base + 8u * (3 * kGemmStages);
-  auto w_full = [&](int s) { return bar_base + 8u * (3 * kGemmStages + 1 + s); };
-  auto w_empty = [&](int s) { return bar_base + 8u * (3 * kGemmStages + 1 + kGemmWStages + s); };
-  uint32_t* tmem_slot = reinterpret_cast<uint32_t*>(smem_al + Smem::kBarOff + 8 * (3 * kGemmStages + 1 + 2 * kGemmWStages));
+  auto empty = [&](int s) { return bar_base + 8u * (kGemmStages + s); };
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
   const int n0 = blockIdx.x * kGemmBN;
   const int m0 = blockIdx.y * kMT;
   const int kb_begin = blockIdx.z * p.kb_per_split;
   const int kb_end = min(p.num_kb, kb_begin + p.kb_per_split);
   const int num_it = max(0, kb_end - kb_begin);
 
-  if (warp == 0 && lane == 0) {
+  if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_x);
     prefetch_tmap(&tmap_w);
     prefetch_tmap(&tmap_s);
     prefetch_tmap(&tmap_z);
     for (int s = 0; s < kGemmStages; ++s) {
-      mbar_init(b_full(s), 1);
-      mbar_init(a_full(s), 4);                   // the four warps (one per TMEM quadrant) that own the stage
-      mbar_init(empty(s), kMcast ? 2 : 1);        // multicast: both CTAs must have released the stage
-    }
-    mbar_init(acc_full, 1);
-    for (int s = 0; s < kGemmWStages; ++s) {
-      mbar_init(w_full(s), 1);
-      mbar_init(w_empty(s), 4);
+      mbar_init(b_full(s), 2);                                   // x producer + weight producer
+      mbar_init(empty(s), (kMcast ? 2 : 1) * (kGemmConsumers / 32));
     }
     fence_mbar_init();
   }
-  if (warp == 2) tmem_alloc<kTmemCols>(smem_u32(tmem_slot));
-  tc_fence_before();
   uint32_t cta_rank = 0;
   if constexpr (kMcast) {
     cg::cluster_group cl = cg::this_cluster();
-    cl.sync();                                     // peer barriers are initialised before any remote arrive
+    cl.sync();                                     // peer barriers are initialised before any remote arrive / multicast
     cta_rank = cl.block_rank();
   } else {
     __syncthreads();
   }
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_slot;
+  float* stage_f32 = reinterpret_cast<float*>(smem_al);  // [kMT][kGemmLd], reuses the ring
 
-  if (warp == 0) {
-    // ================= TMA producer: x tile [kMT rows, 64 k] per stage =================
-    if (lane == 0) {
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ================= x producer: [kMT rows, 64 k] per stage =================
       pdl_wait();   // x comes from the previous kernel in the stream
-      for (int it = 0; it < ((p.debug & 2) ? 0 : num_it); ++it) {
+      for (int it = 0; it < num_it; ++it) {
         const int s = it % kGemmStages;
         const uint32_t ph = (it / kGemmStages) & 1;
         mbar_wait(empty(s), ph ^ 1u);
+        if (p.debug & 2) { mbar_arrive(b_full(s)); continue; }
         mbar_arrive_expect_tx(b_full(s), Smem::kBStage);
         if constexpr (kMcast) {
           tma_load_2d_mcast(smem_base + s * Smem::kBStage + cta_rank * (Smem::kBStage / 2), &tmap_x,
@@ -210,196 +156,160 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
           tma_load_2d(smem_base + s * Smem::kBStage, &tmap_x, (kb_begin + it) * kGemmBK, m0, b_full(s));
         }
       }
-    }
-    __syncwarp();
-  } else if (warp == 3) {
-    // ================= weight producer: packed int4 tile + scale / zero rows of its group(s), deep ring =================
-    // (weights never depend on the previous kernel: no griddepcontrol.wait here)
-    if (lane == 0) {
+    } else if (warp == 1 && lane == 0) {
+      // ================= weight producer: packed int4 tile + scale / zero rows of its group(s) =================
+      // (weights never depend on the previous kernel: no griddepcontrol.wait here)
       const int ngr = p.group_size == 32 ? 2 : 1;            // groups touched by the 64 k of a stage
       const uint32_t bytes = Smem::kWStage + ngr * (kGemmBN * 2 + (kGemmBN / 8) * 4);
-      for (int it = 0; it < ((p.debug & 1) ? 0 : num_it); ++it) {
-        const int ws = it % kGemmWStages;
-        const uint32_t wph = (it / kGemmWStages) & 1;
-        mbar_wait(w_empty(ws), wph ^ 1u);
-        mbar_arrive_expect_tx(w_full(ws), bytes);
+      for (int it = 0; it < num_it; ++it) {
+        const int ws = it % kGemmStages;
+        const uint32_t wph = (it / kGemmStages) & 1;
+        mbar_wait(empty(ws), wph ^ 1u);
+        if (p.debug & 1) { mbar_arrive(b_full(ws)); continue; }
+        mbar_arrive_expect_tx(b_full(ws), bytes);
         const int k0 = (kb_begin + it) * kGemmBK;
         const int g0 = p.gs_log2 >= 0 ? (k0 >> p.gs_log2) : k0 / p.group_size;
-        tma_load_2d(smem_base + Smem::kWOff + ws * Smem::kWStage, &tmap_w, n0, k0 >> 3, w_full(ws));
-        tma_load_2d(smem_base + Smem::kSOff + ws * Smem::kSStage, &tmap_s, n0, g0, w_full(ws));
-        tma_load_2d(smem_base + Smem::kZOff + ws * Smem::kZStage, &tmap_z, n0 >> 3, g0, w_full(ws));
+        tma_load_2d(smem_base + Smem::kWOff + ws * Smem::kWStage, &tmap_w, n0, k0 >> 3, b_full(ws));
+        tma_load_2d(smem_base + Smem::kSOff + ws * Smem::kSStage, &tmap_s, n0, g0, b_full(ws));
+        tma_load_2d(smem_base + Smem::kZOff + ws * Smem::kZStage, &tmap_z, n0 >> 3, g0, b_full(ws));
       }
     }
-    __syncwarp();
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      for (int it = 0; it < num_it; ++it) {
-        const int s = it % kGemmStages;
-        const uint32_t ph = (it / kGemmStages) & 1;
-        if (!(p.debug & 1)) mbar_wait(a_full(s), ph);
-        if (!(p.debug & 2)) mbar_wait(b_full(s), ph);
-        tc_fence_after();
-        const uint64_t bdesc = make_b_desc(smem_base + s * Smem::kBStage);
-#pragma unroll
-        for (int j = 0; j < kGemmBK / 16; ++j) {
-          // A: 8 TMEM columns per 16 k ; B: +32 bytes inside the 128-byte swizzle row
-          umma_ts_f16(tmem_base, tmem_base + kAColBase + s * (kGemmBK / 2) + j * 8, bdesc + 2u * j, kIdesc,
-                      (it > 0 || j > 0) ? 1u : 0u);
-        }
-        if constexpr (kMcast) tc_commit_mcast(empty(s), 0x3);
-        else tc_commit(empty(s));
-      }
-      tc_commit(acc_full);
-    }
-    __syncwarp();
-  } else if (warp >= 4) {
-    // ================= dequant warps (then epilogue) =================
-    // gemm_groups(kMT) groups of four warps (one warp per TMEM lane quadrant) take the pipeline stages round-robin: a
-    // warp expands all 64 k of "its" stages (8 packed words -> 32 TMEM columns, one tcgen05.st.x32).  The chains are
-    // latency-bound (dependent half2 ops, ~0.25 IPC per warp), so throughput comes from the number of groups.
-    const int dw = warp - 4;
-    const int quad = warp & 3;            // TMEM lane quadrant this warp may touch
-    constexpr int kGemmGroups = gemm_groups(kMT);
-    const int grp = dw >> 2;              // handles stages it with it % kGemmGroups == grp
-    const int half = grp;                 // epilogue: which slice of the x rows this warp stores
-    const int nl = quad * 32 + lane;      // weight column inside the tile == TMEM lane
-    const int n = n0 + nl;
-    const bool n_ok = n < p.N;
-    const bool two_groups = p.group_size == 32;        // a 64-k stage then spans two groups
+  } else {
+    setmaxnreg_inc<232>();
+    // ================= consumers: expand W into A fragments, wgmma against the x tile =================
+    // thread (warp w, g = lane / 4, t = lane % 4): A rows c0 = 16 w + g and c0 + 8, k-pair t of every packed word
+    const int cw = warp - 4;                      // consumer warp 0..7
+    const int g = lane >> 2, t = lane & 3;
+    const int c0 = (cw >> 2) * 64 + (cw & 3) * 16 + g;   // weight column inside the tile (second one: c0 + 8)
+    const bool two_groups = p.group_size == 32;           // a 64-k stage then spans two groups
+    const uint32_t* wsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kWOff) + c0;  // [stage][8][128]
+    const uint16_t* ssm = reinterpret_cast<const uint16_t*>(smem_al + Smem::kSOff) + c0;  // [stage][2][128]
+    const uint32_t* zsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kZOff);  // [stage][2][16]
+    const int zsh = 4 * (c0 & 7);  // same for c0 + 8
 
-    // Everything the dequant warps consume (packed words, group scales, packed zero-points) arrives in shared
-    // memory by TMA on the stage's mbarrier: no global addressing in this loop.
-    const int zsh = 4 * (n & 7);
-    auto group_consts = [&](uint32_t s16, uint32_t zword, uint32_t& s2, uint32_t& zc_lo, uint32_t& zc_hi) {
+    auto group_consts = [&](uint32_t s16, uint32_t zword, uint32_t& s2, uint32_t& zc) {
       s2 = s16 | (s16 << 16);
       const uint32_t z = (((zword >> zsh) & 0xFu) + 1u) & 0xFu;
-      if constexpr (!kBf16) {
-        const uint32_t lo = 0x6400u | z;            // fp16(1024 + z)
-        const uint32_t hi = 0xD400u | (z << 4);     // fp16(-(64 + z))
-        zc_lo = lo | (lo << 16);
-        zc_hi = hi | (hi << 16);
-      } else {
-        const uint32_t lo = 0x4300u | z;            // bf16(128 + z)
-        zc_lo = lo | (lo << 16);
-        zc_hi = 0;
+      const uint32_t lo = (kBf16 ? 0x4300u : 0x6400u) | z;    // bf16(128 + z) / fp16(1024 + z)
+      zc = lo | (lo << 16);
+    };
+
+    // 256-row tiles: no registers for a second A set, so every wgmma group retires before the next stage
+    constexpr int kInFlight = kMT == 256 ? 0 : 1;
+    float acc[kMT / 2];
+#pragma unroll
+    for (int i = 0; i < kMT / 2; ++i) acc[i] = 0.f;
+    uint32_t a[2][16];
+
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) {
+        if constexpr (kMcast) {
+          mbar_arrive_cluster(empty(s), 0);
+          mbar_arrive_cluster(empty(s), 1);
+        } else {
+          mbar_arrive(empty(s));
+        }
       }
     };
-    const uint32_t* wsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kWOff) + nl;       // [stage][8][128] words
-    const uint16_t* ssm = reinterpret_cast<const uint16_t*>(smem_al + Smem::kSOff) + nl;       // [stage][2][128]
-    const uint32_t* zsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kZOff) + (nl >> 3);  // [stage][2][16]
 
-    int prev_s = -1;
-    for (int it = grp; it < ((p.debug & 1) ? 0 : num_it); it += kGemmGroups) {
+    auto stage = [&](auto kb_tag, int it) {
+      constexpr int kB = decltype(kb_tag)::value;
       const int s = it % kGemmStages;
-      const uint32_t ph = (it / kGemmStages) & 1;
-      const int ws = it % kGemmWStages;
-      const uint32_t wph = (it / kGemmWStages) & 1;
-      mbar_wait_spin(w_full(ws), wph);
-      const uint32_t* wp = wsm + ws * (Smem::kWStage / 4);
-      uint32_t w8[8];
+      mbar_wait_spin(b_full(s), (it / kGemmStages) & 1);
+      const uint32_t* wp = wsm + s * (Smem::kWStage / 4);
+      const uint16_t* sp = ssm + s * (Smem::kSStage / 2);
+      const uint32_t* zp = zsm + s * (Smem::kZStage / 4);
+      uint32_t s2[2][2], zc[2][2];                         // [column c0 / c0 + 8][group of k 0..31 / 32..63]
 #pragma unroll
-      for (int j = 0; j < 8; ++j) w8[j] = wp[j * kGemmBN];
-      uint32_t s2a, zla, zha, s2b, zlb, zhb;
-      group_consts(ssm[ws * (Smem::kSStage / 2)], zsm[ws * (Smem::kZStage / 4)], s2a, zla, zha);
-      if (two_groups) group_consts(ssm[ws * (Smem::kSStage / 2) + kGemmBN], zsm[ws * (Smem::kZStage / 4) + kGemmBN / 8], s2b, zlb, zhb);
-      else { s2b = s2a; zlb = zla; zhb = zha; }
-      __syncwarp();
-      if (lane == 0) mbar_arrive(w_empty(ws));          // the packed tile is in registers: its slot can be refilled
-      uint32_t v[32];
-#pragma unroll
-      for (int j = 0; j < 4; ++j) dequant_word<kBf16>(w8[j], s2a, zla, zha, &v[4 * j]);
-#pragma unroll
-      for (int j = 4; j < 8; ++j) dequant_word<kBf16>(w8[j], s2b, zlb, zhb, &v[4 * j]);
-      // software pipeline: the TMEM store of this warp's PREVIOUS stage had the whole dequant above to complete
-      if (prev_s >= 0) {
-        tmem_wait_st();
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(a_full(prev_s));
+      for (int c = 0; c < 2; ++c) {
+        const int col = c0 + 8 * c;
+        group_consts(sp[8 * c], zp[(col >> 3)], s2[c][0], zc[c][0]);
+        if (two_groups) group_consts(sp[8 * c + kGemmBN], zp[kGemmBN / 8 + (col >> 3)], s2[c][1], zc[c][1]);
+        else { s2[c][1] = s2[c][0]; zc[c][1] = zc[c][0]; }
       }
-      mbar_wait_spin(empty(s), ph ^ 1u);                // the MMA that last read this TMEM A stage has retired
-      tc_fence_after();
-      tmem_st32(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + kAColBase + s * (kGemmBK / 2), v);
-      prev_s = s;
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {  // k16 slice j = words 2j, 2j + 1
+        const int gi = j >> 1;
+#pragma unroll
+        for (int h = 0; h < 2; ++h)
+#pragma unroll
+          for (int c = 0; c < 2; ++c)
+            a[kB][4 * j + 2 * h + c] = dequant_pair<kBf16>(wp[(2 * j + h) * kGemmBN + 8 * c], t, s2[c][gi], zc[c][gi]);
+      }
+      const uint64_t bdesc = make_b_desc(smem_base + s * Smem::kBStage);
+      wgmma_fence_operands(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wgmma_tile<kMT, kBf16>(acc, &a[kB][4 * j], bdesc + 2u * j);
+      wgmma_commit();
+      wgmma_wait<kInFlight>();
+      wgmma_fence_operands(acc);
+      if (it >= kInFlight) release((it - kInFlight) % kGemmStages);
+    };
+    int it = 0;
+    for (; it + 1 < num_it; it += 2) {
+      stage(std::integral_constant<int, 0>{}, it);
+      stage(std::integral_constant<int, 1>{}, it + 1);
     }
-    if (prev_s >= 0) {
-      tmem_wait_st();
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(a_full(prev_s));
-    }
+    if (it < num_it) stage(std::integral_constant<int, 0>{}, it);
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    if (kInFlight > 0 && num_it > 0) release((num_it - 1) % kGemmStages);
 
-    // ================= epilogue =================
-    // x rows handled by one warp group: kMT / groups, but at least one 16-column TMEM load (surplus groups idle)
-    constexpr int kHalfCols = (kMT / kGemmGroups) >= 16 ? (kMT / kGemmGroups) : 16;
-    constexpr int kChunk = 16;
-    const float bias_v = (p.bias != nullptr && n_ok) ? elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(p.bias)[n]) : 0.f;
-    if (num_it > 0) {
-      mbar_wait(acc_full, 0);
-      tc_fence_after();
-    }
-    float* stage_f32 = reinterpret_cast<float*>(smem_al);    // [kMT][128] fp32, reuses the x stages
-    uint16_t* yp = reinterpret_cast<uint16_t*>(p.y);
-#pragma unroll 1
-    for (int c0 = 0; c0 < kHalfCols; c0 += kChunk) {
-      const int mcol = half * kHalfCols + c0;
-      if (mcol >= kMT) break;                                   // warp-uniform
-      uint32_t acc[kChunk];
-      if (num_it > 0) {
-        tmem_ld16(tmem_base + (static_cast<uint32_t>(quad * 32) << 16) + mcol, acc);
-        tmem_wait_ld();
-      } else {
+    // epilogue: d[4i + 2h + e] = (A row 16 w + g + 8 h, column 8 i + 2 t + e) -> fp32 staging [m][n]
+    consumer_sync();  // both warpgroups are done with the ring
 #pragma unroll
-        for (int i = 0; i < kChunk; ++i) acc[i] = 0;
-      }
-      if (p.split == 1) {
+    for (int i = 0; i < kMT / 8; ++i)
 #pragma unroll
-        for (int i = 0; i < kChunk; ++i) {
-          const int m = m0 + mcol + i;
-          if (n_ok && m < p.M) yp[static_cast<size_t>(m) * p.N + n] = float_to_elt<kBf16>(__uint_as_float(acc[i]) + bias_v);
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) stage_f32[(8 * i + 2 * t + e) * kGemmLd + c0 + 8 * h] = acc[4 * i + 2 * h + e];
+    if (p.split == 1) {
+      consumer_sync();
+      uint16_t* yp = reinterpret_cast<uint16_t*>(p.y);
+      for (int e = threadIdx.x - 128; e < kMT * kGemmBN; e += kGemmConsumers) {
+        const int ml = e / kGemmBN, nl = e % kGemmBN;
+        const int m = m0 + ml, n = n0 + nl;
+        if (m < p.M && n < p.N) {
+          float v = stage_f32[ml * kGemmLd + nl];
+          if (p.bias != nullptr) v += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(p.bias)[n]);
+          yp[static_cast<size_t>(m) * p.N + n] = float_to_elt<kBf16>(v);
         }
-      } else {
-#pragma unroll
-        for (int i = 0; i < kChunk; ++i) stage_f32[(mcol + i) * kGemmBN + nl] = __uint_as_float(acc[i]);
       }
     }
-    tc_fence_before();
   }
 
   if (p.split > 1) {
     // cluster (1,1,split): every CTA holds an fp32 partial tile [kMT][128]; rank r reduces a slice of x rows
     cg::cluster_group cluster = cg::this_cluster();
     cluster.sync();
-    const int rank = static_cast<int>(cluster.block_rank());
-    const int rows_per_rank = (kMT + p.split - 1) / p.split;
-    float* stage_f32 = reinterpret_cast<float*>(smem_al);
-    uint16_t* yp = reinterpret_cast<uint16_t*>(p.y);
-    for (int e = threadIdx.x; e < rows_per_rank * kGemmBN; e += gemm_threads(kMT)) {
-      const int ml = rank * rows_per_rank + e / kGemmBN;
-      const int nl = e % kGemmBN;
-      if (ml < kMT) {
-        float v = 0.f;
-        float rv[8];
+    if (wg > 0) {
+      const int rank = static_cast<int>(cluster.block_rank());
+      const int rows_per_rank = (kMT + p.split - 1) / p.split;
+      uint16_t* yp = reinterpret_cast<uint16_t*>(p.y);
+      for (int e = threadIdx.x - 128; e < rows_per_rank * kGemmBN; e += kGemmConsumers) {
+        const int ml = rank * rows_per_rank + e / kGemmBN;
+        const int nl = e % kGemmBN;
+        if (ml < kMT) {
+          float v = 0.f;
+          float rv[8];
 #pragma unroll
-        for (int r = 0; r < 8; ++r) rv[r] = (r < p.split) ? *cluster.map_shared_rank(&stage_f32[ml * kGemmBN + nl], r) : 0.f;
+          for (int r = 0; r < 8; ++r) rv[r] = (r < p.split) ? *cluster.map_shared_rank(&stage_f32[ml * kGemmLd + nl], r) : 0.f;
 #pragma unroll
-        for (int r = 0; r < 8; ++r) v += rv[r];
-        const int m = m0 + ml, n = n0 + nl;
-        if (m < p.M && n < p.N) {
-          if (p.bias != nullptr) v += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(p.bias)[n]);
-          yp[static_cast<size_t>(m) * p.N + n] = float_to_elt<kBf16>(v);
+          for (int r = 0; r < 8; ++r) v += rv[r];
+          const int m = m0 + ml, n = n0 + nl;
+          if (m < p.M && n < p.N) {
+            if (p.bias != nullptr) v += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(p.bias)[n]);
+            yp[static_cast<size_t>(m) * p.N + n] = float_to_elt<kBf16>(v);
+          }
         }
       }
     }
     cluster.sync();
   } else if constexpr (kMcast) {
     cg::this_cluster().sync();                     // no CTA exits while its peer can still multicast / arrive into it
-  } else {
-    __syncthreads();
   }
-  tc_fence_after();
-  if (warp == 2) tmem_dealloc<kTmemCols>(tmem_base);
 }
 
 // -------------------------------------------------------------------------------------------- host side
@@ -422,7 +332,7 @@ int launch_gemm_inst(const GemmParams& p, const CUtensorMap& tmap, const CUtenso
   }
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3((p.N + kGemmBN - 1) / kGemmBN, m_tiles, p.split);
-  cfg.blockDim = dim3(gemm_threads(kMT), 1, 1);
+  cfg.blockDim = dim3(kGemmThreads, 1, 1);
   cfg.dynamicSmemBytes = smem;
   cfg.stream = stream;
   cudaLaunchAttribute attrs[2];
@@ -461,9 +371,9 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
   const int n_tiles = (a.N + kGemmBN - 1) / kGemmBN;
   int mt = a.tile_m;
   if (mt == 0) {
-    mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : a.M <= 128 ? 128 : 256;
-    // prefer more CTAs over a taller tile while the grid does not fill the machine
-    if (mt == 256 && n_tiles * ((a.M + 255) / 256) < a.sms) mt = 128;
+    // 256-row tiles stay opt-in: their 128 accumulators per thread leave ptxas too few registers to keep wgmma
+    // asynchronous, and a 128 x 128 tile already keeps the tensor cores busier than the weight expansion
+    mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
   }
   if (mt != 32 && mt != 64 && mt != 128 && mt != 256) { snprintf(msg, msg_n, "gemm: x-row tile must be 32/64/128/256 (got %d)", mt); return -1; }
   const int m_tiles = (a.M + mt - 1) / mt;
@@ -478,11 +388,10 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
   const int mcast_req = (a.split_k >> 8) & 3;          // tests: 1 = force off, 2 = force on
   if (split == 0) {
     split = 1;
-    // split-K reduces fp32 tiles through DSMEM (~20 B/clk): only worth it for small tiles
+    // split-K reduces fp32 tiles through DSMEM: only worth it for small tiles
     if (mt <= 64)
       while (split < 8 && n_tiles * m_tiles * split < a.sms && p.num_kb / (split * 2) >= 4) split *= 2;
-    // 128-row tiles: only while the doubled grid still fits one wave (measured, tools/gemm_split_sweep.py: 4096x4096 M=128
-    // 34.2 -> 15.4 us and 11008x4096 82.4 -> 28.3 us at split 4; 4096x11008, 86 column tiles, is best unsplit)
+    // 128-row tiles: only while the doubled grid still fits one wave
     else if (mt == 128)
       while (split < 4 && n_tiles * m_tiles * split * 2 <= a.sms && p.num_kb / (split * 2) >= 4) split *= 2;
   }
@@ -490,7 +399,7 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
   while (split > 1 && split > p.num_kb) split /= 2;
   p.split = split;
   p.kb_per_split = (p.num_kb + split - 1) / split;
-  bool mcast = false;   // measured (tools/gemm_ceiling.py): pair-multicast of x does not pay - the limiter is the A-operand feed
+  bool mcast = false;   // pair-multicast of x: only on request
   if (mcast_req == 1) mcast = false;
   if (mcast_req == 2) {
     if (split != 1 || n_tiles % 2 != 0 || mt < 128) { snprintf(msg, msg_n, "gemm: multicast needs split=1, an even number of N tiles and MT>=128"); return -1; }

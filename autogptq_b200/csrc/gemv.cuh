@@ -3,14 +3,14 @@
 // Roofline: HBM.  Algorithmic bytes per launch = K*N/2 + G*N*2 + G*N/2 (+4K) + 2*M*K + 2*M*N
 // (SURVEY.md 8d); every weight byte is touched exactly once.
 //
-// Design (B200-first, not the reference's exllama/exllamav2 GEMV):
+// Design (not the reference's exllama/exllamav2 GEMV):
 //   * each lane owns 4 adjacent columns and streams 16-byte words (4 cols x 8 k) of qweight with
 //     L1-bypassing loads; a warp row-segment is kLN*16 contiguous bytes (512 B for kLN=32);
 //   * a register ring of kDepth 16-byte loads per thread is issued BEFORE griddepcontrol.wait:
 //     the weight stream of layer i+1 overlaps the tail of layer i (programmatic dependent launch);
 //   * int4 -> fp16 costs ONE LOP3 per nibble pair: the masked nibble is read as an fp16 *subnormal*
-//     (q * 2^-24 or q * 2^-20) and multiplied with x by the sm_100 mixed-precision FMA
-//     (fma.rn.f32.f16 -> SASS FHFMA, fp32 accumulate), so there is no bias subtraction and no fp16
+//     (q * 2^-24 or q * 2^-20) and multiplied with x in fp32 (exact widening: the product
+//     of two 16-bit values is exact, so fmaf rounds once; fp32 accumulate), so there is no bias subtraction and no fp16
 //     rounding anywhere in the K reduction;
 //   * the zero-point is applied per group through sum_k x_k:  y += s*(sum q x - z * sum x);
 //   * K is split over warps (shared memory), row-slots (warp shuffles) and, for small N, over the

@@ -1,4 +1,4 @@
-// Thin inline-PTX wrappers shared by the sm_100a kernels: mbarrier, TMA (cp.async.bulk.tensor), tcgen05 / TMEM.
+// Thin inline-PTX wrappers shared by the sm_90a kernels: mbarrier, TMA (cp.async.bulk.tensor), wgmma.
 #pragma once
 #include <cuda.h>  // CUtensorMap (type only)
 
@@ -59,49 +59,47 @@ __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
 }
 
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
+// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (release at cluster scope).
+__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
+  uint32_t remote;
+  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
+  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
-__device__ __forceinline__ void tc_commit_mcast(uint32_t bar, uint16_t mask) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;" ::"r"(bar), "h"(mask) : "memory");
+
+// Register budget hand-over between warpgroups (all warps of a warpgroup execute it).
+template <int kRegs> __device__ __forceinline__ void setmaxnreg_dec() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+template <int kRegs> __device__ __forceinline__ void setmaxnreg_inc() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(kRegs)); }
+
+// -------------------------------------------------------------------------------------------- wgmma (sm_90a)
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int kN> __device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(kN) : "memory"); }
+template <int kN> __device__ __forceinline__ void wgmma_fence_operands(float (&d)[kN]) {
+#pragma unroll
+  for (int i = 0; i < kN; ++i) asm volatile("" : "+f"(d[i])::"memory");
 }
-template <int kCols>
-__device__ __forceinline__ void tmem_alloc(uint32_t smem_dst) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_dst), "n"(kCols) : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-}
-template <int kCols>
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
-}
-// D[tmem] (+)= A[tmem] * B[smem desc]
-__device__ __forceinline__ void umma_ts_f16(uint32_t d_tmem, uint32_t a_tmem, uint64_t b_desc, uint32_t idesc, uint32_t accumulate) {
-  asm volatile("{\n\t.reg .pred p;\n\tsetp.ne.b32 p, %4, 0;\n\t"
-               "tcgen05.mma.cta_group::1.kind::f16 [%0], [%1], %2, %3, p;\n\t}"
-               ::"r"(d_tmem), "r"(a_tmem), "l"(b_desc), "r"(idesc), "r"(accumulate) : "memory");
-}
-__device__ __forceinline__ void tmem_st16(uint32_t taddr, const uint32_t (&v)[16]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x16.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16};"
-               ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-                 "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]) : "memory");
-}
-__device__ __forceinline__ void tmem_st32(uint32_t taddr, const uint32_t (&v)[32]) {
-  asm volatile("tcgen05.st.sync.aligned.32x32b.x32.b32 [%0], {%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,"
-               "%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32};"
-               ::"r"(taddr), "r"(v[0]), "r"(v[1]), "r"(v[2]), "r"(v[3]), "r"(v[4]), "r"(v[5]), "r"(v[6]), "r"(v[7]),
-                 "r"(v[8]), "r"(v[9]), "r"(v[10]), "r"(v[11]), "r"(v[12]), "r"(v[13]), "r"(v[14]), "r"(v[15]),
-                 "r"(v[16]), "r"(v[17]), "r"(v[18]), "r"(v[19]), "r"(v[20]), "r"(v[21]), "r"(v[22]), "r"(v[23]),
-                 "r"(v[24]), "r"(v[25]), "r"(v[26]), "r"(v[27]), "r"(v[28]), "r"(v[29]), "r"(v[30]), "r"(v[31]) : "memory");
-}
-__device__ __forceinline__ void tmem_wait_st() { asm volatile("tcgen05.wait::st.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_wait_ld() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&v)[16]) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-               : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-                 "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-               : "r"(taddr) : "memory");
-}
+
+// D[64 x N] (fp32 registers) += A[64 x 16] (registers, mma.m16n8k16 A layout per warp) * B[16 x N] (smem descriptor)
+#define AGB_D8(i) "+f"(d[i]), "+f"(d[i + 1]), "+f"(d[i + 2]), "+f"(d[i + 3]), "+f"(d[i + 4]), "+f"(d[i + 5]), "+f"(d[i + 6]), "+f"(d[i + 7])
+#define AGB_WGMMA_RS(N, TY, REGS, AB, ...)                                                                              \
+  __device__ __forceinline__ void wgmma_m64n##N##k16_##TY(float (&d)[N / 2], const uint32_t* a, uint64_t b_desc) { \
+    asm volatile("{\n\t.reg .pred p;\n\tsetp.eq.u32 p, 1, 1;\n\t"                                              \
+                 "wgmma.mma_async.sync.aligned.m64n" #N "k16.f32." #TY "." #TY " {" REGS "}, " AB ", p, 1, 1, 0;\n\t}" \
+                 : __VA_ARGS__ : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(b_desc));                               \
+  }
+#define AGB_R32 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15"
+AGB_WGMMA_RS(32, f16, AGB_R32, "{%16,%17,%18,%19}, %20", AGB_D8(0), AGB_D8(8))
+AGB_WGMMA_RS(32, bf16, AGB_R32, "{%16,%17,%18,%19}, %20", AGB_D8(0), AGB_D8(8))
+#define AGB_R64 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31"
+AGB_WGMMA_RS(64, f16, AGB_R64, "{%32,%33,%34,%35}, %36", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24))
+AGB_WGMMA_RS(64, bf16, AGB_R64, "{%32,%33,%34,%35}, %36", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24))
+#define AGB_R128 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
+AGB_WGMMA_RS(128, f16, AGB_R128, "{%64,%65,%66,%67}, %68", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56))
+AGB_WGMMA_RS(128, bf16, AGB_R128, "{%64,%65,%66,%67}, %68", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56))
+#define AGB_R256 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
+AGB_WGMMA_RS(256, f16, AGB_R256, "{%128,%129,%130,%131}, %132", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56), AGB_D8(64), AGB_D8(72), AGB_D8(80), AGB_D8(88), AGB_D8(96), AGB_D8(104), AGB_D8(112), AGB_D8(120))
+AGB_WGMMA_RS(256, bf16, AGB_R256, "{%128,%129,%130,%131}, %132", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56), AGB_D8(64), AGB_D8(72), AGB_D8(80), AGB_D8(88), AGB_D8(96), AGB_D8(104), AGB_D8(112), AGB_D8(120))
+#undef AGB_WGMMA_RS
+#undef AGB_D8
 
 }  // namespace agb

@@ -1,8 +1,8 @@
 // W4A16 "skinny" kernel for decode batches M <= 8: HBM-bound, straight from the native GPTQ layout.
 //
-// Why a second small-M kernel next to the FHFMA GEMV: at full HBM rate an SM must retire ~46 weights per
+// Why a second small-M kernel next to the CUDA-core GEMV: at full HBM rate an SM must retire ~46 weights per
 // cycle; the CUDA-core GEMV spends 13 + 8*M instructions per 8 weights and is issue-bound above ~60% of the
-// roofline (ncu: profiles/).  Here the multiply-accumulate of 8 weights x 8 activations rows is ONE warp-level
+// roofline.  Here the multiply-accumulate of 8 weights x 8 activations rows is ONE warp-level
 // tensor instruction, so the per-weight instruction cost is ~0.9 and independent of M <= 8:
 //   * a lane loads 16 bytes = 4 adjacent columns x 8 k (one k8-row); lanes (r = lane/4, c = lane%4) of a warp
 //     cover 32 columns x 4 k8-rows per step - four fully used 128-byte lines;

@@ -44,7 +44,7 @@ _PATCH_TARGETS = (
 
 
 def patch_auto_gptq() -> list:
-    """Install the B200 QuantLinear into an importable, unmodified ``auto_gptq``.
+    """Install the H100 QuantLinear into an importable, unmodified ``auto_gptq``.
 
     Rebinds ``dynamically_import_QuantLinear`` in every reference module that imported it by name
     (``modeling/_utils.py:17``, ``modeling/_base.py:44``, ...) so ``AutoGPTQForCausalLM.from_quantized``

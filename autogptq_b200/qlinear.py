@@ -1,10 +1,10 @@
-"""B200-native drop-in for ``auto_gptq.nn_modules.qlinear.*.QuantLinear`` (4-bit GPTQ, W4A16).
+"""H100-native (sm_90a) drop-in for ``auto_gptq.nn_modules.qlinear.*.QuantLinear`` (4-bit GPTQ, W4A16).
 
 Same constructor, same persistent buffers (``qweight / qzeros / scales / g_idx / bias`` - these names
 are the checkpoint keys, reference ``qlinear_cuda_old.py:50-79``), same ``post_init()`` /
 ``forward(x)`` / ``pack()`` contract as the reference modules
 (``qlinear_exllamav2.py:108-195``, ``qlinear_cuda_old.py:23-355``), but one backend only: the
-hand-written sm_100a kernels behind the C ABI in ``include/autogptq_b200.h``.  There is no Triton /
+hand-written sm_90a kernels behind the C ABI in ``include/autogptq_b200.h``.  There is no Triton /
 exllama / marlin dispatch and no CPU or PyTorch fallback: a forward without the CUDA library or on a
 non-CUDA tensor raises.
 """
@@ -66,10 +66,10 @@ class QuantLinear(nn.Module):
         super().__init__()
         if bits != 4:
             # reference: qlinear_exllamav2.py:116-118 / qlinear_exllama.py:56-59
-            raise ValueError(f"The B200 kernels only support bits=4 (GPTQ W4A16); requested bits={bits}.")
+            raise ValueError(f"The H100 kernels only support bits=4 (GPTQ W4A16); requested bits={bits}.")
         if trainable:
             # reference: qlinear_exllamav2.py:119-120
-            raise NotImplementedError("The B200 QuantLinear is inference-only (trainable=True is not supported).")
+            raise NotImplementedError("The H100 QuantLinear is inference-only (trainable=True is not supported).")
         if infeatures % 8 != 0 or outfeatures % 8 != 0:
             raise ValueError("infeatures and outfeatures must be multiples of 8 for 4-bit packing.")
         self.infeatures = infeatures
@@ -124,7 +124,7 @@ class QuantLinear(nn.Module):
                 setattr(self, name, t.contiguous())
         if self.scales.dtype not in _DTYPE_CODE:
             # fp32 checkpoints (reference CPU tests): the kernels compute with 16-bit scales
-            logger.warning("scales are %s; the B200 kernels use float16 scales", self.scales.dtype)
+            logger.warning("scales are %s; the H100 kernels use float16 scales", self.scales.dtype)
         if self.g_idx.numel() != K:
             raise NotImplementedError(
                 f"g_idx has {self.g_idx.numel()} entries for infeatures={K}: fused-QKV g_idx concatenation "
@@ -189,7 +189,7 @@ class QuantLinear(nn.Module):
             # reference casts non-half activations to half (qlinear_exllamav2.py:184-189)
             global _WARNED_CAST
             if not _WARNED_CAST:
-                logger.warning(f"The B200 kernels require float16/bfloat16 activations, got {x_dtype}. Casting to float16.")
+                logger.warning(f"The H100 kernels require float16/bfloat16 activations, got {x_dtype}. Casting to float16.")
                 _WARNED_CAST = True
             cdtype = torch.float16
         K, N = self.infeatures, self.outfeatures
@@ -217,7 +217,7 @@ class QuantLinear(nn.Module):
                     bias.data_ptr() if bias is not None else None, _DTYPE_CODE[cdtype])
             self._plans[cdtype] = plan
         fn, p_qw, p_qz, p_sc, p_perm, p_bias, code = plan
-        # decode batches run straight from the checkpoint layout, except 5..8 rows on >= 100 MB layers (tcgen05 tile)
+        # decode batches run straight from the checkpoint layout, except 5..8 rows on >= 100 MB layers (wgmma tile)
         ws_ptr, ws_bytes, p_tc = None, 0, None
         if M > 4 or self.kernel != _lib.KERNEL_AUTO:
             big_m = M > _lib.IMMA_MAX_M or (M >= 5 and K * N >= 1.0e8 and not (M == 5 and self.group_size % 128 == 0 and K % 128 == 0))
@@ -288,13 +288,13 @@ class QuantLinear(nn.Module):
 
     def extra_repr(self) -> str:
         return (f"in_features={self.infeatures}, out_features={self.outfeatures}, bits=4, "
-                f"group_size={self.group_size}, bias={self.bias is not None}, backend=sm_100a")
+                f"group_size={self.group_size}, bias={self.bias is not None}, backend=sm_90a")
 
 
 # ---------------------------------------------------------------------------------------------------------------
-# Next-layer L2 prefetch (opt-in; measured slower on B200, see csrc/common.cuh).  Decode runs the same sequence of
+# Next-layer L2 prefetch (opt-in; see csrc/common.cuh).  Decode runs the same sequence of
 # QuantLinear launches for every token.  The first time the sequence is seen each launch learns its successor; from then
-# on it tells its kernel which weights come next (agb200_w4_prefetch_hint) and the kernel pulls them into the 126 MB L2
+# on it tells its kernel which weights come next (agb200_w4_prefetch_hint) and the kernel pulls them into the L2
 # while it computes.  Hints only: a changed call order costs some bandwidth until the chain is re-learned, never
 # correctness.
 _CHAIN = {"enabled": False, "last": None}

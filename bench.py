@@ -1,12 +1,12 @@
 #!/usr/bin/env python
 """bench.py - headline benchmark of the W4A16 QuantLinear hot path (driver contract).
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--dump-outputs DIR]
 
 Default workload = BASELINE.json configs[1]: Llama-2-7B int4 g=128 decode, bs=1.  One "step" = one decode
 token = the 224 QuantLinear forwards of the model (32 blocks x {q,k,v,o 4096->4096; gate,up 4096->11008;
 down 11008->4096}) at M=1, chained through their real data dependencies, on synthetic random-packed
-weights (SURVEY.md 8d).  The 3.5 GB weight set is far larger than the 126 MB L2, so every step streams the
+weights (SURVEY.md 8d).  The 3.5 GB weight set is far larger than the 50 MB L2, so every step streams the
 weights from HBM.  N>1: one replica per GPU (the 7B model fits one GPU; north_star shards only models that
 overflow), no data-path collective, weak scaling; value = tokens/s summed over ranks, time = max over ranks.
 
@@ -19,6 +19,8 @@ overflow), no data-path collective, weak scaling; value = tokens/s summed over r
              qlinear_cuda_old.py:291-355) timed on this box's host cores on one decoder block.
 
 --impl reference times that CPU path alone (rank 0 only) and prints the same JSON shape.
+--dump-outputs DIR writes what the timed path computed in its last timed step (rank 0) as DIR/<name>.npy (float32);
+weights and inputs are seeded, so two builds can be compared output for output.
 """
 from __future__ import annotations
 
@@ -68,7 +70,8 @@ def load_peaks():
     try:
         return json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json"))), "measured"
     except Exception:
-        return {"hbm_gbs": 6650.0, "bf16_tflops": 1590.0, "bf16_tflops_sustained": 1400.0}, "fallback"
+        # H100 SXM data sheet (700 W): 3.35 TB/s HBM3, 989 TFLOP/s dense BF16 - not measured figures
+        return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "bf16_tflops_sustained": 989.0}, "fallback (H100 SXM data sheet)"
 
 
 # ------------------------------------------------------------------------------------------- clocks
@@ -333,12 +336,18 @@ def cpu_block_time_qigen(hidden, inter, M, reps):
 def shared_config(workload, desc, n_calls):
     """The `config` object both arms print (the driver compares them): what is measured, nothing about how."""
     return {"workload": workload, "desc": desc, "group_size": GROUP, "layers_per_step": n_calls,
-            "l2": "weight working set 3.5 GB >> 126 MB L2 (no flush needed)"}
+            "l2": "weight working set 3.5 GB >> 50 MB L2 (no flush needed)"}
 
 
 def cpu_rows_for(M):
     # bound the CPU sample for the prefill workload: the python path is O(M) in the matmul only
     return min(M, 64)
+
+
+def dump_outputs(out_dir, arrays):
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, name + ".npy"), t.detach().float().cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------- main arms
@@ -405,7 +414,9 @@ def run_b200(args, rank, world, local_rank):
     bytes_per_step = n_blocks * sum(alg_bytes(M, K, N, GROUP) for (_, K, N) in block_shapes(hidden, inter))
     flops_per_step = n_blocks * sum(2.0 * M * K * N for (_, K, N) in block_shapes(hidden, inter))
 
-    x_dev = torch.randn(M, hidden, dtype=torch.float16, device=dev)
+    gen_x = torch.Generator(device=dev)
+    gen_x.manual_seed(4321 + rank)
+    x_dev = torch.randn(M, hidden, dtype=torch.float16, device=dev, generator=gen_x)
     x_host = torch.randn(M, hidden, dtype=torch.float16).pin_memory()
     y_host = torch.empty(M, hidden, dtype=torch.float16).pin_memory()
     x_in = torch.empty(M, hidden, dtype=torch.float16, device=dev)
@@ -425,7 +436,7 @@ def run_b200(args, rank, world, local_rank):
             try:
                 chain, ch_x, ch_y = build_chain(model, M, dev)
                 chain_info = chain.info()
-            except (NotImplementedError, autogptq_b200._lib.B200KernelError) as exc:
+            except (NotImplementedError, _lib.B200KernelError) as exc:
                 # creation refused (no cooperative launch, not enough shared memory, ...): the per-layer launches are
                 # still this repo's kernels; the line says which path ran
                 chain_error = str(exc)[:300]
@@ -497,6 +508,9 @@ def run_b200(args, rank, world, local_rank):
         ms_dev = timed(g_dev, args.steps)
         t1 = time.time()
         clocks = sampler.stop(t0, t1) if rank == 0 else None
+        if args.dump_outputs and rank == 0:
+            # the token's output after the last timed replay (the e2e graph below overwrites the chain's input)
+            dump_outputs(args.dump_outputs, {"y": ch_y if use_chain else y_dev})
 
         feed = [torch.randn(M, hidden, dtype=torch.float16) for _ in range(4)]
         checksum = [0.0]
@@ -570,7 +584,7 @@ def run_b200(args, rank, world, local_rank):
                 pk = load_peaks()[0]
                 prefill_rec = {"workload": "llama2-7b-prefill-bs8x2048", "M": Mp, "ms_per_step": ms_p, "tflops": fl / ms_p / 1e9,
                                "tokens_per_s": Mp / (ms_p / 1e3), "frac_of_sustained_bf16_peak": fl / ms_p / 1e9 / pk.get("bf16_tflops_sustained", pk["bf16_tflops"]),
-                               "kernel": "w4a16_gemm_kernel (tcgen05 / TMEM / TMA)", "steps": n_p}
+                               "kernel": "w4a16_gemm_kernel (wgmma / TMA)", "steps": n_p}
                 del xp
             except Exception as e:
                 prefill_rec = {"error": f"{type(e).__name__}: {e}"[:200]}
@@ -659,7 +673,7 @@ def build_tp_blocks(hidden, inter, kv, n_blocks, rank, world, dev, log=None):
     return blocks
 
 
-def tp_chain_record(args, rank, world, local_rank, n_blocks=None, steps=None):
+def tp_chain_record(args, rank, world, local_rank, n_blocks=None, steps=None, dump=False):
     """Llama-2-70B decode, QuantLinears column/row-sharded over `world` ranks (BASELINE configs[3]): one persistent
     chain launch per rank and token, the row-parallel all-reduces fused into it (tagged words over NVLink peer memory,
     autogptq_b200.tp.TPDecodeChain), replayed as a CUDA graph.  Returns the record (rank 0) or None."""
@@ -676,7 +690,7 @@ def tp_chain_record(args, rank, world, local_rank, n_blocks=None, steps=None):
               (hidden, inter // world), (hidden, inter // world), (inter // world, hidden)]
     bytes_per_rank_step = n_blocks * sum(alg_bytes(M, K, N, GROUP) for (K, N) in shapes)
     tp = TPDecodeChain(blocks, group=None, M=M, device=dev)
-    x = torch.randn(M, hidden, dtype=torch.float16, device=dev)
+    x = torch.randn(M, hidden, dtype=torch.float16, device=dev, generator=torch.Generator(device=dev).manual_seed(4321))
     stream = torch.cuda.Stream(device=dev)
     with torch.cuda.stream(stream):
         tp.x.copy_(x)
@@ -703,6 +717,8 @@ def tp_chain_record(args, rank, world, local_rank, n_blocks=None, steps=None):
         ms = torch.tensor([e0.elapsed_time(e1)], device=dev, dtype=torch.float64)
         if world > 1:
             dist.all_reduce(ms, op=dist.ReduceOp.MAX)
+        if dump and rank == 0:
+            dump_outputs(args.dump_outputs, {"y": tp.output()})
     ms = float(ms.item())
     info = tp.chain.info()
     del tp, blocks
@@ -735,7 +751,7 @@ def run_tp(args, rank, world, local_rank):
     if rank == 0:
         sampler.start()
     t0 = time.time()
-    rec = tp_chain_record(args, rank, world, local_rank, steps=args.steps)
+    rec = tp_chain_record(args, rank, world, local_rank, steps=args.steps, dump=bool(args.dump_outputs))
     t1 = time.time()
     if rank == 0:
         clocks = sampler.stop(t0, t1)
@@ -767,6 +783,7 @@ def main():
     ap.add_argument("--impl", default="b200", choices=["b200", "reference"])
     ap.add_argument("--workload", default="llama2-7b-decode-bs1", choices=sorted(WORKLOADS) + sorted(TP_WORKLOADS))
     ap.add_argument("--prefetch", action="store_true", help="switch the learned next-layer L2 prefetch of decode launches on (experiment; measured slower)")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's outputs as DIR/<name>.npy")
     ap.add_argument("--siblings", default="chain", choices=["chain", "group", "branches", "serial"],
                     help="how the token's layers are issued: chain = the whole token as one persistent launch (decode, M <= 2); otherwise per-layer launches with sibling layers (q|k|v, gate|up) as one grouped launch, parallel graph branches, or serially")
     args = ap.parse_args()

@@ -1,5 +1,5 @@
 /*
- * autogptq_b200.h - C ABI of the B200-native GPTQ W4A16 QuantLinear hot path.
+ * autogptq_b200.h - C ABI of the H100-native (sm_90a) GPTQ W4A16 QuantLinear hot path.
  *
  * Drop-in boundary (SURVEY.md 8b).  Every entry point replaces a pybind11 torch-extension
  * function the reference's QuantLinear modules call today; the reference interface each
@@ -51,11 +51,11 @@ extern "C" {
 
 /* kernel selection for agb200_w4a16_forward_ex */
 #define AGB200_KERNEL_AUTO 0
-#define AGB200_KERNEL_GEMV 1   /* CUDA-core FHFMA GEMV, M <= AGB200_GEMV_MAX_M per pass (AUTO: M = 1) */
-#define AGB200_KERNEL_GEMM 2   /* tcgen05 / TMEM tensor-core GEMM */
+#define AGB200_KERNEL_GEMV 1   /* CUDA-core GEMV, M <= AGB200_GEMV_MAX_M per pass (AUTO: M = 1) */
+#define AGB200_KERNEL_GEMM 2   /* wgmma tensor-core GEMM (sm_90a) */
 #define AGB200_KERNEL_SKINNY 3 /* decode batches M <= 8: warp-level MMA on subnormal-encoded nibbles, cluster split-K (AUTO: M = 5..8) */
 #define AGB200_KERNEL_DECODE 4 /* experimental: M <= 8, TMA-staged persistent CTAs (not picked by AUTO; AGB200_ENOSUP unless the library was built with -DAGB200_EXPERIMENTAL_KERNELS) */
-#define AGB200_KERNEL_TCDECODE 5 /* experimental: M <= 16 on tcgen05, unpack-only + per-group TMEM accumulators (needs qweight_tc; not picked by AUTO; same build flag) */
+#define AGB200_KERNEL_TCDECODE 5 /* reserved: a tensor-memory decode kernel sm_90a cannot run; always AGB200_ENOSUP */
 #define AGB200_KERNEL_IMMA 6 /* decode batches M <= 8: integer tensor cores on raw nibbles, x as 24-bit block fixed point (AUTO: M = 2..4) */
 #define AGB200_GEMV_MAX_M 4
 #define AGB200_SKINNY_MAX_M 8
@@ -81,7 +81,7 @@ int agb200_device_count(void);
  *   x, y      [M,K] / [M,N], row-major, dtype `dtype`; y is caller-allocated
  *             (qlinear_exllamav2.py:39 torch.empty).
  *   qweight_tc  NULL, or the tensor-core copy of qweight made by agb200_w4_prepare_tc (same shape; nibbles of
- *             every word reordered so that adjacent k unpack into one 16-bit pair).  Needed by the tcgen05 path
+ *             every word reordered so that adjacent k unpack into one 16-bit pair).  Needed by the wgmma path
  *             (M > 8); the decode kernels (M <= 8) read the checkpoint layout `qweight` directly.  This is the
  *             analogue of the load-time shuffle the reference does IN PLACE (exllamav2/cuda/q_matrix.cu:19-42).
  *   perm      NULL, or int32[K]: x column gathered for sorted row j is perm[j]; qweight must then be
@@ -285,7 +285,7 @@ int agb200_w4_dequantize(const int32_t* qweight, const int32_t* qzeros, const vo
 int agb200_permute_columns(const void* x, const int32_t* perm, void* x_out, int M, int K, int dtype,
                            void* stream);
 
-/* Static facts about the build, for logs: returns e.g. "sm_100a tcgen05+tma gemv=fhfma". */
+/* Static facts about the build, for logs: returns e.g. "autogptq_b200 sm_90a: ... gemm=wgmma ...". */
 const char* agb200_build_info(void);
 
 #ifdef __cplusplus

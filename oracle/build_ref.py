@@ -1,4 +1,4 @@
-"""Compile the REFERENCE's own CUDA kernels for sm_100a from the sources where they lie under
+"""Compile the REFERENCE's own CUDA kernels for sm_90a from the sources where they lie under
 /root/reference, outputs only into oracle/_ref/ (git-ignored, travels to the GPU box).
 
     python oracle/build_ref.py [exllamav2] [marlin]
@@ -25,7 +25,7 @@ ALIASES = {"exllamav2": "exllamav2_kernels", "marlin": "autogptq_marlin_cuda"}
 def build(name):
     from torch.utils import cpp_extension
 
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0a")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0a")
     os.environ.setdefault("CXX", "/usr/bin/g++")
     os.environ.setdefault("MAX_JOBS", "4")
     bdir = os.path.join(OUT, name)

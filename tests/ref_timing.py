@@ -1,4 +1,4 @@
-"""Timing of the reference's own CUDA kernels rebuilt for sm_100a (oracle/_ref, built by oracle/build_ref.py) - the on-box
+"""Timing of the reference's own CUDA kernels rebuilt for sm_90a (oracle/_ref, built by oracle/build_ref.py) - the on-box
 performance baselines of tools/microbench.py.  Kept under tests/ because only tests/, smoke() and bench.py's CPU-baseline
 leg may import anything from oracle/; not a test module (no test_ prefix), never imported by the product."""
 import os
@@ -9,7 +9,7 @@ import torch
 
 
 def time_reference(emit, K, N, g, L, quick, alg_bytes):
-    """The reference's own CUDA kernels rebuilt for sm_100a (oracle/_ref): exllamav2 (decode default) and Marlin."""
+    """The reference's own CUDA kernels rebuilt for sm_90a (oracle/_ref): exllamav2 (decode default) and Marlin."""
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     from oracle import ref_kernels
 

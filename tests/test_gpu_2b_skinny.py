@@ -1,4 +1,6 @@
 """GPU parity: the skinny (M <= 8) decode kernel through the QuantLinear module / C ABI vs the oracle."""
+import os
+
 import numpy as np
 import pytest
 import torch
@@ -79,21 +81,20 @@ def test_skinny_agrees_with_gemv_bitwise_tolerance():
     assert_parity(y_s, y_v, rtol=1e-3, atol_rms=6e-4, what="skinny vs gemv")
 
 
-def test_reference_exllamav2_kernel_agrees():
-    """The reference's own default 4-bit CUDA kernel (compiled from /root/reference into oracle/_ref by
-    oracle/build_ref.py) on the same packed buffers - tolerance of tests/test_q4.py:1120,1941."""
-    from oracle import ref_kernels
+def test_reference_exllamav2_kernel_agrees(golden_dir):
+    """The reference's own default 4-bit CUDA kernel (exllamav2) on the same packed buffers - tolerance of
+    tests/test_q4.py:1120,1941.  Its outputs are stored in tests/golden/kernel_exllamav2.npz (written on an H100 by
+    tests/golden/make_golden_kernels.py from the kernel built by oracle/build_ref.py)."""
+    from tests.golden.make_golden_kernels import EXL_G, EXL_K, EXL_MS, EXL_N, EXL_SEED
 
-    if ref_kernels.exllamav2() is None:
-        pytest.skip("oracle/_ref/exllamav2_kernels not built")
-    K, N, g = 1024, 1024, 128
-    d = O.random_packed(K, N, g, seed=43)
+    K, N, g = EXL_K, EXL_N, EXL_G
+    d = O.random_packed(K, N, g, seed=EXL_SEED)
     lin = make_layer(d)
-    ref = ref_kernels.ExllamaV2Layer(lin.qweight, lin.qzeros, lin.scales, K, N)
-    for M in (1, 8, 64):
+    golden = np.load(os.path.join(golden_dir, "kernel_exllamav2.npz"))
+    for M in EXL_MS:
         x = torch.from_numpy(rand_x(M, K, seed=M)).cuda()
         y = lin(x).float()
-        y_ref = ref(x).float()
+        y_ref = torch.from_numpy(golden[f"y_{M}"].astype(np.float32)).cuda()
         torch.cuda.synchronize()
         rms = y_ref.pow(2).mean().sqrt().item()
         assert (y - y_ref).abs().max().item() <= 1e-2 * rms + 2e-2, f"M={M}"

@@ -1,4 +1,4 @@
-"""GPU parity: the tcgen05 tensor-core GEMM through the QuantLinear module / C ABI vs the oracle."""
+"""GPU parity: the wgmma tensor-core GEMM through the QuantLinear module / C ABI vs the oracle."""
 import numpy as np
 import pytest
 import torch

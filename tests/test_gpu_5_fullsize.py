@@ -43,7 +43,7 @@ def test_full_size_vs_dense(K, N, g, M):
 @pytest.mark.parametrize("K,N", [(8192, 28672), (28672, 8192)])
 @pytest.mark.parametrize("M", [1, 3, 5, 16])
 def test_llama70b_layer_sizes_vs_dense(K, N, M):
-    """BASELINE config 4 shapes: GEMV (M=1), persistent integer kernel incl. its K-chunked form (M=3, 5), tcgen05 tile (M=16)."""
+    """BASELINE config 4 shapes: GEMV (M=1), persistent integer kernel incl. its K-chunked form (M=3, 5), wgmma tile (M=16)."""
     d = O.random_packed(K, N, 128, seed=K % 89 + M)
     lin = make_layer(d)
     torch.manual_seed(M)

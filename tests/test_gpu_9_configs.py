@@ -2,7 +2,7 @@
 repo's kernels:
 
   (a) Llama-2-70B layer sizes WITH desc_act (config 4) at decode batches M = 1, 3, 8, 64;
-  (b) the prefill configuration M = 16384 (config 3): multi-M-tile grid of the tcgen05 kernel, strided sample of rows;
+  (b) the prefill configuration M = 16384 (config 3): multi-M-tile grid of the wgmma kernel, strided sample of rows;
   (c) the sweep of config 5: (K, N) in {4096, 11008}^2 x g in {32, -1} x M in {1, 8, 64, 512};
   (d) bit-exact full-size dequantisation (anchors `_dense_ref` of test_gpu_5_fullsize.py);
   (e) two devices driven from ONE process (accelerate device_map style, modeling/_utils.py:341-377);

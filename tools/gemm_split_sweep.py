@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""Sweep of the tcgen05 GEMM's x-row tile and split-K for small M (measurement aid for the launch heuristic)."""
+"""Sweep of the wgmma GEMM's x-row tile and split-K for small M (measurement aid for the launch heuristic)."""
 import json
 import os
 import sys

@@ -80,7 +80,7 @@ def time_config(lib, L, M, kernel, tune, iters=5, dev="cuda"):
 
 
 def time_reference(emit, K, N, g, L, quick):
-    """The reference's own CUDA kernels rebuilt for sm_100a: lives in tests/ (only tests/ may touch oracle/)."""
+    """The reference's own CUDA kernels rebuilt for sm_90a: lives in tests/ (only tests/ may touch oracle/)."""
     sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
     from tests.ref_timing import time_reference as _impl
 

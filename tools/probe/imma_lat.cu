@@ -1,5 +1,5 @@
-// Latency / throughput of mma.sync.m16n8k32.s32.u8.s8 (IMMA.16832) and of the LDS -> LOP3 -> IMMA chain on sm_100a.
-// nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o imma_lat imma_lat.cu && ./imma_lat
+// Latency / throughput of mma.sync.m16n8k32.s32.u8.s8 (IMMA.16832) and of the LDS -> LOP3 -> IMMA chain on sm_90a.
+// nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o imma_lat imma_lat.cu && ./imma_lat
 #include <cstdio>
 #include <cuda_runtime.h>
 __device__ __forceinline__ void imma(int (&d)[4], unsigned a0, unsigned a1, unsigned a2, unsigned a3, unsigned b0, unsigned b1) {

@@ -4,7 +4,7 @@
 // Prints, per kernel boundary: [last CTA of kernel i ends] -> [first / median / last CTA of kernel i+1 passes the wait],
 // how early kernel i+1's CTAs started, and the kernel's own streaming time - for several per-kernel byte counts.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probe/pdl_phase_probe tools/probe/pdl_phase_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probe/pdl_phase_probe tools/probe/pdl_phase_probe.cu
 // Run:   tools/probe/pdl_phase_probe            (one line of JSON per configuration)
 #include <algorithm>
 #include <cstdio>

@@ -1,6 +1,6 @@
-// Issue-rate probe for the instruction mixes the int4 decode kernels are built from (sm_100a).
+// Issue-rate probe for the instruction mixes the int4 decode kernels are built from (sm_90a).
 // Prints cycles per warp-instruction per SM sub-partition (lower = faster) with 8 warps per sub-partition.
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o tools/probe/pipe_probe tools/probe/pipe_probe.cu
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o tools/probe/pipe_probe tools/probe/pipe_probe.cu
 #include <cstdio>
 #include <cstdint>
 #include <cuda_runtime.h>
@@ -8,8 +8,8 @@
 #define REP8(X) X(0) X(1) X(2) X(3) X(4) X(5) X(6) X(7)
 
 enum Kind { FFMA, FHFMA, HFMA2, IMAD, IDP4A, IDP2A, LOP3, SHF, MIX_FH, MIX_DP4, MIX_DP2, MIX_DP4_IMADSHIFT, IMMA, HMMA, MIX_IMMA, MIX_IMMA3, NKIND };
-static const char* kNames[NKIND] = {"ffma", "fhfma(f32+=f16*f16)", "hfma2", "imad", "idp4a", "idp2a", "lop3", "shf",
-                                     "mix: 4lop3+1shf+8fhfma /word", "mix: 2lop3+1shf+4idp4a /word",
+static const char* kNames[NKIND] = {"ffma", "cvt f16->f32 + ffma", "hfma2", "imad", "idp4a", "idp2a", "lop3", "shf",
+                                     "mix: 4lop3+1shf+8(cvt+ffma) /word", "mix: 2lop3+1shf+4idp4a /word",
                                      "mix: 2lop3+1shf+4idp2a /word", "mix: 2lop3+1imad.hi-shift+4idp4a /word",
                                      "imma.m16n8k32.u8.s8", "hmma.m16n8k16.f16.f32acc", "mix: 16B load worth = 4shf+8lop3+2imma", "mix: 4shf+8lop3+6imma (M=8)"};
 static const int kInstrPerIter[NKIND] = {8, 8, 8, 8, 8, 8, 8, 8, 13 * 4, 7 * 4, 7 * 4, 7 * 4, 8, 8, 14, 18};
@@ -33,7 +33,7 @@ __global__ void __launch_bounds__(1024, 1) probe(uint32_t* out, long long* cycle
       REP8(X)
 #undef X
     } else if constexpr (kKind == FHFMA) {
-#define X(i) asm volatile("{.reg .b16 lo, hi, xl, xh; mov.b32 {lo,hi}, %1; mov.b32 {xl,xh}, %2; fma.rn.f32.f16 %0, lo, xl, %0;}" : "+f"(f[i]) : "r"(w[i & 3]), "r"(x[i & 3]));
+#define X(i) asm volatile("{.reg .b16 lo, hi, xl, xh; mov.b32 {lo,hi}, %1; mov.b32 {xl,xh}, %2; .reg .f32 a, b; cvt.f32.f16 a, lo; cvt.f32.f16 b, xl; fma.rn.f32 %0, a, b, %0;}" : "+f"(f[i]) : "r"(w[i & 3]), "r"(x[i & 3]));
       REP8(X)
 #undef X
     } else if constexpr (kKind == HFMA2) {
@@ -69,7 +69,7 @@ __global__ void __launch_bounds__(1024, 1) probe(uint32_t* out, long long* cycle
         asm volatile("and.b32 %0, %1, 0x00f000f0;" : "=r"(q1) : "r"(w[c]));
         asm volatile("and.b32 %0, %1, 0x000f000f;" : "=r"(q2) : "r"(t));
         asm volatile("and.b32 %0, %1, 0x00f000f0;" : "=r"(q3) : "r"(t));
-#define FH(acc, q, xx) asm volatile("{.reg .b16 lo, hi, xl, xh; mov.b32 {lo,hi}, %1; mov.b32 {xl,xh}, %2; fma.rn.f32.f16 %0, lo, xl, %0; fma.rn.f32.f16 %0, hi, xh, %0;}" : "+f"(acc) : "r"(q), "r"(xx));
+#define FH(acc, q, xx) asm volatile("{.reg .b16 lo, hi, xl, xh; mov.b32 {lo,hi}, %1; mov.b32 {xl,xh}, %2; .reg .f32 a, b; cvt.f32.f16 a, lo; cvt.f32.f16 b, xl; fma.rn.f32 %0, a, b, %0; cvt.f32.f16 a, hi; cvt.f32.f16 b, xh; fma.rn.f32 %0, a, b, %0;}" : "+f"(acc) : "r"(q), "r"(xx));
         FH(f[c], q0, x[0]) FH(f[4 + c], q1, x[1]) FH(f[c], q2, x[2]) FH(f[4 + c], q3, x[3])
 #undef FH
         w[c] += r[0];   // keeps the unpack loop-variant (1 extra IADD per word is counted in the loop overhead)
