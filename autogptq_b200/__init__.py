@@ -6,9 +6,11 @@ Only what the path needs lives here:
   import_utils.py  mirror of ``dynamically_import_QuantLinear`` + the patch that installs it into auto_gptq
   sharding.py      column/row tensor-parallel slicing of packed layers (SURVEY.md 8e)
   tp.py            column/row parallel modules: one NCCL all-reduce per row-parallel layer
+  moe.py           QuantExperts: the routed experts of a Mixtral-style block as one grouped forward
   checkpoint.py    safetensors GPTQ checkpoint -> QuantLinear modules, TP-aware (SURVEY.md 8f rank 1; `from autogptq_b200 import checkpoint`)
 """
 __version__ = "0.1.0"
 
 from .import_utils import dynamically_import_QuantLinear, patch_auto_gptq  # noqa: E402,F401
 from .qlinear import QuantLinear, forward_group, set_next_layer_prefetch  # noqa: E402,F401
+from .moe import QuantExperts, group_experts  # noqa: E402,F401

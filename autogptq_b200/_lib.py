@@ -12,7 +12,7 @@ from ctypes import c_char_p, c_int, c_size_t, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 4
+ABI_VERSION = 5
 F16, BF16 = 0, 1
 CHAIN_MAX_M = 2
 CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS = 0, 1, 2
@@ -22,6 +22,9 @@ KERNEL_AUTO, KERNEL_GEMV, KERNEL_GEMM, KERNEL_SKINNY, KERNEL_DECODE, KERNEL_TCDE
 GEMV_MAX_M = 4
 SKINNY_MAX_M = 8
 IMMA_MAX_M = 8
+MOE_DECODE_MAX_T = 8
+MOE_MAX_EXPERTS = 256
+MOE_INDEX_I32, MOE_INDEX_I64, MOE_WEIGHTS_F32 = 0, 1, 2
 
 _lib = None
 
@@ -62,6 +65,11 @@ def _declare(lib):
         "agb200_peer_export": (I, [P, P]),
         "agb200_peer_open": (I, [P, P]),
         "agb200_peer_close": (I, [P]),
+        "agb200_moe_plan_bytes": (S, [I, I, I, I]),
+        "agb200_moe_create": (I, [P, I, I, I, I, I, P, S, P]),
+        "agb200_moe_workspace_bytes": (S, [I, I, I, I, I]),
+        "agb200_moe_forward": (I, [P, P, P, I, P, I, I, I, P, P, S, P]),
+        "agb200_moe_destroy": (I, [P]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 4
+#define AGB200_ABI_VERSION 5
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -233,6 +233,65 @@ int agb200_peer_free(void* ptr);
 int agb200_peer_export(const void* ptr, void* handle_out /* AGB200_PEER_HANDLE_BYTES */);
 int agb200_peer_open(const void* handle /* AGB200_PEER_HANDLE_BYTES */, void** ptr_out);
 int agb200_peer_close(void* ptr);
+
+/*
+ * Grouped mixture-of-experts forward (ABI v5): the routed experts of a Mixtral-style block, every expert's w1 (gate),
+ * w3 (up) and w2 (down) a 4-bit GPTQ layer.
+ *
+ *   out[t] = sum over j < k with 0 <= e_j < E of  w[t,j] * W2_{e_j}( silu(W1_{e_j} x[t]) * W3_{e_j} x[t] ),
+ *   e_j = top_k_index[t, j]
+ *
+ * Replaces the experts loop of transformers' MixtralExperts.forward (transformers/models/mixtral/modeling_mixtral.py:74-98:
+ * nonzero() over the routing mask, then per hit expert QuantLinear calls, act_fn(gate) * up and index_add_) for the
+ * experts the reference quantises (auto_gptq/modeling/mixtral.py:4-39).  An id outside [0, E) contributes nothing (the
+ * `expert_idx == num_experts` skip, modeling_mixtral.py:88).  Routing stays on the device: T and k are the only sizes the
+ * host needs, nothing synchronises with the host, so the call can be captured in a CUDA graph and replayed with new
+ * top_k_index / top_k_weights.  Two runs on the same inputs give bit-identical outputs (no atomics).
+ *
+ *   experts   E descriptors; every expert has the same H (hidden size), I (intermediate size) and group_size
+ *             (-1 = one group over each layer's K).  Act-order layers: qweight is the matrix made by
+ *             agb200_w4_make_sequential and perm its permutation; w1 and w3 of an expert must then share ONE perm
+ *             pointer.  qweight_tc (agb200_w4_prepare_tc of qweight) is needed for T > AGB200_MOE_DECODE_MAX_T and must
+ *             be given for every layer of every expert or for none.  bias may be NULL.
+ *   x, out    [T, H] of `dtype`; top_k_index [T, k] (AGB200_MOE_INDEX_I32 / _I64); top_k_weights [T, k] of `dtype`
+ *             or AGB200_MOE_WEIGHTS_F32.  All device pointers, 16-byte aligned.
+ *   plan      caller-owned DEVICE memory of agb200_moe_plan_bytes(...) bytes, 256-byte aligned, alive and untouched until
+ *             agb200_moe_destroy (expert table, TMA tensor maps, inverse permutations).
+ *   workspace DEVICE scratch of agb200_moe_workspace_bytes(T, k, E, H, I) bytes (routing tables, gathered rows,
+ *             intermediate activations, per-pair outputs).
+ * Constraints (else AGB200_ENOSUP): 1 <= E <= AGB200_MOE_MAX_EXPERTS, H % 128 == 0, I % 128 == 0, group_size 32 or a
+ * multiple of 64 (or -1), 16 * H bytes of x rows fit in shared memory (H <= 13824 on H100).
+ * T <= AGB200_MOE_DECODE_MAX_T runs the decode kernels (weights streamed from the checkpoint layout), larger T the
+ * grouped wgmma GEMM; T = 0 does nothing.
+ */
+#define AGB200_MOE_MAX_EXPERTS 256
+#define AGB200_MOE_DECODE_MAX_T 8
+#define AGB200_MOE_INDEX_I32 0
+#define AGB200_MOE_INDEX_I64 1
+#define AGB200_MOE_WEIGHTS_F32 2   /* weights_dtype: AGB200_F16 / AGB200_BF16 (the activation dtype) or fp32 */
+
+typedef struct agb200_moe_layer {
+  const int32_t* qweight;     /* [K/8, N] (row-sorted copy for act-order layers) */
+  const int32_t* qweight_tc;  /* tensor-core copy or NULL */
+  const int32_t* qzeros;      /* [G, N/8] */
+  const void* scales;         /* [G, N] of the dtype */
+  const int32_t* perm;        /* int32[K] or NULL */
+  const void* bias;           /* [N] or NULL */
+} agb200_moe_layer;
+
+typedef struct agb200_moe_expert {
+  agb200_moe_layer w1;        /* gate: K = H, N = I */
+  agb200_moe_layer w3;        /* up:   K = H, N = I */
+  agb200_moe_layer w2;        /* down: K = I, N = H */
+} agb200_moe_expert;
+
+size_t agb200_moe_plan_bytes(int E, int H, int I, int group_size);
+int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int group_size, int dtype, void* plan,
+                      size_t plan_bytes, void** handle_out);
+size_t agb200_moe_workspace_bytes(int T, int k, int E, int H, int I);
+int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
+                       int weights_dtype, int T, int k, void* out, void* workspace, size_t workspace_bytes, void* stream);
+int agb200_moe_destroy(void* handle);
 
 /*
  * Next-layer prefetch hint (optional, decode): names up to 8 device ranges - typically the packed weights and scales of
