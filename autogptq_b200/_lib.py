@@ -7,12 +7,12 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_char_p, c_int, c_size_t, c_void_p
+from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 5
+ABI_VERSION = 6
 F16, BF16 = 0, 1
 CHAIN_MAX_M = 2
 CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS = 0, 1, 2
@@ -70,6 +70,9 @@ def _declare(lib):
         "agb200_moe_workspace_bytes": (S, [I, I, I, I, I]),
         "agb200_moe_forward": (I, [P, P, P, I, P, I, I, I, P, P, S, P]),
         "agb200_moe_destroy": (I, [P]),
+        "agb200_gptq_hessian_update": (I, [P, P, I, I, I, c_float, c_float, P]),
+        "agb200_gptq_quantize": (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, I, P, S, P]),
+        "agb200_gptq_workspace_bytes": (S, [I, I, I]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

@@ -29,7 +29,7 @@ NVCC_FLAGS = [
 if os.environ.get("AGB200_EXPERIMENTAL", "0") == "1":      # the two decode kernel families AUTO never selects (DESIGN.md 3.6)
     NVCC_FLAGS.append("-DAGB200_EXPERIMENTAL_KERNELS")
 # translation units of the library (compiled in parallel, then linked)
-UNITS = ["abi.cu", "chain.cu", "moe.cu"]
+UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu"]
 # chain.cu holds only the 448-thread persistent chain kernel (one CTA per SM)
 UNIT_FLAGS = {"chain.cu": ["-maxrregcount=112"]}
 

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 5
+#define AGB200_ABI_VERSION 6
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -292,6 +292,47 @@ size_t agb200_moe_workspace_bytes(int T, int k, int E, int H, int I);
 int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
                        int weights_dtype, int T, int k, void* out, void* workspace, size_t workspace_bytes, void* stream);
 int agb200_moe_destroy(void* handle);
+
+/*
+ * GPTQ quantiser (ABI v6): makes the packed 4-bit layers the entry points above run, on the GPU.
+ *
+ * Hessian update: H = alpha * H + beta * x^T x, x [T, K] of `dtype` (row-major), H [K, K] fp32 (DEVICE).
+ *   Replaces GPTQ.add_batch (auto_gptq/quantization/gptq.py:34-60), whose fp32 matmul this computes on tensor cores
+ *   with fp32 accumulation (fp16 x fp16 and bf16 x bf16 products are exact in fp32).  The reference's running mean is
+ *   alpha = n / (n + b), beta = 2 / (n + b) for a batch of b samples after n.  Only the tiles on or above the diagonal
+ *   are computed; H must be symmetric on entry (it is read from its upper triangle) and is symmetric on return.
+ *   T is arbitrary, K % 8 == 0; x and H 16-byte aligned.  The reduction over T runs in a fixed order without atomics:
+ *   two calls on the same inputs give bit-identical H.
+ */
+int agb200_gptq_hessian_update(const void* x, float* H, int T, int K, int dtype, float alpha, float beta, void* stream);
+
+/*
+ * Blocked GPTQ quantisation of one layer, 4 bits, per-channel, blocksize 128, no MSE grid search, in one launch.
+ *   Replaces the column loop of GPTQ.fasterquant (gptq.py:62-194; Quantizer.find_params / quantize, quantizer.py:45-131)
+ *   and the code derivation of QuantLinear.pack (auto_gptq/nn_modules/qlinear/qlinear_cuda_old.py:110-200).  The damping
+ *   and the three Cholesky steps (gptq.py:113-119) stay with the caller (a dense library factorisation).
+ *
+ *   W        [N, K] fp32 (DEVICE), the layer weight in ORIGINAL column order; on return the dequantised Q
+ *            scale * (q - zero), in original column order.
+ *   Hinv     [K, K] fp32, upper Cholesky factor of the damped inverse Hessian, in processing order (permuted by `perm`).
+ *   perm     NULL, or int32[K] for act-order: processing position j quantises original column perm[j] (gptq.py:104-108).
+ *   dead     NULL, or uint8[K] in original order: 1 marks a column whose Hessian diagonal was 0; it is zeroed before
+ *            anything else except the group_size = -1 parameters, which see the initial W (gptq.py:79-86).
+ *   group_size  -1 (one group, parameters from the initial W) or a positive multiple of 8.  G = 1 or ceil(K / group_size).
+ *   sym, static_groups  as the reference (static_groups is ignored for group_size = -1, as there).
+ * Outputs (DEVICE, caller-allocated):
+ *   scale, zero  fp32 [N, G]: what fasterquant returns (gptq.py:189-194).
+ *   scales   [G, N] of `dtype`; qweight int32 [K/8, N]; qzeros int32 [G, N/8] (zero - 1 in each nibble);
+ *   g_idx    int32 [K]: the packed checkpoint layout of this header, with codes in original column order.
+ *   losses   NULL, or fp32 [N, K] in original column order: (w - q)^2 / d^2 / 2 of every element (gptq.py:152, 159).
+ *   workspace  DEVICE scratch of agb200_gptq_workspace_bytes(N, K, perm != NULL) bytes, 256-byte aligned.
+ * Constraints: N % 8 == 0, K % 8 == 0; W and Hinv 16-byte aligned.  Deterministic (no atomics).
+ */
+int agb200_gptq_quantize(float* W, const float* Hinv, const int32_t* perm, const uint8_t* dead, int N, int K,
+                         int group_size, int sym, int static_groups, float* scale, float* zero, void* scales,
+                         int32_t* qweight, int32_t* qzeros, int32_t* g_idx, float* losses, int dtype, void* workspace,
+                         size_t workspace_bytes, void* stream);
+size_t agb200_gptq_workspace_bytes(int N, int K, int act_order);
 
 /*
  * Next-layer prefetch hint (optional, decode): names up to 8 device ranges - typically the packed weights and scales of
