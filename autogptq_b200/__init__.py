@@ -8,7 +8,8 @@ Only what the path needs lives here:
   tp.py            column/row parallel modules: one NCCL all-reduce per row-parallel layer
   moe.py           QuantExperts: the routed experts of a Mixtral-style block as one grouped forward
   gptq.py          GPTQ: the quantiser (Hessian accumulation + blocked quantisation) writing packed 4-bit layers
-  checkpoint.py    safetensors GPTQ checkpoint -> QuantLinear modules, TP-aware (SURVEY.md 8f rank 1; `from autogptq_b200 import checkpoint`)
+  awq.py           AWQ GEMM packed layers -> the GPTQ layout (exact integer re-layout, used by the loader)
+  checkpoint.py    safetensors GPTQ / AWQ checkpoint -> QuantLinear modules, TP-aware (SURVEY.md 8f rank 1; `from autogptq_b200 import checkpoint`)
 """
 __version__ = "0.1.0"
 

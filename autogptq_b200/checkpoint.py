@@ -12,6 +12,11 @@ tensors.  Nothing is repacked (the kernels read the checkpoint layout); with ``t
 rank right after it has been read (``sharding.py``: q/k/v/gate/up by columns, o/down by rows): one FULL layer is in host
 memory at a time, a rank keeps only its share; tensors that are not packed-layer buffers (embeddings, norms, lm_head)
 are never read.  Host-side only: works on CPU tensors; moving to the GPU is ``device=``.
+
+AutoAWQ "GEMM" checkpoints (``quant_config.json``, or ``quantization_config`` in an HF ``config.json``) load the same
+way: each layer is rewritten exactly into the GPTQ layout (``awq.awq_to_gptq``) as it is read, before any TP slicing, so
+the modules are ordinary GPTQ-layout ``QuantLinear``s (the reference converts in a slow fp16 round trip, writes a cache
+file and refuses sharded checkpoints, ``modeling/_base.py:974-1062``).
 """
 from __future__ import annotations
 
@@ -23,10 +28,13 @@ from typing import Callable, Dict, Iterator, Mapping, Optional, Tuple, Union
 
 import torch
 
+from .awq import awq_to_gptq
 from .qlinear import QuantLinear
 from .sharding import shard_column_parallel, shard_row_parallel, shard_to_module
 
 QUANT_CONFIG_FILENAME = "quantize_config.json"            # quantization/config.py:20
+AWQ_CONFIG_FILENAME = "quant_config.json"                 # AutoAWQ
+HF_CONFIG_FILENAME = "config.json"                        # transformers: its "quantization_config" entry
 _PACKED_SUFFIXES = ("qweight", "qzeros", "scales", "g_idx", "bias")
 # Megatron-style plan for Llama-family decoder blocks (SURVEY.md 8e)
 LLAMA_TP_PLAN = {
@@ -46,19 +54,34 @@ class QuantSettings:
     @classmethod
     def from_mapping(cls, d: Mapping) -> "QuantSettings":
         g = lambda *names, default=None: next((d[n] for n in names if n in d), default)   # noqa: E731
-        # synonyms accepted by the reference (quantization/config.py:51-55) and its safetensors metadata keys
+        truthy = lambda v: str(v).lower() in ("true", "1")                                # noqa: E731
+        # synonyms accepted by the reference (quantization/config.py:51-55) and its safetensors metadata keys; AWQ
+        # configs say zero_point instead of sym
+        sym = g("sym", default=None)
         out = cls(bits=int(g("bits", "w_bit", "gptq_bits", default=4)),
                   group_size=int(g("group_size", "q_group_size", "gptq_group_size", default=-1)),
-                  desc_act=str(g("desc_act", "gptq_desc_act", default=False)).lower() in ("true", "1"),
-                  sym=str(g("sym", default=True)).lower() in ("true", "1"),
-                  checkpoint_format=str(g("checkpoint_format", "gptq_checkpoint_format", default="gptq")))
-        if str(g("is_marlin_format", default=False)).lower() in ("true", "1"):
+                  desc_act=truthy(g("desc_act", "gptq_desc_act", default=False)),
+                  sym=truthy(sym) if sym is not None else not truthy(g("zero_point", default=False)),
+                  checkpoint_format=str(g("checkpoint_format", "gptq_checkpoint_format", default="gptq")).lower())
+        if truthy(g("is_marlin_format", default=False)):
             out.checkpoint_format = "marlin"
+        # AWQ: quant_method "awq" (HF) or a bare "version" (AutoAWQ's quant_config.json) names the layout
+        # (quantization/config.py:141-143); AWQ does not reorder rows (:152-154)
+        method = str(g("quant_method", default="")).lower()
+        if method == "awq" or (method == "" and "version" in d):
+            version = str(g("version", default="gemm")).lower()
+            if version != "gemm":
+                raise NotImplementedError(f"AWQ version {version!r}: only AutoAWQ's GEMM layout is read "
+                                          "(GEMV / Marlin / exllama AWQ checkpoints are not)")
+            out.checkpoint_format = "gemm"
+        if out.checkpoint_format == "gemm":
+            out.desc_act = False
         return out
 
 
 def read_quant_settings(path: str) -> Optional[QuantSettings]:
-    """``quantize_config.json`` next to the weights, else the ``gptq_*`` metadata of the first safetensors file."""
+    """``quantize_config.json`` next to the weights, else the ``gptq_*`` metadata of the first safetensors file, else
+    AutoAWQ's ``quant_config.json``, else the ``quantization_config`` of an HF ``config.json``."""
     d = path if os.path.isdir(path) else os.path.dirname(path)
     cfg = os.path.join(d, QUANT_CONFIG_FILENAME)
     if os.path.exists(cfg):
@@ -71,6 +94,14 @@ def read_quant_settings(path: str) -> Optional[QuantSettings]:
         if any(k.startswith("gptq_") for k in meta):
             return QuantSettings.from_mapping(meta)
         break
+    for name, key in ((AWQ_CONFIG_FILENAME, None), (HF_CONFIG_FILENAME, "quantization_config")):
+        cfg = os.path.join(d, name)
+        if os.path.exists(cfg):
+            with open(cfg) as fh:
+                m = json.load(fh)
+            m = m.get(key) if key is not None else m
+            if m:
+                return QuantSettings.from_mapping(m)
     return None
 
 
@@ -139,20 +170,30 @@ def build_quant_linear(tensors: Mapping[str, torch.Tensor], settings: QuantSetti
     """One ``QuantLinear`` from the packed tensors of a layer; ``tp = (mode, rank, world)`` slices it first (the module
     then carries ``tp_mode / tp_rank / tp_world / tp_n_range / tp_k_range / tp_x_index``; a row-parallel shard's bias lives
     on rank 0 only and its outputs are PARTIAL sums - wrap it in ``autogptq_b200.tp.RowParallelQuantLinear`` or run it in a
-    ``TPDecodeChain``)."""
+    ``TPDecodeChain``).  ``settings.checkpoint_format == "gemm"`` (AWQ) converts the layer to the GPTQ layout first, on
+    ``device`` when that is a CUDA device."""
     if settings.bits != 4:
         raise NotImplementedError(f"{settings.bits}-bit GPTQ checkpoints are outside the H100 hot path (4-bit only)")
-    if settings.checkpoint_format != "gptq":
-        raise NotImplementedError(f"checkpoint_format={settings.checkpoint_format!r}: only the GPTQ pack layout is read "
-                                  "(Marlin / AWQ checkpoints must be converted back, cf. marlin_utils.py:118-198)")
+    if settings.checkpoint_format not in ("gptq", "gemm"):
+        raise NotImplementedError(f"checkpoint_format={settings.checkpoint_format!r}: only the GPTQ and AWQ GEMM pack "
+                                  "layouts are read (Marlin checkpoints must be converted back, cf. marlin_utils.py:118-198)")
     qweight, qzeros, scales = tensors["qweight"], tensors["qzeros"], tensors["scales"]
+    awq = settings.checkpoint_format == "gemm"
+    if awq:
+        if device is not None and torch.device(device).type == "cuda":
+            qweight, qzeros, scales = (t.to(device) for t in (qweight, qzeros, scales))
+        qweight, qzeros = awq_to_gptq(qweight, qzeros, scales)
     K, N = qweight.shape[0] * 8, qweight.shape[1]
     G = scales.shape[0]
     group_size = settings.group_size if settings.group_size != -1 else K
     if G != -(-K // group_size) or qzeros.shape != (G, N // 8) or scales.shape != (G, N):
+        hint = ""
+        if not awq and qweight.dim() == 2 and scales.dim() == 2 and scales.shape[1] == 8 * qweight.shape[1]:
+            hint = (" - these are the shapes of an AWQ GEMM layer (qweight [K, N/8], packed along N): load it with "
+                    "checkpoint_format='gemm'")
         raise ValueError(f"packed tensor shapes do not match group_size={settings.group_size}: qweight {tuple(qweight.shape)}, "
-                         f"qzeros {tuple(qzeros.shape)}, scales {tuple(scales.shape)}")
-    g_idx = tensors.get("g_idx")
+                         f"qzeros {tuple(qzeros.shape)}, scales {tuple(scales.shape)}{hint}")
+    g_idx = None if awq else tensors.get("g_idx")     # AWQ has no act-order: groups are sequential
     if g_idx is None:
         g_idx = torch.arange(K, dtype=torch.int32) // group_size
     bias = tensors.get("bias")
@@ -183,7 +224,7 @@ def build_quant_linear(tensors: Mapping[str, torch.Tensor], settings: QuantSetti
 def load_quant_linears(source: Union[str, Mapping[str, torch.Tensor]], settings: Optional[QuantSettings] = None, device=None,
                        tp_rank: int = 0, tp_world: int = 1, tp_plan: Optional[Mapping[str, str]] = None,
                        select: Optional[Callable[[str], bool]] = None, allow_gathered_input: bool = False) -> Dict[str, QuantLinear]:
-    """All packed layers of a GPTQ checkpoint as ``{prefix: QuantLinear}``.
+    """All packed layers of a GPTQ or AWQ GEMM checkpoint as ``{prefix: QuantLinear}`` (GPTQ layout either way).
 
     ``tp_world > 1``: layers whose prefix matches a pattern of ``tp_plan`` (default: the Llama plan) are sliced for
     ``tp_rank`` ("column" / "row"); the others are replicated.  ``select(prefix)`` filters layers (e.g. one decoder
