@@ -12,8 +12,9 @@ from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 6
+ABI_VERSION = 7
 F16, BF16 = 0, 1
+ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
 CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS = 0, 1, 2
 CHAIN_DEBUG_NO_DEPS, CHAIN_DEBUG_NO_MATH = 1, 2
@@ -25,6 +26,7 @@ IMMA_MAX_M = 8
 MOE_DECODE_MAX_T = 8
 MOE_MAX_EXPERTS = 256
 MOE_INDEX_I32, MOE_INDEX_I64, MOE_WEIGHTS_F32 = 0, 1, 2
+GATE_UP_AUTO, GATE_UP_DECODE, GATE_UP_GEMM = 0, 1, 2
 
 _lib = None
 
@@ -70,6 +72,9 @@ def _declare(lib):
         "agb200_moe_workspace_bytes": (S, [I, I, I, I, I]),
         "agb200_moe_forward": (I, [P, P, P, I, P, I, I, I, P, P, S, P]),
         "agb200_moe_destroy": (I, [P]),
+        "agb200_w4a16_gate_up": (I, [P, P, P, P, I, I, I, I, I, P, S, P]),
+        "agb200_w4a16_gate_up_ex": (I, [P, P, P, P, I, I, I, I, I, P, S, P, I, I, I]),
+        "agb200_w4a16_gate_up_workspace_bytes": (S, [I, I, I]),
         "agb200_gptq_hessian_update": (I, [P, P, I, I, I, c_float, c_float, P]),
         "agb200_gptq_quantize": (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, I, P, S, P]),
         "agb200_gptq_workspace_bytes": (S, [I, I, I]),

@@ -304,6 +304,9 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   int inflight = 0;
   if (const char* e = getenv("AGB200_CHAIN_INFLIGHT")) { const int v = atoi(e); if (v >= 1) inflight = v; }
 
+  // the plan is caller memory a stream-ordered allocator may have just recycled from a tensor that kernels queued on a
+  // non-blocking stream still write; the legacy-stream copies below are not ordered after them (create time only)
+  CH_CUDA(cudaDeviceSynchronize());
   CH_CUDA(cudaMemset(d_flags, 0, kFlagsBytes + kProfBytes));
   if (ll_total > 0) CH_CUDA(cudaMemset(d_ll, 0, ll_total));
   CH_CUDA(cudaMemcpy(d_stages, hs.data(), size_t(n_stages) * sizeof(agb::ChainStage), cudaMemcpyHostToDevice));

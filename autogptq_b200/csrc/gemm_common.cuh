@@ -1,5 +1,6 @@
-// Device helpers shared by the wgmma W4A16 GEMMs (gemm_tcgen05.cuh: one layer; moe.cuh: grouped experts): tile
-// constants, shared-memory ring layout, the x-tile descriptor, the int4 -> 16-bit A-fragment expansion and the wgmma call.
+// Device helpers shared by the wgmma W4A16 GEMMs (gemm_tcgen05.cuh: one layer; moe.cuh: grouped experts and the dense
+// gate/up pair): tile constants, shared-memory ring layout, the x-tile descriptor, the int4 -> 16-bit A-fragment
+// expansion, the wgmma call and the gate/up (silu * mul) epilogue.
 #pragma once
 #include <type_traits>
 
@@ -63,5 +64,23 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[kMT / 2], const uint32_t* 
 }
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kGemmConsumers) : "memory"); }
+
+// h = silu(g) * u on 16-bit tensors (the reference MLP's act_fn(gate) * up): g and u are values of the dtype, silu(g) is
+// rounded to the dtype, then the product is formed in fp32 (the caller rounds it).  Same rule as the chain's X_SILU_MUL.
+template <bool kBf16>
+__device__ __forceinline__ float silu_mul_elt(uint16_t g, uint16_t u) {
+  const float fg = elt_to_float<kBf16>(g);
+  const float s = fg / (1.f + __expf(-fg));
+  return elt_to_float<kBf16>(float_to_elt<kBf16>(s)) * elt_to_float<kBf16>(u);
+}
+
+// Gate/up epilogue of one output element: g and u are the fp32 sums of column nn; adds the biases, rounds g and u to
+// the dtype and stores round(silu(g) * u) at out[dst].
+template <bool kBf16>
+__device__ __forceinline__ void store_gate_up(uint16_t* out, float gv, float uv, const void* bias_g, const void* bias_u, int nn) {
+  if (bias_g != nullptr) gv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(bias_g)[nn]);
+  if (bias_u != nullptr) uv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(bias_u)[nn]);
+  *out = float_to_elt<kBf16>(silu_mul_elt<kBf16>(float_to_elt<kBf16>(gv), float_to_elt<kBf16>(uv)));
+}
 
 }  // namespace agb

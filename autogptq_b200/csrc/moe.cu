@@ -108,7 +108,7 @@ int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType d
 
 template <bool kBf16, bool kGateUp>
 int decode_setup(size_t smem, int& occ) {
-  auto kern = agb::moe_decode_kernel<kBf16, kGateUp>;
+  auto kern = agb::moe_decode_kernel<kBf16, kGateUp, agb::MoeRouted>;
   MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   MOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, agb::kMdThreads, smem));
   if (occ < 1) return failf(AGB200_ENOSUP, "moe: decode kernel with %zu B of shared memory does not fit an SM", smem);
@@ -116,19 +116,21 @@ int decode_setup(size_t smem, int& occ) {
 }
 
 template <bool kGateUp>
-int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, int max_items, cudaStream_t stream) {
+int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, const agb::MoeRouted& src, int max_items, cudaStream_t stream) {
   const size_t smem = kGateUp ? m.up_smem : m.down_smem;
   const int occ = kGateUp ? m.up_occ : m.down_occ;
   const int grid = std::max(1, std::min(max_items, m.sms * occ));
-  if (m.dtype == AGB200_BF16) agb::moe_decode_kernel<true, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p);
-  else agb::moe_decode_kernel<false, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p);
+  if (m.dtype == AGB200_BF16) agb::moe_decode_kernel<true, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
+  else agb::moe_decode_kernel<false, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
   MOE_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <int kMT, bool kBf16, bool kGateUp>
-int launch_gemm_inst(const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, int n_tiles, int m_tiles, cudaStream_t stream) {
-  auto kern = agb::moe_gemm_kernel<kMT, kBf16, kGateUp>;
+// One GEMM launch; split > 1 (dense gate/up only) runs as clusters of `split` CTAs along z.
+template <int kMT, bool kBf16, bool kGateUp, class Src>
+int launch_gemm_inst(const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, const Src& src, int n_tiles, int m_tiles,
+                     cudaStream_t stream) {
+  auto kern = agb::moe_gemm_kernel<kMT, kBf16, kGateUp, Src>;
   constexpr int smem = agb::MoeGemmSmem<kMT>::kTotal;
   static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
   const int dev = agb::current_device_index();
@@ -136,19 +138,34 @@ int launch_gemm_inst(const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, int
     MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
     attr_set_dev[dev] = true;
   }
-  kern<<<dim3(n_tiles, m_tiles, 1), agb::kGemmThreads, smem, stream>>>(p, tmap_x);
+  if (p.split == 1) {
+    kern<<<dim3(n_tiles, m_tiles, 1), agb::kGemmThreads, smem, stream>>>(p, tmap_x, src);
+  } else {
+    cudaLaunchConfig_t cfg{};
+    cfg.gridDim = dim3(n_tiles, m_tiles, p.split);
+    cfg.blockDim = dim3(agb::kGemmThreads, 1, 1);
+    cfg.dynamicSmemBytes = smem;
+    cfg.stream = stream;
+    cudaLaunchAttribute attr;
+    attr.id = cudaLaunchAttributeClusterDimension;
+    attr.val.clusterDim.x = 1;
+    attr.val.clusterDim.y = 1;
+    attr.val.clusterDim.z = p.split;
+    cfg.attrs = &attr;
+    cfg.numAttrs = 1;
+    MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tmap_x, src));
+  }
   MOE_CUDA(cudaGetLastError());
   return 0;
 }
 
-template <bool kGateUp>
-int launch_gemm(const Moe& m, int mt, const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, int n_tiles, int m_tiles,
-                cudaStream_t s) {
-  const bool bf = m.dtype == AGB200_BF16;
+template <bool kGateUp, class Src>
+int launch_gemm(bool bf, int mt, const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, const Src& src, int n_tiles,
+                int m_tiles, cudaStream_t s) {
   switch (mt) {
-    case 32: return bf ? launch_gemm_inst<32, true, kGateUp>(p, tmap_x, n_tiles, m_tiles, s) : launch_gemm_inst<32, false, kGateUp>(p, tmap_x, n_tiles, m_tiles, s);
-    case 64: return bf ? launch_gemm_inst<64, true, kGateUp>(p, tmap_x, n_tiles, m_tiles, s) : launch_gemm_inst<64, false, kGateUp>(p, tmap_x, n_tiles, m_tiles, s);
-    default: return bf ? launch_gemm_inst<128, true, kGateUp>(p, tmap_x, n_tiles, m_tiles, s) : launch_gemm_inst<128, false, kGateUp>(p, tmap_x, n_tiles, m_tiles, s);
+    case 32: return bf ? launch_gemm_inst<32, true, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s) : launch_gemm_inst<32, false, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s);
+    case 64: return bf ? launch_gemm_inst<64, true, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s) : launch_gemm_inst<64, false, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s);
+    default: return bf ? launch_gemm_inst<128, true, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s) : launch_gemm_inst<128, false, kGateUp>(p, tmap_x, src, n_tiles, m_tiles, s);
   }
 }
 
@@ -263,12 +280,15 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
     return failf(AGB200_ECUDA, "moe: %s: %s", what, cudaGetErrorString(e));
   };
   cudaError_t ce;
+  // Wait for all work on the device before writing the plan (load time only).  The plan buffer is caller memory that a
+  // stream-ordered allocator may have just recycled from a tensor that kernels queued on a non-blocking stream still
+  // write (the copies below run on the legacy stream, which is not ordered after such streams); the permutations were
+  // also made on the caller's streams.
+  if ((ce = cudaDeviceSynchronize()) != cudaSuccess) return cleanup_fail(ce, "cudaDeviceSynchronize");
   if (!maps.empty() && (ce = cudaMemcpy(d_maps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice)) != cudaSuccess)
     return cleanup_fail(ce, "copy tensor maps");
   if ((ce = cudaMemcpy(d_ex, table.data(), size_t(E) * sizeof(agb::MoeExpertDev), cudaMemcpyHostToDevice)) != cudaSuccess)
     return cleanup_fail(ce, "copy expert table");
-  // the permutations were made on the caller's streams: wait for them, invert, and wait again (load time only)
-  if ((ce = cudaDeviceSynchronize()) != cudaSuccess) return cleanup_fail(ce, "cudaDeviceSynchronize");
   for (int e = 0; e < E; ++e)
     if (experts[e].w2.perm != nullptr)
       agb::moe_invert_perm_kernel<<<(I + 255) / 256, 256>>>(experts[e].w2.perm, d_inv + size_t(e) * I, I);
@@ -317,16 +337,18 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
   uint16_t* hs = reinterpret_cast<uint16_t*>(ws + w.hs);
   const bool bf = m->dtype == AGB200_BF16;
   const dim3 cgrid(T, (H + 255) / 256, 1);
+  agb::MoeRouted src{};
+  src.ex = m->d_ex; src.r = r; src.k = k; src.maps = m->d_maps;
   if (decode) {
     float* part = reinterpret_cast<float*>(ws + w.ys);
     agb::MoeDecodeParams p{};
-    p.ex = m->d_ex; p.r = r; p.k = k; p.P = P;
+    p.P = P;
     p.x = x; p.out = hs; p.K = H; p.N = I; p.rows = H / 8; p.rows_per_group = m->gs13 / 8;
     p.rows_per_split = m->up_rps; p.split = 1; p.tiles = I / agb::kMdTN;
-    if (int rc = launch_decode<true>(*m, p, std::min(E, P) * p.tiles, s)) return rc;
+    if (int rc = launch_decode<true>(*m, p, src, std::min(E, P) * p.tiles, s)) return rc;
     p.x = hs; p.out = part; p.K = I; p.N = H; p.rows = I / 8; p.rows_per_group = m->gs2 / 8;
     p.rows_per_split = m->down_rps; p.split = m->down_split; p.tiles = H / agb::kMdTN;
-    if (int rc = launch_decode<false>(*m, p, std::min(E, P) * p.tiles * p.split, s)) return rc;
+    if (int rc = launch_decode<false>(*m, p, src, std::min(E, P) * p.tiles * p.split, s)) return rc;
     if (bf) agb::moe_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
                                                                 nullptr, part, m->down_split, m->d_ex, static_cast<uint16_t*>(out));
     else agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
@@ -348,11 +370,13 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
   if (int rc = encode_2d(encode, &tx, xdt, xs, H, w.rows, size_t(H) * 2, agb::kGemmBK, mt, true, "gathered x")) return rc;
   if (int rc = encode_2d(encode, &th, xdt, hs, I, w.rows, size_t(I) * 2, agb::kGemmBK, mt, true, "h")) return rc;
   agb::MoeGemmParams p{};
-  p.maps = m->d_maps; p.ex = m->d_ex; p.r = r;
+  p.split = 1;
   p.out = hs; p.K = H; p.N = I; p.group_size = m->gs13; p.gs_log2 = gs_log2(m->gs13); p.num_kb = (H + agb::kGemmBK - 1) / agb::kGemmBK;
-  if (int rc = launch_gemm<true>(*m, mt, p, tx, I / (agb::kGemmBN / 2), m_tiles, s)) return rc;
+  p.kb_per_split = p.num_kb;
+  if (int rc = launch_gemm<true>(bf, mt, p, tx, src, I / (agb::kGemmBN / 2), m_tiles, s)) return rc;
   p.out = ys; p.K = I; p.N = H; p.group_size = m->gs2; p.gs_log2 = gs_log2(m->gs2); p.num_kb = (I + agb::kGemmBK - 1) / agb::kGemmBK;
-  if (int rc = launch_gemm<false>(*m, mt, p, th, H / agb::kGemmBN, m_tiles, s)) return rc;
+  p.kb_per_split = p.num_kb;
+  if (int rc = launch_gemm<false>(bf, mt, p, th, src, H / agb::kGemmBN, m_tiles, s)) return rc;
   if (bf) agb::moe_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
                                                               ys, nullptr, 0, m->d_ex, static_cast<uint16_t*>(out));
   else agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
@@ -368,6 +392,158 @@ int agb200_moe_destroy(void* handle) {
   m->magic = 0;
   delete m;
   return 0;
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ dense gate/up pair
+// h = silu(x Wg + bg) * (x Wu + bu) for the MLP of a dense model (agb200_w4a16_gate_up*): the experts' gate/up kernels
+// with the DenseRows / DenseGemmRows work sources.
+namespace {
+
+size_t gate_up_decode_smem(int K) { return size_t(round_up(K / 8, 32)) * agb::kMdRows * 16 + agb::kMdRedBytes; }
+
+template <bool kBf16>
+int launch_gate_up_decode(const agb::DenseRows& src, const agb::MoeDecodeParams& p, size_t smem, int smem_optin,
+                          cudaStream_t stream) {
+  auto kern = agb::moe_decode_kernel<kBf16, true, agb::DenseRows>;
+  static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
+  const int dev = agb::current_device_index();
+  if (!attr_set_dev[dev]) {
+    MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+    attr_set_dev[dev] = true;
+  }
+  kern<<<p.tiles, agb::kMdThreads, smem, stream>>>(p, src);   // one CTA per 32-column tile
+  MOE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+// Split-K of the GEMM path: the number of K splits (1/2/4/8, >= 4 blocks of 64 k each) with the fewest modelled time
+// units, ceil(CTAs * split / SMs) waves of (blocks per split + 4) - the 4 stands for the ring fill and the DSMEM reduction.
+int gate_up_auto_split(int ctas, int num_kb, int sms) {
+  int best = 1;
+  long best_cost = -1;
+  for (int s = 1; s <= 8; s *= 2) {
+    if (s > 1 && num_kb / s < 4) break;
+    const long waves = (static_cast<long>(ctas) * s + sms - 1) / sms;
+    const long cost = waves * ((num_kb + s - 1) / s + 4);
+    if (best_cost < 0 || cost < best_cost) { best = s; best_cost = cost; }
+  }
+  return best;
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t agb200_w4a16_gate_up_workspace_bytes(int M, int K, int I) {
+  (void)I;
+  if (M <= 0 || K <= 0) return 0;
+  return align_up(size_t(M) * K * 2, 256);   // x gathered through the act-order permutation (GEMM path)
+}
+
+int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
+                            int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream,
+                            int kernel, int tile_m, int split_k) {
+  if (!gate || !up) return failf(AGB200_EINVAL, "gate_up: null layer descriptor");
+  if (M < 0 || K <= 0 || I <= 0) return failf(AGB200_EINVAL, "gate_up: M >= 0, K > 0 and I > 0 (got M=%d, K=%d, I=%d)", M, K, I);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16) return failf(AGB200_EINVAL, "gate_up: dtype must be AGB200_F16 or AGB200_BF16");
+  if (kernel != AGB200_GATE_UP_AUTO && kernel != AGB200_GATE_UP_DECODE && kernel != AGB200_GATE_UP_GEMM)
+    return failf(AGB200_EINVAL, "gate_up: unknown kernel %d", kernel);
+  if (M == 0) return 0;
+  if (!x || !h) return failf(AGB200_EINVAL, "gate_up: null x or h");
+  for (const agb200_moe_layer* L : {gate, up}) {
+    if (!L->qweight || !L->qzeros || !L->scales) return failf(AGB200_EINVAL, "gate_up: null qweight/qzeros/scales");
+    if (!aligned16(L->qweight) || !aligned16(L->qzeros) || !aligned16(L->scales) || !aligned16(L->bias) ||
+        !aligned16(L->qweight_tc) || !aligned16(L->perm))
+      return failf(AGB200_EINVAL, "gate_up: layer buffers must be 16-byte aligned");
+  }
+  if (!aligned16(x) || !aligned16(h)) return failf(AGB200_EINVAL, "gate_up: x and h must be 16-byte aligned");
+  if (K % 8 != 0 || I % 32 != 0) return failf(AGB200_ENOSUP, "gate_up: K %% 8 == 0 and I %% 32 == 0 (got K=%d, I=%d)", K, I);
+  if (gate->perm != up->perm)
+    return failf(AGB200_ENOSUP, "gate_up: gate and up must share one act-order permutation of x (same pointer, or both NULL)");
+  const int gs = group_size == -1 ? K : group_size;
+  if (gs <= 0) return failf(AGB200_EINVAL, "gate_up: group_size must be positive or -1 (got %d)", group_size);
+  int dev = 0, smem_optin = 0, sms = 0;
+  MOE_CUDA(cudaGetDevice(&dev));
+  if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "gate_up: device index %d out of range", dev);
+  MOE_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  MOE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  const bool bf = dtype == AGB200_BF16;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+
+  // decode kernel: all of K of the M <= 8 rows in shared memory, group boundaries on 32-row steps of k
+  const size_t dsmem = gate_up_decode_smem(K);
+  const bool decode_ok = M <= agb::kMoeDecodeMaxT && (gs % 32 == 0 || gs >= K) && dsmem <= static_cast<size_t>(smem_optin);
+  bool decode = kernel == AGB200_GATE_UP_DECODE || (kernel == AGB200_GATE_UP_AUTO && decode_ok);
+  if (decode) {
+    if (!decode_ok)
+      return failf(AGB200_ENOSUP, "gate_up: the decode kernel needs M <= %d, group_size %% 32 == 0 (or one group) and "
+                   "%zu B of shared memory <= %d (got M=%d, group_size=%d)", agb::kMoeDecodeMaxT, dsmem, smem_optin, M, gs);
+    agb::DenseRows src{};
+    src.M = M;
+    src.lay.qweight[0] = gate->qweight; src.lay.qzeros[0] = gate->qzeros; src.lay.scales[0] = gate->scales; src.lay.bias[0] = gate->bias;
+    src.lay.qweight[1] = up->qweight;   src.lay.qzeros[1] = up->qzeros;   src.lay.scales[1] = up->scales;   src.lay.bias[1] = up->bias;
+    src.lay.perm13 = gate->perm;
+    agb::MoeDecodeParams p{};
+    p.x = x; p.out = h; p.K = K; p.N = I; p.P = M; p.rows = K / 8; p.rows_per_group = gs / 8;
+    p.rows_per_split = round_up(K / 8, 32); p.split = 1; p.tiles = I / agb::kMdTN;
+    return bf ? launch_gate_up_decode<true>(src, p, dsmem, smem_optin, s) : launch_gate_up_decode<false>(src, p, dsmem, smem_optin, s);
+  }
+
+  // wgmma GEMM over 64 gate + 64 up columns per CTA
+  if (!gate->qweight_tc || !up->qweight_tc)
+    return failf(AGB200_ENOSUP, "gate_up: the tensor-core GEMM (M=%d) needs qweight_tc of both layers", M);
+  if (gs != 32 && gs % 64 != 0)
+    return failf(AGB200_ENOSUP, "gate_up: group_size=%d must be 32 or a multiple of 64 on the GEMM path", gs);
+  const void* xa = x;
+  if (gate->perm != nullptr) {
+    const size_t need = size_t(M) * K * 2;
+    if (!workspace || workspace_bytes < need)
+      return failf(AGB200_EWORKSPACE, "gate_up: act-order needs a %zu-byte workspace for the gathered x (got %zu)", need, workspace_bytes);
+    if (!aligned16(workspace)) return failf(AGB200_EINVAL, "gate_up: the workspace must be 16-byte aligned");
+    if (int rc = agb200_permute_columns(x, gate->perm, workspace, M, K, dtype, stream)) return rc;
+    xa = workspace;
+  }
+  int mt = tile_m;
+  if (mt == 0) mt = M <= 32 ? 32 : M <= 64 ? 64 : 128;
+  if (mt != 32 && mt != 64 && mt != 128) return failf(AGB200_EINVAL, "gate_up: x-row tile must be 32/64/128 (got %d)", mt);
+  const int n_tiles = (I + agb::kGemmBN / 2 - 1) / (agb::kGemmBN / 2);
+  const int m_tiles = (M + mt - 1) / mt;
+  if (m_tiles > 65535) return failf(AGB200_ENOSUP, "gate_up: %d row tiles exceed the grid limit", m_tiles);
+  agb::MoeGemmParams p{};
+  p.out = h; p.K = K; p.N = I; p.group_size = gs; p.gs_log2 = gs_log2(gs); p.num_kb = (K + agb::kGemmBK - 1) / agb::kGemmBK;
+  int split = split_k == 0 ? gate_up_auto_split(n_tiles * m_tiles, p.num_kb, sms) : split_k;
+  if (split != 1 && split != 2 && split != 4 && split != 8) return failf(AGB200_EINVAL, "gate_up: split-K must be 1/2/4/8 (got %d)", split);
+  while (split > 1 && split > p.num_kb) split /= 2;
+  p.split = split;
+  p.kb_per_split = (p.num_kb + split - 1) / split;
+
+  agb::EncodeTiledFn encode = agb::get_encode_fn();
+  if (encode == nullptr) return failf(AGB200_ECUDA, "gate_up: cuTensorMapEncodeTiled entry point not available");
+  const CUtensorMapDataType xdt = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  CUtensorMap tx;
+  if (int rc = encode_2d(encode, &tx, xdt, xa, K, M, size_t(K) * 2, agb::kGemmBK, mt, true, "x")) return rc;
+  agb::DenseGemmRows src{};
+  src.M = M;
+  src.lay.bias[0] = gate->bias;
+  src.lay.bias[1] = up->bias;
+  const int G = (K + gs - 1) / gs;
+  const uint32_t ngr = gs == 32 ? 2 : 1;
+  const agb200_moe_layer* L[2] = {gate, up};
+  for (int l = 0; l < 2; ++l) {
+    CUtensorMap* mp = src.maps + 3 * l;
+    if (int rc = encode_2d(encode, mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qweight_tc, I, K / 8, size_t(I) * 4, 64, 8, false, "qweight_tc")) return rc;
+    if (int rc = encode_2d(encode, mp + 1, xdt, L[l]->scales, I, G, size_t(I) * 2, 64, ngr, false, "scales")) return rc;
+    if (int rc = encode_2d(encode, mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qzeros, I / 8, G, size_t(I / 8) * 4, 8, ngr, false, "qzeros")) return rc;
+  }
+  return launch_gemm<true>(bf, mt, p, tx, src, n_tiles, m_tiles, s);
+}
+
+int agb200_w4a16_gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
+                         int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream) {
+  return agb200_w4a16_gate_up_ex(x, gate, up, h, M, K, I, group_size, dtype, workspace, workspace_bytes, stream,
+                                 AGB200_GATE_UP_AUTO, 0, 0);
 }
 
 }  // extern "C"

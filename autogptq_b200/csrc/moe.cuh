@@ -11,7 +11,11 @@
 //   moe_combine_kernel      out[t] = sum_j w[t, j] * y_pair in slot order, fp32, one rounding (no atomics)
 // The gate/up stage computes w1 and w3 of the same columns in one CTA and writes h = silu(g) * u (g, u rounded to the
 // dtype first, like the reference's act_fn(gate) * up); g and u never leave the SM.
+// The decode and GEMM kernels take their rows from a work source (template parameter): MoeRouted reads the routing
+// table; DenseRows / DenseGemmRows run one gate/up pair over all M rows of x (agb200_w4a16_gate_up, a dense MLP), the
+// GEMM then with split-K over a thread-block cluster whose partial tiles are reduced through DSMEM before silu * mul.
 #pragma once
+#include <cooperative_groups.h>
 #include <cuda.h>
 
 #include "common.cuh"
@@ -58,13 +62,55 @@ __device__ __forceinline__ int moe_load_id(const void* ids, int ids64, int i) {
                : reinterpret_cast<const int*>(ids)[i];
 }
 
-template <bool kBf16>
-__device__ __forceinline__ float moe_silu_mul(uint16_t g, uint16_t u) {
-  // F.silu(gate) * up on 16-bit tensors: silu rounded to the dtype, then the product (same rule as the chain's X_SILU_MUL)
-  const float fg = elt_to_float<kBf16>(g);
-  const float s = fg / (1.f + __expf(-fg));
-  return elt_to_float<kBf16>(float_to_elt<kBf16>(s)) * elt_to_float<kBf16>(u);
-}
+// ------------------------------------------------------------------------------------------------ work sources
+// A "row group" is the rows of x that go through one layer set: an active expert's pairs, or all M rows of a dense MLP.
+// Rows of a group are numbered by position (pair-list order for experts); gate/up writes h row `pos`.
+struct MoeRouted {
+  static constexpr bool kSplitK = false;
+  const MoeExpertDev* ex;
+  MoeRoute r;
+  int k;                        // slots per token
+  const CUtensorMap* maps;      // GEMM path: [E][3 layers][weights (tensor-core copy), scales, zeros]
+  __device__ __forceinline__ int groups() const { return r.meta[0]; }
+  __device__ __forceinline__ int expert(int i) const { return r.active[i]; }
+  __device__ __forceinline__ int count(int e) const { return r.counts[e]; }
+  __device__ __forceinline__ int offset(int e) const { return r.offsets[e]; }
+  __device__ __forceinline__ const MoeExpertDev& layers(int e) const { return ex[e]; }
+  __device__ __forceinline__ int x_row(int pos) const { return r.pairs[pos] / k; }
+  // GEMM row tile -> expert, first (padded) row, valid rows; false past the last used tile
+  __device__ __forceinline__ bool gemm_tile(int tile, int mt, int& e, int& m0, int& m_valid) const {
+    if (tile >= r.meta[1]) return false;
+    e = r.tile_e[tile];
+    m0 = r.tile_m0[tile];
+    m_valid = min(mt, r.counts[e] - (m0 - r.pad_off[e]));
+    return true;
+  }
+  __device__ __forceinline__ const CUtensorMap* gemm_maps(int e, int layer) const { return maps + (e * 3 + layer) * 3; }
+};
+
+struct DenseRows {
+  static constexpr bool kSplitK = false;
+  MoeExpertDev lay;             // gate = layer 0, up = layer 1 (perm13: the shared act-order permutation or null)
+  int M;
+  __device__ __forceinline__ int groups() const { return 1; }
+  __device__ __forceinline__ int expert(int) const { return 0; }
+  __device__ __forceinline__ int count(int) const { return M; }
+  __device__ __forceinline__ int offset(int) const { return 0; }
+  __device__ __forceinline__ const MoeExpertDev& layers(int) const { return lay; }
+  __device__ __forceinline__ int x_row(int pos) const { return pos; }
+};
+
+struct DenseGemmRows : DenseRows {
+  static constexpr bool kSplitK = true;
+  CUtensorMap maps[6];          // gate {weights, scales, zeros}, up {weights, scales, zeros}
+  __device__ __forceinline__ bool gemm_tile(int tile, int mt, int& e, int& m0, int& m_valid) const {
+    e = 0;
+    m0 = tile * mt;
+    m_valid = min(mt, M - m0);
+    return true;                // the grid has exactly ceil(M / mt) row tiles: no CTA of a split-K cluster leaves early
+  }
+  __device__ __forceinline__ const CUtensorMap* gemm_maps(int, int layer) const { return maps + layer * 3; }
+};
 
 // ------------------------------------------------------------------------------------------------ routing
 // One CTA of 1024 threads.  Counts by shared-memory atomics (the totals do not depend on the order), then placement in
@@ -128,9 +174,6 @@ moe_route_kernel(const void* ids, int ids64, int P, int E, int MT, MoeRoute r) {
 // ------------------------------------------------------------------------------------------------ decode path (T <= 8)
 struct MoeDecodeParams {
   const void* x;              // gate/up: x [T, K]; down: h [T*k, K] in pair-list order
-  const MoeExpertDev* ex;
-  MoeRoute r;
-  int k;                      // slots per token
   void* out;                  // gate/up: h [T*k, N] in pair-list order; down: fp32 partial sums [split][T*k, N]
   int K, N, P;
   int rows;                   // K / 8
@@ -144,10 +187,10 @@ struct MoeDecodeParams {
 // columns and K range; down: all 8 warps stream w2.  Inside a warp the arithmetic is the skinny kernel's: a lane loads 16
 // bytes = 4 columns x 8 k, the masked nibbles are fp16/bf16 subnormal (or biased) operands of mma.m16n8k16 against the
 // expert's x rows (at most 8 per pass; a pass is repeated for experts with more rows), fp32 accumulate, scale and
-// zero point once per group and column.
-template <bool kBf16, bool kGateUp>
+// zero point once per group and column.  Src: MoeRouted (experts) or DenseRows (gate/up of a dense MLP, M <= 8 rows).
+template <bool kBf16, bool kGateUp, class Src>
 __global__ void __launch_bounds__(kMdThreads, 2)
-moe_decode_kernel(const MoeDecodeParams p) {
+moe_decode_kernel(const MoeDecodeParams p, const __grid_constant__ Src src) {
   constexpr int D = kGateUp ? kMdDepth - 2 : kMdDepth;   // gate/up: fewer loads in flight leave room for its epilogue (128 registers, 2 CTAs per SM)
   constexpr int kWarpsPerLayer = kGateUp ? 4 : 8;
   extern __shared__ __align__(16) unsigned char smem_raw[];
@@ -168,15 +211,15 @@ moe_decode_kernel(const MoeDecodeParams p) {
   constexpr uint32_t kMaskLo = 0x000f000fu, kMaskHi = 0x00f000f0u;
   constexpr uint32_t kMagic = kBf16 ? 0x43004300u : 0x64006400u;
 
-  const int n_items = p.r.meta[0] * p.tiles * p.split;
+  const int n_items = src.groups() * p.tiles * p.split;
   for (int item = blockIdx.x; item < n_items; item += gridDim.x) {
     const int s = item % p.split;
     const int rest = item / p.split;
     const int tile = rest % p.tiles;
-    const int e = p.r.active[rest / p.tiles];
-    const int cnt = p.r.counts[e];
-    const int off = p.r.offsets[e];
-    const MoeExpertDev& X = p.ex[e];
+    const int e = src.expert(rest / p.tiles);
+    const int cnt = src.count(e);
+    const int off = src.offset(e);
+    const MoeExpertDev& X = src.layers(e);
     const int32_t* qweight = X.qweight[layer];
     const int32_t* qzeros = X.qzeros[layer];
     const uint16_t* sc = reinterpret_cast<const uint16_t*>(X.scales[layer]);
@@ -223,7 +266,7 @@ moe_decode_kernel(const MoeDecodeParams p) {
         for (int idx = tid; idx < chunk_rows * M; idx += kMdThreads) {
           const int m = idx / chunk_rows, rc = idx - m * chunk_rows;
           const int k0 = (r_begin + rc) * kPack;
-          const int src_row = kGateUp ? p.r.pairs[off + rb + m] / p.k : off + rb + m;
+          const int src_row = kGateUp ? src.x_row(off + rb + m) : off + rb + m;
           const uint16_t* xr = xg + static_cast<size_t>(src_row) * p.K;
           uint4 v;
           if (perm == nullptr) {
@@ -355,16 +398,14 @@ moe_decode_kernel(const MoeDecodeParams p) {
               gv += red[(w * kMdRows + m) * kMdTN + col];
               uv += red[((w + 4) * kMdRows + m) * kMdTN + col];
             }
-            if (X.bias[0] != nullptr) gv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(X.bias[0])[nn]);
-            if (X.bias[1] != nullptr) uv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(X.bias[1])[nn]);
-            const float h = moe_silu_mul<kBf16>(float_to_elt<kBf16>(gv), float_to_elt<kBf16>(uv));
             const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
-            reinterpret_cast<uint16_t*>(p.out)[static_cast<size_t>(pos) * p.N + dst] = float_to_elt<kBf16>(h);
+            store_gate_up<kBf16>(reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(pos) * p.N + dst, gv, uv,
+                                 X.bias[0], X.bias[1], nn);
           } else {
             float v = 0.f;
 #pragma unroll
             for (int w = 0; w < kMdWarps; ++w) v += red[(w * kMdRows + m) * kMdTN + col];
-            const int pair = p.r.pairs[pos];
+            const int pair = src.r.pairs[pos];
             reinterpret_cast<float*>(p.out)[(static_cast<size_t>(s) * p.P + pair) * p.N + nn] = v;
           }
         }
@@ -410,36 +451,35 @@ struct MoeGemmSmem : GemmSmem<kMT> {
 };
 
 struct MoeGemmParams {
-  const CUtensorMap* maps;    // plan: [E][3 layers][weights (tensor-core copy), scales, zeros]
-  const MoeExpertDev* ex;
-  MoeRoute r;
   void* out;                  // gate/up: h [padded rows, N]; down: y_pair [T*k, N]
   int K, N;
   int group_size;
   int gs_log2;                // log2(group_size) when it is a power of two, else -1
   int num_kb;                 // ceil(K / 64)
+  int kb_per_split;           // 64-k blocks of one K split (num_kb without split-K)
+  int split;                  // K splits = cluster size along z (1 for the experts)
 };
 
-// The wgmma GEMM of gemm_tcgen05.cuh (no split-K, no multicast) over the row tiles of the routing table.  A CTA owns 128
-// weight columns as two halves of 64 (one wgmma M = 64 slice per consumer warpgroup): gate/up = the same 64 columns of
-// w1 (half 0) and w3 (half 1), so the epilogue sees g and u of a column side by side; down = 128 columns of w2.  Each
-// half is its own TMA box ([8 k8-rows][64 columns], scale and zero rows of 64 columns) from the expert's tensor maps,
-// which live in the plan buffer.  Row tiles past the last used one exit at once.
-template <int kMT, bool kBf16, bool kGateUp>
+// The wgmma GEMM of gemm_tcgen05.cuh (no multicast) over the row tiles of the work source.  A CTA owns 128 weight
+// columns as two halves of 64 (one wgmma M = 64 slice per consumer warpgroup): gate/up = the same 64 columns of w1
+// (half 0) and w3 (half 1), so the epilogue sees g and u of a column side by side; down = 128 columns of w2.  Each half
+// is its own TMA box ([8 k8-rows][64 columns], scale and zero rows of 64 columns) from the source's tensor maps (plan
+// buffer for the experts, kernel parameters for a dense pair).  Row tiles past the last used one exit at once.
+// Split-K (DenseGemmRows only): the `split` CTAs of a cluster each take kb_per_split blocks of K; their fp32 tiles are
+// summed through DSMEM in rank order, then the gate/up epilogue runs on the sums.
+template <int kMT, bool kBf16, bool kGateUp, class Src>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_x) {
+moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ Src src) {
   using Smem = MoeGemmSmem<kMT>;
   constexpr int kStages = Smem::kStages;
   constexpr int kHalf = kGemmBN / 2;
-  const int tile = blockIdx.y;
-  if (tile >= p.r.meta[1]) return;
-  const int e = p.r.tile_e[tile];
-  const int m0 = p.r.tile_m0[tile];
-  const int m_valid = min(kMT, p.r.counts[e] - (m0 - p.r.pad_off[e]));
+  int e, m0, m_valid;
+  if (!src.gemm_tile(blockIdx.y, kMT, e, m0, m_valid)) return;
   const int n0 = blockIdx.x * (kGateUp ? kHalf : kGemmBN);
-  const CUtensorMap* maps0 = p.maps + (e * 3 + (kGateUp ? 0 : 2)) * 3;
-  const CUtensorMap* maps1 = p.maps + (e * 3 + (kGateUp ? 1 : 2)) * 3;
+  const CUtensorMap* maps0 = src.gemm_maps(e, kGateUp ? 0 : 2);
+  const CUtensorMap* maps1 = src.gemm_maps(e, kGateUp ? 1 : 2);
   const int col1 = kGateUp ? n0 : n0 + kHalf;
+  const int kb_begin = Src::kSplitK ? static_cast<int>(blockIdx.z) * p.kb_per_split : 0;
 
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
@@ -450,7 +490,7 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int wg = warp >> 2;
-  const int num_it = p.num_kb;
+  const int num_it = Src::kSplitK ? max(0, min(p.num_kb, kb_begin + p.kb_per_split) - kb_begin) : p.num_kb;
 
   if (threadIdx.x == 0) {
     prefetch_tmap(&tmap_x);
@@ -471,7 +511,7 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
         const int s = it % kStages;
         mbar_wait(empty(s), ((it / kStages) & 1) ^ 1u);
         mbar_arrive_expect_tx(b_full(s), Smem::kBStage);
-        tma_load_2d(smem_base + s * Smem::kBStage, &tmap_x, it * kGemmBK, m0, b_full(s));
+        tma_load_2d(smem_base + s * Smem::kBStage, &tmap_x, (kb_begin + it) * kGemmBK, m0, b_full(s));
       }
     } else if (warp == 1 && lane == 0) {
       const int ngr = p.group_size == 32 ? 2 : 1;
@@ -480,7 +520,7 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
         const int ws = it % kStages;
         mbar_wait(empty(ws), ((it / kStages) & 1) ^ 1u);
         mbar_arrive_expect_tx(b_full(ws), bytes);
-        const int k0 = it * kGemmBK;
+        const int k0 = (kb_begin + it) * kGemmBK;
         const int g0 = p.gs_log2 >= 0 ? (k0 >> p.gs_log2) : k0 / p.group_size;
         const uint32_t w_at = smem_base + Smem::kWOff + ws * Smem::kWStage;
         const uint32_t s_at = smem_base + Smem::kSOff + ws * Smem::kSStage;
@@ -574,37 +614,65 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
       for (int h = 0; h < 2; ++h)
 #pragma unroll
         for (int e2 = 0; e2 < 2; ++e2) stage_f32[(8 * i + 2 * t + e2) * kGemmLd + c0 + 8 * h] = acc[4 * i + 2 * h + e2];
-    consumer_sync();
-
-    const MoeExpertDev& X = p.ex[e];
+    const MoeExpertDev& X = src.layers(e);
     uint16_t* yp = reinterpret_cast<uint16_t*>(p.out);
-    if constexpr (kGateUp) {
-      const uint16_t* b1 = reinterpret_cast<const uint16_t*>(X.bias[0]);
-      const uint16_t* b3 = reinterpret_cast<const uint16_t*>(X.bias[1]);
-      for (int idx = threadIdx.x - 128; idx < kMT * kHalf; idx += kGemmConsumers) {
-        const int ml = idx / kHalf, nl = idx % kHalf;
-        if (ml < m_valid) {
+    if (!Src::kSplitK || p.split == 1) {
+      consumer_sync();
+      if constexpr (kGateUp) {
+        for (int idx = threadIdx.x - 128; idx < kMT * kHalf; idx += kGemmConsumers) {
+          const int ml = idx / kHalf, nl = idx % kHalf;
           const int nn = n0 + nl;
-          float gv = stage_f32[ml * kGemmLd + nl], uv = stage_f32[ml * kGemmLd + kHalf + nl];
-          if (b1 != nullptr) gv += elt_to_float<kBf16>(b1[nn]);
-          if (b3 != nullptr) uv += elt_to_float<kBf16>(b3[nn]);
-          const float h = moe_silu_mul<kBf16>(float_to_elt<kBf16>(gv), float_to_elt<kBf16>(uv));
-          const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
-          yp[static_cast<size_t>(m0 + ml) * p.N + dst] = float_to_elt<kBf16>(h);
+          if (ml < m_valid && nn < p.N) {
+            const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
+            store_gate_up<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + dst, stage_f32[ml * kGemmLd + nl],
+                                 stage_f32[ml * kGemmLd + kHalf + nl], X.bias[0], X.bias[1], nn);
+          }
+        }
+      } else {
+        const uint16_t* b2 = reinterpret_cast<const uint16_t*>(X.bias[2]);
+        const int pos0 = src.r.offsets[e] + (m0 - src.r.pad_off[e]);
+        for (int idx = threadIdx.x - 128; idx < kMT * kGemmBN; idx += kGemmConsumers) {
+          const int ml = idx / kGemmBN, nl = idx % kGemmBN;
+          if (ml < m_valid) {
+            const int nn = n0 + nl;
+            float v = stage_f32[ml * kGemmLd + nl];
+            if (b2 != nullptr) v += elt_to_float<kBf16>(b2[nn]);
+            yp[static_cast<size_t>(src.r.pairs[pos0 + ml]) * p.N + nn] = float_to_elt<kBf16>(v);
+          }
         }
       }
-    } else {
-      const uint16_t* b2 = reinterpret_cast<const uint16_t*>(X.bias[2]);
-      const int pos0 = p.r.offsets[e] + (m0 - p.r.pad_off[e]);
-      for (int idx = threadIdx.x - 128; idx < kMT * kGemmBN; idx += kGemmConsumers) {
-        const int ml = idx / kGemmBN, nl = idx % kGemmBN;
-        if (ml < m_valid) {
+    }
+  }
+
+  if constexpr (Src::kSplitK && kGateUp) {
+    if (p.split > 1) {
+      // cluster (1, 1, split): every CTA holds fp32 partial g | u tiles [kMT][64 | 64]; rank r reduces a slice of x rows
+      // (sum over the ranks in rank order), then forms h
+      cooperative_groups::cluster_group cluster = cooperative_groups::this_cluster();
+      cluster.sync();
+      if (wg > 0) {
+        const int rank = static_cast<int>(cluster.block_rank());
+        const int rows_per_rank = (kMT + p.split - 1) / p.split;
+        const MoeExpertDev& X = src.layers(e);
+        uint16_t* yp = reinterpret_cast<uint16_t*>(p.out);
+        for (int idx = threadIdx.x - 128; idx < rows_per_rank * kHalf; idx += kGemmConsumers) {
+          const int ml = rank * rows_per_rank + idx / kHalf, nl = idx % kHalf;
           const int nn = n0 + nl;
-          float v = stage_f32[ml * kGemmLd + nl];
-          if (b2 != nullptr) v += elt_to_float<kBf16>(b2[nn]);
-          yp[static_cast<size_t>(p.r.pairs[pos0 + ml]) * p.N + nn] = float_to_elt<kBf16>(v);
+          if (ml < m_valid && nn < p.N) {
+            float gr[8], ur[8];
+#pragma unroll
+            for (int r = 0; r < 8; ++r) {
+              gr[r] = r < p.split ? *cluster.map_shared_rank(&stage_f32[ml * kGemmLd + nl], r) : 0.f;
+              ur[r] = r < p.split ? *cluster.map_shared_rank(&stage_f32[ml * kGemmLd + kHalf + nl], r) : 0.f;
+            }
+            float gv = 0.f, uv = 0.f;
+#pragma unroll
+            for (int r = 0; r < 8; ++r) { gv += gr[r]; uv += ur[r]; }
+            store_gate_up<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + nn, gv, uv, X.bias[0], X.bias[1], nn);
+          }
         }
       }
+      cluster.sync();
     }
   }
 }

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 6
+#define AGB200_ABI_VERSION 7
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -292,6 +292,43 @@ size_t agb200_moe_workspace_bytes(int T, int k, int E, int H, int I);
 int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
                        int weights_dtype, int T, int k, void* out, void* workspace, size_t workspace_bytes, void* stream);
 int agb200_moe_destroy(void* handle);
+
+/*
+ * Fused gate/up of a dense MLP (ABI v7): the gate and up projections of a Llama / Mistral / Qwen2 MLP and the SiLU * mul
+ * between them in one launch,
+ *
+ *   h[M, I] = round(round(silu(g)) * u),  g = round(x Wg + bg),  u = round(x Wu + bu)   (every round: to `dtype`)
+ *
+ * so that g and u never reach device memory.  Replaces, for 4-bit layers, the first half of the reference's fused MLP
+ * (auto_gptq/nn_modules/fused_llama_mlp.py:131-245, FusedLlamaMLPForQuantizedModel: its Triton quant_fused_matmul_248 of
+ * gate and up with act_fn(gate) * up, and the unfused LlamaMLP.forward down_proj(act_fn(gate_proj(x)) * up_proj(x)),
+ * transformers/models/llama/modeling_llama.py).  The down projection stays an ordinary agb200_w4a16_forward.
+ *
+ *   gate, up  layer descriptors (agb200_moe_layer) of two 4-bit layers with the same K, N = I, group_size and dtype.
+ *             Act-order layers: qweight is the matrix made by agb200_w4_make_sequential and perm its permutation; gate
+ *             and up must then share ONE perm pointer (they are quantised on the same input).  qweight_tc
+ *             (agb200_w4_prepare_tc) is needed on the GEMM path; bias may be NULL.
+ *   x, h      [M, K] / [M, I] of `dtype`, device memory, 16-byte aligned.
+ *   workspace DEVICE scratch of agb200_w4a16_gate_up_workspace_bytes(M, K, I) bytes: the gathered x of an act-order
+ *             pair on the GEMM path (may be NULL otherwise).
+ * Kernels: M <= AGB200_MOE_DECODE_MAX_T runs the experts' decode kernel over dense rows (weights streamed from the
+ * checkpoint layout, fp32 accumulation; needs 16 * K bytes of x in shared memory, K <= 13824 on H100, and
+ * group_size % 32 == 0 or one group); larger M the wgmma GEMM with 64 gate + 64 up columns per CTA and split-K over a
+ * thread-block cluster (partial sums reduced through DSMEM, then silu * mul).
+ * Constraints (else AGB200_ENOSUP): K % 8 == 0, I % 32 == 0; GEMM path: group_size 32 or a multiple of 64 (-1 = K).
+ * No host synchronisation (CUDA-graph capturable); two calls on the same inputs give bit-identical h.
+ */
+#define AGB200_GATE_UP_AUTO 0
+#define AGB200_GATE_UP_DECODE 1   /* M <= AGB200_MOE_DECODE_MAX_T */
+#define AGB200_GATE_UP_GEMM 2
+int agb200_w4a16_gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
+                         int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream);
+/* Same, with an explicit kernel (AGB200_GATE_UP_*) and GEMM tuning (tests / benchmarks): tile_m = x-row tile
+ * (32|64|128, 0 = auto), split_k = K splits (1|2|4|8, 0 = auto). */
+int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
+                            int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream,
+                            int kernel, int tile_m, int split_k);
+size_t agb200_w4a16_gate_up_workspace_bytes(int M, int K, int I);
 
 /*
  * GPTQ quantiser (ABI v6): makes the packed 4-bit layers the entry points above run, on the GPU.
