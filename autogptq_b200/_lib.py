@@ -12,7 +12,7 @@ from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 7
+ABI_VERSION = 8
 F16, BF16 = 0, 1
 ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
@@ -61,6 +61,7 @@ def _declare(lib):
         "agb200_chain_destroy": (I, [P]),
         "agb200_chain_info": (I, [P, P, P, P]),
         "agb200_chain_profile": (I, [P, P, I]),
+        "agb200_chain_tuning": (I, [P, P, P, P, P]),
         "agb200_peer_alloc": (I, [S, P]),
         "agb200_chain_diag": (I, [P]),
         "agb200_peer_free": (I, [P]),

@@ -30,8 +30,6 @@ if os.environ.get("AGB200_EXPERIMENTAL", "0") == "1":      # the two decode kern
     NVCC_FLAGS.append("-DAGB200_EXPERIMENTAL_KERNELS")
 # translation units of the library (compiled in parallel, then linked)
 UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu"]
-# chain.cu holds only the 448-thread persistent chain kernel (one CTA per SM)
-UNIT_FLAGS = {"chain.cu": ["-maxrregcount=112"]}
 
 
 def _nvcc() -> str:
@@ -50,7 +48,6 @@ def _sources_digest() -> str:
             h.update(f.encode())
             h.update(open(p, "rb").read())
     h.update(" ".join(NVCC_FLAGS).encode())
-    h.update(repr(sorted(UNIT_FLAGS.items())).encode())
     return h.hexdigest()
 
 
@@ -68,7 +65,7 @@ def build_extension(force: bool = False, verbose: bool = False) -> str:
         objs.append(obj)
         if only and unit not in only.split(",") and os.path.exists(obj):
             continue
-        cmd = [nvcc, *NVCC_FLAGS, *UNIT_FLAGS.get(unit, []), "-c", "-o", obj, os.path.join(CSRC, unit)]
+        cmd = [nvcc, *NVCC_FLAGS, "-c", "-o", obj, os.path.join(CSRC, unit)]
         if verbose:
             cmd.insert(1, "-Xptxas=-v")
             print(" ".join(cmd), flush=True)

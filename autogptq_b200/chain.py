@@ -163,21 +163,28 @@ class DecodeChain:
         lib = _lib.load()
         a, b, c = ctypes.c_int(), ctypes.c_int(), ctypes.c_int()
         _lib.check(lib.agb200_chain_info(self._handle, ctypes.byref(a), ctypes.byref(b), ctypes.byref(c)), "agb200_chain_info")
-        return {"ring_slots": a.value, "smem_bytes": b.value, "grid": c.value, "stages": len(self._stages)}
+        la, la_max, inflight, backoff = (ctypes.c_int() for _ in range(4))
+        _lib.check(lib.agb200_chain_tuning(self._handle, ctypes.byref(la), ctypes.byref(la_max), ctypes.byref(inflight),
+                                           ctypes.byref(backoff)), "agb200_chain_tuning")
+        return {"ring_slots": a.value, "smem_bytes": b.value, "grid": c.value, "stages": len(self._stages),
+                "l2_lookahead": la.value, "l2_lookahead_max": la_max.value, "inflight": inflight.value,
+                "poll_backoff": backoff.value}
 
     def profile(self):
-        """Cycle counters of the last run(debug_flags=8) as an int64 array [grid, 3 consumer groups, 8 categories]:
-        total, wait for x, convert x, wait for weights, unpack + MMA, flush, tile end, stage end.  Measurement aid."""
+        """Counters of the last run(debug_flags=8) as an int64 array [grid, 4, 8].  Rows 0..2, one warp per consumer
+        group, in cycles: total, wait for x, convert x, wait for weights, unpack + MMA, flush, tile end, stage end.
+        Row 3, the producer: total cycles, cycles blocked on a full ring, cycles blocked on the in-flight cap, slots
+        issued, slots prefetched into L2, then three zeros.  Measurement aid."""
         import numpy as np
 
         lib = _lib.load()
         torch.cuda.synchronize(self.device)
-        n = self.info()["grid"] * 3 * 8
+        n = self.info()["grid"] * 4 * 8
         buf = (ctypes.c_longlong * n)()
         rc = lib.agb200_chain_profile(self._handle, buf, n)
         if rc < 0:
             _lib.check(rc, "agb200_chain_profile")
-        return np.frombuffer(buf, dtype=np.int64).reshape(-1, 3, 8).copy()
+        return np.frombuffer(buf, dtype=np.int64).reshape(-1, 4, 8).copy()
 
     def __del__(self):
         try:

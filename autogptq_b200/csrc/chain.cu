@@ -35,12 +35,19 @@ int failf(int code, const char* fmt, ...) {
   } while (0)
 
 constexpr uint32_t kMagic = 0x43484e32u;   // "CHN2"
+// Measured on one H100 80GB HBM3 at a 400 W power limit, bench.py's Llama-2-7B token (tools/chain_lookahead_sweep.py,
+// DESIGN 3.5).  L2 lookahead: 1-3 slots no faster, 4-7 slots 5-10 % slower, so it is off.  In-flight cap: 3 slots was the
+// fastest setting of the sweep (cap off / 3 / 4 / 6: 1525 / 1451 / 1489 / 1579 us per token); bench.py measured 700-705
+// tokens/s with it against 671-672 without (three alternating runs each).  Poll back-off 0..800 cycles made no difference.
+constexpr int kDefaultLookahead = 0;
+constexpr int kDefaultInflight = 3;
 
 struct Chain {
   uint32_t magic;
   int device;
   int n_stages, M, dtype;
   int slots, rows_pad_max, grid;
+  int lookahead_max;
   size_t smem;
   int smem_optin;
   agb::ChainParams params;
@@ -48,7 +55,7 @@ struct Chain {
 
 size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 constexpr size_t kFlagsBytes = 256;
-constexpr size_t kProfBytes = 256 * agb::kChGroups * agb::kChProfSlots * sizeof(long long);   // up to 256 CTAs
+constexpr size_t kProfBytes = 256 * agb::kChProfRows * agb::kChProfSlots * sizeof(long long);   // up to 256 CTAs
 size_t stages_bytes(int n) { return align_up(size_t(n) * sizeof(agb::ChainStage), 128); }
 size_t maps_bytes(int n) { return size_t(n) * agb::kChMaxGroup * 3 * sizeof(CUtensorMap); }
 size_t ll_bytes(const agb200_chain_stage* stages, int n, int M) {
@@ -300,9 +307,18 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   if (slots > agb::kChMaxSlots) slots = agb::kChMaxSlots;
   if (const char* e = getenv("AGB200_CHAIN_SLOTS")) { const int v = atoi(e); if (v >= agb::kChGroups && v < slots) slots = v; }
   // Any ring size works: the landed-barriers come in pairs per ring position (chain.cuh), so a position that changes its
-  // owner group from lap to lap cannot be mistaken for its previous use.  `inflight` stays as a measurement knob.
-  int inflight = 0;
-  if (const char* e = getenv("AGB200_CHAIN_INFLIGHT")) { const int v = atoi(e); if (v >= 1) inflight = v; }
+  // owner group from lap to lap cannot be mistaken for its previous use.  `inflight` caps the slots in flight
+  // (AGB200_CHAIN_INFLIGHT, 0 = no cap); a cap at or above the ring size does nothing.
+  int inflight = kDefaultInflight;
+  if (const char* e = getenv("AGB200_CHAIN_INFLIGHT")) { const int v = atoi(e); if (v >= 0) inflight = v; }
+  // L2 lookahead (chain.cuh, producer): the slots prefetched into L2 while the ring is full must still be there when the
+  // consumers resume, next to the weights every other SM is streaming through L2 at the same time: all CTAs together keep
+  // at most a third of the L2 in lookahead slots (H100: 7 slots)
+  int l2_bytes = 0;
+  CH_CUDA(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev));
+  const int lookahead_max = static_cast<int>(static_cast<size_t>(l2_bytes) / 3 / (size_t(agb::kChSlotBytes) * sms));
+  int lookahead = std::min(kDefaultLookahead, lookahead_max);
+  if (const char* e = getenv("AGB200_CHAIN_L2_LOOKAHEAD")) { const int v = atoi(e); if (v >= 0) lookahead = std::min(v, lookahead_max); }
 
   // the plan is caller memory a stream-ordered allocator may have just recycled from a tensor that kernels queued on a
   // non-blocking stream still write; the legacy-stream copies below are not ordered after them (create time only)
@@ -322,8 +338,10 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   c->params.n_stages = n_stages; c->params.slots = slots; c->params.rows_pad_max = rows_pad_max; c->params.debug = 0;
   c->params.xs_bytes = xs_bytes;
   c->params.inflight = inflight;
+  c->params.lookahead = lookahead;
+  c->lookahead_max = lookahead_max;
   c->params.diag = diag_device_ptr();
-  c->params.poll_backoff = 400;    // cycles after a failed poll of x (AGB200_CHAIN_POLL_BACKOFF; not tuned on H100)
+  c->params.poll_backoff = 400;    // cycles after a failed poll of x (AGB200_CHAIN_POLL_BACKOFF; 0..800 measured the same on H100)
   if (const char* e = getenv("AGB200_CHAIN_POLL_BACKOFF")) { const int v = atoi(e); if (v >= 0 && v <= 100000) c->params.poll_backoff = v; }
   *handle_out = c;
   return 0;
@@ -350,6 +368,16 @@ int agb200_chain_info(void* handle, int* slots, int* smem_bytes, int* grid) {
   return 0;
 }
 
+int agb200_chain_tuning(void* handle, int* lookahead, int* lookahead_max, int* inflight, int* poll_backoff) {
+  Chain* c = static_cast<Chain*>(handle);
+  if (!c || c->magic != kMagic) return failf(AGB200_EINVAL, "chain: bad handle");
+  if (lookahead) *lookahead = c->params.lookahead;
+  if (lookahead_max) *lookahead_max = c->lookahead_max;
+  if (inflight) *inflight = c->params.inflight;
+  if (poll_backoff) *poll_backoff = c->params.poll_backoff;
+  return 0;
+}
+
 int agb200_chain_diag(int* out5) {
   if (!out5) return failf(AGB200_EINVAL, "chain diag: null output");
   for (int i = 0; i < 5; ++i) out5[i] = g_diag_host != nullptr ? g_diag_host[i] : 0;
@@ -359,7 +387,7 @@ int agb200_chain_diag(int* out5) {
 int agb200_chain_profile(void* handle, long long* out_host, int max_entries) {
   Chain* c = static_cast<Chain*>(handle);
   if (!c || c->magic != kMagic || !out_host) return failf(AGB200_EINVAL, "chain: bad handle");
-  const int n = c->grid * agb::kChGroups * agb::kChProfSlots;
+  const int n = c->grid * agb::kChProfRows * agb::kChProfSlots;
   if (max_entries < n) return failf(AGB200_EWORKSPACE, "chain profile: need room for %d entries", n);
   CH_CUDA(cudaMemcpy(out_host, c->params.prof, size_t(n) * sizeof(long long), cudaMemcpyDeviceToHost));
   return n;

@@ -11,7 +11,8 @@
 //     zero-word rows they need) filled with cp.async.bulk.tensor (TMA)
 //     loads.  It never waits for a layer boundary, only for a free slot, so it runs a stage or more AHEAD of the
 //     arithmetic; the arithmetic is faster than the stream in bursts, so the ring is what keeps HBM busy while a
-//     stage boundary stalls it;
+//     stage boundary stalls it.  When even the ring is full, the producer prefetches the next slots into L2
+//     (`lookahead`) so that HBM keeps streaming until the consumers resume;
 //   * dependencies are DATA FLOW, not barriers: a stage's y is published as 8-byte {two 16-bit values, launch tag} words
 //     (single-copy atomic stores, the "LL" idea of NCCL's low-latency protocol); the consumers of the next stage poll the
 //     very words they need.  No flag, no fence, no atomic, no grid barrier sits between a tile's last MMA and the next
@@ -69,6 +70,8 @@ constexpr int kChMaxPeers = 8;
 enum ChainXMode { kChXPlain = 0, kChXSiluMul = 1, kChXSumParts = 2 };
 enum ChainDebug { kChDbgNoDeps = 1, kChDbgNoMath = 2, kChDbgNoConvert = 4, kChDbgProfile = 8 };
 constexpr int kChProfSlots = 8;   // per CTA and profiled warp: total, wait for x, convert, wait for weights, MMA, flush, tile end, -
+constexpr int kChProfRows = kChGroups + 1;   // one warp per consumer group, then the producer: total, blocked on a full
+                                             // ring, blocked on the in-flight cap, slots issued, slots prefetched into L2, -, -, -
 
 struct ChainLayer {
   const void* bias;     // [N] or null
@@ -101,11 +104,12 @@ struct ChainParams {
   const ChainStage* stages;    // [n_stages] device
   const CUtensorMap* maps;     // 3 per layer (weights, scales, zeros), indexed by ChainStage::map_base
   unsigned* flags;             // [0] = launches completed, [1] = CTAs finished
-  long long* prof;             // [grid][kChGroups warps][kChProfSlots] cycle counters (kChDbgProfile)
+  long long* prof;             // [grid][kChProfRows][kChProfSlots] cycle counters (kChDbgProfile)
   int n_stages, slots, rows_pad_max, debug;
   int xs_bytes;                // shared-memory staging of x for act-order gathers (0 when no stage has a perm)
   int inflight;                // 0, or the most ring slots the producer keeps in flight (landed slots do not count)
   int poll_backoff;            // cycles a thread waits after a failed poll of x before the next one
+  int lookahead;               // 0, or the most slots past a blocked one that the producer prefetches into L2
   int* diag;                   // host-mapped words {site, stage, CTA, warp, extra} written before a protocol timeout traps, or null
 };
 
@@ -196,6 +200,50 @@ __device__ __forceinline__ void ch_copy_desc_store(uint32_t* dst, int lane, cons
   dst[lane + 32] = r.w1;
   dst[lane + 64] = r.w2;
 }
+// Position of a producer cursor in this CTA's walk over (stage, tile, 1024-k chunk), with the fields of its stage that the
+// walk needs.  The issue cursor and the L2 lookahead cursor both move with these helpers, so they visit the same slots in
+// the same order.
+struct ChWalk {
+  int s, tile, j;
+  int C, total, lb, map_base, n_layers;
+  int tb1, tb2, tb3;            // tile_begin of layers 1..3 (layer 0 starts at tile 0)
+};
+// enter stage s at this CTA's first tile (tile >= total: the CTA has no tile in it); kLdg: read the descriptor from global
+// memory through the read-only path instead of from the producer's shared-memory copy
+template <bool kLdg>
+__device__ __forceinline__ void ch_walk_enter(ChWalk& w, const ChainStage* st, int s, int bid, int G) {
+  auto ld = [](const int* a) { return kLdg ? __ldg(a) : *a; };
+  w.s = s;
+  w.j = 0;
+  w.C = ld(&st->chunks);
+  w.total = ld(&st->total_tiles);
+  w.lb = ld(&st->bpg_log2);
+  w.map_base = ld(&st->map_base);
+  w.n_layers = ld(&st->n_layers);
+  w.tb1 = ld(&st->layer[1].tile_begin);
+  w.tb2 = ld(&st->layer[2].tile_begin);
+  w.tb3 = ld(&st->layer[3].tile_begin);
+  const int vb = bid - ld(&st->rot);
+  w.tile = vb < 0 ? vb + G : vb;
+}
+// next slot inside the stage; false once the walk has left it
+__device__ __forceinline__ bool ch_walk_next(ChWalk& w, int G) {
+  if (++w.j == w.C) { w.j = 0; w.tile += G; }
+  return w.tile < w.total;
+}
+// the three TMA boxes of the slot under the cursor: box(b, map, c0, c1) with b = 0 weights [128 k8-rows x 32 columns],
+// 1 the 8 scale rows, 2 the 8 zero-word rows
+template <typename F>
+__device__ __forceinline__ void ch_walk_boxes(const ChWalk& w, const CUtensorMap* maps, F&& box) {
+  const int li = (w.n_layers > 1 && w.tile >= w.tb1) + (w.n_layers > 2 && w.tile >= w.tb2) + (w.n_layers > 3 && w.tile >= w.tb3);
+  const int tl = w.tile - (li == 0 ? 0 : li == 1 ? w.tb1 : li == 2 ? w.tb2 : w.tb3);
+  const CUtensorMap* m3 = maps + w.map_base + 3 * li;
+  const int grow = (w.j * 8) >> w.lb;
+  box(0, m3, tl * 32, w.j * kChSlotRows);
+  box(1, m3 + 1, tl * 32, grow);
+  box(2, m3 + 2, tl * 4, grow);
+}
+
 __device__ __forceinline__ int ch_locate(const ChainStage& st, int tile, int& li) {
   li = 0;
 #pragma unroll
@@ -344,45 +392,76 @@ w4a16_chain_kernel(const ChainParams p) {
     __syncwarp();
     int slot = 0;
     int lap = 0;                                       // times the producer went around the ring
-    // optional cap on the bytes in flight (measurement knob AGB200_CHAIN_INFLIGHT, off by default: it costs stream rate)
+    // cap on the slots in flight (AGB200_CHAIN_INFLIGHT; chain.cu has the default and the measurement behind it)
     const int F = p.inflight > 0 && p.inflight < S ? p.inflight : 0;
     int lslot = 0;                                     // oldest slot that may still be in flight
     int llap = 0;
     int ahead = 0;                                     // slots issued and not yet known to have landed
+    // L2 lookahead: while the ring is full (the consumers wait for x at a stage boundary and this SM's share of HBM would
+    // idle), the slots after the blocked one are prefetched into L2 by a second cursor, at most P ahead; once the
+    // consumers resume, their loads hit L2 and the ring refills at L2 speed.  A ring that is not full issues nothing extra.
+    const int P = p.lookahead;
+    ChWalk la{};                                       // next slot to prefetch, la_n slots past the issue cursor
+    int la_n = 0;
+    bool la_end = false;                               // the lookahead cursor has walked past the last stage
+    long long pr_t0 = kProf ? clock64() : 0, pr_full = 0, pr_cap = 0, pr_issued = 0, pr_pref = 0;
     for (int s = 0; s < p.n_stages; ++s) {
       if (s + 1 < p.n_stages) ch_copy_desc_load(p.stages + s + 1, lane, dr);     // latency hidden behind this stage's loads
       if (lane == 0) {
-        const ChainStage& st = *reinterpret_cast<const ChainStage*>(pdesc + (s & 1) * kChDescWords);
-        const CUtensorMap* mp = p.maps + st.map_base;
-        const int C = st.chunks, lb = st.bpg_log2;
-        int vb = bid - st.rot;
-        if (vb < 0) vb += G;
-        for (int tile = vb; tile < st.total_tiles; tile += G) {
-          int li;
-          const int tl = ch_locate(st, tile, li);
-          const CUtensorMap* m3 = mp + 3 * li;
-          for (int j = 0; j < C; ++j) {
-            if (F > 0 && ahead >= F) {
-              ch_wait(full(lslot, llap), (llap >> 1) & 1, p.diag, kChSiteLanded, s, lslot);   // the oldest request has landed
-              if (++lslot == S) { lslot = 0; ++llap; }
-              --ahead;
-            }
-            ch_wait(empty(slot), (lap & 1) ^ 1, p.diag, kChSiteEmpty, s, slot);
-            const uint32_t fb = full(slot, lap);
-            mbar_arrive_expect_tx(fb, kChSlotTx);
-            ++ahead;
-            const uint32_t dst = smem_base + slot * kChSlotBytes;
-            const int grow = (j * 8) >> lb;
-            tma_load_2d(dst, m3, tl * 32, j * kChSlotRows, fb);
-            tma_load_2d(dst + kChWBytes, m3 + 1, tl * 32, grow, fb);
-            tma_load_2d(dst + kChWBytes + kChSBytes, m3 + 2, tl * 4, grow, fb);
-            if (++slot == S) { slot = 0; ++lap; }
+        ChWalk w;
+        ch_walk_enter<false>(w, reinterpret_cast<const ChainStage*>(pdesc + (s & 1) * kChDescWords), s, bid, G);
+        for (bool more = w.tile < w.total; more; more = ch_walk_next(w, G)) {
+          if (F > 0 && ahead >= F) {
+            const long long t0 = kProf ? clock64() : 0;
+            ch_wait(full(lslot, llap), (llap >> 1) & 1, p.diag, kChSiteLanded, s, lslot);   // the oldest request has landed
+            if constexpr (kProf) pr_cap += clock64() - t0;
+            if (++lslot == S) { lslot = 0; ++llap; }
+            --ahead;
           }
+          const uint32_t eb = empty(slot), ep = (lap & 1) ^ 1;
+          if (!mbar_test_wait(eb, ep)) {                 // the ring is full
+            const long long t0 = kProf ? clock64() : 0;
+            while (la_n < P) {
+              if (la_n == 0) { la = w; la_end = false; }
+              if (la_end) break;
+              ch_walk_boxes(la, p.maps, [](int, const CUtensorMap* m, int c0, int c1) { tma_prefetch_l2_2d(m, c0, c1); });
+              ++la_n;
+              if constexpr (kProf) ++pr_pref;
+              if (!ch_walk_next(la, G)) {                // into the next stage that has a tile for this CTA
+                la_end = true;
+                for (int s2 = la.s + 1; s2 < p.n_stages && la_end; ++s2) {
+                  ch_walk_enter<true>(la, p.stages + s2, s2, bid, G);
+                  la_end = la.tile >= la.total;
+                }
+              }
+              if (mbar_test_wait(eb, ep)) break;
+            }
+            ch_wait(eb, ep, p.diag, kChSiteEmpty, s, slot);
+            if constexpr (kProf) pr_full += clock64() - t0;
+          }
+          if (la_n > 0) --la_n;                          // the issue cursor moves up to the lookahead cursor
+          const uint32_t fb = full(slot, lap);
+          mbar_arrive_expect_tx(fb, kChSlotTx);
+          ++ahead;
+          if constexpr (kProf) ++pr_issued;
+          const uint32_t dst = smem_base + slot * kChSlotBytes;
+          ch_walk_boxes(w, p.maps, [&](int b, const CUtensorMap* m, int c0, int c1) {
+            tma_load_2d(dst + (b == 0 ? 0u : b == 1 ? uint32_t(kChWBytes) : uint32_t(kChWBytes + kChSBytes)), m, c0, c1, fb);
+          });
+          if (++slot == S) { slot = 0; ++lap; }
         }
       }
       __syncwarp();
       if (s + 1 < p.n_stages) ch_copy_desc_store(pdesc + ((s + 1) & 1) * kChDescWords, lane, dr);
       __syncwarp();
+    }
+    if constexpr (kProf) {
+      if (lane == 0) {
+        long long* dst = p.prof + (static_cast<size_t>(bid) * kChProfRows + kChGroups) * kChProfSlots;
+        const long long row[kChProfSlots] = {clock64() - pr_t0, pr_full, pr_cap, pr_issued, pr_pref, 0, 0, 0};
+#pragma unroll
+        for (int i = 0; i < kChProfSlots; ++i) dst[i] = row[i];
+      }
     }
     return;
   }
@@ -940,7 +1019,7 @@ w4a16_chain_kernel(const ChainParams p) {
   if constexpr (kProf) {
     if (prof_on) {
       pc[0] = clock64() - tstart;
-      long long* dst = p.prof + (static_cast<size_t>(bid) * kChGroups + grp) * kChProfSlots;
+      long long* dst = p.prof + (static_cast<size_t>(bid) * kChProfRows + grp) * kChProfSlots;
 #pragma unroll
       for (int i = 0; i < kChProfSlots; ++i) dst[i] = pc[i];
     }

@@ -44,6 +44,13 @@ __device__ __forceinline__ void mbar_wait_spin(uint32_t bar, uint32_t parity) {
     if (++polls > (1u << 26)) __trap();
   }
 }
+// Non-blocking test of a phase (try_wait may suspend the thread for a while first)
+__device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.test_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
+               : "=r"(done) : "r"(bar), "r"(parity) : "memory");
+  return done != 0;
+}
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
 __device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
@@ -54,6 +61,10 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
 __device__ __forceinline__ void tma_load_2d_mcast(uint32_t smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar, uint16_t mask) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
                ::"r"(smem_dst), "l"(tmap), "r"(bar), "h"(mask), "r"(c0), "r"(c1) : "memory");
+}
+// Same box, fetched into L2 only: no shared memory, no barrier; a later load of the box hits L2
+__device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* tmap, int c0, int c1) {
+  asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");

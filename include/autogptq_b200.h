@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 7
+#define AGB200_ABI_VERSION 8
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -211,9 +211,15 @@ int agb200_chain_forward(void* handle, int flags, void* stream);
 int agb200_chain_destroy(void* handle);
 /* Facts about a created chain for logs / benchmarks: ring slots, dynamic shared memory bytes, grid size. */
 int agb200_chain_info(void* handle, int* slots, int* smem_bytes, int* grid);
-/* After a forward with AGB200_CHAIN_DEBUG_PROFILE (and a stream synchronisation): copies grid x 3 x 8 cycle counters
- * {total, wait for x, convert x, wait for weights, unpack + MMA, flush, tile end, -} of one warp per consumer
- * group to out_host; returns the number of entries or a negative error.  Measurement aid. */
+/* The chain's weight-stream settings: `lookahead` ring slots the producer may prefetch into L2 while the ring is full
+ * (0: none; at most `lookahead_max`, which keeps them within a third of the L2; AGB200_CHAIN_L2_LOOKAHEAD at create time
+ * overrides the default), the in-flight cap (0: none) and the back-off in cycles after a failed poll of x. */
+int agb200_chain_tuning(void* handle, int* lookahead, int* lookahead_max, int* inflight, int* poll_backoff);
+/* After a forward with AGB200_CHAIN_DEBUG_PROFILE (and a stream synchronisation): copies grid x 4 x 8 counters to out_host:
+ * rows 0..2 = one warp per consumer group, cycles {total, wait for x, convert x, wait for weights, unpack + MMA, flush,
+ * tile end, -}; row 3 = the producer {total cycles, cycles blocked on a full ring, cycles blocked on the in-flight cap,
+ * slots issued, slots prefetched into L2, -, -, -}.  Returns the number of entries or a negative error.  Measurement aid
+ * (ABI 7 had the three consumer rows only). */
 int agb200_chain_profile(void* handle, long long* out_host, int max_entries);
 /* Every wait inside the chain kernel is bounded; a timeout (a protocol bug, or a peer rank that died) traps the launch
  * after writing {site (0 = none), stage, CTA, warp, detail} to host-mapped words.  They stay readable after the CUDA

@@ -100,16 +100,19 @@ def main():
             raise
         print(f"[probe] {name}: {us:.1f} us", file=sys.stderr, flush=True)
         out[name] = {"us": round(us, 1), "gbs": round(nbytes / us / 1e3, 1)}
-    # where the consumer warps spend their cycles (one warp per consumer group and CTA)
-    cats = ["total", "wait_x", "convert", "wait_w", "mma", "flush", "tile_end", "stage_end"]
+    # where the consumer warps spend their cycles (one warp per consumer group and CTA), and how long the producer sits
+    # on a full ring
+    from tools.chain_lookahead_sweep import CONSUMER as cats, profile_summary
     for name, flags in (("full", 8), ("no_deps", 9)):
         with torch.cuda.stream(stream):
             ch.run(flags)
             torch.cuda.synchronize()
-        pr = ch.profile().astype("float64")
+        raw = ch.profile()
+        pr = raw[:, :3, :].astype("float64")
         tot = pr[:, :, 0].mean()
         out["profile_" + name] = {"total_cycles": round(tot), **{c: round(float(pr[:, :, i].mean() / tot), 3) for i, c in enumerate(cats) if i > 0},
                                   "max_over_ctas": {c: round(float(pr[:, :, i].max() / tot), 3) for i, c in enumerate(cats) if i > 0}}
+        out["producer_" + name] = profile_summary(raw)[1]
 
     def per_layer():
         xx = x
