@@ -12,14 +12,14 @@ from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 8
+ABI_VERSION = 9
 F16, BF16 = 0, 1
 ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
 CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS = 0, 1, 2
 CHAIN_DEBUG_NO_DEPS, CHAIN_DEBUG_NO_MATH = 1, 2
 PEER_HANDLE_BYTES = 64
-KERNEL_AUTO, KERNEL_GEMV, KERNEL_GEMM, KERNEL_SKINNY, KERNEL_DECODE, KERNEL_TCDECODE, KERNEL_IMMA = 0, 1, 2, 3, 4, 5, 6
+KERNEL_AUTO, KERNEL_GEMV, KERNEL_GEMM, KERNEL_SKINNY, KERNEL_IMMA = 0, 1, 2, 3, 6
 GEMV_MAX_M = 4
 SKINNY_MAX_M = 8
 IMMA_MAX_M = 8

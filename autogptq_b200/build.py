@@ -26,8 +26,6 @@ NVCC_FLAGS = [
     "-Xcompiler", "-fPIC",
     "-DAGB200_NO_FAST_MATH",
 ]
-if os.environ.get("AGB200_EXPERIMENTAL", "0") == "1":      # the two decode kernel families AUTO never selects (DESIGN.md 3.6)
-    NVCC_FLAGS.append("-DAGB200_EXPERIMENTAL_KERNELS")
 # translation units of the library (compiled in parallel, then linked)
 UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu"]
 

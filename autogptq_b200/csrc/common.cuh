@@ -18,58 +18,23 @@ inline int current_device_index() {
 }
 
 // ---------------------------------------------------------------- memory
-// Weights are read exactly once per forward: stream them past L1.
-__device__ __forceinline__ uint4 ldg_stream_v4(const void* p) {
-  uint4 r;
-  asm volatile("ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];"
-               : "=r"(r.x), "=r"(r.y), "=r"(r.z), "=r"(r.w)
-               : "l"(p));
-  return r;
-}
-// Predicated forms: the destination keeps its old value when !pred.  Written as one asm block so the compiler
+// Predicated loads: the destination keeps its old value when !pred.  Written as one asm block so the compiler
 // sees a plain read-modify-write of the destination registers (no control flow, no phi copies that would
-// put a scoreboard wait right behind the load).
+// put a scoreboard wait right behind the load).  Weights are read exactly once per forward: the stream form
+// keeps them out of L1.
 __device__ __forceinline__ void ldg_stream_v4_pred(uint4& r, const void* p, bool pred) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %5, 0;\n\t"
                "@q ld.global.nc.L1::no_allocate.v4.u32 {%0,%1,%2,%3}, [%4];\n\t}"
                : "+r"(r.x), "+r"(r.y), "+r"(r.z), "+r"(r.w)
                : "l"(p), "r"(static_cast<uint32_t>(pred)));
 }
-__device__ __forceinline__ void ldg_stream_u32_pred(uint32_t& r, const void* p, bool pred) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.global.nc.L1::no_allocate.u32 %0, [%1];\n\t}"
-               : "+r"(r) : "l"(p), "r"(static_cast<uint32_t>(pred)));
-}
 __device__ __forceinline__ void ldg_nc_u32_pred(uint32_t& r, const void* p, bool pred) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.global.nc.u32 %0, [%1];\n\t}"
                : "+r"(r) : "l"(p), "r"(static_cast<uint32_t>(pred)));
 }
-__device__ __forceinline__ void ldg_nc_u16_pred(uint16_t& r, const void* p, bool pred) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.global.nc.u16 %0, [%1];\n\t}"
-               : "+h"(r) : "l"(p), "r"(static_cast<uint32_t>(pred)));
-}
 __device__ __forceinline__ void ldg_nc_v2_pred(uint2& r, const void* p, bool pred) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %3, 0;\n\t@q ld.global.nc.v2.u32 {%0,%1}, [%2];\n\t}"
                : "+r"(r.x), "+r"(r.y) : "l"(p), "r"(static_cast<uint32_t>(pred)));
-}
-__device__ __forceinline__ uint32_t ldg_stream_u32(const void* p) {
-  uint32_t r;
-  asm volatile("ld.global.nc.L1::no_allocate.u32 %0, [%1];" : "=r"(r) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ uint2 ldg_nc_v2(const void* p) {
-  uint2 r;
-  asm volatile("ld.global.nc.v2.u32 {%0,%1}, [%2];" : "=r"(r.x), "=r"(r.y) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ uint32_t ldg_nc_u32(const void* p) {
-  uint32_t r;
-  asm volatile("ld.global.nc.u32 %0, [%1];" : "=r"(r) : "l"(p));
-  return r;
-}
-__device__ __forceinline__ uint16_t ldg_nc_u16(const void* p) {
-  uint16_t r;
-  asm volatile("ld.global.nc.u16 %0, [%1];" : "=h"(r) : "l"(p));
-  return r;
 }
 
 // ---------------------------------------------------------------- programmatic dependent launch

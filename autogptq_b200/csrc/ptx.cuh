@@ -52,7 +52,6 @@ __device__ __forceinline__ bool mbar_test_wait(uint32_t bar, uint32_t parity) {
   return done != 0;
 }
 __device__ __forceinline__ void fence_mbar_init() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
-__device__ __forceinline__ void fence_proxy_async() { asm volatile("fence.proxy.async.shared::cta;" ::: "memory"); }
 
 __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
