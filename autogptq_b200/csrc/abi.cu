@@ -13,6 +13,7 @@
 #include "internal.h"
 #include "aux_kernels.cuh"
 #include "gemm_tcgen05.cuh"   // the wgmma GEMM (file name kept from the first target)
+#include "dgrad.cuh"
 #include "gemv.cuh"
 #include "skinny.cuh"
 #include "decode_imma.cuh"
@@ -698,6 +699,78 @@ int agb200_w4_dequantize(const int32_t* qweight, const int32_t* qzeros, const vo
                                                           static_cast<uint16_t*>(w_out), K / 8, N, group_size);
   AGB_CUDA(cudaGetLastError());
   return 0;
+}
+
+size_t agb200_w4a16_dgrad_workspace_bytes(int M, int K, int) {
+  // the row-sorted dx of an act-order layer on the tensor-core path
+  return (static_cast<size_t>(M) * K * 2 + 255) / 256 * 256;
+}
+
+int agb200_w4a16_dgrad_ex(const void* dy, const int32_t* qweight, const int32_t* qzeros, const void* scales, const int32_t* perm,
+                          void* dx, int M, int K, int N, int group_size, int dtype, void* workspace, size_t workspace_bytes,
+                          void* stream_, int kernel, int tile_m, int split_k) {
+  if (int rc = check_common(dy, qweight, qzeros, scales, dx, M, K, N, group_size, dtype)) return rc;
+  if (dy == dx) return fail(AGB200_EINVAL, "dgrad: dy and dx must not alias");
+  if (M == 0) return 0;
+  DeviceInfo di;
+  if (int rc = get_device_info(di)) return rc;
+  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
+  const bool bf16 = dtype == AGB200_BF16;
+  const bool tc_ok = agb::dgrad_tc_supported(K, N, group_size);
+  if (kernel == AGB200_DGRAD_AUTO) kernel = tc_ok ? AGB200_DGRAD_WGMMA : AGB200_DGRAD_CUDA_CORE;
+  if (kernel == AGB200_DGRAD_CUDA_CORE) {
+    dim3 grid((K + 127) / 128, M < 65535 ? M : 65535);
+    if (bf16)
+      agb::w4a16_dgrad_simt_kernel<true><<<grid, 128, 0, stream>>>(
+          static_cast<const uint16_t*>(dy), reinterpret_cast<const uint32_t*>(qweight), reinterpret_cast<const uint32_t*>(qzeros),
+          static_cast<const uint16_t*>(scales), perm, static_cast<uint16_t*>(dx), M, K, N, group_size);
+    else
+      agb::w4a16_dgrad_simt_kernel<false><<<grid, 128, 0, stream>>>(
+          static_cast<const uint16_t*>(dy), reinterpret_cast<const uint32_t*>(qweight), reinterpret_cast<const uint32_t*>(qzeros),
+          static_cast<const uint16_t*>(scales), perm, static_cast<uint16_t*>(dx), M, K, N, group_size);
+    AGB_CUDA(cudaGetLastError());
+    return 0;
+  }
+  if (kernel != AGB200_DGRAD_WGMMA) return fail(AGB200_EINVAL, "dgrad: unknown kernel selector %d", kernel);
+  if (!tc_ok)
+    return fail(AGB200_ENOSUP, "dgrad: the tensor-core path needs N %% 32 == 0 and group_size >= 32 with group_size %% 16 == 0 "
+                               "(or one group); got K=%d N=%d group_size=%d", K, N, group_size);
+  void* out = dx;
+  if (perm != nullptr) {
+    const size_t need = static_cast<size_t>(M) * K * 2;
+    if (workspace == nullptr || workspace_bytes < need)
+      return fail(AGB200_EWORKSPACE, "dgrad: act-order needs a %zu-byte workspace for the row-sorted dx (got %zu)", need, workspace_bytes);
+    if (!aligned16(workspace)) return fail(AGB200_EINVAL, "dgrad: workspace must be 16-byte aligned");
+    out = workspace;
+  }
+  agb::DgradArgs a{};
+  a.dy = dy; a.qweight = qweight; a.qzeros = qzeros; a.scales = scales; a.dx = out;
+  a.M = M; a.K = K; a.N = N; a.group_size = group_size; a.bf16 = bf16;
+  a.tile_m = tile_m; a.split_k = split_k; a.sms = di.sms;
+  char msg[400] = "";
+  if (int rc = agb::launch_w4a16_dgrad(a, stream, msg, sizeof(msg))) return fail(rc, "%s", msg);
+  if (perm != nullptr) {
+    const size_t smem = static_cast<size_t>(K) * 2;
+    if (smem > static_cast<size_t>(di.smem_optin))
+      return fail(AGB200_ENOSUP, "dgrad: act-order row of K=%d does not fit in shared memory", K);
+    static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
+    const int attr_dev = agb::current_device_index();
+    if (!attr_set_dev[attr_dev]) {
+      AGB_CUDA(cudaFuncSetAttribute(agb::unpermute_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, di.smem_optin));
+      attr_set_dev[attr_dev] = true;
+    }
+    const int grid = M < 8 * di.sms ? M : 8 * di.sms;
+    agb::unpermute_columns_kernel<<<grid, 256, smem, stream>>>(static_cast<const uint16_t*>(out), perm, static_cast<uint16_t*>(dx), M, K);
+    AGB_CUDA(cudaGetLastError());
+  }
+  return 0;
+}
+
+int agb200_w4a16_dgrad(const void* dy, const int32_t* qweight, const int32_t* qzeros, const void* scales, const int32_t* perm,
+                       void* dx, int M, int K, int N, int group_size, int dtype, void* workspace, size_t workspace_bytes,
+                       void* stream) {
+  return agb200_w4a16_dgrad_ex(dy, qweight, qzeros, scales, perm, dx, M, K, N, group_size, dtype, workspace, workspace_bytes,
+                               stream, AGB200_DGRAD_AUTO, 0, 0);
 }
 
 int agb200_permute_columns(const void* x, const int32_t* perm, void* x_out, int M, int K, int dtype, void* stream) {

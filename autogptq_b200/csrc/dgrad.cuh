@@ -1,0 +1,404 @@
+// W4A16 input gradient on the Hopper warpgroup tensor cores (sm_90a): dx[M,K] = dy[M,N] * dequant(W)[K,N]^T, issued as
+// D[k, m] = sum_n W[k, n] * dy[m, n].  Compared with the forward GEMM (gemm_tcgen05.cuh) the reduction now runs over N,
+// the contiguous axis of qweight, and the output over K, the packed axis; the zero point and scale vary along the
+// reduction.  A = dequantised W straight from the checkpoint layout, expanded in REGISTERS: each consumer thread owns two
+// k rows (nibble g of two adjacent word rows) and gathers the adjacent-n pairs of the wgmma A fragment from two adjacent
+// words with one 8-byte shared-memory load and one byte permute, so no dgrad-specific copy of the weights exists.
+// B = dy tile [kMT rows x 64 n] by TMA, K-major SWIZZLE_128B (the forward's x-tile layout); D = fp32 registers.
+// 384 threads: warpgroup 0 = producers (dy after griddepcontrol.wait; packed words, scales, zeros at once), warpgroups
+// 1, 2 = consumers of k rows 0..63 / 64..127 of the CTA's tile.  Split over N: thread-block cluster, DSMEM reduction in
+// rank order (no atomics: repeated calls are bit-identical).
+#pragma once
+#include <cooperative_groups.h>
+#include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched through the runtime)
+
+#include <cstdio>
+#include <type_traits>
+
+#include "common.cuh"
+#include "gemm_common.cuh"
+#include "ptx.cuh"
+#include "tmap.cuh"
+
+namespace agb {
+namespace cg = cooperative_groups;
+
+constexpr int kDgBK = 128;      // k (dx columns) per CTA: two consumer warpgroups x 64 wgmma rows
+constexpr int kDgBN = 64;       // n per pipeline stage: one 128-byte swizzle row of 16-bit dy
+constexpr int kDgGroups = 5;    // quantisation groups a 128-row tile can touch when group_size >= 32
+constexpr int kDgLd = kDgBK + 4;
+
+// The tensor-core path needs whole 16-row blocks per group (a thread's two rows r, r + 8 then share one group), at
+// most kDgGroups groups per tile, and 16-byte TMA rows of qzeros.
+__host__ __device__ constexpr bool dgrad_tc_supported(int K, int N, int group_size) {
+  return N % 32 == 0 && ((group_size % 16 == 0 && group_size >= 32) || group_size >= K);
+}
+
+template <int kMT>
+struct DgradSmem {
+  static constexpr int kStages = 6;
+  static constexpr int kBStage = kMT * 128;                       // dy [kMT rows][64 n], 16-bit, swizzled
+  static constexpr int kWStage = (kDgBK / 8) * kDgBN * 4;         // packed words [16 word rows][64 n] = 4 KB
+  static constexpr int kSStage = kDgGroups * kDgBN * 2;           // scales [5 groups][64 n] (640 B)
+  static constexpr int kZStage = 256;                             // packed zeros [5 groups][8 words], padded
+  static constexpr int kWOff = kBStage * kStages;
+  static constexpr int kSOff = kWOff + kWStage * kStages;
+  static constexpr int kZOff = kSOff + kSStage * kStages;
+  static constexpr int kRing = kZOff + kZStage * kStages;
+  static constexpr int kStaging = kMT * kDgLd * 4;                // fp32 [kMT][kDgLd], reuses the ring
+  static constexpr int kBarOff = (kRing > kStaging ? kRing : kStaging);
+  static constexpr int kTotal = kBarOff + 256 + 1024;
+};
+
+struct DgradParams {
+  void* dx;            // [M, K] (the row-sorted order of qweight for act-order layers)
+  int M, K, N;
+  int group_size;
+  int num_nb;          // ceil(N / 64)
+  int nb_per_split;
+  int split;
+};
+
+// s * (q - z) of the 16-bit pair b = {magic | q_lo, magic | q_hi}, rounded once (the forward's dequant_pair rule)
+template <bool kBf16>
+__device__ __forceinline__ uint32_t dgrad_sub_mul(uint32_t b, uint32_t s2, uint32_t zc) {
+  uint32_t out;
+  if constexpr (!kBf16) {
+    const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2*>(&b), *reinterpret_cast<const __half2*>(&zc)),
+                              *reinterpret_cast<const __half2*>(&s2));
+    out = *reinterpret_cast<const uint32_t*>(&v);
+  } else {
+    const __nv_bfloat162 v = __hmul2(__hsub2(*reinterpret_cast<const __nv_bfloat162*>(&b), *reinterpret_cast<const __nv_bfloat162*>(&zc)),
+                                     *reinterpret_cast<const __nv_bfloat162*>(&s2));
+    out = *reinterpret_cast<const uint32_t*>(&v);
+  }
+  return out;
+}
+
+template <int kMT, bool kBf16>
+__global__ void __launch_bounds__(kGemmThreads, 1)
+w4a16_dgrad_kernel(const DgradParams p, const __grid_constant__ CUtensorMap tmap_dy, const __grid_constant__ CUtensorMap tmap_w,
+                   const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_z) {
+  using Smem = DgradSmem<kMT>;
+  constexpr int kStages = Smem::kStages;
+
+  extern __shared__ unsigned char smem_dyn[];
+  const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
+  unsigned char* smem_al = smem_dyn + (smem_base - smem_u32(smem_dyn));
+  const uint32_t bar_base = smem_base + Smem::kBarOff;
+  auto full = [&](int s) { return bar_base + 8u * s; };
+  auto empty = [&](int s) { return bar_base + 8u * (kStages + s); };
+
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int wg = warp >> 2;
+  const int k0 = blockIdx.x * kDgBK;
+  const int m0 = blockIdx.y * kMT;
+  const int nb_begin = blockIdx.z * p.nb_per_split;
+  const int nb_end = min(p.num_nb, nb_begin + p.nb_per_split);
+  const int num_it = max(0, nb_end - nb_begin);
+  const int g_lo = k0 / p.group_size;           // first group of the tile: row 0 of the staged scales / zeros
+
+  if (threadIdx.x == 0) {
+    prefetch_tmap(&tmap_dy);
+    prefetch_tmap(&tmap_w);
+    prefetch_tmap(&tmap_s);
+    prefetch_tmap(&tmap_z);
+    for (int s = 0; s < kStages; ++s) {
+      mbar_init(full(s), 2);                                     // dy producer + weight producer
+      mbar_init(empty(s), kGemmConsumers / 32);
+    }
+    fence_mbar_init();
+  }
+  __syncthreads();
+  float* stage_f32 = reinterpret_cast<float*>(smem_al);  // [kMT][kDgLd], reuses the ring
+
+  if (wg == 0) {
+    setmaxnreg_dec<40>();
+    if (warp == 0 && lane == 0) {
+      // ================= dy producer: [kMT rows, 64 n] per stage =================
+      pdl_wait();   // dy comes from the previous kernel in the stream
+      for (int it = 0; it < num_it; ++it) {
+        const int s = it % kStages;
+        mbar_wait(empty(s), ((it / kStages) & 1) ^ 1u);
+        mbar_arrive_expect_tx(full(s), Smem::kBStage);
+        tma_load_2d(smem_base + s * Smem::kBStage, &tmap_dy, (nb_begin + it) * kDgBN, m0, full(s));
+      }
+    } else if (warp == 1 && lane == 0) {
+      // ================= weight producer: packed words of the tile's 128 rows + scale / zero rows of its groups ========
+      constexpr uint32_t bytes = Smem::kWStage + Smem::kSStage + kDgGroups * (kDgBN / 8) * 4;
+      for (int it = 0; it < num_it; ++it) {
+        const int s = it % kStages;
+        mbar_wait(empty(s), ((it / kStages) & 1) ^ 1u);
+        mbar_arrive_expect_tx(full(s), bytes);
+        const int n0 = (nb_begin + it) * kDgBN;
+        tma_load_2d(smem_base + Smem::kWOff + s * Smem::kWStage, &tmap_w, n0, k0 >> 3, full(s));
+        tma_load_2d(smem_base + Smem::kSOff + s * Smem::kSStage, &tmap_s, n0, g_lo, full(s));
+        tma_load_2d(smem_base + Smem::kZOff + s * Smem::kZStage, &tmap_z, n0 >> 3, g_lo, full(s));
+      }
+    }
+  } else {
+    setmaxnreg_inc<232>();
+    // ================= consumers: expand W into A fragments, wgmma against the dy tile =================
+    // thread (warp w, g = lane / 4, t = lane % 4): A rows r0 = 16 w + g and r0 + 8 (k), columns 2t, 2t + 1 and
+    // 2t + 8, 2t + 9 of every 16-n slice.  Rows r0 and r0 + 8 are nibble g of word rows r0 / 8 and r0 / 8 + 1.
+    const int cw = warp - 4;                                   // consumer warp 0..7
+    const int g = lane >> 2, t = lane & 3;
+    const int r0 = (cw >> 2) * 64 + (cw & 3) * 16 + g;        // tile row (second one: r0 + 8, same group)
+    int gi = (k0 + r0) / p.group_size - g_lo;                 // staged group row of both rows
+    if (gi > kDgGroups - 1) gi = kDgGroups - 1;               // rows past K of a single-group layer (never stored)
+    const uint32_t* wsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kWOff) + (r0 >> 3) * kDgBN + 2 * t;
+    const uint16_t* ssm = reinterpret_cast<const uint16_t*>(smem_al + Smem::kSOff) + gi * kDgBN + 2 * t;
+    const uint32_t* zsm = reinterpret_cast<const uint32_t*>(smem_al + Smem::kZOff) + gi * (kDgBN / 8);
+    const uint32_t magic = kBf16 ? 0x43004300u : 0x64006400u;   // bf16(128 + v) / fp16(1024 + v) pairs
+    const int sh = 4 * g;
+
+    float acc[kMT / 2];
+#pragma unroll
+    for (int i = 0; i < kMT / 2; ++i) acc[i] = 0.f;
+    uint32_t a[2][16];
+
+    auto release = [&](int s) {
+      __syncwarp();
+      if (lane == 0) mbar_arrive(empty(s));
+    };
+
+    auto stage = [&](auto kb_tag, int it) {
+      constexpr int kB = decltype(kb_tag)::value;
+      const int s = it % kStages;
+      mbar_wait_spin(full(s), (it / kStages) & 1);
+      const uint32_t* wp = wsm + s * (Smem::kWStage / 4);
+      const uint16_t* sp = ssm + s * (Smem::kSStage / 2);
+      const uint32_t* zp = zsm + s * (Smem::kZStage / 4);
+#pragma unroll
+      for (int jh = 0; jh < 8; ++jh) {        // columns 8 jh + 2t, +1: k16 slice jh / 2, half jh % 2
+        // scale pair and zero pair of the two columns (zero nibbles 2t, 2t + 1 of word jh, wrapped (z + 1) & 0xF)
+        const uint32_t s2 = *reinterpret_cast<const uint32_t*>(sp + 8 * jh);
+        const uint32_t v = zp[jh] >> (8 * t);
+        const uint32_t zc = lop3_and_or(((v & 0xFu) | ((v & 0xF0u) << 12)) + 0x00010001u, 0x000F000Fu, magic);
+        const uint2 wa = *reinterpret_cast<const uint2*>(wp + 8 * jh);            // row r0: words of columns n, n + 1
+        const uint2 wb = *reinterpret_cast<const uint2*>(wp + kDgBN + 8 * jh);    // row r0 + 8
+        const uint32_t ba = lop3_and_or(__byte_perm(wa.x >> sh, wa.y >> sh, 0x5410), 0x000F000Fu, magic);
+        const uint32_t bb = lop3_and_or(__byte_perm(wb.x >> sh, wb.y >> sh, 0x5410), 0x000F000Fu, magic);
+        a[kB][4 * (jh >> 1) + 2 * (jh & 1) + 0] = dgrad_sub_mul<kBf16>(ba, s2, zc);
+        a[kB][4 * (jh >> 1) + 2 * (jh & 1) + 1] = dgrad_sub_mul<kBf16>(bb, s2, zc);
+      }
+      const uint64_t bdesc = make_b_desc(smem_base + s * Smem::kBStage);
+      wgmma_fence_operands(acc);
+      wgmma_fence();
+#pragma unroll
+      for (int j = 0; j < 4; ++j) wgmma_tile<kMT, kBf16>(acc, &a[kB][4 * j], bdesc + 2u * j);
+      wgmma_commit();
+      wgmma_wait<1>();
+      wgmma_fence_operands(acc);
+      if (it >= 1) release((it - 1) % kStages);
+    };
+    int it = 0;
+    for (; it + 1 < num_it; it += 2) {
+      stage(std::integral_constant<int, 0>{}, it);
+      stage(std::integral_constant<int, 1>{}, it + 1);
+    }
+    if (it < num_it) stage(std::integral_constant<int, 0>{}, it);
+    wgmma_wait<0>();
+    wgmma_fence_operands(acc);
+    if (num_it > 0) release((num_it - 1) % kStages);
+
+    // epilogue: d[4i + 2h + e] = (A row r0 + 8 h, dy row 8 i + 2 t + e) -> fp32 staging [m][k]
+    consumer_sync();  // both warpgroups are done with the ring
+    const int c0 = r0;
+#pragma unroll
+    for (int i = 0; i < kMT / 8; ++i)
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+#pragma unroll
+        for (int e = 0; e < 2; ++e) stage_f32[(8 * i + 2 * t + e) * kDgLd + c0 + 8 * h] = acc[4 * i + 2 * h + e];
+    if (p.split == 1) {
+      consumer_sync();
+      uint16_t* dx = reinterpret_cast<uint16_t*>(p.dx);
+      for (int e = threadIdx.x - 128; e < kMT * kDgBK; e += kGemmConsumers) {
+        const int ml = e / kDgBK, kl = e % kDgBK;
+        const int m = m0 + ml, k = k0 + kl;
+        if (m < p.M && k < p.K) dx[static_cast<size_t>(m) * p.K + k] = float_to_elt<kBf16>(stage_f32[ml * kDgLd + kl]);
+      }
+    }
+  }
+
+  if (p.split > 1) {
+    // cluster (1,1,split): every CTA holds an fp32 partial tile [kMT][128]; rank r reduces a slice of dy rows, adding
+    // the partials in rank order
+    cg::cluster_group cluster = cg::this_cluster();
+    cluster.sync();
+    if (wg > 0) {
+      const int rank = static_cast<int>(cluster.block_rank());
+      const int rows_per_rank = (kMT + p.split - 1) / p.split;
+      uint16_t* dx = reinterpret_cast<uint16_t*>(p.dx);
+      for (int e = threadIdx.x - 128; e < rows_per_rank * kDgBK; e += kGemmConsumers) {
+        const int ml = rank * rows_per_rank + e / kDgBK;
+        const int kl = e % kDgBK;
+        if (ml < kMT) {
+          float rv[8];
+#pragma unroll
+          for (int r = 0; r < 8; ++r) rv[r] = (r < p.split) ? *cluster.map_shared_rank(&stage_f32[ml * kDgLd + kl], r) : 0.f;
+          float v = 0.f;
+#pragma unroll
+          for (int r = 0; r < 8; ++r) v += rv[r];
+          const int m = m0 + ml, k = k0 + kl;
+          if (m < p.M && k < p.K) dx[static_cast<size_t>(m) * p.K + k] = float_to_elt<kBf16>(v);
+        }
+      }
+    }
+    cluster.sync();
+  }
+}
+
+// CUDA-core form for the layers the tensor-core path does not take (group sizes below 32 or not a multiple of 16,
+// N % 32 != 0): one thread per dx element, the same weight rounding, fp32 accumulation in order of n.  Writes the
+// original column order directly (perm[k] for act-order layers).
+template <bool kBf16>
+__global__ void w4a16_dgrad_simt_kernel(const uint16_t* __restrict__ dy, const uint32_t* __restrict__ qweight,
+                                        const uint32_t* __restrict__ qzeros, const uint16_t* __restrict__ scales,
+                                        const int32_t* __restrict__ perm, uint16_t* __restrict__ dx, int M, int K, int N,
+                                        int group_size) {
+  const int k = blockIdx.x * blockDim.x + threadIdx.x;
+  if (k >= K) return;
+  const int grp = k / group_size;
+  const uint32_t* wrow = qweight + static_cast<size_t>(k >> 3) * N;
+  const uint32_t* zrow = qzeros + static_cast<size_t>(grp) * (N >> 3);
+  const uint16_t* srow = scales + static_cast<size_t>(grp) * N;
+  const int sh = 4 * (k & 7);
+  const int col = perm != nullptr ? perm[k] : k;
+  for (int m = blockIdx.y; m < M; m += gridDim.y) {
+    const uint16_t* dyr = dy + static_cast<size_t>(m) * N;
+    float acc = 0.f;
+    for (int n = 0; n < N; ++n) {
+      const int q = static_cast<int>((wrow[n] >> sh) & 0xFu);
+      const int z = zero_from_nibble((zrow[n >> 3] >> (4 * (n & 7))) & 0xFu);
+      const float w = elt_to_float<kBf16>(float_to_elt<kBf16>(elt_to_float<kBf16>(srow[n]) * static_cast<float>(q - z)));
+      acc = fmaf(elt_to_float<kBf16>(dyr[n]), w, acc);
+    }
+    dx[static_cast<size_t>(m) * K + col] = float_to_elt<kBf16>(acc);
+  }
+}
+
+// out[m, perm[j]] = in[m, j]: one CTA per row at a time through shared memory, so that both the read of the sorted row
+// and the write of the original-order row are coalesced (no inverse permutation needed)
+__global__ void unpermute_columns_kernel(const uint16_t* __restrict__ in, const int32_t* __restrict__ perm,
+                                         uint16_t* __restrict__ out, int M, int K) {
+  extern __shared__ uint16_t row_buf[];
+  for (int m = blockIdx.x; m < M; m += gridDim.x) {
+    const uint16_t* src = in + static_cast<size_t>(m) * K;
+    for (int j = threadIdx.x; j < K; j += blockDim.x) row_buf[perm[j]] = src[j];
+    __syncthreads();
+    uint16_t* dst = out + static_cast<size_t>(m) * K;
+    for (int c = threadIdx.x; c < K; c += blockDim.x) dst[c] = row_buf[c];
+    __syncthreads();
+  }
+}
+
+// -------------------------------------------------------------------------------------------- host side
+struct DgradArgs {
+  const void* dy; const int32_t* qweight; const int32_t* qzeros; const void* scales; void* dx;
+  int M, K, N, group_size; bool bf16; int tile_m, split_k, sms;
+};
+
+template <int kMT, bool kBf16>
+int launch_dgrad_inst(const DgradParams& p, const CUtensorMap& tmap_dy, const CUtensorMap& tmap_w, const CUtensorMap& tmap_s,
+                      const CUtensorMap& tmap_z, int k_tiles, int m_tiles, cudaStream_t stream, char* msg, size_t msg_n) {
+  auto kern = w4a16_dgrad_kernel<kMT, kBf16>;
+  constexpr int smem = DgradSmem<kMT>::kTotal;
+  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
+  const int attr_dev = current_device_index();
+  if (!attr_set_dev[attr_dev]) {
+    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
+    if (e != cudaSuccess) { snprintf(msg, msg_n, "dgrad: cudaFuncSetAttribute(%d B): %s", smem, cudaGetErrorString(e)); return -2; }
+    attr_set_dev[attr_dev] = true;
+  }
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(k_tiles, m_tiles, p.split);
+  cfg.blockDim = dim3(kGemmThreads, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attrs[2];
+  int na = 0;
+  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attrs[na].val.programmaticStreamSerializationAllowed = 1;
+  ++na;
+  if (p.split > 1) {
+    attrs[na].id = cudaLaunchAttributeClusterDimension;
+    attrs[na].val.clusterDim.x = 1;
+    attrs[na].val.clusterDim.y = 1;
+    attrs[na].val.clusterDim.z = p.split;
+    ++na;
+  }
+  cfg.attrs = attrs;
+  cfg.numAttrs = na;
+  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p, tmap_dy, tmap_w, tmap_s, tmap_z);
+  if (e != cudaSuccess) { snprintf(msg, msg_n, "dgrad launch (MT=%d split=%d): %s", kMT, p.split, cudaGetErrorString(e)); return -2; }
+  return 0;
+}
+
+// dx (row-sorted order for act-order layers) = dy * W^T on the tensor cores; the caller has checked dgrad_tc_supported
+inline int launch_w4a16_dgrad(const DgradArgs& a, cudaStream_t stream, char* msg, size_t msg_n) {
+  const int k_tiles = (a.K + kDgBK - 1) / kDgBK;
+  int mt = a.tile_m;
+  if (mt == 0) mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
+  if (mt != 32 && mt != 64 && mt != 128) { snprintf(msg, msg_n, "dgrad: dy-row tile must be 32/64/128 (got %d)", mt); return -1; }
+  const int m_tiles = (a.M + mt - 1) / mt;
+  if (m_tiles > 65535) { snprintf(msg, msg_n, "dgrad: M=%d needs more than 65535 row tiles of %d", a.M, mt); return -1; }
+  DgradParams p{};
+  p.dx = a.dx; p.M = a.M; p.K = a.K; p.N = a.N; p.group_size = a.group_size;
+  p.num_nb = (a.N + kDgBN - 1) / kDgBN;
+  int split = a.split_k;
+  if (split == 0) split = gemm_auto_split(mt, k_tiles * m_tiles, p.num_nb, a.sms);
+  if (split != 1 && split != 2 && split != 4 && split != 8) { snprintf(msg, msg_n, "dgrad: split must be 1/2/4/8 (got %d)", split); return -1; }
+  while (split > 1 && split > p.num_nb) split /= 2;
+  p.split = split;
+  p.nb_per_split = (p.num_nb + split - 1) / split;
+
+  EncodeTiledFn encode = get_encode_fn();
+  if (encode == nullptr) { snprintf(msg, msg_n, "dgrad: cuTensorMapEncodeTiled entry point not available"); return -2; }
+  if (cudaError_t e = ensure_context()) { snprintf(msg, msg_n, "dgrad: no CUDA context: %s", cudaGetErrorString(e)); return -2; }
+  const CUtensorMapDataType t16 = a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const cuuint32_t one[2] = {1, 1};
+  const int G = (a.K + a.group_size - 1) / a.group_size;
+  CUtensorMap tmap_dy, tmap_w, tmap_s, tmap_z;
+  const cuuint64_t ddim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.M)};
+  const cuuint64_t dstride[1] = {static_cast<cuuint64_t>(a.N) * 2};
+  const cuuint32_t dbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(mt)};
+  const cuuint64_t wdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.K / 8)};
+  const cuuint64_t wstride[1] = {static_cast<cuuint64_t>(a.N) * 4};
+  const cuuint32_t wbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(kDgBK / 8)};
+  const cuuint64_t sdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(G)};
+  const cuuint64_t sstride[1] = {static_cast<cuuint64_t>(a.N) * 2};
+  const cuuint32_t sbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(kDgGroups)};
+  const cuuint64_t zdim[2] = {static_cast<cuuint64_t>(a.N / 8), static_cast<cuuint64_t>(G)};
+  const cuuint64_t zstride[1] = {static_cast<cuuint64_t>(a.N / 8) * 4};
+  const cuuint32_t zbox[2] = {static_cast<cuuint32_t>(kDgBN / 8), static_cast<cuuint32_t>(kDgGroups)};
+  const CUresult r0 = encode(&tmap_dy, t16, 2, const_cast<void*>(a.dy), ddim, dstride, dbox, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r1 = encode(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qweight), wdim, wstride, wbox, one,
+                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r2 = encode(&tmap_s, t16, 2, const_cast<void*>(a.scales), sdim, sstride, sbox, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  const CUresult r3 = encode(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qzeros), zdim, zstride, zbox, one,
+                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+  if (r0 != CUDA_SUCCESS || r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS || r3 != CUDA_SUCCESS) {
+    snprintf(msg, msg_n, "dgrad: cuTensorMapEncodeTiled failed (dy %d, qweight %d, scales %d, qzeros %d)", static_cast<int>(r0),
+             static_cast<int>(r1), static_cast<int>(r2), static_cast<int>(r3));
+    return -2;
+  }
+#define AGB_DGRAD_CASE(MT)                                                                                         \
+  case MT:                                                                                                         \
+    return a.bf16 ? launch_dgrad_inst<MT, true>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream, msg, msg_n) \
+                  : launch_dgrad_inst<MT, false>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream, msg, msg_n);
+  switch (mt) {
+    AGB_DGRAD_CASE(32)
+    AGB_DGRAD_CASE(64)
+    AGB_DGRAD_CASE(128)
+  }
+#undef AGB_DGRAD_CASE
+  return -1;
+}
+
+}  // namespace agb

@@ -16,6 +16,18 @@ constexpr int kGemmBK = 64;       // k per pipeline stage   (one 128-byte swizzl
 constexpr int kGemmLd = kGemmBN + 4;   // fp32 staging row pitch: conflict-free fragment stores
 __host__ __device__ constexpr int gemm_stages(int mt) { return mt == 256 ? 5 : 6; }
 
+// Reduction split over a thread-block cluster (DSMEM reduction) for `tiles` output tiles of `mt` rows and `num_kb`
+// 64-wide reduction stages: small tiles split while the grid is under one wave, 128-row tiles only while the doubled
+// grid still fits one wave; every split keeps >= 4 stages per CTA.  Shared by the forward GEMM and the dgrad kernel.
+inline int gemm_auto_split(int mt, int tiles, int num_kb, int sms) {
+  int split = 1;
+  if (mt <= 64)
+    while (split < 8 && tiles * split < sms && num_kb / (split * 2) >= 4) split *= 2;
+  else if (mt == 128)
+    while (split < 4 && tiles * split * 2 <= sms && num_kb / (split * 2) >= 4) split *= 2;
+  return split;
+}
+
 // K-major SWIZZLE_128B shared-memory matrix descriptor (wgmma): start>>4 [0,14) | LBO>>4 [16,30) (unused for swizzled
 // K-major, 1) | SBO>>4 [32,46) = 1024 B between 8-row groups | layout [62,64) = 1 (128B swizzle)
 __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {

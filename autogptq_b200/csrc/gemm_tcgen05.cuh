@@ -331,15 +331,7 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
   p.debug = (a.split_k >> 12) & 3;
   int split = a.split_k & 0xff;
   const int mcast_req = (a.split_k >> 8) & 3;          // tests: 1 = force off, 2 = force on
-  if (split == 0) {
-    split = 1;
-    // split-K reduces fp32 tiles through DSMEM: only worth it for small tiles
-    if (mt <= 64)
-      while (split < 8 && n_tiles * m_tiles * split < a.sms && p.num_kb / (split * 2) >= 4) split *= 2;
-    // 128-row tiles: only while the doubled grid still fits one wave
-    else if (mt == 128)
-      while (split < 4 && n_tiles * m_tiles * split * 2 <= a.sms && p.num_kb / (split * 2) >= 4) split *= 2;
-  }
+  if (split == 0) split = gemm_auto_split(mt, n_tiles * m_tiles, p.num_kb, a.sms);
   if (split != 1 && split != 2 && split != 4 && split != 8) { snprintf(msg, msg_n, "gemm: split-K must be 1/2/4/8 (got %d)", split); return -1; }
   while (split > 1 && split > p.num_kb) split /= 2;
   p.split = split;
@@ -353,6 +345,7 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
 
   EncodeTiledFn encode = get_encode_fn();
   if (encode == nullptr) { snprintf(msg, msg_n, "gemm: cuTensorMapEncodeTiled entry point not available"); return -2; }
+  if (cudaError_t e = ensure_context()) { snprintf(msg, msg_n, "gemm: no CUDA context: %s", cudaGetErrorString(e)); return -2; }
   CUtensorMap tmap;
   const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(a.K), static_cast<cuuint64_t>(a.M)};
   const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(a.K) * 2};

@@ -21,4 +21,23 @@ inline EncodeTiledFn get_encode_fn() {
   return fn;
 }
 
+// cuTensorMapEncodeTiled needs a current context.  A host thread whose first CUDA work is an encode (autograd's
+// backward worker thread, a checkpoint recomputation) has none yet: bind the current device's primary context there.
+inline cudaError_t ensure_context() {
+  using CtxGetFn = CUresult (*)(CUcontext*);
+  static CtxGetFn get = nullptr;
+  if (get == nullptr) {
+    void* p = nullptr;
+    cudaDriverEntryPointQueryResult qres;
+    if (cudaGetDriverEntryPoint("cuCtxGetCurrent", &p, cudaEnableDefault, &qres) == cudaSuccess &&
+        qres == cudaDriverEntryPointSuccess)
+      get = reinterpret_cast<CtxGetFn>(p);
+  }
+  CUcontext ctx = nullptr;
+  if (get != nullptr && get(&ctx) == CUDA_SUCCESS && ctx != nullptr) return cudaSuccess;
+  int dev = 0;
+  cudaError_t e = cudaGetDevice(&dev);
+  return e != cudaSuccess ? e : cudaSetDevice(dev);
+}
+
 }  // namespace agb

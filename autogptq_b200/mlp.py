@@ -83,10 +83,17 @@ def forward_gate_up(gate_proj, up_proj, x: torch.Tensor, *, kernel: int = _lib.G
     run at M > 8, activations other than fp16 / bf16) run the unfused expression instead, and so do batches of more
     than ``FUSED_MAX_M`` rows, where the unfused layers measured faster.  ``kernel`` / ``tile_m`` /
     ``split_k`` force a kernel and its tuning (``agb200_w4a16_gate_up_ex``; tests and benchmarks): a forced call never
-    falls back and raises what the library reports."""
+    falls back and raises what the library reports.
+
+    When autograd records (grad mode on and ``x.requires_grad``) the unfused expression runs, through the layers'
+    differentiable ``forward()``: output and gradients are then those of the unfused layers (a forced kernel raises)."""
     if x.device.type != "cuda":
         raise RuntimeError("autogptq_b200.forward_gate_up needs a CUDA tensor (no CPU fallback).")
     forced = kernel != _lib.GATE_UP_AUTO or tile_m or split_k
+    if x.requires_grad and torch.is_grad_enabled():
+        if forced:
+            raise NotImplementedError("forward_gate_up: the fused kernels have no backward; x requires grad")
+        return _unfused(gate_proj, up_proj, x)
     why = _fusable(gate_proj, up_proj)
     if not why and x.dtype not in _DTYPE_CODE:
         why = f"activations are {x.dtype}"

@@ -148,6 +148,11 @@ class QuantExperts(nn.Module):
     def forward(self, hidden_states: torch.Tensor, top_k_index: torch.Tensor, top_k_weights: torch.Tensor) -> torch.Tensor:
         if hidden_states.device.type != "cuda":
             raise RuntimeError("autogptq_b200.QuantExperts.forward needs CUDA tensors (there is no CPU fallback).")
+        if torch.is_grad_enabled() and (hidden_states.requires_grad or top_k_weights.requires_grad):
+            raise NotImplementedError(
+                "QuantExperts is inference-only: the grouped expert kernels have no backward, so hidden_states and "
+                "top_k_weights must not require grad (run it under torch.no_grad(), or use the experts' QuantLinear "
+                "layers one by one, which do propagate input gradients).")
         device = hidden_states.device
         if top_k_index.device != device or top_k_weights.device != device:
             raise RuntimeError("hidden_states, top_k_index and top_k_weights must be on the same CUDA device")

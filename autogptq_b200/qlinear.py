@@ -16,6 +16,7 @@ from logging import getLogger
 import numpy as np
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 
@@ -69,7 +70,9 @@ class QuantLinear(nn.Module):
             raise ValueError(f"The H100 kernels only support bits=4 (GPTQ W4A16); requested bits={bits}.")
         if trainable:
             # reference: qlinear_exllamav2.py:119-120
-            raise NotImplementedError("The H100 QuantLinear is inference-only (trainable=True is not supported).")
+            raise NotImplementedError(
+                "trainable=True is not supported by the H100 QuantLinear; it is not needed for adapter training: input "
+                "gradients flow through forward() whenever x requires grad (the 4-bit weights stay frozen).")
         if infeatures % 8 != 0 or outfeatures % 8 != 0:
             raise ValueError("infeatures and outfeatures must be multiples of 8 for 4-bit packing.")
         self.infeatures = infeatures
@@ -179,6 +182,13 @@ class QuantLinear(nn.Module):
 
     # ------------------------------------------------------------------ forward
     def forward(self, x: torch.Tensor) -> torch.Tensor:
+        """y = x W (+ bias).  When autograd records (grad mode on and ``x.requires_grad``), y carries a backward that
+        computes dx = dy Wᵀ on the GPU (``agb200_w4a16_dgrad``); the packed weights are frozen and get no gradient."""
+        if x.requires_grad and torch.is_grad_enabled():
+            return _QuantLinearFunction.apply(x, self)
+        return self._forward(x)
+
+    def _forward(self, x: torch.Tensor) -> torch.Tensor:
         if x.device.type != "cuda":
             raise RuntimeError("autogptq_b200.QuantLinear.forward needs a CUDA tensor (no CPU fallback).")
         if not self._ready or self._qweight_run is None or self._qweight_run.device != x.device:
@@ -250,6 +260,48 @@ class QuantLinear(nn.Module):
         y = y.reshape(out_shape)
         return y if x_dtype == cdtype else y.to(x_dtype)
 
+    # ------------------------------------------------------------------ input gradient
+    def input_grad(self, dy: torch.Tensor, *, kernel: int = _lib.DGRAD_AUTO, tile_m: int = 0, split_k: int = 0) -> torch.Tensor:
+        """dx = dy Wᵀ in dy's 16-bit dtype (fp32 dy is computed in fp16, as the forward does), with the dtype-rounded
+        scales the forward uses, in the original column order of x for act-order layers.  ``kernel`` / ``tile_m`` /
+        ``split_k`` force the kernel and its tuning (``agb200_w4a16_dgrad_ex``; tests and benchmarks)."""
+        if dy.device.type != "cuda":
+            raise RuntimeError("autogptq_b200.QuantLinear.input_grad needs a CUDA tensor (no CPU fallback).")
+        if not self._ready or self._qweight_run is None or self._qweight_run.device != dy.device:
+            self.post_init()
+        K, N = self.infeatures, self.outfeatures
+        if dy.shape[-1] != N:
+            raise RuntimeError(f"gradient has {dy.shape[-1]} features, layer has {N} outputs")
+        cdtype = dy.dtype if dy.dtype in _DTYPE_CODE else torch.float16
+        dy2 = dy.reshape(-1, N)
+        if dy2.dtype != cdtype:
+            dy2 = dy2.to(cdtype)
+        if not dy2.is_contiguous() or dy2.data_ptr() % 16:
+            dy2 = dy2.clone(memory_format=torch.contiguous_format)
+        M = dy2.shape[0]
+        dx = torch.empty((M, K), dtype=cdtype, device=dy.device)
+        if M > 0:
+            lib = _lib.load()
+            scales, _ = self._run_tensors(cdtype)
+            ws_ptr, ws_bytes = None, 0
+            if self._perm is not None:
+                ws_bytes = int(lib.agb200_w4a16_dgrad_workspace_bytes(M, K, N))
+                ws_ptr = _workspace(dy.device, ws_bytes).data_ptr()
+            dev_index = dy.device.index
+            cur = _current_device()
+            if cur != dev_index:
+                torch.cuda.set_device(dev_index)
+            try:
+                rc = lib.agb200_w4a16_dgrad_ex(
+                    dy2.data_ptr(), self._qweight_run.data_ptr(), self.qzeros.data_ptr(), scales.data_ptr(),
+                    self._perm.data_ptr() if self._perm is not None else None, dx.data_ptr(), M, K, N, self.group_size,
+                    _DTYPE_CODE[cdtype], ws_ptr, ws_bytes, _raw_stream(dev_index), kernel, tile_m, split_k)
+            finally:
+                if cur != dev_index:
+                    torch.cuda.set_device(cur)
+            _lib.check(rc, "agb200_w4a16_dgrad")
+        return dx.reshape(dy.shape[:-1] + (K,))
+
     # ------------------------------------------------------------------ pack (offline; builds fixtures)
     def pack(self, linear, scales, zeros, g_idx=None):
         """fp weights + per-group ``scales[N, G]`` / ``zeros[N, G]`` -> packed buffers.
@@ -289,6 +341,24 @@ class QuantLinear(nn.Module):
     def extra_repr(self) -> str:
         return (f"in_features={self.infeatures}, out_features={self.outfeatures}, bits=4, "
                 f"group_size={self.group_size}, bias={self.bias is not None}, backend=sm_90a")
+
+
+class _QuantLinearFunction(torch.autograd.Function):
+    """y = QuantLinear._forward(x) with dx = dy Wᵀ as its backward (reference: QuantLinearFunction,
+    auto_gptq/nn_modules/triton_utils/kernels.py:408-426, grad_input only).  Saves no activations: dx needs only the
+    frozen weights."""
+
+    @staticmethod
+    def forward(ctx, x, lin):
+        ctx.lin = lin
+        ctx.x_dtype = x.dtype
+        return lin._forward(x)
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        dx = ctx.lin.input_grad(dy)
+        return (dx if dx.dtype == ctx.x_dtype else dx.to(ctx.x_dtype)), None
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -389,10 +459,14 @@ def forward_group(layers, x: torch.Tensor):
     For decode batches (M <= 8 rows) all of them execute in ONE kernel launch through
     ``agb200_w4a16_forward_group``; the checkpoint tensors stay separate (the reference's fused-QKV
     injection concatenates them instead, ``fused_llama_attn.py:171-207``).  Larger M: plain per-layer calls.
+    When autograd records (grad mode on and ``x.requires_grad``) the layers always run one by one through their
+    differentiable ``forward()``: outputs and gradients are then those of the unfused layers.
     """
     layers = list(layers)
     if not layers:
         return []
+    if x.requires_grad and torch.is_grad_enabled():
+        return [l(x) for l in layers]
     first = layers[0]
     if x.device.type != "cuda":
         raise RuntimeError("autogptq_b200.forward_group needs a CUDA tensor (no CPU fallback).")

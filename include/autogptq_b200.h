@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 9
+#define AGB200_ABI_VERSION 10
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -115,6 +115,44 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
                             int kernel, int tune0, int tune1, int flags);
 
 size_t agb200_w4a16_workspace_bytes(int M, int K, int N);
+
+/*
+ * Input gradient of a 4-bit layer (ABI v10): dx[M,K] = dy[M,N] * dequant(qweight,qzeros,scales)^T, all pointers DEVICE
+ * memory.  The weights are frozen: there is no weight, scale or zero gradient.
+ *
+ * Replaces, for 4-bit layers, the backward of the reference's trainable Triton QuantLinear:
+ *   QuantLinearFunction.backward          auto_gptq/nn_modules/triton_utils/kernels.py:408-426 (grad_input only)
+ *   transpose_quant_matmul_248            auto_gptq/nn_modules/triton_utils/kernels.py:377-405
+ * and the autograd of the pure-PyTorch dequantise + torch.matmul path (qlinear_cuda_old.py:291-355) that training
+ * falls back to when the exllama / exllamav2 / marlin backends refuse trainable mode (modeling/_base.py:860-869).
+ *
+ * Arithmetic: every weight is rounded once to `dtype` as scales * (q - z) (the rule of the wgmma forward), products
+ * accumulate in fp32 and dx is rounded once to `dtype`.  Pass the same `dtype`-rounded scales the forward used: dx is
+ * then the gradient of the function the forward computed.
+ *   dy, dx    [M,N] / [M,K], row-major, dtype `dtype`; dx is caller-allocated and must not alias dy.
+ *   qweight   the matrix the forward runs (for act-order layers the agb200_w4_make_sequential copy), with `perm`:
+ *             dx comes out in the ORIGINAL column order of x (sorted row j is x column perm[j]).
+ *   workspace DEVICE scratch of agb200_w4a16_dgrad_workspace_bytes(M,K,N) bytes, needed by the tensor-core path of
+ *             act-order layers only (the row-sorted dx before the column scatter); may be NULL otherwise.
+ *   stream    cudaStream_t the work is enqueued on (no host synchronisation: forward + backward can be captured in a
+ *             CUDA graph).
+ * Kernels: a wgmma kernel (sm_90a; weights expanded from the checkpoint layout on chip, split over N through a
+ * thread-block cluster) for N % 32 == 0 and group_size >= 32 with group_size % 16 == 0 or one group; a CUDA-core
+ * kernel for every other layer agb200_w4a16_forward accepts.  No atomics: two calls give bit-identical dx.
+ * Constraints: K % 8 == 0, N % 8 == 0, pointers 16-byte aligned.
+ */
+#define AGB200_DGRAD_AUTO 0
+#define AGB200_DGRAD_CUDA_CORE 1   /* one thread per dx element, any layer */
+#define AGB200_DGRAD_WGMMA 2       /* tensor cores; AGB200_ENOSUP for layers it does not take */
+int agb200_w4a16_dgrad(const void* dy, const int32_t* qweight, const int32_t* qzeros, const void* scales,
+                       const int32_t* perm, void* dx, int M, int K, int N, int group_size, int dtype,
+                       void* workspace, size_t workspace_bytes, void* stream);
+/* Same, with an explicit kernel (AGB200_DGRAD_*) and wgmma tuning (tests / benchmarks): tile_m = dy-row tile
+ * (32|64|128, 0 = auto), split_k = splits of the N reduction (1|2|4|8, 0 = auto). */
+int agb200_w4a16_dgrad_ex(const void* dy, const int32_t* qweight, const int32_t* qzeros, const void* scales,
+                          const int32_t* perm, void* dx, int M, int K, int N, int group_size, int dtype,
+                          void* workspace, size_t workspace_bytes, void* stream, int kernel, int tile_m, int split_k);
+size_t agb200_w4a16_dgrad_workspace_bytes(int M, int K, int N);
 
 /*
  * Grouped forward: `n_layers` (<= 4) sibling layers that consume the SAME x (q|k|v, gate|up) in ONE launch, for
