@@ -123,8 +123,8 @@ def forward_gate_up(gate_proj, up_proj, x: torch.Tensor, *, kernel: int = _lib.G
             raise NotImplementedError("forward_gate_up: gate_proj and up_proj have different act-order permutations")
         return _unfused(gate_proj, up_proj, x)
     x2 = x.reshape(-1, K)
-    if not x2.is_contiguous():
-        x2 = x2.contiguous()
+    if not x2.is_contiguous() or x2.data_ptr() % 16:        # the kernels read x in 16-byte words
+        x2 = x2.clone(memory_format=torch.contiguous_format)
     M = x2.shape[0]
     out_shape = x.shape[:-1] + (I,)
     if M == 0:

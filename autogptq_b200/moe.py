@@ -167,6 +167,8 @@ class QuantExperts(nn.Module):
         if T == 0:
             return torch.empty(out_shape, dtype=x_dtype, device=device)
         x = x.to(cdtype).contiguous()
+        if x.data_ptr() % 16:                        # the kernels read x in 16-byte words
+            x = x.clone()
         idx = top_k_index.reshape(T, -1)
         k = idx.shape[1]
         if idx.dtype not in (torch.int32, torch.int64):

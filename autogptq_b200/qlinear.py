@@ -208,8 +208,8 @@ class QuantLinear(nn.Module):
         x2 = x.reshape(-1, K)
         if x2.dtype != cdtype:
             x2 = x2.to(cdtype)
-        if not x2.is_contiguous():
-            x2 = x2.contiguous()
+        if not x2.is_contiguous() or x2.data_ptr() % 16:    # the kernels read x in 16-byte words
+            x2 = x2.clone(memory_format=torch.contiguous_format)
         M = x2.shape[0]
         dev_index = x.device.index
         y = torch.empty((M, N), dtype=cdtype, device=x.device)
@@ -482,8 +482,8 @@ def forward_group(layers, x: torch.Tensor):
     for l in layers:
         if not l._ready or l._qweight_run is None or l._qweight_run.device != x.device:
             l.post_init()
-    if not x2.is_contiguous():
-        x2 = x2.contiguous()
+    if not x2.is_contiguous() or x2.data_ptr() % 16:        # the kernels read x in 16-byte words
+        x2 = x2.clone(memory_format=torch.contiguous_format)
     key = (id(first), len(layers), x2.dtype)
     ga = first.__dict__.setdefault("_group_cache", {}).get(key)
     sig = tuple((id(l), l._qweight_run.data_ptr(), l.qzeros.data_ptr(), l.scales.data_ptr()) for l in layers)
