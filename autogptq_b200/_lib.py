@@ -77,6 +77,12 @@ def _declare(lib):
         "agb200_moe_workspace_bytes": (S, [I, I, I, I, I]),
         "agb200_moe_forward": (I, [P, P, P, I, P, I, I, I, P, P, S, P]),
         "agb200_moe_destroy": (I, [P]),
+        "agb200_moe_saved_bytes": (S, [I, I, I, I, I]),
+        "agb200_moe_forward_saving": (I, [P, P, P, I, P, I, I, I, P, P, S, P, S, P]),
+        "agb200_moe_grad_plan_bytes": (S, [I, I, I, I]),
+        "agb200_moe_grad_attach": (I, [P, P, P, S]),
+        "agb200_moe_backward_workspace_bytes": (S, [I, I, I, I, I]),
+        "agb200_moe_backward": (I, [P, P, P, I, P, I, I, I, P, S, P, P, P, S, P]),
         "agb200_w4a16_gate_up": (I, [P, P, P, P, I, I, I, I, I, P, S, P]),
         "agb200_w4a16_gate_up_ex": (I, [P, P, P, P, I, I, I, I, I, P, S, P, I, I, I]),
         "agb200_w4a16_gate_up_workspace_bytes": (S, [I, I, I]),

@@ -16,39 +16,13 @@
 #include <type_traits>
 
 #include "common.cuh"
+#include "dgrad_common.cuh"
 #include "gemm_common.cuh"
 #include "ptx.cuh"
 #include "tmap.cuh"
 
 namespace agb {
 namespace cg = cooperative_groups;
-
-constexpr int kDgBK = 128;      // k (dx columns) per CTA: two consumer warpgroups x 64 wgmma rows
-constexpr int kDgBN = 64;       // n per pipeline stage: one 128-byte swizzle row of 16-bit dy
-constexpr int kDgGroups = 5;    // quantisation groups a 128-row tile can touch when group_size >= 32
-constexpr int kDgLd = kDgBK + 4;
-
-// The tensor-core path needs whole 16-row blocks per group (a thread's two rows r, r + 8 then share one group), at
-// most kDgGroups groups per tile, and 16-byte TMA rows of qzeros.
-__host__ __device__ constexpr bool dgrad_tc_supported(int K, int N, int group_size) {
-  return N % 32 == 0 && ((group_size % 16 == 0 && group_size >= 32) || group_size >= K);
-}
-
-template <int kMT>
-struct DgradSmem {
-  static constexpr int kStages = 6;
-  static constexpr int kBStage = kMT * 128;                       // dy [kMT rows][64 n], 16-bit, swizzled
-  static constexpr int kWStage = (kDgBK / 8) * kDgBN * 4;         // packed words [16 word rows][64 n] = 4 KB
-  static constexpr int kSStage = kDgGroups * kDgBN * 2;           // scales [5 groups][64 n] (640 B)
-  static constexpr int kZStage = 256;                             // packed zeros [5 groups][8 words], padded
-  static constexpr int kWOff = kBStage * kStages;
-  static constexpr int kSOff = kWOff + kWStage * kStages;
-  static constexpr int kZOff = kSOff + kSStage * kStages;
-  static constexpr int kRing = kZOff + kZStage * kStages;
-  static constexpr int kStaging = kMT * kDgLd * 4;                // fp32 [kMT][kDgLd], reuses the ring
-  static constexpr int kBarOff = (kRing > kStaging ? kRing : kStaging);
-  static constexpr int kTotal = kBarOff + 256 + 1024;
-};
 
 struct DgradParams {
   void* dx;            // [M, K] (the row-sorted order of qweight for act-order layers)
@@ -58,22 +32,6 @@ struct DgradParams {
   int nb_per_split;
   int split;
 };
-
-// s * (q - z) of the 16-bit pair b = {magic | q_lo, magic | q_hi}, rounded once (the forward's dequant_pair rule)
-template <bool kBf16>
-__device__ __forceinline__ uint32_t dgrad_sub_mul(uint32_t b, uint32_t s2, uint32_t zc) {
-  uint32_t out;
-  if constexpr (!kBf16) {
-    const __half2 v = __hmul2(__hsub2(*reinterpret_cast<const __half2*>(&b), *reinterpret_cast<const __half2*>(&zc)),
-                              *reinterpret_cast<const __half2*>(&s2));
-    out = *reinterpret_cast<const uint32_t*>(&v);
-  } else {
-    const __nv_bfloat162 v = __hmul2(__hsub2(*reinterpret_cast<const __nv_bfloat162*>(&b), *reinterpret_cast<const __nv_bfloat162*>(&zc)),
-                                     *reinterpret_cast<const __nv_bfloat162*>(&s2));
-    out = *reinterpret_cast<const uint32_t*>(&v);
-  }
-  return out;
-}
 
 template <int kMT, bool kBf16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
@@ -169,19 +127,7 @@ w4a16_dgrad_kernel(const DgradParams p, const __grid_constant__ CUtensorMap tmap
       const uint32_t* wp = wsm + s * (Smem::kWStage / 4);
       const uint16_t* sp = ssm + s * (Smem::kSStage / 2);
       const uint32_t* zp = zsm + s * (Smem::kZStage / 4);
-#pragma unroll
-      for (int jh = 0; jh < 8; ++jh) {        // columns 8 jh + 2t, +1: k16 slice jh / 2, half jh % 2
-        // scale pair and zero pair of the two columns (zero nibbles 2t, 2t + 1 of word jh, wrapped (z + 1) & 0xF)
-        const uint32_t s2 = *reinterpret_cast<const uint32_t*>(sp + 8 * jh);
-        const uint32_t v = zp[jh] >> (8 * t);
-        const uint32_t zc = lop3_and_or(((v & 0xFu) | ((v & 0xF0u) << 12)) + 0x00010001u, 0x000F000Fu, magic);
-        const uint2 wa = *reinterpret_cast<const uint2*>(wp + 8 * jh);            // row r0: words of columns n, n + 1
-        const uint2 wb = *reinterpret_cast<const uint2*>(wp + kDgBN + 8 * jh);    // row r0 + 8
-        const uint32_t ba = lop3_and_or(__byte_perm(wa.x >> sh, wa.y >> sh, 0x5410), 0x000F000Fu, magic);
-        const uint32_t bb = lop3_and_or(__byte_perm(wb.x >> sh, wb.y >> sh, 0x5410), 0x000F000Fu, magic);
-        a[kB][4 * (jh >> 1) + 2 * (jh & 1) + 0] = dgrad_sub_mul<kBf16>(ba, s2, zc);
-        a[kB][4 * (jh >> 1) + 2 * (jh & 1) + 1] = dgrad_sub_mul<kBf16>(bb, s2, zc);
-      }
+      dgrad_build_a<kBf16>(a[kB], wp, sp, zp, t, sh, magic);
       const uint64_t bdesc = make_b_desc(smem_base + s * Smem::kBStage);
       wgmma_fence_operands(acc);
       wgmma_fence();

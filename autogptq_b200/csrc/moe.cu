@@ -3,6 +3,9 @@
 //   route -> [T <= 8] decode gate/up -> decode down -> combine
 //         -> [T > 8]  gather x -> GEMM gate/up -> GEMM down -> combine
 // all on the caller's stream, without a host synchronisation.  Kernels: moe.cuh.
+// The backward (agb200_moe_backward; kernels: moe_dgrad.cuh) runs
+//   route -> combine backward (dw, dy_pair rows) -> dgrad down (dg | du) -> dgrad gate/up (dx_pair) -> dx combine
+// on the values the saving forward kept, with the tensor maps and inverse permutations of the grad plan.
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -15,6 +18,7 @@
 #include "../../include/autogptq_b200.h"
 #include "internal.h"
 #include "moe.cuh"
+#include "moe_dgrad.cuh"
 #include "tmap.cuh"
 
 namespace {
@@ -52,6 +56,8 @@ struct Moe {
   int up_rps, down_rps, down_split;    // decode path: k8-rows per work item, K splits of the down stage
   size_t up_smem, down_smem;
   int up_occ, down_occ;                // decode path: resident CTAs per SM
+  CUtensorMap* g_maps;                 // grad plan (agb200_moe_grad_attach), or null
+  agb::MoeGradExpertDev* g_ex;
 };
 
 size_t maps_bytes(int E) { return align_up(size_t(E) * 9 * sizeof(CUtensorMap), 256); }
@@ -106,22 +112,22 @@ int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType d
   return 0;
 }
 
-template <bool kBf16, bool kGateUp>
+template <bool kBf16, bool kGateUp, class Src = agb::MoeRouted>
 int decode_setup(size_t smem, int& occ) {
-  auto kern = agb::moe_decode_kernel<kBf16, kGateUp, agb::MoeRouted>;
+  auto kern = agb::moe_decode_kernel<kBf16, kGateUp, Src>;
   MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
   MOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, agb::kMdThreads, smem));
   if (occ < 1) return failf(AGB200_ENOSUP, "moe: decode kernel with %zu B of shared memory does not fit an SM", smem);
   return 0;
 }
 
-template <bool kGateUp>
-int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, const agb::MoeRouted& src, int max_items, cudaStream_t stream) {
+template <bool kGateUp, class Src>
+int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, const Src& src, int max_items, cudaStream_t stream) {
   const size_t smem = kGateUp ? m.up_smem : m.down_smem;
   const int occ = kGateUp ? m.up_occ : m.down_occ;
   const int grid = std::max(1, std::min(max_items, m.sms * occ));
-  if (m.dtype == AGB200_BF16) agb::moe_decode_kernel<true, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
-  else agb::moe_decode_kernel<false, kGateUp><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
+  if (m.dtype == AGB200_BF16) agb::moe_decode_kernel<true, kGateUp, Src><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
+  else agb::moe_decode_kernel<false, kGateUp, Src><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
   MOE_CUDA(cudaGetLastError());
   return 0;
 }
@@ -273,6 +279,10 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
   m->up_rps = up_rps; m->down_rps = down_rps; m->down_split = down_split; m->up_smem = up_smem; m->down_smem = down_smem;
   int rc = dtype == AGB200_BF16 ? decode_setup<true, true>(up_smem, m->up_occ) : decode_setup<false, true>(up_smem, m->up_occ);
   if (rc == 0) rc = dtype == AGB200_BF16 ? decode_setup<true, false>(down_smem, m->down_occ) : decode_setup<false, false>(down_smem, m->down_occ);
+  int save_occ = 0;   // the saving gate/up kernel (agb200_moe_forward_saving) runs with the grid of the plain one
+  if (rc == 0)
+    rc = dtype == AGB200_BF16 ? decode_setup<true, true, agb::MoeRoutedSave>(up_smem, save_occ)
+                              : decode_setup<false, true, agb::MoeRoutedSave>(up_smem, save_occ);
   if (rc != 0) { delete m; return rc; }
 
   auto cleanup_fail = [&](cudaError_t e, const char* what) {
@@ -298,8 +308,20 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
   return 0;
 }
 
-int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
-                       int weights_dtype, int T, int k, void* out, void* workspace, size_t workspace_bytes, void* stream) {
+}  // extern "C"
+
+namespace {
+
+size_t saved_bytes(int T, int k, int H, int I) {
+  const size_t P = size_t(T) * k;
+  return 2 * align_up(P * I * 2, 256) + align_up(P * H * 2, 256);
+}
+
+// agb200_moe_forward, and with `saved` (agb200_moe_forward_saving) also g, u and y_pair of every pair at saved:
+// g [T*k, I] | u [T*k, I] | y_pair [T*k, H], 256-byte aligned parts, pair-id rows
+int moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
+                int weights_dtype, int T, int k, void* out, void* saved, size_t saved_bytes_given, void* workspace,
+                size_t workspace_bytes, void* stream) {
   Moe* m = static_cast<Moe*>(handle);
   if (!m || m->magic != kMagic) return failf(AGB200_EINVAL, "moe: bad handle");
   if (T < 0 || k < 1) return failf(AGB200_EINVAL, "moe: T >= 0 and k >= 1 (got T=%d, k=%d)", T, k);
@@ -317,6 +339,18 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
   const int E = m->E, H = m->H, I = m->I;
   const WsLayout w = ws_layout(T, k, E, H, I);
   if (workspace_bytes < w.total) return failf(AGB200_EWORKSPACE, "moe: workspace needs %zu bytes (got %zu)", w.total, workspace_bytes);
+  uint16_t* sv_g = nullptr;
+  uint16_t* sv_u = nullptr;
+  uint16_t* sv_y = nullptr;
+  if (saved != nullptr) {
+    const size_t need = saved_bytes(T, k, H, I);
+    if (saved_bytes_given < need || (reinterpret_cast<uintptr_t>(saved) & 255u))
+      return failf(AGB200_EWORKSPACE, "moe: saved buffer needs %zu bytes, 256-byte aligned (got %zu)", need, saved_bytes_given);
+    const size_t gu = align_up(size_t(T) * k * I * 2, 256);
+    sv_g = static_cast<uint16_t*>(saved);
+    sv_u = reinterpret_cast<uint16_t*>(static_cast<unsigned char*>(saved) + gu);
+    sv_y = reinterpret_cast<uint16_t*>(static_cast<unsigned char*>(saved) + 2 * gu);
+  }
   const bool decode = T <= agb::kMoeDecodeMaxT;
   if (!decode && !m->has_tc)
     return failf(AGB200_ENOSUP, "moe: T=%d > %d runs the tensor-core GEMM, which needs qweight_tc for every layer", T, agb::kMoeDecodeMaxT);
@@ -339,26 +373,36 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
   const dim3 cgrid(T, (H + 255) / 256, 1);
   agb::MoeRouted src{};
   src.ex = m->d_ex; src.r = r; src.k = k; src.maps = m->d_maps;
+  agb::MoeRoutedSave save_src{};
+  static_cast<agb::MoeRouted&>(save_src) = src;
+  save_src.g = sv_g; save_src.u = sv_u;
   if (decode) {
     float* part = reinterpret_cast<float*>(ws + w.ys);
     agb::MoeDecodeParams p{};
     p.P = P;
     p.x = x; p.out = hs; p.K = H; p.N = I; p.rows = H / 8; p.rows_per_group = m->gs13 / 8;
     p.rows_per_split = m->up_rps; p.split = 1; p.tiles = I / agb::kMdTN;
-    if (int rc = launch_decode<true>(*m, p, src, std::min(E, P) * p.tiles, s)) return rc;
+    if (int rc = saved != nullptr ? launch_decode<true>(*m, p, save_src, std::min(E, P) * p.tiles, s)
+                                  : launch_decode<true>(*m, p, src, std::min(E, P) * p.tiles, s)) return rc;
     p.x = hs; p.out = part; p.K = I; p.N = H; p.rows = I / 8; p.rows_per_group = m->gs2 / 8;
     p.rows_per_split = m->down_rps; p.split = m->down_split; p.tiles = H / agb::kMdTN;
     if (int rc = launch_decode<false>(*m, p, src, std::min(E, P) * p.tiles * p.split, s)) return rc;
-    if (bf) agb::moe_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
-                                                                nullptr, part, m->down_split, m->d_ex, static_cast<uint16_t*>(out));
-    else agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
-                                                              nullptr, part, m->down_split, m->d_ex, static_cast<uint16_t*>(out));
+    const int wf32 = weights_dtype == AGB200_MOE_WEIGHTS_F32;
+    uint16_t* o16 = static_cast<uint16_t*>(out);
+    if (saved != nullptr) {
+      if (bf) agb::moe_combine_kernel<true, true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, wf32, k, E, H, P, nullptr, part, m->down_split, m->d_ex, o16, sv_y);
+      else agb::moe_combine_kernel<false, true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, wf32, k, E, H, P, nullptr, part, m->down_split, m->d_ex, o16, sv_y);
+    } else if (bf) {
+      agb::moe_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, wf32, k, E, H, P, nullptr, part, m->down_split, m->d_ex, o16);
+    } else {
+      agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, wf32, k, E, H, P, nullptr, part, m->down_split, m->d_ex, o16);
+    }
     MOE_CUDA(cudaGetLastError());
     return 0;
   }
 
   uint16_t* xs = reinterpret_cast<uint16_t*>(ws + w.xs);
-  uint16_t* ys = reinterpret_cast<uint16_t*>(ws + w.ys);
+  uint16_t* ys = saved != nullptr ? sv_y : reinterpret_cast<uint16_t*>(ws + w.ys);   // y_pair rows by pair id
   const int m_tiles = (P + mt - 1) / mt + E;
   if (m_tiles > 65535) return failf(AGB200_ENOSUP, "moe: %d row tiles exceed the grid limit", m_tiles);
   agb::moe_gather_x_kernel<<<P, 128, 0, s>>>(static_cast<const uint16_t*>(x), top_k_index, ids64, k, H, E, r, m->d_ex, xs);
@@ -373,7 +417,8 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
   p.split = 1;
   p.out = hs; p.K = H; p.N = I; p.group_size = m->gs13; p.gs_log2 = gs_log2(m->gs13); p.num_kb = (H + agb::kGemmBK - 1) / agb::kGemmBK;
   p.kb_per_split = p.num_kb;
-  if (int rc = launch_gemm<true>(bf, mt, p, tx, src, I / (agb::kGemmBN / 2), m_tiles, s)) return rc;
+  if (int rc = saved != nullptr ? launch_gemm<true>(bf, mt, p, tx, save_src, I / (agb::kGemmBN / 2), m_tiles, s)
+                                : launch_gemm<true>(bf, mt, p, tx, src, I / (agb::kGemmBN / 2), m_tiles, s)) return rc;
   p.out = ys; p.K = I; p.N = H; p.group_size = m->gs2; p.gs_log2 = gs_log2(m->gs2); p.num_kb = (I + agb::kGemmBK - 1) / agb::kGemmBK;
   p.kb_per_split = p.num_kb;
   if (int rc = launch_gemm<false>(bf, mt, p, th, src, H / agb::kGemmBN, m_tiles, s)) return rc;
@@ -381,6 +426,261 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
                                                               ys, nullptr, 0, m->d_ex, static_cast<uint16_t*>(out));
   else agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
                                                             ys, nullptr, 0, m->d_ex, static_cast<uint16_t*>(out));
+  MOE_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int index_dtype, const void* top_k_weights,
+                       int weights_dtype, int T, int k, void* out, void* workspace, size_t workspace_bytes, void* stream) {
+  return moe_forward(handle, x, top_k_index, index_dtype, top_k_weights, weights_dtype, T, k, out, nullptr, 0, workspace,
+                     workspace_bytes, stream);
+}
+
+size_t agb200_moe_saved_bytes(int T, int k, int E, int H, int I) {
+  if (T < 0 || k < 1 || E < 1 || H < 1 || I < 1) return 0;
+  return saved_bytes(T, k, H, I);
+}
+
+int agb200_moe_forward_saving(void* handle, const void* x, const void* top_k_index, int index_dtype,
+                              const void* top_k_weights, int weights_dtype, int T, int k, void* out, void* saved,
+                              size_t saved_bytes, void* workspace, size_t workspace_bytes, void* stream) {
+  if (saved == nullptr && T > 0) return failf(AGB200_EINVAL, "moe: null saved buffer");
+  return moe_forward(handle, x, top_k_index, index_dtype, top_k_weights, weights_dtype, T, k, out, saved, saved_bytes,
+                     workspace, workspace_bytes, stream);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ backward
+namespace {
+
+size_t grad_table_bytes(int E) { return align_up(size_t(E) * sizeof(agb::MoeGradExpertDev), 256); }
+
+// Backward workspace: routing tables | padded row of every pair | dy_pair [rows, H] | dg | du [rows, 2 I] | fp32
+// dx_pair [rows, H], with rows = P + min(E, P) * (MT - 1) >= the padded rows of the routing (MT = the backward's row tile)
+struct BwdLayout {
+  WsLayout w;               // routing part (max_tiles, route offset)
+  int mt, rows;
+  size_t prow, dyp, dgu, dxp, total;
+};
+
+int bwd_tile(int P, int E) {
+  const int avg = (P + std::min(E, P) - 1) / std::min(E, P);
+  return avg <= 32 ? 32 : avg <= 64 ? 64 : 128;
+}
+
+BwdLayout bwd_layout(int T, int k, int E, int H, int I) {
+  BwdLayout b{};
+  const int P = T * k;
+  b.w.P = P;
+  b.w.max_tiles = (P + 31) / 32 + E;
+  b.mt = bwd_tile(P, E);
+  b.rows = P + std::min(E, P) * (b.mt - 1);
+  const size_t ints = size_t(E) * 4 + 4 + 2 * size_t(b.w.max_tiles) + P;
+  b.prow = align_up(ints * 4, 256);
+  b.dyp = b.prow + align_up(size_t(P) * 4, 256);
+  b.dgu = b.dyp + align_up(size_t(b.rows) * H * 2, 256);
+  b.dxp = b.dgu + align_up(size_t(b.rows) * 2 * I * 2, 256);
+  b.total = b.dxp + align_up(size_t(b.rows) * H * 4, 256);
+  return b;
+}
+
+template <int kMT, bool kBf16, bool kDown>
+int launch_moe_dgrad_inst(const agb::MoeDgradParams& p, const CUtensorMap& tb, const agb::MoeRoute& r, const CUtensorMap* maps,
+                          const agb::MoeGradExpertDev* gx, int k_tiles, int m_tiles, cudaStream_t stream) {
+  auto kern = agb::moe_dgrad_kernel<kMT, kBf16, kDown>;
+  constexpr int smem = agb::DgradSmem<kMT>::kTotal;
+  static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
+  const int dev = agb::current_device_index();
+  if (!attr_set_dev[dev]) {
+    MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
+    attr_set_dev[dev] = true;
+  }
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(k_tiles, m_tiles, p.split);
+  cfg.blockDim = dim3(agb::kGemmThreads, 1, 1);
+  cfg.dynamicSmemBytes = smem;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr;
+  attr.id = cudaLaunchAttributeClusterDimension;
+  attr.val.clusterDim.x = 1;
+  attr.val.clusterDim.y = 1;
+  attr.val.clusterDim.z = p.split;
+  cfg.attrs = &attr;
+  cfg.numAttrs = p.split > 1 ? 1 : 0;
+  MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tb, r, maps, gx));
+  return 0;
+}
+
+template <bool kDown>
+int launch_moe_dgrad(const Moe& m, int mt, int P, agb::MoeDgradParams p, const CUtensorMap& tb, const agb::MoeRoute& r,
+                     cudaStream_t s) {
+  const int k_tiles = p.K / agb::kDgBK;
+  const int m_tiles = (P + mt - 1) / mt + m.E;           // grid bound; CTAs past the used tiles exit
+  if (m_tiles > 65535) return failf(AGB200_ENOSUP, "moe backward: %d row tiles exceed the grid limit", m_tiles);
+  // the wave model of the dense dgrad on the tiles the routing can use: ceil(P / MT) plus one partial tile per hit expert
+  const int used = std::min(m_tiles, (P + mt - 1) / mt + std::min(m.E, P) - 1);
+  int split = agb::gemm_auto_split(mt, k_tiles * used, p.num_nb, m.sms);
+  while (split > 1 && split > p.num_nb) split /= 2;
+  p.split = split;
+  p.nb_per_split = (p.num_nb + split - 1) / split;
+  const bool bf = m.dtype == AGB200_BF16;
+#define AGB_MOE_DGRAD_CASE(MT)                                                                                          \
+  case MT:                                                                                                             \
+    return bf ? launch_moe_dgrad_inst<MT, true, kDown>(p, tb, r, m.g_maps, m.g_ex, k_tiles, m_tiles, s)                \
+              : launch_moe_dgrad_inst<MT, false, kDown>(p, tb, r, m.g_maps, m.g_ex, k_tiles, m_tiles, s);
+  switch (mt) {
+    AGB_MOE_DGRAD_CASE(32)
+    AGB_MOE_DGRAD_CASE(64)
+    AGB_MOE_DGRAD_CASE(128)
+  }
+#undef AGB_MOE_DGRAD_CASE
+  return failf(AGB200_EINVAL, "moe backward: row tile %d", mt);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t agb200_moe_grad_plan_bytes(int E, int H, int I, int group_size) {
+  (void)I; (void)group_size;
+  if (E < 1 || H < 1) return 0;
+  return maps_bytes(E) + grad_table_bytes(E) + align_up(size_t(E) * H * 4, 256);
+}
+
+int agb200_moe_grad_attach(void* handle, const agb200_moe_expert* experts, void* grad_plan, size_t grad_plan_bytes) {
+  Moe* m = static_cast<Moe*>(handle);
+  if (!m || m->magic != kMagic) return failf(AGB200_EINVAL, "moe: bad handle");
+  if (!experts || !grad_plan) return failf(AGB200_EINVAL, "moe grad: null pointer argument");
+  const int E = m->E, H = m->H, I = m->I;
+  const size_t need = agb200_moe_grad_plan_bytes(E, H, I, 0);
+  if (grad_plan_bytes < need || (reinterpret_cast<uintptr_t>(grad_plan) & 255u))
+    return failf(AGB200_EWORKSPACE, "moe grad: plan buffer needs %zu bytes, 256-byte aligned (got %zu)", need, grad_plan_bytes);
+  int dev = 0;
+  MOE_CUDA(cudaGetDevice(&dev));
+  if (dev != m->device) return failf(AGB200_EINVAL, "moe grad: created on device %d, current device is %d", m->device, dev);
+  // every configuration agb200_moe_create accepts (H, I multiples of 128; group 32, a multiple of 64, or one group)
+  // has whole 16-row groups: the tensor-core dgrad takes all three layers
+  if (!agb::dgrad_tc_supported(H, I, m->gs13) || !agb::dgrad_tc_supported(I, H, m->gs2))
+    return failf(AGB200_ENOSUP, "moe grad: H=%d, I=%d, group sizes %d / %d are outside the tensor-core dgrad", H, I, m->gs13, m->gs2);
+  agb::EncodeTiledFn encode = agb::get_encode_fn();
+  if (encode == nullptr) return failf(AGB200_ECUDA, "moe grad: cuTensorMapEncodeTiled entry point not available");
+  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "moe grad: no CUDA context: %s", cudaGetErrorString(e));
+  unsigned char* base = static_cast<unsigned char*>(grad_plan);
+  CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base);
+  agb::MoeGradExpertDev* d_ex = reinterpret_cast<agb::MoeGradExpertDev*>(base + maps_bytes(E));
+  int32_t* d_inv = reinterpret_cast<int32_t*>(base + maps_bytes(E) + grad_table_bytes(E));
+  const CUtensorMapDataType sdt = m->dtype == AGB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  std::vector<CUtensorMap> maps;
+  std::vector<agb::MoeGradExpertDev> table(E);
+  for (int e = 0; e < E; ++e) {
+    const agb200_moe_layer* L[3] = {&experts[e].w1, &experts[e].w3, &experts[e].w2};
+    for (int l = 0; l < 3; ++l) {
+      const agb200_moe_layer& X = *L[l];
+      if (!X.qweight || !X.qzeros || !X.scales) return failf(AGB200_EINVAL, "moe grad expert %d layer %d: null qweight/qzeros/scales", e, l);
+      if (!aligned16(X.qweight) || !aligned16(X.qzeros) || !aligned16(X.scales))
+        return failf(AGB200_EINVAL, "moe grad expert %d layer %d: buffers must be 16-byte aligned", e, l);
+      const int K = l == 2 ? I : H, N = l == 2 ? H : I, gs = l == 2 ? m->gs2 : m->gs13;
+      const int G = (K + gs - 1) / gs;
+      CUtensorMap mw, ms, mz;   // the dgrad kernel's boxes: [16 word rows][64 n], [5 groups][64 n], [5 groups][8 words]
+      if (int rc = encode_2d(encode, &mw, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "qweight")) return rc;
+      if (int rc = encode_2d(encode, &ms, sdt, X.scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "scales")) return rc;
+      if (int rc = encode_2d(encode, &mz, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "qzeros")) return rc;
+      maps.push_back(mw); maps.push_back(ms); maps.push_back(mz);
+    }
+    if (experts[e].w1.perm != experts[e].w3.perm)
+      return failf(AGB200_ENOSUP, "moe grad expert %d: w1 and w3 must share one act-order permutation of x", e);
+    table[e].perm2 = experts[e].w2.perm;
+    table[e].inv13 = experts[e].w1.perm != nullptr ? d_inv + size_t(e) * H : nullptr;
+  }
+  cudaError_t ce;
+  // load time only: as agb200_moe_create, wait for the device before writing caller memory with the legacy stream
+  if ((ce = cudaDeviceSynchronize()) != cudaSuccess) return failf(AGB200_ECUDA, "moe grad: cudaDeviceSynchronize: %s", cudaGetErrorString(ce));
+  if ((ce = cudaMemcpy(d_maps, maps.data(), maps.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice)) != cudaSuccess ||
+      (ce = cudaMemcpy(d_ex, table.data(), size_t(E) * sizeof(agb::MoeGradExpertDev), cudaMemcpyHostToDevice)) != cudaSuccess)
+    return failf(AGB200_ECUDA, "moe grad: copy plan: %s", cudaGetErrorString(ce));
+  for (int e = 0; e < E; ++e)
+    if (experts[e].w1.perm != nullptr)
+      agb::moe_invert_perm_kernel<<<(H + 255) / 256, 256>>>(experts[e].w1.perm, d_inv + size_t(e) * H, H);
+  if ((ce = cudaGetLastError()) != cudaSuccess || (ce = cudaDeviceSynchronize()) != cudaSuccess)
+    return failf(AGB200_ECUDA, "moe grad: invert permutations: %s", cudaGetErrorString(ce));
+  m->g_maps = d_maps;
+  m->g_ex = d_ex;
+  return 0;
+}
+
+size_t agb200_moe_backward_workspace_bytes(int T, int k, int E, int H, int I) {
+  if (T < 0 || k < 1 || E < 1 || H < 1 || I < 1) return 0;
+  return bwd_layout(T, k, E, H, I).total;
+}
+
+int agb200_moe_backward(void* handle, const void* dy, const void* top_k_index, int index_dtype, const void* top_k_weights,
+                        int weights_dtype, int T, int k, const void* saved, size_t saved_bytes_given, void* dx, void* dw,
+                        void* workspace, size_t workspace_bytes, void* stream) {
+  Moe* m = static_cast<Moe*>(handle);
+  if (!m || m->magic != kMagic) return failf(AGB200_EINVAL, "moe: bad handle");
+  if (T < 0 || k < 1) return failf(AGB200_EINVAL, "moe backward: T >= 0 and k >= 1 (got T=%d, k=%d)", T, k);
+  if (T == 0 || (dx == nullptr && dw == nullptr)) return 0;
+  if (static_cast<long long>(T) * k > (1ll << 30)) return failf(AGB200_ENOSUP, "moe backward: T*k=%lld pairs is too many", static_cast<long long>(T) * k);
+  if (m->g_maps == nullptr) return failf(AGB200_EINVAL, "moe backward: no grad plan (call agb200_moe_grad_attach first)");
+  int dev = 0;
+  MOE_CUDA(cudaGetDevice(&dev));
+  if (dev != m->device) return failf(AGB200_EINVAL, "moe backward: created on device %d, current device is %d", m->device, dev);
+  if (!dy || !top_k_index || !top_k_weights || !saved || !workspace) return failf(AGB200_EINVAL, "moe backward: null pointer argument");
+  if (!aligned16(dy) || !aligned16(dx) || !aligned16(dw) || (reinterpret_cast<uintptr_t>(saved) & 255u) ||
+      (reinterpret_cast<uintptr_t>(workspace) & 255u))
+    return failf(AGB200_EINVAL, "moe backward: dy, dx and dw must be 16-byte aligned, saved and the workspace 256-byte aligned");
+  if (index_dtype != AGB200_MOE_INDEX_I32 && index_dtype != AGB200_MOE_INDEX_I64) return failf(AGB200_EINVAL, "moe backward: unknown index dtype %d", index_dtype);
+  if (weights_dtype != m->dtype && weights_dtype != AGB200_MOE_WEIGHTS_F32)
+    return failf(AGB200_EINVAL, "moe backward: top_k_weights must be fp32 or the activation dtype");
+  const int E = m->E, H = m->H, I = m->I;
+  if (saved_bytes_given < saved_bytes(T, k, H, I))
+    return failf(AGB200_EWORKSPACE, "moe backward: saved buffer needs %zu bytes (got %zu)", saved_bytes(T, k, H, I), saved_bytes_given);
+  const BwdLayout b = bwd_layout(T, k, E, H, I);
+  if (workspace_bytes < b.total) return failf(AGB200_EWORKSPACE, "moe backward: workspace needs %zu bytes (got %zu)", b.total, workspace_bytes);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  const agb::MoeRoute r = route_views(ws, E, b.w);
+  const int P = b.w.P;
+  const int ids64 = index_dtype == AGB200_MOE_INDEX_I64;
+  const int wf32 = weights_dtype == AGB200_MOE_WEIGHTS_F32;
+  const bool bf = m->dtype == AGB200_BF16;
+  const size_t gu = align_up(size_t(P) * I * 2, 256);
+  const uint16_t* sv_g = static_cast<const uint16_t*>(saved);
+  const uint16_t* sv_u = reinterpret_cast<const uint16_t*>(static_cast<const unsigned char*>(saved) + gu);
+  const uint16_t* sv_y = reinterpret_cast<const uint16_t*>(static_cast<const unsigned char*>(saved) + 2 * gu);
+  int* prow = reinterpret_cast<int*>(ws + b.prow);
+  uint16_t* dyp = dx != nullptr ? reinterpret_cast<uint16_t*>(ws + b.dyp) : nullptr;
+
+  agb::moe_route_kernel<<<1, agb::kMoeRouteThreads, 0, s>>>(top_k_index, ids64, P, E, b.mt, r);
+  MOE_CUDA(cudaGetLastError());
+  const uint16_t* dy16 = static_cast<const uint16_t*>(dy);
+  if (bf) agb::moe_combine_bwd_kernel<true><<<P, 256, 0, s>>>(dy16, top_k_index, ids64, top_k_weights, wf32, k, E, H, r, sv_y, prow, dyp, dw);
+  else agb::moe_combine_bwd_kernel<false><<<P, 256, 0, s>>>(dy16, top_k_index, ids64, top_k_weights, wf32, k, E, H, r, sv_y, prow, dyp, dw);
+  MOE_CUDA(cudaGetLastError());
+  if (dx == nullptr) return 0;
+
+  agb::EncodeTiledFn encode = agb::get_encode_fn();
+  if (encode == nullptr) return failf(AGB200_ECUDA, "moe backward: cuTensorMapEncodeTiled entry point not available");
+  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "moe backward: no CUDA context: %s", cudaGetErrorString(e));
+  const CUtensorMapDataType t16 = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  uint16_t* dgu = reinterpret_cast<uint16_t*>(ws + b.dgu);
+  float* dxp = reinterpret_cast<float*>(ws + b.dxp);
+  CUtensorMap t_dyp, t_dgu;
+  if (int rc = encode_2d(encode, &t_dyp, t16, dyp, H, b.rows, size_t(H) * 2, agb::kDgBN, b.mt, true, "dy_pair")) return rc;
+  if (int rc = encode_2d(encode, &t_dgu, t16, dgu, 2 * I, b.rows, size_t(2 * I) * 2, agb::kDgBN, b.mt, true, "dg | du")) return rc;
+  agb::MoeDgradParams p{};
+  p.out = dgu; p.K = I; p.N = H; p.I = I; p.group_size = m->gs2; p.num_nb = H / agb::kDgBN; p.g = sv_g; p.u = sv_u;
+  if (int rc = launch_moe_dgrad<true>(*m, b.mt, P, p, t_dyp, r, s)) return rc;
+  p.out = dxp; p.K = H; p.N = 2 * I; p.group_size = m->gs13; p.num_nb = 2 * I / agb::kDgBN; p.g = nullptr; p.u = nullptr;
+  if (int rc = launch_moe_dgrad<false>(*m, b.mt, P, p, t_dgu, r, s)) return rc;
+  const dim3 cgrid(T, (H + 255) / 256, 1);
+  if (bf) agb::moe_dx_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, k, E, H, prow, dxp, m->g_ex, static_cast<uint16_t*>(dx));
+  else agb::moe_dx_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, k, E, H, prow, dxp, m->g_ex, static_cast<uint16_t*>(dx));
   MOE_CUDA(cudaGetLastError());
   return 0;
 }

@@ -14,6 +14,8 @@
 // The decode and GEMM kernels take their rows from a work source (template parameter): MoeRouted reads the routing
 // table; DenseRows / DenseGemmRows run one gate/up pair over all M rows of x (agb200_w4a16_gate_up, a dense MLP), the
 // GEMM then with split-K over a thread-block cluster whose partial tiles are reduced through DSMEM before silu * mul.
+// MoeRoutedSave (agb200_moe_forward_saving) is MoeRouted whose gate/up epilogue also keeps g and u for the backward
+// (moe_dgrad.cuh); the other sources compile to the code they had before it existed.
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda.h>
@@ -67,6 +69,7 @@ __device__ __forceinline__ int moe_load_id(const void* ids, int ids64, int i) {
 // Rows of a group are numbered by position (pair-list order for experts); gate/up writes h row `pos`.
 struct MoeRouted {
   static constexpr bool kSplitK = false;
+  static constexpr bool kSave = false;
   const MoeExpertDev* ex;
   MoeRoute r;
   int k;                        // slots per token
@@ -88,8 +91,18 @@ struct MoeRouted {
   __device__ __forceinline__ const CUtensorMap* gemm_maps(int e, int layer) const { return maps + (e * 3 + layer) * 3; }
 };
 
+// The routed rows of a forward that keeps what the backward reads (agb200_moe_forward_saving): the gate/up stage also
+// stores g and u (bias added, rounded: the values silu_mul_elt consumed) of every pair, at row = pair id t * k + j and in
+// h's column order (w2's sorted order for an act-order w2).
+struct MoeRoutedSave : MoeRouted {
+  static constexpr bool kSave = true;
+  uint16_t* g;                  // [T * k, I]
+  uint16_t* u;                  // [T * k, I]
+};
+
 struct DenseRows {
   static constexpr bool kSplitK = false;
+  static constexpr bool kSave = false;
   MoeExpertDev lay;             // gate = layer 0, up = layer 1 (perm13: the shared act-order permutation or null)
   int M;
   __device__ __forceinline__ int groups() const { return 1; }
@@ -111,6 +124,18 @@ struct DenseGemmRows : DenseRows {
   }
   __device__ __forceinline__ const CUtensorMap* gemm_maps(int, int layer) const { return maps + layer * 3; }
 };
+
+// store_gate_up that also keeps the rounded g and u (MoeRoutedSave) at g_out / u_out
+template <bool kBf16>
+__device__ __forceinline__ void store_gate_up_saving(uint16_t* out, float gv, float uv, const void* bias_g, const void* bias_u,
+                                                     int nn, uint16_t* g_out, uint16_t* u_out) {
+  if (bias_g != nullptr) gv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(bias_g)[nn]);
+  if (bias_u != nullptr) uv += elt_to_float<kBf16>(reinterpret_cast<const uint16_t*>(bias_u)[nn]);
+  const uint16_t g16 = float_to_elt<kBf16>(gv), u16 = float_to_elt<kBf16>(uv);
+  *g_out = g16;
+  *u_out = u16;
+  *out = float_to_elt<kBf16>(silu_mul_elt<kBf16>(g16, u16));
+}
 
 // ------------------------------------------------------------------------------------------------ routing
 // One CTA of 1024 threads.  Counts by shared-memory atomics (the totals do not depend on the order), then placement in
@@ -399,8 +424,13 @@ moe_decode_kernel(const MoeDecodeParams p, const __grid_constant__ Src src) {
               uv += red[((w + 4) * kMdRows + m) * kMdTN + col];
             }
             const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
-            store_gate_up<kBf16>(reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(pos) * p.N + dst, gv, uv,
-                                 X.bias[0], X.bias[1], nn);
+            uint16_t* hp = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(pos) * p.N + dst;
+            if constexpr (Src::kSave) {
+              const size_t at = static_cast<size_t>(src.r.pairs[pos]) * p.N + dst;
+              store_gate_up_saving<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn, src.g + at, src.u + at);
+            } else {
+              store_gate_up<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn);
+            }
           } else {
             float v = 0.f;
 #pragma unroll
@@ -624,8 +654,15 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
           const int nn = n0 + nl;
           if (ml < m_valid && nn < p.N) {
             const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
-            store_gate_up<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + dst, stage_f32[ml * kGemmLd + nl],
-                                 stage_f32[ml * kGemmLd + kHalf + nl], X.bias[0], X.bias[1], nn);
+            if constexpr (Src::kSave) {
+              const int pair = src.r.pairs[src.r.offsets[e] + (m0 - src.r.pad_off[e]) + ml];
+              const size_t at = static_cast<size_t>(pair) * p.N + dst;
+              store_gate_up_saving<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + dst, stage_f32[ml * kGemmLd + nl],
+                                          stage_f32[ml * kGemmLd + kHalf + nl], X.bias[0], X.bias[1], nn, src.g + at, src.u + at);
+            } else {
+              store_gate_up<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + dst, stage_f32[ml * kGemmLd + nl],
+                                   stage_f32[ml * kGemmLd + kHalf + nl], X.bias[0], X.bias[1], nn);
+            }
           }
         }
       } else {
@@ -679,11 +716,12 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
 
 // ------------------------------------------------------------------------------------------------ combine
 // out[t, n] = sum_j w[t, j] * y_pair[t*k + j, n] over the slots with a valid id, in slot order, fp32, one rounding.
-// Decode path: y_pair = round(sum_s partial[s] + bias2) first (the split-K partial sums of the down stage).
-template <bool kBf16>
+// Decode path: y_pair = round(sum_s partial[s] + bias2) first (the split-K partial sums of the down stage); kSave also
+// stores that y_pair at ysave[t*k + j] (the GEMM path's down stage writes its y_pair there itself).
+template <bool kBf16, bool kSave = false>
 __global__ void moe_combine_kernel(const void* ids, int ids64, const void* w, int w_f32, int k, int E, int N, int P,
                                    const uint16_t* ypair, const float* part, int split, const MoeExpertDev* ex,
-                                   uint16_t* out) {
+                                   uint16_t* out, uint16_t* ysave = nullptr) {
   const int t = blockIdx.x;
   const int nn = blockIdx.y * blockDim.x + threadIdx.x;
   if (nn >= N) return;
@@ -699,7 +737,9 @@ __global__ void moe_combine_kernel(const void* ids, int ids64, const void* w, in
       for (int s = 0; s < split; ++s) v += part[(static_cast<size_t>(s) * P + i) * N + nn];
       const uint16_t* b2 = reinterpret_cast<const uint16_t*>(ex[e].bias[2]);
       if (b2 != nullptr) v += elt_to_float<kBf16>(b2[nn]);
-      y = elt_to_float<kBf16>(float_to_elt<kBf16>(v));
+      const uint16_t y16 = float_to_elt<kBf16>(v);
+      if constexpr (kSave) ysave[static_cast<size_t>(i) * N + nn] = y16;
+      y = elt_to_float<kBf16>(y16);
     } else {
       y = elt_to_float<kBf16>(ypair[static_cast<size_t>(i) * N + nn]);
     }

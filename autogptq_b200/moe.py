@@ -11,6 +11,10 @@ reference loop finds the hit experts with ``nonzero()`` (a host synchronisation)
 plus a dozen small ops per hit expert; here the routing stays on the device and the block is one fixed sequence of
 launches (CUDA-graph capturable, replayable with new routing).  The checkpoint tensors of the experts stay where they
 are: the library reads them in place.  There is no CPU fallback.
+
+``QuantExperts(..., input_grad=True)`` also backpropagates: ``hidden_states`` and ``top_k_weights`` get their gradients
+from the grouped backward (``agb200_moe_backward``), so adapters of earlier layers and the router train on a frozen 4-bit
+MoE checkpoint.  The expert weights get no gradient.
 """
 from __future__ import annotations
 
@@ -21,6 +25,8 @@ from typing import Dict, Mapping
 
 import torch
 import torch.nn as nn
+
+from torch.autograd.function import once_differentiable
 
 from . import _lib
 from .qlinear import _DTYPE_CODE, QuantLinear, _workspace
@@ -42,10 +48,12 @@ def _ptr(t):
 
 
 class _Plan:
-    """A created ``agb200_moe`` handle with its plan buffer and the tensors it points to."""
+    """A created ``agb200_moe`` handle with its plan buffer and the tensors it points to (``arr``: the expert descriptors;
+    ``grad``: the buffer of ``agb200_moe_grad_attach`` once attached)."""
 
-    def __init__(self, handle, plan, keep):
-        self.handle, self.plan, self.keep = handle, plan, keep
+    def __init__(self, handle, plan, keep, arr=None):
+        self.handle, self.plan, self.keep, self.arr = handle, plan, keep, arr
+        self.grad = None
 
     def __del__(self):
         if self.handle is not None and _lib._lib is not None:
@@ -56,9 +64,13 @@ class _Plan:
 class QuantExperts(nn.Module):
     """E experts, each ``w2(silu(w1(x)) * w3(x))`` with 4-bit GPTQ ``QuantLinear`` layers, routed per token.
 
-    All experts share the hidden size H (w1 / w3 in, w2 out), the intermediate size I and the group size."""
+    All experts share the hidden size H (w1 / w3 in, w2 out), the intermediate size I and the group size.
 
-    def __init__(self, w1s, w3s, w2s):
+    ``input_grad=True``: in grad mode, when ``hidden_states`` or ``top_k_weights`` requires grad, the forward keeps g, u
+    and the per-pair outputs, ``(2 I + H) * T * k`` 16-bit values, until backward, which then computes both input
+    gradients.  The default refuses grad mode instead, so that an inference model never holds that memory silently."""
+
+    def __init__(self, w1s, w3s, w2s, *, input_grad: bool = False):
         super().__init__()
         w1s, w3s, w2s = list(w1s), list(w3s), list(w2s)
         if not w1s or not (len(w1s) == len(w3s) == len(w2s)):
@@ -94,16 +106,18 @@ class QuantExperts(nn.Module):
         self.w1, self.w3, self.w2 = nn.ModuleList(w1s), nn.ModuleList(w3s), nn.ModuleList(w2s)
         self.num_experts, self.hidden_size, self.intermediate_size = E, H, I
         self.group_size = group_size
+        self.input_grad = bool(input_grad)
         self._plans: Dict = {}     # (dtype, device index, with tensor-core copies) -> _Plan
         self._tc = False           # tensor-core copies built (first call with T > MOE_DECODE_MAX_T)
 
     @classmethod
-    def from_linears(cls, w1s, w3s, w2s) -> "QuantExperts":
-        return cls(w1s, w3s, w2s)
+    def from_linears(cls, w1s, w3s, w2s, *, input_grad: bool = False) -> "QuantExperts":
+        return cls(w1s, w3s, w2s, input_grad=input_grad)
 
     def extra_repr(self) -> str:
         return (f"num_experts={self.num_experts}, hidden_size={self.hidden_size}, "
-                f"intermediate_size={self.intermediate_size}, group_size={self.group_size}, backend=sm_90a")
+                f"intermediate_size={self.intermediate_size}, group_size={self.group_size}, input_grad={self.input_grad}, "
+                "backend=sm_90a")
 
     def _layers(self):
         return list(self.w1) + list(self.w3) + list(self.w2)
@@ -141,18 +155,32 @@ class QuantExperts(nn.Module):
             rc = lib.agb200_moe_create(ctypes.cast(arr, c_void_p), E, H, I, self.group_size, _DTYPE_CODE[dtype],
                                        buf.data_ptr(), nbytes, ctypes.byref(handle))
         _lib.check(rc, "agb200_moe_create")
-        plan = _Plan(handle.value, buf, keep)
+        plan = _Plan(handle.value, buf, keep, arr)
         self._plans[key] = plan
         return plan
+
+    def _attach_grad(self, plan: _Plan, device) -> None:
+        """Build the backward's per-expert data (tensor maps, inverse permutations) once per plan; synchronises."""
+        if plan.grad is not None:
+            return
+        lib = _lib.load()
+        nbytes = int(lib.agb200_moe_grad_plan_bytes(self.num_experts, self.hidden_size, self.intermediate_size,
+                                                    self.group_size))
+        buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        with torch.cuda.device(device):
+            rc = lib.agb200_moe_grad_attach(plan.handle, ctypes.cast(plan.arr, c_void_p), buf.data_ptr(), nbytes)
+        _lib.check(rc, "agb200_moe_grad_attach")
+        plan.grad = buf
 
     def forward(self, hidden_states: torch.Tensor, top_k_index: torch.Tensor, top_k_weights: torch.Tensor) -> torch.Tensor:
         if hidden_states.device.type != "cuda":
             raise RuntimeError("autogptq_b200.QuantExperts.forward needs CUDA tensors (there is no CPU fallback).")
-        if torch.is_grad_enabled() and (hidden_states.requires_grad or top_k_weights.requires_grad):
+        grad = torch.is_grad_enabled() and (hidden_states.requires_grad or top_k_weights.requires_grad)
+        if grad and not self.input_grad:
             raise NotImplementedError(
-                "QuantExperts is inference-only: the grouped expert kernels have no backward, so hidden_states and "
-                "top_k_weights must not require grad (run it under torch.no_grad(), or use the experts' QuantLinear "
-                "layers one by one, which do propagate input gradients).")
+                "QuantExperts is inference-only unless built with input_grad=True: hidden_states and top_k_weights must "
+                "not require grad (run it under torch.no_grad(), pass input_grad=True to QuantExperts / group_experts "
+                "for the grouped backward, or use the experts' QuantLinear layers one by one).")
         device = hidden_states.device
         if top_k_index.device != device or top_k_weights.device != device:
             raise RuntimeError("hidden_states, top_k_index and top_k_weights must be on the same CUDA device")
@@ -164,12 +192,13 @@ class QuantExperts(nn.Module):
         x = hidden_states.reshape(-1, H)
         T = x.shape[0]
         out_shape = hidden_states.shape[:-1] + (H,)
-        if T == 0:
+        if T == 0 and not grad:
             return torch.empty(out_shape, dtype=x_dtype, device=device)
+        # the conversions are differentiable torch ops: gradients reach fp32 inputs in their own dtype
         x = x.to(cdtype).contiguous()
         if x.data_ptr() % 16:                        # the kernels read x in 16-byte words
             x = x.clone()
-        idx = top_k_index.reshape(T, -1)
+        idx = top_k_index.reshape(T, -1) if T else top_k_index.reshape(0, top_k_index.shape[-1])
         k = idx.shape[1]
         if idx.dtype not in (torch.int32, torch.int64):
             idx = idx.to(torch.int64)
@@ -178,31 +207,101 @@ class QuantExperts(nn.Module):
         if w.dtype not in (torch.float32, cdtype):
             w = w.float()
         w = w.contiguous()
+        if grad:
+            out = _QuantExpertsFunction.apply(x, w, idx, self)
+        else:
+            out = self._forward(x, idx, w)[0]
+        out = out.reshape(out_shape)
+        return out if x_dtype == cdtype else out.to(x_dtype)
+
+    def _forward(self, x: torch.Tensor, idx: torch.Tensor, w: torch.Tensor, save: bool = False):
+        """(out [T, H], saved or None) of the grouped forward on prepared inputs (x [T, H] of the compute dtype,
+        contiguous and 16-byte aligned; idx [T, k] int32 / int64; w [T, k] fp32 or the compute dtype).  ``save``: also
+        keep what the backward reads (``agb200_moe_forward_saving``)."""
+        device, cdtype = x.device, x.dtype
+        T, k = idx.shape
+        H, E, I = self.hidden_size, self.num_experts, self.intermediate_size
+        out = torch.empty((T, H), dtype=cdtype, device=device)
+        if T == 0:
+            return out, (torch.empty(0, dtype=torch.uint8, device=device) if save else None)
         if T > _lib.MOE_DECODE_MAX_T and not self._tc:
             self._tc = True                          # same lazy rule as QuantLinear: tensor-core copies on first need
         plan = self._plan(cdtype, device)
         lib = _lib.load()
-        E, I = self.num_experts, self.intermediate_size
         ws_bytes = int(lib.agb200_moe_workspace_bytes(T, k, E, H, I))
         ws = _workspace(device, ws_bytes)
-        out = torch.empty((T, H), dtype=cdtype, device=device)
-        with torch.cuda.device(device):
-            rc = lib.agb200_moe_forward(
-                plan.handle, x.data_ptr(), idx.data_ptr(),
+        args = (plan.handle, x.data_ptr(), idx.data_ptr(),
                 _lib.MOE_INDEX_I64 if idx.dtype == torch.int64 else _lib.MOE_INDEX_I32, w.data_ptr(),
-                _lib.MOE_WEIGHTS_F32 if w.dtype == torch.float32 else _DTYPE_CODE[cdtype], T, k, out.data_ptr(),
+                _lib.MOE_WEIGHTS_F32 if w.dtype == torch.float32 else _DTYPE_CODE[cdtype], T, k, out.data_ptr())
+        saved = None
+        with torch.cuda.device(device):
+            if not save:
+                rc = lib.agb200_moe_forward(*args, ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream)
+            else:
+                self._attach_grad(plan, device)
+                nsaved = int(lib.agb200_moe_saved_bytes(T, k, E, H, I))
+                saved = torch.empty(nsaved, dtype=torch.uint8, device=device)
+                rc = lib.agb200_moe_forward_saving(*args, saved.data_ptr(), nsaved, ws.data_ptr(), ws.numel(),
+                                                   torch.cuda.current_stream(device).cuda_stream)
+        _lib.check(rc, "agb200_moe_forward_saving" if save else "agb200_moe_forward")
+        return out, saved
+
+    def _backward(self, dy: torch.Tensor, idx: torch.Tensor, w: torch.Tensor, saved: torch.Tensor, need_dx: bool,
+                  need_dw: bool):
+        """(dx [T, H] of the compute dtype or None, dw [T, k] of w's dtype or None) from dy [T, H] and the saved
+        values of ``_forward(..., save=True)`` on the same x / idx / w."""
+        T, k = idx.shape
+        H, E, I = self.hidden_size, self.num_experts, self.intermediate_size
+        device, cdtype = dy.device, dy.dtype
+        dx = torch.empty((T, H), dtype=cdtype, device=device) if need_dx else None
+        dw = torch.empty((T, k), dtype=w.dtype, device=device) if need_dw else None
+        if T == 0 or not (need_dx or need_dw):
+            return dx, dw
+        plan = self._plan(cdtype, device)
+        lib = _lib.load()
+        ws_bytes = int(lib.agb200_moe_backward_workspace_bytes(T, k, E, H, I))
+        ws = _workspace(device, ws_bytes)
+        with torch.cuda.device(device):
+            rc = lib.agb200_moe_backward(
+                plan.handle, dy.data_ptr(), idx.data_ptr(),
+                _lib.MOE_INDEX_I64 if idx.dtype == torch.int64 else _lib.MOE_INDEX_I32, w.data_ptr(),
+                _lib.MOE_WEIGHTS_F32 if w.dtype == torch.float32 else _DTYPE_CODE[cdtype], T, k, saved.data_ptr(),
+                saved.numel(), dx.data_ptr() if dx is not None else None, dw.data_ptr() if dw is not None else None,
                 ws.data_ptr(), ws.numel(), torch.cuda.current_stream(device).cuda_stream)
-        _lib.check(rc, "agb200_moe_forward")
-        out = out.reshape(out_shape)
-        return out if x_dtype == cdtype else out.to(x_dtype)
+        _lib.check(rc, "agb200_moe_backward")
+        return dx, dw
 
 
-def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTERN) -> Dict[str, nn.Module]:
+class _QuantExpertsFunction(torch.autograd.Function):
+    """out = QuantExperts._forward(x, idx, w) with dx and dw from ``agb200_moe_backward`` (the expert weights are frozen,
+    top_k_index gets no gradient).  x and w arrive converted and contiguous; the conversions happen outside, as torch ops."""
+
+    @staticmethod
+    def forward(ctx, x, w, idx, qe):
+        out, saved = qe._forward(x, idx, w, save=True)
+        ctx.qe = qe
+        ctx.save_for_backward(idx, w, saved)
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, dy):
+        idx, w, saved = ctx.saved_tensors
+        need_dx, need_dw = ctx.needs_input_grad[0], ctx.needs_input_grad[1]
+        dy = dy.contiguous()
+        if dy.data_ptr() % 16:
+            dy = dy.clone()
+        dx, dw = ctx.qe._backward(dy, idx, w, saved, need_dx, need_dw)
+        return dx, dw, None, None
+
+
+def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTERN, *,
+                  input_grad: bool = False) -> Dict[str, nn.Module]:
     """``{prefix: QuantLinear}`` (e.g. from ``checkpoint.load_quant_linears``) -> the same mapping with every
     ``<experts prefix>.<i>.w1|w2|w3`` family replaced by ONE ``QuantExperts`` under ``<experts prefix>``.
 
     ``pattern`` has three groups: the experts prefix, the expert number and the layer name (w1, w2 or w3).  Every
-    other layer stays as it was."""
+    other layer stays as it was.  ``input_grad`` is passed to every ``QuantExperts`` (see there)."""
     rx = re.compile(pattern)
     out: Dict[str, nn.Module] = {}
     groups: Dict[str, Dict[int, Dict[str, QuantLinear]]] = {}
@@ -221,7 +320,7 @@ def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTE
             if missing:
                 raise ValueError(f"{prefix}.{i}: missing {sorted(missing)}")
         out[prefix] = QuantExperts.from_linears([experts[i]["w1"] for i in ids], [experts[i]["w3"] for i in ids],
-                                                [experts[i]["w2"] for i in ids])
+                                                [experts[i]["w2"] for i in ids], input_grad=input_grad)
     return out
 
 

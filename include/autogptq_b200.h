@@ -334,6 +334,45 @@ int agb200_moe_forward(void* handle, const void* x, const void* top_k_index, int
 int agb200_moe_destroy(void* handle);
 
 /*
+ * Backward of the grouped experts (additions to ABI v10): with the expert weights frozen,
+ *
+ *   dx = dL/d x            [T, H] of `dtype`, in x's column order
+ *   dw = dL/d top_k_weights [T, k] of weights_dtype (fp32 or `dtype`); 0 for ids outside [0, E)
+ *
+ * from dy = dL/d out [T, H] of `dtype` and what agb200_moe_forward_saving kept.  Rounding points ("round" = to the
+ * activation dtype; every sum fp32 in a fixed order, no atomics, so repeated calls are bit-identical):
+ *   saved g, u   the rounded gate / up values (+ bias) that silu * mul consumed; saved y_pair the rounded per-pair outputs
+ *   dw[t, j]     = sum_n dy[t, n] * y_pair[t*k + j, n], one rounding to weights_dtype
+ *   dy_pair      = round(w[t, j] * dy[t])
+ *   dh           = dy_pair * W2^T (W rounded once as s * (q - z)), unrounded
+ *   dg, du       = round(dh * u * silu'(g)), round(dh * round(silu(g))),  silu'(g) = s(g) (1 + g (1 - s(g)))
+ *   dx_pair      = dg * W1^T + du * W3^T in ONE fp32 sum, unrounded
+ *   dx[t]        = round(sum_j dx_pair[t*k + j]) in slot order
+ *
+ *   agb200_moe_saved_bytes       size of `saved`: g [T*k, I] | u [T*k, I] | y_pair [T*k, H], pair-id rows (t*k + j),
+ *                                whichever forward path ran.  DEVICE memory, 256-byte aligned.
+ *   agb200_moe_forward_saving    agb200_moe_forward (same result, bit for bit) that also fills `saved`.
+ *   agb200_moe_grad_attach       builds the backward's per-expert data into caller-owned DEVICE memory of
+ *                                agb200_moe_grad_plan_bytes(...) bytes (256-byte aligned, alive until agb200_moe_destroy):
+ *                                TMA tensor maps of qweight (the checkpoint layout), scales and qzeros of every layer with
+ *                                the dgrad boxes, and the inverse of each expert's w1 / w3 permutation.  `experts` are the
+ *                                descriptors given to agb200_moe_create (qweight_tc is not used).  Synchronises the device:
+ *                                call it at load time, outside stream capture.
+ *   agb200_moe_backward          dx and / or dw (NULL: not computed; dw alone runs no GEMM).  Explicit stream, no host
+ *                                synchronisation: capturable in a CUDA graph.  workspace: agb200_moe_backward_workspace_bytes.
+ */
+size_t agb200_moe_saved_bytes(int T, int k, int E, int H, int I);
+int agb200_moe_forward_saving(void* handle, const void* x, const void* top_k_index, int index_dtype,
+                              const void* top_k_weights, int weights_dtype, int T, int k, void* out, void* saved,
+                              size_t saved_bytes, void* workspace, size_t workspace_bytes, void* stream);
+size_t agb200_moe_grad_plan_bytes(int E, int H, int I, int group_size);
+int agb200_moe_grad_attach(void* handle, const agb200_moe_expert* experts, void* grad_plan, size_t grad_plan_bytes);
+size_t agb200_moe_backward_workspace_bytes(int T, int k, int E, int H, int I);
+int agb200_moe_backward(void* handle, const void* dy, const void* top_k_index, int index_dtype, const void* top_k_weights,
+                        int weights_dtype, int T, int k, const void* saved, size_t saved_bytes, void* dx, void* dw,
+                        void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Fused gate/up of a dense MLP (ABI v7): the gate and up projections of a Llama / Mistral / Qwen2 MLP and the SiLU * mul
  * between them in one launch,
  *
