@@ -86,6 +86,11 @@ def _declare(lib):
         "agb200_w4a16_gate_up": (I, [P, P, P, P, I, I, I, I, I, P, S, P]),
         "agb200_w4a16_gate_up_ex": (I, [P, P, P, P, I, I, I, I, I, P, S, P, I, I, I]),
         "agb200_w4a16_gate_up_workspace_bytes": (S, [I, I, I]),
+        "agb200_w4a16_gate_up_saving": (I, [P, P, P, P, P, P, I, I, I, I, I, P, S, P]),
+        "agb200_w4a16_gate_up_saving_ex": (I, [P, P, P, P, P, P, I, I, I, I, I, P, S, P, I, I, I]),
+        "agb200_w4a16_mlp_backward_workspace_bytes": (S, [I, I, I]),
+        "agb200_w4a16_mlp_backward": (I, [P, P, P, P, P, P, P, I, I, I, I, I, I, P, S, P]),
+        "agb200_w4a16_mlp_backward_ex": (I, [P, P, P, P, P, P, P, I, I, I, I, I, I, P, S, P, I, I]),
         "agb200_gptq_hessian_update": (I, [P, P, I, I, I, c_float, c_float, P]),
         "agb200_gptq_quantize": (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, I, P, S, P]),
         "agb200_gptq_workspace_bytes": (S, [I, I, I]),

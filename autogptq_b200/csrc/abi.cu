@@ -448,6 +448,25 @@ int check_common(const void* x, const int32_t* qweight, const int32_t* qzeros, c
 
 int agb_internal_fail(int code, const char* msg) { return fail(code, "%s", msg); }
 
+int agb_internal_unpermute_columns(const void* in, const int* perm, void* out, int M, int K, void* stream) {
+  DeviceInfo di;
+  if (int rc = get_device_info(di)) return rc;
+  const size_t smem = static_cast<size_t>(K) * 2;
+  if (smem > static_cast<size_t>(di.smem_optin))
+    return fail(AGB200_ENOSUP, "dgrad: act-order row of K=%d does not fit in shared memory", K);
+  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
+  const int attr_dev = agb::current_device_index();
+  if (!attr_set_dev[attr_dev]) {
+    AGB_CUDA(cudaFuncSetAttribute(agb::unpermute_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, di.smem_optin));
+    attr_set_dev[attr_dev] = true;
+  }
+  const int grid = M < 8 * di.sms ? M : 8 * di.sms;
+  agb::unpermute_columns_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(in), perm,
+                                                                                       static_cast<uint16_t*>(out), M, K);
+  AGB_CUDA(cudaGetLastError());
+  return 0;
+}
+
 // ================================================================================================
 extern "C" {
 
@@ -749,20 +768,7 @@ int agb200_w4a16_dgrad_ex(const void* dy, const int32_t* qweight, const int32_t*
   a.tile_m = tile_m; a.split_k = split_k; a.sms = di.sms;
   char msg[400] = "";
   if (int rc = agb::launch_w4a16_dgrad(a, stream, msg, sizeof(msg))) return fail(rc, "%s", msg);
-  if (perm != nullptr) {
-    const size_t smem = static_cast<size_t>(K) * 2;
-    if (smem > static_cast<size_t>(di.smem_optin))
-      return fail(AGB200_ENOSUP, "dgrad: act-order row of K=%d does not fit in shared memory", K);
-    static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-    const int attr_dev = agb::current_device_index();
-    if (!attr_set_dev[attr_dev]) {
-      AGB_CUDA(cudaFuncSetAttribute(agb::unpermute_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, di.smem_optin));
-      attr_set_dev[attr_dev] = true;
-    }
-    const int grid = M < 8 * di.sms ? M : 8 * di.sms;
-    agb::unpermute_columns_kernel<<<grid, 256, smem, stream>>>(static_cast<const uint16_t*>(out), perm, static_cast<uint16_t*>(dx), M, K);
-    AGB_CUDA(cudaGetLastError());
-  }
+  if (perm != nullptr) return agb_internal_unpermute_columns(out, perm, dx, M, K, stream);
   return 0;
 }
 

@@ -489,10 +489,10 @@ BwdLayout bwd_layout(int T, int k, int E, int H, int I) {
   return b;
 }
 
-template <int kMT, bool kBf16, bool kDown>
-int launch_moe_dgrad_inst(const agb::MoeDgradParams& p, const CUtensorMap& tb, const agb::MoeRoute& r, const CUtensorMap* maps,
-                          const agb::MoeGradExpertDev* gx, int k_tiles, int m_tiles, cudaStream_t stream) {
-  auto kern = agb::moe_dgrad_kernel<kMT, kBf16, kDown>;
+template <int kMT, bool kBf16, bool kDown, class Rows>
+int launch_moe_dgrad_inst(const agb::MoeDgradParams& p, const CUtensorMap& tb, const Rows& rows, int k_tiles, int m_tiles,
+                          cudaStream_t stream) {
+  auto kern = agb::moe_dgrad_kernel<kMT, kBf16, kDown, Rows>;
   constexpr int smem = agb::DgradSmem<kMT>::kTotal;
   static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
   const int dev = agb::current_device_index();
@@ -512,8 +512,25 @@ int launch_moe_dgrad_inst(const agb::MoeDgradParams& p, const CUtensorMap& tb, c
   attr.val.clusterDim.z = p.split;
   cfg.attrs = &attr;
   cfg.numAttrs = p.split > 1 ? 1 : 0;
-  MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tb, r, maps, gx));
+  MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tb, rows));
   return 0;
+}
+
+// One moe_dgrad_kernel launch with row tile mt (32 / 64 / 128)
+template <bool kDown, class Rows>
+int launch_dgrad_rows(bool bf, int mt, const agb::MoeDgradParams& p, const CUtensorMap& tb, const Rows& rows, int k_tiles,
+                      int m_tiles, cudaStream_t s) {
+#define AGB_MOE_DGRAD_CASE(MT)                                                                          \
+  case MT:                                                                                             \
+    return bf ? launch_moe_dgrad_inst<MT, true, kDown>(p, tb, rows, k_tiles, m_tiles, s)               \
+              : launch_moe_dgrad_inst<MT, false, kDown>(p, tb, rows, k_tiles, m_tiles, s);
+  switch (mt) {
+    AGB_MOE_DGRAD_CASE(32)
+    AGB_MOE_DGRAD_CASE(64)
+    AGB_MOE_DGRAD_CASE(128)
+  }
+#undef AGB_MOE_DGRAD_CASE
+  return failf(AGB200_EINVAL, "dgrad: row tile must be 32/64/128 (got %d)", mt);
 }
 
 template <bool kDown>
@@ -528,18 +545,9 @@ int launch_moe_dgrad(const Moe& m, int mt, int P, agb::MoeDgradParams p, const C
   while (split > 1 && split > p.num_nb) split /= 2;
   p.split = split;
   p.nb_per_split = (p.num_nb + split - 1) / split;
-  const bool bf = m.dtype == AGB200_BF16;
-#define AGB_MOE_DGRAD_CASE(MT)                                                                                          \
-  case MT:                                                                                                             \
-    return bf ? launch_moe_dgrad_inst<MT, true, kDown>(p, tb, r, m.g_maps, m.g_ex, k_tiles, m_tiles, s)                \
-              : launch_moe_dgrad_inst<MT, false, kDown>(p, tb, r, m.g_maps, m.g_ex, k_tiles, m_tiles, s);
-  switch (mt) {
-    AGB_MOE_DGRAD_CASE(32)
-    AGB_MOE_DGRAD_CASE(64)
-    AGB_MOE_DGRAD_CASE(128)
-  }
-#undef AGB_MOE_DGRAD_CASE
-  return failf(AGB200_EINVAL, "moe backward: row tile %d", mt);
+  agb::MoeGradRows rows{};
+  rows.r = r; rows.maps = m.g_maps; rows.gx = m.g_ex;
+  return launch_dgrad_rows<kDown>(m.dtype == AGB200_BF16, mt, p, tb, rows, k_tiles, m_tiles, s);
 }
 
 }  // namespace
@@ -703,10 +711,9 @@ namespace {
 
 size_t gate_up_decode_smem(int K) { return size_t(round_up(K / 8, 32)) * agb::kMdRows * 16 + agb::kMdRedBytes; }
 
-template <bool kBf16>
-int launch_gate_up_decode(const agb::DenseRows& src, const agb::MoeDecodeParams& p, size_t smem, int smem_optin,
-                          cudaStream_t stream) {
-  auto kern = agb::moe_decode_kernel<kBf16, true, agb::DenseRows>;
+template <bool kBf16, class Src>
+int launch_gate_up_decode(const Src& src, const agb::MoeDecodeParams& p, size_t smem, int smem_optin, cudaStream_t stream) {
+  auto kern = agb::moe_decode_kernel<kBf16, true, Src>;
   static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
   const int dev = agb::current_device_index();
   if (!attr_set_dev[dev]) {
@@ -732,19 +739,10 @@ int gate_up_auto_split(int ctas, int num_kb, int sms) {
   return best;
 }
 
-}  // namespace
-
-extern "C" {
-
-size_t agb200_w4a16_gate_up_workspace_bytes(int M, int K, int I) {
-  (void)I;
-  if (M <= 0 || K <= 0) return 0;
-  return align_up(size_t(M) * K * 2, 256);   // x gathered through the act-order permutation (GEMM path)
-}
-
-int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
-                            int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream,
-                            int kernel, int tile_m, int split_k) {
+// agb200_w4a16_gate_up_ex, and with g / u (agb200_w4a16_gate_up_saving_ex) also the rounded g and u of every row
+int gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, void* g, void* u, int M, int K,
+            int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream, int kernel, int tile_m,
+            int split_k) {
   if (!gate || !up) return failf(AGB200_EINVAL, "gate_up: null layer descriptor");
   if (M < 0 || K <= 0 || I <= 0) return failf(AGB200_EINVAL, "gate_up: M >= 0, K > 0 and I > 0 (got M=%d, K=%d, I=%d)", M, K, I);
   if (dtype != AGB200_F16 && dtype != AGB200_BF16) return failf(AGB200_EINVAL, "gate_up: dtype must be AGB200_F16 or AGB200_BF16");
@@ -759,6 +757,9 @@ int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const a
       return failf(AGB200_EINVAL, "gate_up: layer buffers must be 16-byte aligned");
   }
   if (!aligned16(x) || !aligned16(h)) return failf(AGB200_EINVAL, "gate_up: x and h must be 16-byte aligned");
+  const bool save = g != nullptr;
+  if (save && (u == nullptr || !aligned16(g) || !aligned16(u)))
+    return failf(AGB200_EINVAL, "gate_up: the saved g and u must both be given, 16-byte aligned");
   if (K % 8 != 0 || I % 32 != 0) return failf(AGB200_ENOSUP, "gate_up: K %% 8 == 0 and I %% 32 == 0 (got K=%d, I=%d)", K, I);
   if (gate->perm != up->perm)
     return failf(AGB200_ENOSUP, "gate_up: gate and up must share one act-order permutation of x (same pointer, or both NULL)");
@@ -788,6 +789,12 @@ int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const a
     agb::MoeDecodeParams p{};
     p.x = x; p.out = h; p.K = K; p.N = I; p.P = M; p.rows = K / 8; p.rows_per_group = gs / 8;
     p.rows_per_split = round_up(K / 8, 32); p.split = 1; p.tiles = I / agb::kMdTN;
+    if (save) {
+      agb::DenseRowsSave ss{};
+      static_cast<agb::DenseRows&>(ss) = src;
+      ss.g = static_cast<uint16_t*>(g); ss.u = static_cast<uint16_t*>(u);
+      return bf ? launch_gate_up_decode<true>(ss, p, dsmem, smem_optin, s) : launch_gate_up_decode<false>(ss, p, dsmem, smem_optin, s);
+    }
     return bf ? launch_gate_up_decode<true>(src, p, dsmem, smem_optin, s) : launch_gate_up_decode<false>(src, p, dsmem, smem_optin, s);
   }
 
@@ -837,13 +844,180 @@ int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const a
     if (int rc = encode_2d(encode, mp + 1, xdt, L[l]->scales, I, G, size_t(I) * 2, 64, ngr, false, "scales")) return rc;
     if (int rc = encode_2d(encode, mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qzeros, I / 8, G, size_t(I / 8) * 4, 8, ngr, false, "qzeros")) return rc;
   }
+  if (save) {
+    agb::DenseGemmRowsSave ss{};
+    static_cast<agb::DenseGemmRows&>(ss) = src;
+    ss.g = static_cast<uint16_t*>(g); ss.u = static_cast<uint16_t*>(u);
+    return launch_gemm<true>(bf, mt, p, tx, ss, n_tiles, m_tiles, s);
+  }
   return launch_gemm<true>(bf, mt, p, tx, src, n_tiles, m_tiles, s);
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t agb200_w4a16_gate_up_workspace_bytes(int M, int K, int I) {
+  (void)I;
+  if (M <= 0 || K <= 0) return 0;
+  return align_up(size_t(M) * K * 2, 256);   // x gathered through the act-order permutation (GEMM path)
+}
+
+int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
+                            int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream,
+                            int kernel, int tile_m, int split_k) {
+  return gate_up(x, gate, up, h, nullptr, nullptr, M, K, I, group_size, dtype, workspace, workspace_bytes, stream, kernel,
+                 tile_m, split_k);
 }
 
 int agb200_w4a16_gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, int M, int K,
                          int I, int group_size, int dtype, void* workspace, size_t workspace_bytes, void* stream) {
   return agb200_w4a16_gate_up_ex(x, gate, up, h, M, K, I, group_size, dtype, workspace, workspace_bytes, stream,
                                  AGB200_GATE_UP_AUTO, 0, 0);
+}
+
+int agb200_w4a16_gate_up_saving_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, void* g,
+                                   void* u, int M, int K, int I, int group_size, int dtype, void* workspace,
+                                   size_t workspace_bytes, void* stream, int kernel, int tile_m, int split_k) {
+  if (M > 0 && (g == nullptr || u == nullptr)) return failf(AGB200_EINVAL, "gate_up_saving: null g or u");
+  return gate_up(x, gate, up, h, g, u, M, K, I, group_size, dtype, workspace, workspace_bytes, stream, kernel, tile_m,
+                 split_k);
+}
+
+int agb200_w4a16_gate_up_saving(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, void* g,
+                                void* u, int M, int K, int I, int group_size, int dtype, void* workspace,
+                                size_t workspace_bytes, void* stream) {
+  return agb200_w4a16_gate_up_saving_ex(x, gate, up, h, g, u, M, K, I, group_size, dtype, workspace, workspace_bytes, stream,
+                                        AGB200_GATE_UP_AUTO, 0, 0);
+}
+
+}  // extern "C"
+
+// ------------------------------------------------------------------------------------------------ dense MLP backward
+// dx = d/dx of down(silu(gate x) * up x) from dy and the g, u the saving gate/up kept (agb200_w4a16_mlp_backward): the
+// grouped dgrad kernel over the M rows (DenseGradRows), down stage -> [dg | du] in the workspace, gate/up stage -> dx
+// (the row-sorted order of an act-order gate / up pair goes through the workspace and unpermute_columns_kernel).
+namespace {
+
+struct MlpBwdLayout {
+  size_t dgu, dxs, total;
+};
+
+MlpBwdLayout mlp_bwd_layout(int M, int H, int I) {
+  MlpBwdLayout b{};
+  b.dgu = 0;
+  b.dxs = align_up(size_t(M) * 2 * I * 2, 256);
+  b.total = b.dxs + align_up(size_t(M) * H * 2, 256);
+  return b;
+}
+
+// the dgrad tensor maps of one layer (K rows, N columns) at mp[0..2]: packed words, scales, zeros
+int encode_dgrad_layer(agb::EncodeTiledFn encode, CUtensorMap* mp, const agb200_moe_layer* L, int K, int N, int gs,
+                       CUtensorMapDataType sdt) {
+  const int G = (K + gs - 1) / gs;
+  if (int rc = encode_2d(encode, mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "qweight")) return rc;
+  if (int rc = encode_2d(encode, mp + 1, sdt, L->scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "scales")) return rc;
+  return encode_2d(encode, mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "qzeros");
+}
+
+}  // namespace
+
+extern "C" {
+
+size_t agb200_w4a16_mlp_backward_workspace_bytes(int M, int H, int I) {
+  if (M < 0 || H <= 0 || I <= 0) return 0;
+  return mlp_bwd_layout(M, H, I).total;
+}
+
+int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, const agb200_moe_layer* up,
+                                 const agb200_moe_layer* down, const void* g, const void* u, void* dx, int M, int H, int I,
+                                 int group_size_13, int group_size_2, int dtype, void* workspace, size_t workspace_bytes,
+                                 void* stream, int tile_m, int split_k) {
+  if (!gate || !up || !down) return failf(AGB200_EINVAL, "mlp_backward: null layer descriptor");
+  if (M < 0 || H <= 0 || I <= 0) return failf(AGB200_EINVAL, "mlp_backward: M >= 0, H > 0 and I > 0 (got M=%d, H=%d, I=%d)", M, H, I);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16) return failf(AGB200_EINVAL, "mlp_backward: dtype must be AGB200_F16 or AGB200_BF16");
+  if (M == 0) return 0;
+  if (!dy || !g || !u || !dx || !workspace) return failf(AGB200_EINVAL, "mlp_backward: null pointer argument");
+  for (const agb200_moe_layer* L : {gate, up, down}) {
+    if (!L->qweight || !L->qzeros || !L->scales) return failf(AGB200_EINVAL, "mlp_backward: null qweight/qzeros/scales");
+    if (!aligned16(L->qweight) || !aligned16(L->qzeros) || !aligned16(L->scales))
+      return failf(AGB200_EINVAL, "mlp_backward: layer buffers must be 16-byte aligned");
+  }
+  if (!aligned16(dy) || !aligned16(g) || !aligned16(u) || !aligned16(dx) || (reinterpret_cast<uintptr_t>(workspace) & 255u))
+    return failf(AGB200_EINVAL, "mlp_backward: dy, g, u and dx must be 16-byte aligned, the workspace 256-byte aligned");
+  if (dy == dx) return failf(AGB200_EINVAL, "mlp_backward: dy and dx must not alias");
+  if (gate->perm != up->perm)
+    return failf(AGB200_ENOSUP, "mlp_backward: gate and up must share one act-order permutation of x (same pointer, or both NULL)");
+  const int gs13 = group_size_13 == -1 ? H : group_size_13, gs2 = group_size_2 == -1 ? I : group_size_2;
+  if (gs13 <= 0 || gs2 <= 0) return failf(AGB200_EINVAL, "mlp_backward: group sizes must be positive or -1");
+  // the gate/up stage switches from w1 to w3 at n = I, which must fall on a 64-n stage boundary
+  if (H % 8 != 0 || I % 64 != 0 || !agb::dgrad_tc_supported(H, I, gs13) || !agb::dgrad_tc_supported(I, H, gs2))
+    return failf(AGB200_ENOSUP, "mlp_backward: needs H %% 8 == 0, I %% 64 == 0 and the tensor-core dgrad for both stages "
+                 "(got H=%d, I=%d, group sizes %d / %d)", H, I, gs13, gs2);
+  const size_t need = agb200_w4a16_mlp_backward_workspace_bytes(M, H, I);
+  if (workspace_bytes < need) return failf(AGB200_EWORKSPACE, "mlp_backward: workspace needs %zu bytes (got %zu)", need, workspace_bytes);
+  int mt = tile_m;
+  if (mt == 0) mt = M <= 32 ? 32 : M <= 64 ? 64 : 128;
+  if (mt != 32 && mt != 64 && mt != 128) return failf(AGB200_EINVAL, "mlp_backward: row tile must be 32/64/128 (got %d)", mt);
+  if (split_k != 0 && split_k != 1 && split_k != 2 && split_k != 4 && split_k != 8)
+    return failf(AGB200_EINVAL, "mlp_backward: split must be 1/2/4/8 (got %d)", split_k);
+  const int m_tiles = (M + mt - 1) / mt;
+  if (m_tiles > 65535) return failf(AGB200_ENOSUP, "mlp_backward: %d row tiles exceed the grid limit", m_tiles);
+  int dev = 0, sms = 0, smem_optin = 0;
+  MOE_CUDA(cudaGetDevice(&dev));
+  MOE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  MOE_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  if (gate->perm != nullptr && size_t(H) * 2 > static_cast<size_t>(smem_optin))
+    return failf(AGB200_ENOSUP, "mlp_backward: act-order row of H=%d does not fit in shared memory", H);
+  agb::EncodeTiledFn encode = agb::get_encode_fn();
+  if (encode == nullptr) return failf(AGB200_ECUDA, "mlp_backward: cuTensorMapEncodeTiled entry point not available");
+  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "mlp_backward: no CUDA context: %s", cudaGetErrorString(e));
+  const bool bf = dtype == AGB200_BF16;
+  const CUtensorMapDataType t16 = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const MlpBwdLayout b = mlp_bwd_layout(M, H, I);
+  unsigned char* ws = static_cast<unsigned char*>(workspace);
+  uint16_t* dgu = reinterpret_cast<uint16_t*>(ws + b.dgu);
+  uint16_t* dxs = gate->perm != nullptr ? reinterpret_cast<uint16_t*>(ws + b.dxs) : static_cast<uint16_t*>(dx);
+
+  agb::DenseGradRows rows{};
+  rows.M = M;
+  rows.perm2_ = down->perm;
+  if (int rc = encode_dgrad_layer(encode, rows.maps + 0, gate, H, I, gs13, t16)) return rc;
+  if (int rc = encode_dgrad_layer(encode, rows.maps + 3, up, H, I, gs13, t16)) return rc;
+  if (int rc = encode_dgrad_layer(encode, rows.maps + 6, down, I, H, gs2, t16)) return rc;
+  CUtensorMap t_dy, t_dgu;
+  if (int rc = encode_2d(encode, &t_dy, t16, dy, H, M, size_t(H) * 2, agb::kDgBN, mt, true, "dy")) return rc;
+  if (int rc = encode_2d(encode, &t_dgu, t16, dgu, 2 * I, M, size_t(2 * I) * 2, agb::kDgBN, mt, true, "dg | du")) return rc;
+
+  // split over n by the wave model of the dense dgrad (no host synchronisation, no atomics)
+  auto plan = [&](agb::MoeDgradParams& p, int k_tiles) {
+    int split = split_k != 0 ? split_k : agb::gemm_auto_split(mt, k_tiles * m_tiles, p.num_nb, sms);
+    while (split > 1 && split > p.num_nb) split /= 2;
+    p.split = split;
+    p.nb_per_split = (p.num_nb + split - 1) / split;
+  };
+  agb::MoeDgradParams p{};
+  p.out = dgu; p.K = I; p.N = H; p.I = I; p.group_size = gs2; p.num_nb = (H + agb::kDgBN - 1) / agb::kDgBN;
+  p.g = static_cast<const uint16_t*>(g); p.u = static_cast<const uint16_t*>(u);
+  int k_tiles = (I + agb::kDgBK - 1) / agb::kDgBK;
+  plan(p, k_tiles);
+  if (int rc = launch_dgrad_rows<true>(bf, mt, p, t_dy, rows, k_tiles, m_tiles, s)) return rc;
+  p.out = dxs; p.K = H; p.N = 2 * I; p.group_size = gs13; p.num_nb = 2 * I / agb::kDgBN; p.g = nullptr; p.u = nullptr;
+  k_tiles = (H + agb::kDgBK - 1) / agb::kDgBK;
+  plan(p, k_tiles);
+  if (int rc = launch_dgrad_rows<false>(bf, mt, p, t_dgu, rows, k_tiles, m_tiles, s)) return rc;
+  if (gate->perm != nullptr)
+    return agb_internal_unpermute_columns(dxs, gate->perm, dx, M, H, s);
+  return 0;
+}
+
+int agb200_w4a16_mlp_backward(const void* dy, const agb200_moe_layer* gate, const agb200_moe_layer* up,
+                              const agb200_moe_layer* down, const void* g, const void* u, void* dx, int M, int H, int I,
+                              int group_size_13, int group_size_2, int dtype, void* workspace, size_t workspace_bytes,
+                              void* stream) {
+  return agb200_w4a16_mlp_backward_ex(dy, gate, up, down, g, u, dx, M, H, I, group_size_13, group_size_2, dtype, workspace,
+                                      workspace_bytes, stream, 0, 0);
 }
 
 }  // extern "C"

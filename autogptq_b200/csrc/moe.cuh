@@ -15,7 +15,10 @@
 // table; DenseRows / DenseGemmRows run one gate/up pair over all M rows of x (agb200_w4a16_gate_up, a dense MLP), the
 // GEMM then with split-K over a thread-block cluster whose partial tiles are reduced through DSMEM before silu * mul.
 // MoeRoutedSave (agb200_moe_forward_saving) is MoeRouted whose gate/up epilogue also keeps g and u for the backward
-// (moe_dgrad.cuh); the other sources compile to the code they had before it existed.
+// (moe_dgrad.cuh); DenseRowsSave / DenseGemmRowsSave (agb200_w4a16_gate_up_saving) do the same for a dense MLP, the GEMM
+// also on its split-K path (the rank that forms h after the DSMEM reduction stores g and u).  The source decides which
+// saved row a position goes to (save_row / gemm_save_row: the pair id for routed rows, the row itself for dense rows);
+// the other sources compile to the code they had before saving existed.
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda.h>
@@ -98,6 +101,11 @@ struct MoeRoutedSave : MoeRouted {
   static constexpr bool kSave = true;
   uint16_t* g;                  // [T * k, I]
   uint16_t* u;                  // [T * k, I]
+  // saved row of h row `pos` (decode path) and of row ml of the GEMM tile (e, m0): the pair id
+  __device__ __forceinline__ int save_row(int pos) const { return r.pairs[pos]; }
+  __device__ __forceinline__ int gemm_save_row(int e, int m0, int ml) const {
+    return r.pairs[r.offsets[e] + (m0 - r.pad_off[e]) + ml];
+  }
 };
 
 struct DenseRows {
@@ -125,7 +133,23 @@ struct DenseGemmRows : DenseRows {
   __device__ __forceinline__ const CUtensorMap* gemm_maps(int, int layer) const { return maps + layer * 3; }
 };
 
-// store_gate_up that also keeps the rounded g and u (MoeRoutedSave) at g_out / u_out
+// The dense rows of a forward that keeps what the dense MLP backward reads (agb200_w4a16_gate_up_saving): g and u (bias
+// added, rounded) of row m at row m, in I's natural column order.
+struct DenseRowsSave : DenseRows {
+  static constexpr bool kSave = true;
+  uint16_t* g;                  // [M, I]
+  uint16_t* u;                  // [M, I]
+  __device__ __forceinline__ int save_row(int pos) const { return pos; }
+};
+
+struct DenseGemmRowsSave : DenseGemmRows {
+  static constexpr bool kSave = true;
+  uint16_t* g;                  // [M, I]
+  uint16_t* u;                  // [M, I]
+  __device__ __forceinline__ int gemm_save_row(int, int m0, int ml) const { return m0 + ml; }
+};
+
+// store_gate_up that also keeps the rounded g and u (the saving work sources) at g_out / u_out
 template <bool kBf16>
 __device__ __forceinline__ void store_gate_up_saving(uint16_t* out, float gv, float uv, const void* bias_g, const void* bias_u,
                                                      int nn, uint16_t* g_out, uint16_t* u_out) {
@@ -426,7 +450,7 @@ moe_decode_kernel(const MoeDecodeParams p, const __grid_constant__ Src src) {
             const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
             uint16_t* hp = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(pos) * p.N + dst;
             if constexpr (Src::kSave) {
-              const size_t at = static_cast<size_t>(src.r.pairs[pos]) * p.N + dst;
+              const size_t at = static_cast<size_t>(src.save_row(pos)) * p.N + dst;
               store_gate_up_saving<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn, src.g + at, src.u + at);
             } else {
               store_gate_up<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn);
@@ -655,8 +679,7 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
           if (ml < m_valid && nn < p.N) {
             const int dst = X.inv2 != nullptr ? X.inv2[nn] : nn;
             if constexpr (Src::kSave) {
-              const int pair = src.r.pairs[src.r.offsets[e] + (m0 - src.r.pad_off[e]) + ml];
-              const size_t at = static_cast<size_t>(pair) * p.N + dst;
+              const size_t at = static_cast<size_t>(src.gemm_save_row(e, m0, ml)) * p.N + dst;
               store_gate_up_saving<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + dst, stage_f32[ml * kGemmLd + nl],
                                           stage_f32[ml * kGemmLd + kHalf + nl], X.bias[0], X.bias[1], nn, src.g + at, src.u + at);
             } else {
@@ -705,7 +728,13 @@ moe_gemm_kernel(const MoeGemmParams p, const __grid_constant__ CUtensorMap tmap_
             float gv = 0.f, uv = 0.f;
 #pragma unroll
             for (int r = 0; r < 8; ++r) { gv += gr[r]; uv += ur[r]; }
-            store_gate_up<kBf16>(yp + static_cast<size_t>(m0 + ml) * p.N + nn, gv, uv, X.bias[0], X.bias[1], nn);
+            uint16_t* hp = yp + static_cast<size_t>(m0 + ml) * p.N + nn;
+            if constexpr (Src::kSave) {
+              const size_t at = static_cast<size_t>(src.gemm_save_row(e, m0, ml)) * p.N + nn;
+              store_gate_up_saving<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn, src.g + at, src.u + at);
+            } else {
+              store_gate_up<kBf16>(hp, gv, uv, X.bias[0], X.bias[1], nn);
+            }
           }
         }
       }

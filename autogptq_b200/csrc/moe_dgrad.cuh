@@ -15,6 +15,8 @@
 // exit), the weight, scale and zero tensor maps of the tile's expert from the grad plan, A expanded straight from the
 // checkpoint layout, split over n by a cluster with the DSMEM reduction in rank order.  No atomics: repeated calls are
 // bit-identical.  No host synchronisation.
+// The dense MLP backward (agb200_w4a16_mlp_backward) runs the same two stages over the M rows of one MLP (row source
+// DenseGradRows): dy W2^T -> [dg | du], then [dg | du] [W1 | W3]^T -> dx, rounded once.
 #pragma once
 #include <cooperative_groups.h>
 #include <cuda.h>
@@ -36,14 +38,58 @@ struct MoeGradExpertDev {
 };
 
 struct MoeDgradParams {
-  void* out;                // down: [dg | du] 16-bit [rows, 2 I]; gate/up: fp32 dx_pair [rows, H]
+  void* out;                // down: [dg | du] 16-bit [rows, 2 I]; gate/up: fp32 dx_pair [rows, H] (dense: 16-bit dx)
   int K, N, I;              // down: K = I, N = H; gate/up: K = H, N = 2 I
   int group_size;
-  int num_nb;               // N / 64
+  int num_nb;               // N / 64 (dense down stage: ceil(H / 64))
   int nb_per_split;
   int split;
-  const uint16_t* g;        // saved g, u [T * k, I] (pair-id rows, h's column order); down only
+  const uint16_t* g;        // saved g, u (the row source's saved rows and column order, see there); down only
   const uint16_t* u;
+};
+
+// Row sources of moe_dgrad_kernel (as the forward's kernels take work sources).  A source maps blockIdx.y to a row tile
+// (expert e, first row m0, valid rows), names the tile's tensor maps ([w1, w3, w2][weights, scales, zeros], dgrad
+// boxes), the saved g / u row of a tile row and w2's permutation.
+// MoeGradRows: the routed pairs of agb200_moe_backward.  Rows are the routing table's padded rows; saved g, u are in
+// pair-id rows and w2's sorted column order (the order h was written in), so the down stage reads them at sorted row kk;
+// the gate/up stage leaves dx_pair unrounded in fp32 for the slot sum.
+struct MoeGradRows {
+  static constexpr bool kDense = false;
+  MoeRoute r;
+  const CUtensorMap* maps;            // grad plan: [E][w1, w3, w2][weights, scales, zeros]
+  const MoeGradExpertDev* gx;
+  __device__ __forceinline__ bool tile(int t, int mt, int& e, int& m0, int& m_valid) const {
+    if (t >= r.meta[1]) return false;       // every CTA of a cluster has the same tile: they leave together
+    e = r.tile_e[t];
+    m0 = r.tile_m0[t];
+    m_valid = min(mt, r.counts[e] - (m0 - r.pad_off[e]));
+    return true;
+  }
+  __device__ __forceinline__ const CUtensorMap* layer_maps(int e) const { return maps + e * 9; }
+  __device__ __forceinline__ int saved_row(int e, int m0, int ml) const { return r.pairs[r.offsets[e] + (m0 - r.pad_off[e]) + ml]; }
+  __device__ __forceinline__ int saved_col(int, int kk) const { return kk; }
+  __device__ __forceinline__ const int32_t* perm2(int e) const { return gx[e].perm2; }
+};
+
+// DenseGradRows: the M rows of a dense MLP (agb200_w4a16_mlp_backward), tile t = rows [t MT, t MT + MT).  The tensor
+// maps are kernel parameters.  Saved g, u are in I's natural column order, so the down stage reads sorted row kk of an
+// act-order w2 at column perm2[kk], where it also writes dg and du; the gate/up stage rounds dx once to the dtype.
+struct DenseGradRows {
+  static constexpr bool kDense = true;
+  int M;
+  const int32_t* perm2_;              // w2's act-order permutation or null
+  CUtensorMap maps[9];                // [w1, w3, w2][weights, scales, zeros]
+  __device__ __forceinline__ bool tile(int t, int mt, int& e, int& m0, int& m_valid) const {
+    e = 0;
+    m0 = t * mt;
+    m_valid = min(mt, M - m0);
+    return true;                      // the grid has exactly ceil(M / MT) row tiles
+  }
+  __device__ __forceinline__ const CUtensorMap* layer_maps(int) const { return maps; }
+  __device__ __forceinline__ int saved_row(int, int m0, int ml) const { return m0 + ml; }
+  __device__ __forceinline__ int saved_col(int, int kk) const { return perm2_ != nullptr ? perm2_[kk] : kk; }
+  __device__ __forceinline__ const int32_t* perm2(int) const { return perm2_; }
 };
 
 // dg = round(dh * u * silu'(g)), du = round(dh * round(silu(g))) from the saved 16-bit g, u; silu(g) is formed exactly as
@@ -58,18 +104,14 @@ __device__ __forceinline__ void silu_mul_backward(float dh, uint16_t g16, uint16
   du = float_to_elt<kBf16>(dh * sg);
 }
 
-template <int kMT, bool kBf16, bool kDown>
+template <int kMT, bool kBf16, bool kDown, class Rows>
 __global__ void __launch_bounds__(kGemmThreads, 1)
-moe_dgrad_kernel(const MoeDgradParams p, const __grid_constant__ CUtensorMap tmap_b, const MoeRoute r,
-                 const CUtensorMap* __restrict__ maps, const MoeGradExpertDev* __restrict__ gx) {
+moe_dgrad_kernel(const MoeDgradParams p, const __grid_constant__ CUtensorMap tmap_b, const __grid_constant__ Rows rows) {
   using Smem = DgradSmem<kMT>;
   constexpr int kStages = Smem::kStages;
-  const int tile = blockIdx.y;
-  if (tile >= r.meta[1]) return;                 // every CTA of a cluster has the same tile: they leave together
-  const int e = r.tile_e[tile];
-  const int m0 = r.tile_m0[tile];
-  const int m_valid = min(kMT, r.counts[e] - (m0 - r.pad_off[e]));
-  const CUtensorMap* emaps = maps + e * 9;
+  int e, m0, m_valid;
+  if (!rows.tile(blockIdx.y, kMT, e, m0, m_valid)) return;
+  const CUtensorMap* emaps = rows.layer_maps(e);
 
   extern __shared__ unsigned char smem_dyn[];
   const uint32_t smem_base = (smem_u32(smem_dyn) + 1023u) & ~1023u;
@@ -102,16 +144,20 @@ moe_dgrad_kernel(const MoeDgradParams p, const __grid_constant__ CUtensorMap tma
   auto store = [&](int ml, int kl, float v) {
     if (ml >= m_valid) return;
     const int row = m0 + ml, kk = k0 + kl;
+    if constexpr (Rows::kDense) {
+      if (kk >= p.K) return;                     // K = I or H need not fill the last 128-k tile
+    }
     if constexpr (kDown) {
-      const int pair = r.pairs[r.offsets[e] + (m0 - r.pad_off[e]) + ml];
-      const size_t at = static_cast<size_t>(pair) * p.I + kk;
+      const size_t at = static_cast<size_t>(rows.saved_row(e, m0, ml)) * p.I + rows.saved_col(e, kk);
       uint16_t dg, du;
       silu_mul_backward<kBf16>(v, p.g[at], p.u[at], dg, du);
-      const int32_t* perm2 = gx[e].perm2;
+      const int32_t* perm2 = rows.perm2(e);
       const int col = perm2 != nullptr ? perm2[kk] : kk;
       uint16_t* o = reinterpret_cast<uint16_t*>(p.out) + static_cast<size_t>(row) * (2 * p.I);
       o[col] = dg;
       o[p.I + col] = du;
+    } else if constexpr (Rows::kDense) {
+      reinterpret_cast<uint16_t*>(p.out)[static_cast<size_t>(row) * p.K + kk] = float_to_elt<kBf16>(v);
     } else {
       reinterpret_cast<float*>(p.out)[static_cast<size_t>(row) * p.K + kk] = v;
     }

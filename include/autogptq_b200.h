@@ -410,6 +410,48 @@ int agb200_w4a16_gate_up_ex(const void* x, const agb200_moe_layer* gate, const a
 size_t agb200_w4a16_gate_up_workspace_bytes(int M, int K, int I);
 
 /*
+ * Backward of a dense MLP (additions to ABI v10):  y = down(h),  h = round(round(silu(g)) * u)  as above, with the
+ * three 4-bit layers frozen.
+ *
+ *   agb200_w4a16_gate_up_saving[_ex]  agb200_w4a16_gate_up[_ex] (same h, bit for bit, same kernels and arguments) that
+ *                                     also writes g and u, [M, I] of `dtype` each (bias added, rounded: the values
+ *                                     silu * mul consumed), in I's natural column order.  16-byte aligned device memory.
+ *   agb200_w4a16_mlp_backward[_ex]    dx [M, H] of `dtype` in x's column order, from dy [M, H] (= dL/dy) and that g, u.
+ *
+ * Rounding points ("round" = to `dtype`; every sum fp32 in a fixed order, no atomics, so repeated calls are bit-identical):
+ *   dh      = dy * W2^T (W rounded once as s * (q - z)), unrounded
+ *   dg, du  = round(dh * u * silu'(g)), round(dh * round(silu(g))),  silu'(g) = s(g) (1 + g (1 - s(g)))
+ *   dx      = round(dg * W1^T + du * W3^T), ONE fp32 sum over the 2 I terms, one rounding
+ * so dh, dg and du never round-trip through autograd's separate 16-bit tensors.
+ *
+ *   gate, up, down  layer descriptors as for agb200_w4a16_gate_up (qweight_tc and bias are not read: dgrad expands the
+ *                   checkpoint layout, and biases have no input gradient).  gate and up: K = H, N = I, group_size_13, one
+ *                   shared perm pointer (or none); down: K = I, N = H, group_size_2, its own perm (or none).  -1 = one group.
+ *   workspace       DEVICE scratch of agb200_w4a16_mlp_backward_workspace_bytes(M, H, I) bytes, 256-byte aligned: the
+ *                   [dg | du] rows [M, 2 I] and, for an act-order gate / up pair, the row-sorted dx [M, H].
+ *   tile_m, split_k (_ex; tests / benchmarks) row tile 32|64|128 and n splits 1|2|4|8 of both stages, 0 = auto.
+ * Constraints (else AGB200_ENOSUP): H % 8 == 0, I % 64 == 0 (the gate/up stage switches from W1 to W3 at n = I on a
+ * 64-n stage boundary), and the tensor-core dgrad for both stages: H % 32 == 0, I % 32 == 0, each group size >= 32 and a
+ * multiple of 16, or one group.  M = 0 does nothing.  Explicit stream, no host synchronisation: capturable in a CUDA
+ * graph together with the saving forward.
+ */
+int agb200_w4a16_gate_up_saving(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, void* g,
+                                void* u, int M, int K, int I, int group_size, int dtype, void* workspace,
+                                size_t workspace_bytes, void* stream);
+int agb200_w4a16_gate_up_saving_ex(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer* up, void* h, void* g,
+                                   void* u, int M, int K, int I, int group_size, int dtype, void* workspace,
+                                   size_t workspace_bytes, void* stream, int kernel, int tile_m, int split_k);
+size_t agb200_w4a16_mlp_backward_workspace_bytes(int M, int H, int I);
+int agb200_w4a16_mlp_backward(const void* dy, const agb200_moe_layer* gate, const agb200_moe_layer* up,
+                              const agb200_moe_layer* down, const void* g, const void* u, void* dx, int M, int H, int I,
+                              int group_size_13, int group_size_2, int dtype, void* workspace, size_t workspace_bytes,
+                              void* stream);
+int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, const agb200_moe_layer* up,
+                                 const agb200_moe_layer* down, const void* g, const void* u, void* dx, int M, int H, int I,
+                                 int group_size_13, int group_size_2, int dtype, void* workspace, size_t workspace_bytes,
+                                 void* stream, int tile_m, int split_k);
+
+/*
  * GPTQ quantiser (ABI v6): makes the packed 4-bit layers the entry points above run, on the GPU.
  *
  * Hessian update: H = alpha * H + beta * x^T x, x [T, K] of `dtype` (row-major), H [K, K] fp32 (DEVICE).
