@@ -404,6 +404,9 @@ w4a16_chain_kernel(const ChainParams p) {
     ChWalk la{};                                       // next slot to prefetch, la_n slots past the issue cursor
     int la_n = 0;
     bool la_end = false;                               // the lookahead cursor has walked past the last stage
+    // Every weight byte is read once per token and the token's 3.5 GB pass through a 50 MB L2: the lines are marked
+    // evict-first, so that they do not push out the tagged words of x that every CTA polls
+    const uint64_t wpol = l2_policy_evict_first();
     long long pr_t0 = kProf ? clock64() : 0, pr_full = 0, pr_cap = 0, pr_issued = 0, pr_pref = 0;
     for (int s = 0; s < p.n_stages; ++s) {
       if (s + 1 < p.n_stages) ch_copy_desc_load(p.stages + s + 1, lane, dr);     // latency hidden behind this stage's loads
@@ -446,7 +449,7 @@ w4a16_chain_kernel(const ChainParams p) {
           if constexpr (kProf) ++pr_issued;
           const uint32_t dst = smem_base + slot * kChSlotBytes;
           ch_walk_boxes(w, p.maps, [&](int b, const CUtensorMap* m, int c0, int c1) {
-            tma_load_2d(dst + (b == 0 ? 0u : b == 1 ? uint32_t(kChWBytes) : uint32_t(kChWBytes + kChSBytes)), m, c0, c1, fb);
+            tma_load_2d_hint(dst + (b == 0 ? 0u : b == 1 ? uint32_t(kChWBytes) : uint32_t(kChWBytes + kChSBytes)), m, c0, c1, fb, wpol);
           });
           if (++slot == S) { slot = 0; ++lap; }
         }

@@ -57,6 +57,16 @@ __device__ __forceinline__ void tma_load_2d(uint32_t smem_dst, const CUtensorMap
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
                ::"r"(smem_dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1) : "memory");
 }
+// The same load with an L2 eviction policy (createpolicy) for the lines it brings in
+__device__ __forceinline__ void tma_load_2d_hint(uint32_t smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar, uint64_t policy) {
+  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.L2::cache_hint [%0], [%1, {%3, %4}], [%2], %5;"
+               ::"r"(smem_dst), "l"(tmap), "r"(bar), "r"(c0), "r"(c1), "l"(policy) : "memory");
+}
+__device__ __forceinline__ uint64_t l2_policy_evict_first() {
+  uint64_t p;
+  asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
+  return p;
+}
 __device__ __forceinline__ void tma_load_2d_mcast(uint32_t smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar, uint16_t mask) {
   asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
                ::"r"(smem_dst), "l"(tmap), "r"(bar), "h"(mask), "r"(c0), "r"(c1) : "memory");
