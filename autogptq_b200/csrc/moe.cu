@@ -112,10 +112,12 @@ int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType d
   return 0;
 }
 
+// The attribute is the kernel's, shared by every plan in the process: it is raised to the device's opt-in limit, never
+// set to this plan's need, so creating a plan whose H or I is smaller cannot turn an earlier plan's launches down.
 template <bool kBf16, bool kGateUp, class Src = agb::MoeRouted>
-int decode_setup(size_t smem, int& occ) {
+int decode_setup(size_t smem, int smem_optin, int& occ) {
   auto kern = agb::moe_decode_kernel<kBf16, kGateUp, Src>;
-  MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, static_cast<int>(smem)));
+  MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
   MOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, agb::kMdThreads, smem));
   if (occ < 1) return failf(AGB200_ENOSUP, "moe: decode kernel with %zu B of shared memory does not fit an SM", smem);
   return 0;
@@ -277,12 +279,12 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
   m->magic = kMagic; m->device = dev; m->E = E; m->H = H; m->I = I; m->gs13 = gs13; m->gs2 = gs2; m->dtype = dtype;
   m->has_tc = has_tc; m->d_ex = d_ex; m->d_maps = d_maps; m->sms = sms;
   m->up_rps = up_rps; m->down_rps = down_rps; m->down_split = down_split; m->up_smem = up_smem; m->down_smem = down_smem;
-  int rc = dtype == AGB200_BF16 ? decode_setup<true, true>(up_smem, m->up_occ) : decode_setup<false, true>(up_smem, m->up_occ);
-  if (rc == 0) rc = dtype == AGB200_BF16 ? decode_setup<true, false>(down_smem, m->down_occ) : decode_setup<false, false>(down_smem, m->down_occ);
+  int rc = dtype == AGB200_BF16 ? decode_setup<true, true>(up_smem, smem_optin, m->up_occ) : decode_setup<false, true>(up_smem, smem_optin, m->up_occ);
+  if (rc == 0) rc = dtype == AGB200_BF16 ? decode_setup<true, false>(down_smem, smem_optin, m->down_occ) : decode_setup<false, false>(down_smem, smem_optin, m->down_occ);
   int save_occ = 0;   // the saving gate/up kernel (agb200_moe_forward_saving) runs with the grid of the plain one
   if (rc == 0)
-    rc = dtype == AGB200_BF16 ? decode_setup<true, true, agb::MoeRoutedSave>(up_smem, save_occ)
-                              : decode_setup<false, true, agb::MoeRoutedSave>(up_smem, save_occ);
+    rc = dtype == AGB200_BF16 ? decode_setup<true, true, agb::MoeRoutedSave>(up_smem, smem_optin, save_occ)
+                              : decode_setup<false, true, agb::MoeRoutedSave>(up_smem, smem_optin, save_occ);
   if (rc != 0) { delete m; return rc; }
 
   auto cleanup_fail = [&](cudaError_t e, const char* what) {
