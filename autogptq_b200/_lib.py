@@ -16,7 +16,8 @@ ABI_VERSION = 10
 F16, BF16 = 0, 1
 ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
-CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS = 0, 1, 2
+CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS, CHAIN_X_RMSNORM, CHAIN_X_ADD_RMSNORM = 0, 1, 2, 3, 4
+CHAIN_NORM_MAX_K = 16384
 CHAIN_DEBUG_NO_DEPS, CHAIN_DEBUG_NO_MATH = 1, 2
 PEER_HANDLE_BYTES = 64
 KERNEL_AUTO, KERNEL_GEMV, KERNEL_GEMM, KERNEL_SKINNY, KERNEL_IMMA = 0, 1, 2, 3, 6
@@ -61,6 +62,8 @@ def _declare(lib):
         "agb200_chain_plan_bytes": (S, [P, I, I]),
         "agb200_chain_parts_bytes": (S, [I, I, I]),
         "agb200_chain_create": (I, [P, I, I, I, P, S, P]),
+        "agb200_chain_plan_bytes_norm": (S, [P, P, I, I]),
+        "agb200_chain_create_norm": (I, [P, P, I, I, I, P, S, P]),
         "agb200_chain_forward": (I, [P, I, P]),
         "agb200_chain_destroy": (I, [P]),
         "agb200_chain_info": (I, [P, P, P, P]),

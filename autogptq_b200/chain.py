@@ -18,14 +18,16 @@ layers, and every layer is its own launch (``exllamav2/cuda/q_gemm.cu:47,85``).
 from __future__ import annotations
 
 import ctypes
-from ctypes import c_int32, c_int64, c_void_p
+from ctypes import c_float, c_int32, c_int64, c_void_p
 
 import torch
 
 from . import _lib
 from .qlinear import _DTYPE_CODE, QuantLinear
 
-_X_MODES = {"plain": _lib.CHAIN_X_PLAIN, "silu_mul": _lib.CHAIN_X_SILU_MUL, "sum_parts": _lib.CHAIN_X_SUM_PARTS}
+_X_MODES = {"plain": _lib.CHAIN_X_PLAIN, "silu_mul": _lib.CHAIN_X_SILU_MUL, "sum_parts": _lib.CHAIN_X_SUM_PARTS,
+            "rmsnorm": _lib.CHAIN_X_RMSNORM, "add_rmsnorm": _lib.CHAIN_X_ADD_RMSNORM}
+_NORM_MODES = (_lib.CHAIN_X_RMSNORM, _lib.CHAIN_X_ADD_RMSNORM)
 
 
 class _CLayer(ctypes.Structure):
@@ -37,6 +39,38 @@ class _CStage(ctypes.Structure):
     _fields_ = [("x", c_void_p), ("x2", c_void_p), ("perm", c_void_p), ("K", c_int32), ("group_size", c_int32),
                 ("n_layers", c_int32), ("x_mode", c_int32), ("x_parts", c_int32), ("reserved", c_int32),
                 ("x_part_stride", c_int64), ("layer", _CLayer * 4)]
+
+
+class _CNorm(ctypes.Structure):
+    _fields_ = [("weight", c_void_p), ("residual_out", c_void_p), ("eps", c_float), ("reserved", c_int32)]
+
+
+def check_norm_args(x_mode: str, M: int, K: int, dtype: torch.dtype, device, x2, norm_weight, norm_eps):
+    """Validate the norm keywords of ``DecodeChain.stage``; raises ValueError / NotImplementedError naming the problem."""
+    norm = x_mode in ("rmsnorm", "add_rmsnorm")
+    if not norm:
+        if norm_weight is not None:
+            raise ValueError(f"norm_weight is only used by x_mode='rmsnorm' or 'add_rmsnorm' (got x_mode={x_mode!r})")
+        return
+    if norm_weight is None:
+        raise ValueError(f"x_mode={x_mode!r} needs norm_weight (the RMSNorm weight, a [{K}] tensor)")
+    if not isinstance(norm_weight, torch.Tensor) or tuple(norm_weight.shape) != (K,):
+        raise ValueError(f"norm_weight has shape {tuple(getattr(norm_weight, 'shape', ()))}, expected ({K},)")
+    if norm_weight.dtype != dtype:
+        raise ValueError(f"norm_weight has dtype {norm_weight.dtype}, expected the chain's {dtype}")
+    if norm_weight.device != torch.device(device):
+        raise ValueError(f"norm_weight is on {norm_weight.device}, expected the chain's device {device}")
+    if not norm_weight.is_contiguous():
+        raise ValueError("norm_weight must be contiguous")
+    if not (isinstance(norm_eps, (int, float)) and norm_eps > 0):
+        raise ValueError(f"norm_eps must be a positive number (got {norm_eps!r})")
+    if K > _lib.CHAIN_NORM_MAX_K:
+        raise NotImplementedError(f"norm stages take infeatures <= {_lib.CHAIN_NORM_MAX_K} (got {K}): the normalised x "
+                                  "is staged in shared memory")
+    if x_mode == "add_rmsnorm" and x2 is None:
+        raise ValueError("x_mode='add_rmsnorm' needs the residual as x2")
+    if x_mode == "rmsnorm" and x2 is not None:
+        raise ValueError("x_mode='rmsnorm' takes no x2 (use 'add_rmsnorm' to add a residual)")
 
 
 def chain_supported(layers, M: int) -> bool:
@@ -56,7 +90,7 @@ class DecodeChain:
         self.device = torch.device("cuda", torch.cuda.current_device()) if device is None else torch.device(device)
         if self.device.type != "cuda":
             raise RuntimeError("DecodeChain needs a CUDA device (there is no CPU fallback)")
-        self._stages = []          # (layers, x, x2, mode, parts, stride, ys)
+        self._stages = []          # (layers, x, x2, mode, parts, stride, ys, peer_tables, perm, (norm_weight, eps, h) or None)
         self._producer = {}        # data_ptr of a chain-owned buffer -> index of the stage that writes it
         self._keep = []
         self._handle = None
@@ -70,12 +104,18 @@ class DecodeChain:
         return t
 
     def stage(self, layers, x: torch.Tensor, x2: torch.Tensor | None = None, x_mode: str = "plain", x_parts: int = 0,
-              x_part_stride: int = 0, outputs=None, peer_tables=None):
+              x_part_stride: int = 0, outputs=None, peer_tables=None, *, norm_weight: torch.Tensor | None = None,
+              norm_eps: float = 1e-6):
         """Append a stage of sibling layers reading ``x``; returns their output buffers [M, N] (one per layer).
 
         ``x_mode="sum_parts"``: ``x`` is an int64 tensor of 8-byte words [x_parts, x_part_stride] that the peers fill
         (tensor parallelism, see ``autogptq_b200.tp``).  ``peer_tables``: per layer None or an int64 device tensor with the
-        addresses this layer's output words are sent to instead of staying in the chain."""
+        addresses this layer's output words are sent to instead of staying in the chain.
+
+        ``x_mode="rmsnorm"``: the layers read RMSNorm(x) with ``norm_weight`` [K] and ``norm_eps`` (a block's
+        input_layernorm).  ``x_mode="add_rmsnorm"``: they read RMSNorm(x + x2), ``x2`` being the residual, and the
+        returned list ends with one more buffer [M, K], the new residual h = x + x2, which later stages may read as
+        their ``x`` or ``x2``.  Rounding as transformers' LlamaDecoderLayer / LlamaRMSNorm (``include/autogptq_b200.h``)."""
         if self._handle is not None:
             raise RuntimeError("DecodeChain.build() has already been called")
         layers = list(layers)
@@ -83,7 +123,10 @@ class DecodeChain:
             raise NotImplementedError("DecodeChain needs 1..4 sibling QuantLinear layers with infeatures % 128 == 0, "
                                       "group_size % 128 == 0 (or -1) and outfeatures % 32 == 0")
         K = layers[0].infeatures
+        if x_mode not in _X_MODES:
+            raise ValueError(f"unknown x_mode {x_mode!r}; one of {sorted(_X_MODES)}")
         mode = _X_MODES[x_mode]
+        check_norm_args(x_mode, self.M, K, self.dtype, self.device, x2, norm_weight, norm_eps)
         for t in (x, x2):
             want = torch.int64 if (mode == _lib.CHAIN_X_SUM_PARTS and t is x) else self.dtype
             if t is not None and (t.device != self.device or t.dtype != want or not t.is_contiguous()):
@@ -94,6 +137,8 @@ class DecodeChain:
             raise ValueError(f"stage input has shape {tuple(x.shape)}, expected {(self.M, K)}")
         if mode == _lib.CHAIN_X_SILU_MUL and (x2 is None or tuple(x2.shape) != (self.M, K)):
             raise ValueError("x_mode='silu_mul' needs x2 of the same shape as x")
+        if mode == _lib.CHAIN_X_ADD_RMSNORM and tuple(x2.shape) != (self.M, K):
+            raise ValueError(f"x_mode='add_rmsnorm': the residual x2 has shape {tuple(x2.shape)}, expected {(self.M, K)}")
         for lin in layers:
             if not lin._ready or lin._qweight_run is None or lin._qweight_run.device != self.device:
                 lin.post_init()
@@ -103,14 +148,17 @@ class DecodeChain:
                 raise NotImplementedError("act-order sibling layers of a stage must share one permutation of x")
         ys = outputs if outputs is not None else [torch.zeros((self.M, lin.outfeatures), dtype=self.dtype, device=self.device) for lin in layers]
         peer_tables = list(peer_tables) if peer_tables is not None else [None] * len(layers)
+        res = torch.zeros((self.M, K), dtype=self.dtype, device=self.device) if mode == _lib.CHAIN_X_ADD_RMSNORM else None
+        norm = (norm_weight, float(norm_eps), res) if mode in _NORM_MODES else None
         idx = len(self._stages)
-        self._stages.append((layers, x, x2, mode, x_parts, x_part_stride, ys, peer_tables, perms[0]))
-        for y in ys:
+        self._stages.append((layers, x, x2, mode, x_parts, x_part_stride, ys, peer_tables, perms[0], norm))
+        outs = list(ys) + ([res] if res is not None else [])
+        for y in outs:
             self._producer[y.data_ptr()] = idx
-        self._keep.extend(ys)
+        self._keep.extend(outs)
         self._keep.extend(t for t in peer_tables if t is not None)
-        self._keep.extend(t for t in (x, x2) if t is not None)
-        return ys
+        self._keep.extend(t for t in (x, x2, norm_weight) if t is not None)
+        return outs
 
     def build(self):
         lib = _lib.load()
@@ -118,7 +166,12 @@ class DecodeChain:
         if n == 0:
             raise RuntimeError("DecodeChain has no stages")
         arr = (_CStage * n)()
-        for i, (layers, x, x2, mode, parts, stride, ys, peer_tables, perm) in enumerate(self._stages):
+        norms = (_CNorm * n)() if any(s[9] is not None for s in self._stages) else None
+        for i, (layers, x, x2, mode, parts, stride, ys, peer_tables, perm, norm) in enumerate(self._stages):
+            if norm is not None:
+                w, eps, res = norm
+                norms[i].weight, norms[i].eps = w.data_ptr(), eps
+                norms[i].residual_out = res.data_ptr() if res is not None else None
             st = arr[i]
             st.x, st.x2 = x.data_ptr(), (x2.data_ptr() if x2 is not None else None)
             st.perm = perm.data_ptr() if perm is not None else None
@@ -132,14 +185,20 @@ class DecodeChain:
                 if pt is not None:
                     L.y_peers, L.n_peers = pt.data_ptr(), pt.numel()
                 self._keep.extend((lin._qweight_run, lin.qzeros, scales, bias))
-        nbytes = int(lib.agb200_chain_plan_bytes(arr, n, self.M))
+        if norms is None:
+            nbytes = int(lib.agb200_chain_plan_bytes(arr, n, self.M))
+        else:
+            nbytes = int(lib.agb200_chain_plan_bytes_norm(arr, norms, n, self.M))
         self._plan = torch.zeros(nbytes + 256, dtype=torch.uint8, device=self.device)
         base = (self._plan.data_ptr() + 255) // 256 * 256
         h = c_void_p()
         with torch.cuda.device(self.device):
             torch.cuda.synchronize(self.device)
-            _lib.check(lib.agb200_chain_create(arr, n, self.M, _DTYPE_CODE[self.dtype], base, nbytes, ctypes.byref(h)),
-                       "agb200_chain_create")
+            if norms is None:
+                rc = lib.agb200_chain_create(arr, n, self.M, _DTYPE_CODE[self.dtype], base, nbytes, ctypes.byref(h))
+            else:
+                rc = lib.agb200_chain_create_norm(arr, norms, n, self.M, _DTYPE_CODE[self.dtype], base, nbytes, ctypes.byref(h))
+            _lib.check(rc, "agb200_chain_create")
         self._handle = h
         return self
 

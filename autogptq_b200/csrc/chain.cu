@@ -58,11 +58,16 @@ constexpr size_t kFlagsBytes = 256;
 constexpr size_t kProfBytes = 256 * agb::kChProfRows * agb::kChProfSlots * sizeof(long long);   // up to 256 CTAs
 size_t stages_bytes(int n) { return align_up(size_t(n) * sizeof(agb::ChainStage), 128); }
 size_t maps_bytes(int n) { return size_t(n) * agb::kChMaxGroup * 3 * sizeof(CUtensorMap); }
-size_t ll_bytes(const agb200_chain_stage* stages, int n, int M) {
+bool publishes_residual(const agb200_chain_stage& st, const agb200_chain_norm* norm) {
+  return st.x_mode == AGB200_CHAIN_X_ADD_RMSNORM && norm != nullptr && norm->residual_out != nullptr && st.K > 0;
+}
+size_t ll_bytes(const agb200_chain_stage* stages, const agb200_chain_norm* norms, int n, int M) {
   size_t total = 0;
-  for (int i = 0; i < n; ++i)
+  for (int i = 0; i < n; ++i) {
     for (int l = 0; l < stages[i].n_layers && l < agb::kChMaxGroup; ++l)
       if (stages[i].layer[l].y != nullptr && stages[i].layer[l].N > 0) total += align_up(size_t(M) * stages[i].layer[l].N * 4, 128);
+    if (norms && publishes_residual(stages[i], norms + i)) total += align_up(size_t(M) * stages[i].K * 4, 128);
+  }
   return total;
 }
 
@@ -107,6 +112,7 @@ const char* site_name(int site) {
     case agb::kChSiteEmpty: return "the producer waiting for a ring slot to be released";
     case agb::kChSitePoll: return "a consumer thread polling the tagged words of x";
     case agb::kChSiteLanded: return "the producer waiting for its oldest request to land";
+    case agb::kChSiteNormPoll: return "a consumer thread polling the tagged words of a norm stage's x or residual";
     default: return "unknown site";
   }
 }
@@ -146,9 +152,13 @@ int launch_m(const Chain& c, int flags, cudaStream_t stream) {
 
 extern "C" {
 
-size_t agb200_chain_plan_bytes(const agb200_chain_stage* stages, int n_stages, int M) {
+size_t agb200_chain_plan_bytes_norm(const agb200_chain_stage* stages, const agb200_chain_norm* norms, int n_stages, int M) {
   if (n_stages <= 0 || !stages || M < 1) return 0;
-  return kFlagsBytes + kProfBytes + stages_bytes(n_stages) + maps_bytes(n_stages) + ll_bytes(stages, n_stages, M);
+  return kFlagsBytes + kProfBytes + stages_bytes(n_stages) + maps_bytes(n_stages) + ll_bytes(stages, norms, n_stages, M);
+}
+
+size_t agb200_chain_plan_bytes(const agb200_chain_stage* stages, int n_stages, int M) {
+  return agb200_chain_plan_bytes_norm(stages, nullptr, n_stages, M);
 }
 
 size_t agb200_chain_parts_bytes(int parts, int M, int K) {
@@ -158,6 +168,11 @@ size_t agb200_chain_parts_bytes(int parts, int M, int K) {
 
 int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, int dtype, void* plan, size_t plan_bytes,
                         void** handle_out) {
+  return agb200_chain_create_norm(stages, nullptr, n_stages, M, dtype, plan, plan_bytes, handle_out);
+}
+
+int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chain_norm* norms, int n_stages, int M,
+                             int dtype, void* plan, size_t plan_bytes, void** handle_out) {
   if (!stages || !plan || !handle_out) return failf(AGB200_EINVAL, "chain: null pointer argument");
   *handle_out = nullptr;
   if (n_stages < 1 || n_stages > 65535) return failf(AGB200_EINVAL, "chain: 1 <= n_stages <= 65535 (got %d)", n_stages);
@@ -166,7 +181,7 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   for (int i = 0; i < n_stages; ++i)
     if (stages[i].n_layers < 1 || stages[i].n_layers > agb::kChMaxGroup)
       return failf(AGB200_EINVAL, "chain stage %d: 1 <= n_layers <= 4 (got %d)", i, stages[i].n_layers);
-  const size_t need = agb200_chain_plan_bytes(stages, n_stages, M);
+  const size_t need = agb200_chain_plan_bytes_norm(stages, norms, n_stages, M);
   if (plan_bytes < need || (reinterpret_cast<uintptr_t>(plan) & 255u))
     return failf(AGB200_EWORKSPACE, "chain: plan buffer needs %zu bytes, 256-byte aligned (got %zu)", need, plan_bytes);
 
@@ -190,7 +205,7 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
   agb::ChainStage* d_stages = reinterpret_cast<agb::ChainStage*>(base + kFlagsBytes + kProfBytes);
   CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base + kFlagsBytes + kProfBytes + stages_bytes(n_stages));
   unsigned char* d_ll = base + kFlagsBytes + kProfBytes + stages_bytes(n_stages) + maps_bytes(n_stages);
-  const size_t ll_total = ll_bytes(stages, n_stages, M);
+  const size_t ll_total = ll_bytes(stages, norms, n_stages, M);
 
   struct Out { const void* y; uint2* ll; int N; };
   std::vector<Out> outs;            // every output of the chain so far: later stages find their x here
@@ -211,7 +226,24 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
     if (K <= 0 || K % 128 != 0 || K > max_k) return failf(AGB200_ENOSUP, "chain stage %d: K=%d must be a multiple of 128, at most %d for M=%d", i, K, max_k, M);
     if (g <= 0 || g % 128 != 0) return failf(AGB200_ENOSUP, "chain stage %d: group_size=%d must be a multiple of 128 (pass K for -1)", i, g);
     if (!in.x || !aligned16(in.x)) return failf(AGB200_EINVAL, "chain stage %d: x must be a 16-byte aligned device pointer", i);
-    if (in.x_mode < 0 || in.x_mode > AGB200_CHAIN_X_SUM_PARTS) return failf(AGB200_EINVAL, "chain stage %d: unknown x_mode %d", i, in.x_mode);
+    if (in.x_mode < 0 || in.x_mode > AGB200_CHAIN_X_ADD_RMSNORM) return failf(AGB200_EINVAL, "chain stage %d: unknown x_mode %d", i, in.x_mode);
+    const bool norm_stage = in.x_mode == AGB200_CHAIN_X_RMSNORM || in.x_mode == AGB200_CHAIN_X_ADD_RMSNORM;
+    if (norm_stage) {
+      const agb200_chain_norm* nm = norms ? norms + i : nullptr;
+      if (!nm) return failf(AGB200_EINVAL, "chain stage %d: a norm stage needs agb200_chain_create_norm with a norm entry", i);
+      if (!nm->weight || !aligned16(nm->weight)) return failf(AGB200_EINVAL, "chain stage %d: the norm weight must be a 16-byte aligned device pointer", i);
+      if (!(nm->eps > 0.f)) return failf(AGB200_EINVAL, "chain stage %d: norm eps must be > 0", i);
+      if (K > AGB200_CHAIN_NORM_MAX_K) return failf(AGB200_ENOSUP, "chain stage %d: norm stages take K <= %d (got %d)", i, AGB200_CHAIN_NORM_MAX_K, K);
+      if (in.x_mode == AGB200_CHAIN_X_ADD_RMSNORM) {
+        if (!in.x2 || !aligned16(in.x2)) return failf(AGB200_EINVAL, "chain stage %d: X_ADD_RMSNORM needs the residual as x2", i);
+        if (!nm->residual_out || !aligned16(nm->residual_out))
+          return failf(AGB200_EINVAL, "chain stage %d: X_ADD_RMSNORM needs a 16-byte aligned residual_out", i);
+      } else if (nm->residual_out) {
+        return failf(AGB200_EINVAL, "chain stage %d: X_RMSNORM publishes no residual (residual_out must be NULL)", i);
+      }
+      st.norm_w = nm->weight;
+      st.norm_eps = nm->eps;
+    }
     st.K = K; st.rows = K / 8;
     st.chunks = (st.rows + agb::kChSlotRows - 1) / agb::kChSlotRows;
     st.n_layers = in.n_layers; st.map_base = static_cast<int>(hm.size());
@@ -246,8 +278,15 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
         if ((src2 != nullptr) != (src != nullptr)) return failf(AGB200_EINVAL, "chain stage %d: x and x2 must both be chain outputs or both be external", i);
         if (src2 && src2->N != K) return failf(AGB200_EINVAL, "chain stage %d: x2 is the output of a layer with N=%d but K=%d", i, src2->N, K);
         st.x2 = in.x2; st.x2_ll = src2 ? src2->ll : nullptr;
+      } else if (in.x_mode == AGB200_CHAIN_X_ADD_RMSNORM) {
+        // each operand is polled or read plain on its own: the residual of a block's first norm comes from the previous
+        // launch while o_proj's output comes from this one
+        const Out* src2 = find(in.x2);
+        if (src2 && src2->N != K) return failf(AGB200_EINVAL, "chain stage %d: x2 is the output of a layer with N=%d but K=%d", i, src2->N, K);
+        st.x2 = in.x2; st.x2_ll = src2 ? src2->ll : nullptr;
       }
     }
+    if (norm_stage) xs_bytes = std::max(xs_bytes, static_cast<int>(align_up(size_t(M) * K * 2, 128)));
     rows_pad_max = std::max(rows_pad_max, st.chunks * agb::kChSlotRows);
     if (in.perm != nullptr) {
       if (reinterpret_cast<uintptr_t>(in.perm) & 15u) return failf(AGB200_EINVAL, "chain stage %d: perm must be 16-byte aligned", i);
@@ -282,6 +321,12 @@ int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, i
       hm.push_back(mw); hm.push_back(ms); hm.push_back(mz);
     }
     st.total_tiles = tiles;
+    if (publishes_residual(in, norms ? norms + i : nullptr)) {     // h is an output of this stage like a layer's y
+      st.res = norms[i].residual_out;
+      st.res_ll = reinterpret_cast<uint2*>(d_ll + ll_off);
+      ll_off += align_up(size_t(M) * K * 4, 128);
+      outs.push_back(Out{st.res, st.res_ll, K});
+    }
     // tiles are dealt round-robin over the CTAs, continuing where the previous stage stopped: every SM streams the same
     // number of bytes over a few stages although single stages have 0.86 .. 4.65 tiles per SM
     st.rot = static_cast<int>(tiles_so_far % sms);

@@ -36,7 +36,9 @@
 //     buffers (mbarriers) and the epilogue warp combines the digits, adds bias, rounds and publishes.
 // Optional x transforms at a stage input: silu(a) * b (gate|up -> down of an MLP, fused_llama_mlp.py:131-245 in the
 // reference) and the sum of `parts` partial vectors (row-parallel tensor parallelism: the all-reduce of SURVEY 8e, read
-// from peer-written LL buffers - a one-shot all-reduce over NVLink with one-way latency).
+// from peer-written LL buffers - a one-shot all-reduce over NVLink with one-way latency), and RMSNorm(x) or
+// RMSNorm(x + residual) with the new residual published as a stage output (the residual adds and norms of a decoder
+// layer; ch_norm_prepass).
 //
 // Requires: group_size % 128 == 0 (or group_size == K), K % 128 == 0, N % 32 == 0, K <= 32768.
 // Roofline: HBM, algorithmic bytes per stage = sum over its layers of SURVEY 8d's formula.
@@ -67,7 +69,7 @@ constexpr int kChMaxChunks = 32;                    // ring slots (1024 k) per t
 
 constexpr int kChMaxPeers = 8;
 
-enum ChainXMode { kChXPlain = 0, kChXSiluMul = 1, kChXSumParts = 2 };
+enum ChainXMode { kChXPlain = 0, kChXSiluMul = 1, kChXSumParts = 2, kChXRmsNorm = 3, kChXAddRmsNorm = 4 };
 enum ChainDebug { kChDbgNoDeps = 1, kChDbgNoMath = 2, kChDbgNoConvert = 4, kChDbgProfile = 8 };
 constexpr int kChProfSlots = 8;   // per CTA and profiled warp: total, wait for x, convert, wait for weights, MMA, flush, tile end, -
 constexpr int kChProfRows = kChGroups + 1;   // one warp per consumer group, then the producer: total, blocked on a full
@@ -95,6 +97,11 @@ struct ChainStage {
   const uint2* next_x_ll;                        // tagged words of the NEXT stage's x when they can be prefetched (plain, no gather)
   int next_K, next_rows;
   ChainLayer layer[kChMaxGroup];
+  const void* norm_w;   // kChXRmsNorm / kChXAddRmsNorm: [K] norm weight
+  void* res;            // kChXAddRmsNorm: [M, K] plain h = x + x2
+  uint2* res_ll;        // kChXAddRmsNorm: [M, K/2] {two values of h, tag}: what later stages of this chain read
+  float norm_eps;
+  int norm_pad_;
 };
 constexpr int kChStageWords = sizeof(ChainStage) / 4;
 constexpr int kChDescWords = 96;   // shared-memory copy of a stage descriptor
@@ -253,7 +260,8 @@ __device__ __forceinline__ int ch_locate(const ChainStage& st, int tile, int& li
 }
 // A protocol bug must not hang the GPU: every wait is bounded.  Before the trap the waiter says where it was (host-mapped
 // words, readable after the context died: agb200_chain_diag).
-enum ChainWaitSite { kChSiteFull = 1, kChSiteXrdy = 2, kChSiteRedFree = 3, kChSiteRedFull = 4, kChSiteEmpty = 5, kChSitePoll = 6, kChSiteLanded = 7 };
+enum ChainWaitSite { kChSiteFull = 1, kChSiteXrdy = 2, kChSiteRedFree = 3, kChSiteRedFull = 4, kChSiteEmpty = 5, kChSitePoll = 6, kChSiteLanded = 7,
+                     kChSiteNormPoll = 8 };
 __device__ __noinline__ void ch_fail(int* diag, int site, int stage, int extra) {
   if (diag != nullptr) {
     if (atomicCAS(diag, 0, site) == 0) {
@@ -266,12 +274,13 @@ __device__ __noinline__ void ch_fail(int* diag, int site, int stage, int extra) 
   }
   __trap();
 }
-__device__ __forceinline__ void ch_watchdog(unsigned& polls, unsigned long long& t0, int* diag, int stage, int extra) {
+__device__ __forceinline__ void ch_watchdog(unsigned& polls, unsigned long long& t0, int* diag, int stage, int extra,
+                                            int site = kChSitePoll) {
   if ((++polls & 4095u) == 0) {
     unsigned long long now;
     asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(now));
     if (t0 == 0) t0 = now;
-    else if (now - t0 > 4000000000ull) ch_fail(diag, kChSitePoll, stage, extra);   // 4 s
+    else if (now - t0 > 4000000000ull) ch_fail(diag, site, stage, extra);   // 4 s
   }
 }
 __device__ __forceinline__ void ch_wait(uint32_t bar, uint32_t parity, int* diag, int site, int stage, int extra) {
@@ -324,6 +333,136 @@ __device__ __noinline__ void ch_prefetch_rows(const uint2* nx, int nrows, int nK
       for (int m = 0; m < kM; ++m) ch_prefetch_l1(nx + static_cast<size_t>(m) * (nK >> 1) + static_cast<size_t>(row) * 4);
     }
   }
+}
+
+// one k8-row (8 consecutive k) of an operand of a norm stage: plain 16-bit values (ready before the launch) or the
+// tagged words of a chain output; false while one of those is not there yet
+__device__ __forceinline__ bool ch_norm_read(const uint16_t* plain, const uint2* ll, size_t off, unsigned tag, uint4& out) {
+  if (ll == nullptr) {
+    out = ch_ld_v4(plain + off);
+    return true;
+  }
+  const uint2* src = ll + (off >> 1);
+  const uint4 a = ch_ld_gpu_v4(src), b = ch_ld_gpu_v4(src + 2);
+  out = make_uint4(a.x, a.z, b.x, b.z);
+  return a.y == tag && a.w == tag && b.y == tag && b.w == tag;
+}
+
+// Norm stage input (kChXRmsNorm / kChXAddRmsNorm), run by the 12 consumer warps before the digit conversion, which then
+// reads the staged rows instead of polling x.  It is inlined: as an out-of-line call it made ptxas save the slot loop's
+// per-thread constants around the call site (new spills in three of the eight instantiations), while inlined every
+// non-profiling instantiation keeps exactly the registers and spill counts it had before norm stages existed.  The norm needs the whole row, so every
+// CTA reads all of x (and x2):
+//   h = rnd(x + x2)                    (kChXAddRmsNorm; else h = x), staged in XS in storage order;
+//   r = 1 / sqrt(Σh² / K + eps)        fp32; Σh² per thread in row order, then a fixed shuffle tree per warp and the 12
+//                                      warps in order: the same bits in every CTA and every launch;
+//   n = rnd(rnd(h·r)·w)                written over h in XS, where the conversion reads it (through `perm` for act-order).
+// These are the rounding points of transformers' LlamaDecoderLayer (residual + hidden_states in the activation dtype)
+// and LlamaRMSNorm (fp32 variance, rounded to the dtype before the weight multiplies).  kChXAddRmsNorm also publishes h:
+// 1024-k chunk c by CTA c mod grid, as plain values and as tagged words that later stages poll like a layer's y.
+// `red` is kChWarps * kM floats of scratch (the DS table, which the conversion only writes after this returns).
+template <int kM, bool kBf16>
+__device__ __forceinline__ void ch_norm_prepass(const ChainStage& st, uint32_t xs_u32, float* red, unsigned tag, int s,
+                                             int* diag, int backoff, bool no_deps) {
+  const int ctid = threadIdx.x, lane = ctid & 31, warp = ctid >> 5;
+  const int K = st.K, rows = st.rows, G = gridDim.x;
+  const bool add = st.x_mode == kChXAddRmsNorm;
+  const uint16_t* xg = reinterpret_cast<const uint16_t*>(st.x);
+  const uint16_t* xg2 = reinterpret_cast<const uint16_t*>(st.x2);
+  const uint2* xl = no_deps ? nullptr : st.x_ll;
+  const uint2* xl2 = no_deps ? nullptr : st.x2_ll;
+  uint16_t* res = reinterpret_cast<uint16_t*>(st.res);
+  uint2* res_ll = st.res_ll;
+  float ss[kM];
+#pragma unroll
+  for (int m = 0; m < kM; ++m) ss[m] = 0.f;
+  for (int row = ctid; row < rows; row += kChConsumers) {
+    const bool publish = add && (row / kChSlotRows) % G == static_cast<int>(blockIdx.x);
+#pragma unroll
+    for (int m = 0; m < kM; ++m) {
+      const size_t off = static_cast<size_t>(m) * K + static_cast<size_t>(row) * kPack;
+      uint4 a, b = make_uint4(0, 0, 0, 0);
+      unsigned polls = 0;
+      unsigned long long t0 = 0;
+      while (true) {
+        bool ok = ch_norm_read(xg, xl, off, tag, a);
+        if (add) ok = ch_norm_read(xg2, xl2, off, tag, b) && ok;
+        if (ok) break;
+        ch_watchdog(polls, t0, diag, s, row, kChSiteNormPoll);
+        if (backoff > 0) {
+          const long long tb = clock64();
+          while (clock64() - tb < static_cast<long long>(backoff)) {}
+        }
+      }
+      uint32_t hw[4] = {a.x, a.y, a.z, a.w};
+      if (add) {
+        const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
+#pragma unroll
+        for (int i = 0; i < 4; ++i) {
+          const uint32_t lo = float_to_elt<kBf16>(elt_to_float<kBf16>(static_cast<uint16_t>(hw[i] & 0xffffu)) +
+                                                  elt_to_float<kBf16>(static_cast<uint16_t>(bw[i] & 0xffffu)));
+          const uint32_t hi = float_to_elt<kBf16>(elt_to_float<kBf16>(static_cast<uint16_t>(hw[i] >> 16)) +
+                                                  elt_to_float<kBf16>(static_cast<uint16_t>(bw[i] >> 16)));
+          hw[i] = lo | (hi << 16);
+        }
+      }
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const float f0 = elt_to_float<kBf16>(static_cast<uint16_t>(hw[i] & 0xffffu));
+        const float f1 = elt_to_float<kBf16>(static_cast<uint16_t>(hw[i] >> 16));
+        ss[m] = fmaf(f0, f0, ss[m]);
+        ss[m] = fmaf(f1, f1, ss[m]);
+      }
+      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(xs_u32 + static_cast<uint32_t>(off * 2)), "r"(hw[0]), "r"(hw[1]),
+                   "r"(hw[2]), "r"(hw[3]) : "memory");
+      if (publish) {
+        *reinterpret_cast<uint4*>(res + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+#pragma unroll
+        for (int i = 0; i < 4; ++i) ch_st_gpu_v2(res_ll + (off >> 1) + i, hw[i], tag);
+      }
+    }
+  }
+#pragma unroll
+  for (int m = 0; m < kM; ++m) {
+    float v = ss[m];
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    if (lane == 0) red[warp * kM + m] = v;
+  }
+  ch_consumer_barrier();
+  float r[kM];
+#pragma unroll
+  for (int m = 0; m < kM; ++m) {
+    float tot = 0.f;
+    for (int w = 0; w < kChWarps; ++w) tot += red[w * kM + m];
+    r[m] = __frsqrt_rn(__fadd_rn(__fdiv_rn(tot, static_cast<float>(K)), st.norm_eps));
+  }
+  const uint16_t* nw = reinterpret_cast<const uint16_t*>(st.norm_w);
+  for (int row = ctid; row < rows; row += kChConsumers) {
+    const uint4 wv = __ldg(reinterpret_cast<const uint4*>(nw + static_cast<size_t>(row) * kPack));
+    const uint32_t ww[4] = {wv.x, wv.y, wv.z, wv.w};
+#pragma unroll
+    for (int m = 0; m < kM; ++m) {
+      const uint32_t a = xs_u32 + static_cast<uint32_t>((static_cast<size_t>(m) * K + static_cast<size_t>(row) * kPack) * 2);
+      const uint4 hv = ch_lds_v4(a);
+      const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w};
+      uint32_t nv[4];
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        uint32_t o[2];
+#pragma unroll
+        for (int j = 0; j < 2; ++j) {
+          const float h = elt_to_float<kBf16>(static_cast<uint16_t>(j ? hw[i] >> 16 : hw[i] & 0xffffu));
+          const float w = elt_to_float<kBf16>(static_cast<uint16_t>(j ? ww[i] >> 16 : ww[i] & 0xffffu));
+          const float t = elt_to_float<kBf16>(float_to_elt<kBf16>(__fmul_rn(h, r[m])));
+          o[j] = float_to_elt<kBf16>(__fmul_rn(t, w));
+        }
+        nv[i] = o[0] | (o[1] << 16);
+      }
+      asm volatile("st.shared.v4.u32 [%0], {%1,%2,%3,%4};" ::"r"(a), "r"(nv[0]), "r"(nv[1]), "r"(nv[2]), "r"(nv[3]) : "memory");
+    }
+  }
+  ch_consumer_barrier();
 }
 
 template <int kM, bool kBf16, bool kProf>
@@ -712,7 +851,12 @@ w4a16_chain_kernel(const ChainParams p) {
           }
         }
       };
-      if (perm != nullptr) {
+      // x staged in XS in storage order: the normalised x of a norm stage, the gather source of an act-order stage
+      const bool staged = perm != nullptr || xmode >= kChXRmsNorm;
+      if (xmode >= kChXRmsNorm) {
+        ch_norm_prepass<kM, kBf16>(st, xs_u32, reinterpret_cast<float*>(smem_al + (ds_u32 - smem_base)), tag, s, p.diag,
+                                   p.poll_backoff, no_deps);
+      } else if (perm != nullptr) {
         // act-order: stage x in storage order in shared memory (XS), then every thread gathers its sorted rows from there
         for (int cc0 = cmap; cc0 < C; cc0 += kChGroups * kR) {
           uint4 vv[kM][kR];
@@ -732,8 +876,18 @@ w4a16_chain_kernel(const ChainParams p) {
       }
       for (int cc0 = cmap; cc0 < C; cc0 += kChGroups * kR) {
         uint4 vv[kM][kR];
-        if (perm == nullptr) {
+        if (!staged) {
           fetch_batch(cc0, vv);
+        } else if (perm == nullptr) {
+#pragma unroll
+          for (int m = 0; m < kM; ++m) {
+#pragma unroll
+            for (int r = 0; r < kR; ++r) {
+              const int row = (cc0 + kChGroups * r) * kChSlotRows + crow;
+              vv[m][r] = make_uint4(0, 0, 0, 0);
+              if (cc0 + kChGroups * r < C && row < rows) vv[m][r] = ch_lds_v4(xs_u32 + static_cast<uint32_t>((m * rows + row) * 16));
+            }
+          }
         } else {
 #pragma unroll
           for (int m = 0; m < kM; ++m) {

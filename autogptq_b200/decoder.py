@@ -1,0 +1,276 @@
+"""Greedy decoding of a GPTQ Llama / Mistral / Qwen2 model with one decode-chain launch per decoder block.
+
+    dec = ChainDecoder(model, batch=1, max_length=2048)    # model: transformers *ForCausalLM with QuantLinear projections
+    tokens = dec.generate(input_ids, max_new_tokens=128)   # prefill on the HF model, then one CUDA graph per token
+
+Between two attentions a decoder layer is QuantLinears, elementwise work and one row reduction:
+
+    o_proj(attn) -> h1 = x + o -> n2 = post_attention_layernorm(h1) -> gate|up -> silu*mul -> down
+                 -> x' = h1 + down -> n1' = next input_layernorm(x') -> next q|k|v
+
+The decode chain's norm stage inputs (``x_mode="add_rmsnorm"``) cover the adds and norms, so block i is one chain
+
+    chain_0 = [input_layernorm_0 -> q|k|v_0]
+    chain_i = [o_i, add_rmsnorm -> gate|up_i, silu_mul -> down_i, add_rmsnorm(input_layernorm_i+1) -> q|k|v_i+1]
+
+(the last block ends at down_i).  Attention needs the KV cache and runs in torch between two chains: the model's own
+rotary embedding and ``apply_rotary_pos_emb``, a static [batch, kv_heads, max_length, head_dim] cache written at a
+device-side position, and ``F.scaled_dot_product_attention`` with GQA and a length mask; its output goes straight into
+the next chain's o_proj input buffer.  The final add, ``model.model.norm`` and ``lm_head`` run in torch.  One token is
+then n_layers + 1 chain launches and n_layers attentions, captured together in one CUDA graph.
+
+Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  What does not fit raises
+NotImplementedError naming the module.
+"""
+from __future__ import annotations
+
+import torch
+import torch.nn.functional as F
+
+from . import _lib
+from .chain import DecodeChain, chain_supported
+from .mlp import FusedQuantMLP, _is_silu
+from .qlinear import QuantLinear
+
+_RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm")
+
+
+def _norm_of(mod, name: str):
+    """(weight, eps) of an RMSNorm with transformers' Llama rounding: weight · rnd(h · rsqrt(mean(h²) + eps))."""
+    if type(mod).__name__ not in _RMSNORMS or not hasattr(mod, "weight") or not hasattr(mod, "variance_epsilon"):
+        raise NotImplementedError(f"ChainDecoder: {name} is {type(mod).__name__}; only Llama-style RMSNorm "
+                                  f"({', '.join(_RMSNORMS)}) runs inside the decode chain")
+    return mod.weight, float(mod.variance_epsilon)
+
+
+def _plan_layer(i: int, layer, batch: int, dtype):
+    """The modules of decoder layer i that the chains read, after checking that they fit."""
+    attn, mlp = getattr(layer, "self_attn", None), getattr(layer, "mlp", None)
+    if attn is None or mlp is None:
+        raise NotImplementedError(f"ChainDecoder: model.layers.{i} has no self_attn / mlp")
+    names = ("q_proj", "k_proj", "v_proj", "o_proj")
+    for n in names:
+        if not isinstance(getattr(attn, n, None), QuantLinear):
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.self_attn.{n} is "
+                                      f"{type(getattr(attn, n, None)).__name__}, not autogptq_b200.QuantLinear")
+    if not isinstance(mlp, FusedQuantMLP):
+        if not all(hasattr(mlp, n) for n in ("gate_proj", "up_proj", "down_proj")):
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp ({type(mlp).__name__}) is not a "
+                                      "gate/up/down MLP")
+        if not _is_silu(getattr(mlp, "act_fn", None)):
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp.act_fn is "
+                                      f"{type(getattr(mlp, 'act_fn', None)).__name__}, not SiLU")
+    for n in ("gate_proj", "up_proj", "down_proj"):
+        if not isinstance(getattr(mlp, n), QuantLinear):
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp.{n} is {type(getattr(mlp, n)).__name__}, "
+                                      "not autogptq_b200.QuantLinear")
+    groups = {"self_attn.q_proj|k_proj|v_proj": [attn.q_proj, attn.k_proj, attn.v_proj], "self_attn.o_proj": [attn.o_proj],
+              "mlp.gate_proj|up_proj": [mlp.gate_proj, mlp.up_proj], "mlp.down_proj": [mlp.down_proj]}
+    for n, ls in groups.items():
+        if not chain_supported(ls, batch):
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.{n} cannot run in a decode chain (needs "
+                                      "infeatures % 128 == 0, group_size % 128 == 0 or -1, outfeatures % 32 == 0, "
+                                      "sibling layers of one shape)")
+    ln1 = _norm_of(getattr(layer, "input_layernorm", None), f"model.layers.{i}.input_layernorm")
+    ln2 = _norm_of(getattr(layer, "post_attention_layernorm", None), f"model.layers.{i}.post_attention_layernorm")
+    for w, n in ((ln1[0], "input_layernorm"), (ln2[0], "post_attention_layernorm")):
+        if w.dtype != dtype:
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.{n}.weight is {w.dtype}, the activations "
+                                      f"{dtype}")
+    if attn.q_proj.infeatures > _lib.CHAIN_NORM_MAX_K:
+        raise NotImplementedError(f"ChainDecoder: model.layers.{i}: hidden size {attn.q_proj.infeatures} > "
+                                  f"{_lib.CHAIN_NORM_MAX_K}, the largest a chain norm stage takes")
+    return attn, mlp, ln1, ln2
+
+
+def _check_window(config, max_length: int):
+    sw = getattr(config, "sliding_window", None)
+    if getattr(config, "use_sliding_window", True) is False:
+        sw = None
+    if sw is not None and sw < max_length:
+        raise NotImplementedError(f"ChainDecoder: the model attends through a sliding window of {sw} tokens, below "
+                                  f"max_length={max_length}; the static cache holds full attention only")
+
+
+class ChainDecoder:
+    """Greedy decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
+    projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too)."""
+
+    def __init__(self, model, batch: int = 1, max_length: int = 2048):
+        if not 1 <= batch <= _lib.CHAIN_MAX_M:
+            raise NotImplementedError(f"ChainDecoder: batch {batch}; the decode chain runs 1..{_lib.CHAIN_MAX_M} rows")
+        inner = getattr(model, "model", None)
+        if inner is None or not hasattr(inner, "layers") or not hasattr(model, "lm_head"):
+            raise NotImplementedError(f"ChainDecoder: {type(model).__name__} is not a *ForCausalLM with model.layers "
+                                      "and lm_head")
+        for n in ("embed_tokens", "rotary_emb", "norm"):
+            if not hasattr(inner, n):
+                raise NotImplementedError(f"ChainDecoder: model.model has no {n}")
+        self.model, self.batch, self.max_length = model, batch, int(max_length)
+        cfg = model.config
+        _check_window(cfg, self.max_length)
+        self.dtype = inner.embed_tokens.weight.dtype
+        if self.dtype not in (torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"ChainDecoder: activations are {self.dtype}; the chain computes in fp16 / bf16")
+        self.device = inner.embed_tokens.weight.device
+        if self.device.type != "cuda":
+            raise RuntimeError("ChainDecoder needs the model on a CUDA device")
+        plans = [_plan_layer(i, layer, batch, self.dtype) for i, layer in enumerate(inner.layers)]
+        if not plans:
+            raise NotImplementedError("ChainDecoder: the model has no decoder layers")
+        fw, feps = _norm_of(inner.norm, "model.norm")
+        attn0 = plans[0][0]
+        self.head_dim = attn0.head_dim
+        self.scaling = attn0.scaling
+        self.n_heads = attn0.q_proj.outfeatures // self.head_dim
+        self.n_kv = attn0.k_proj.outfeatures // self.head_dim
+        H = attn0.q_proj.infeatures
+
+        B, L, dev, dt = batch, len(plans), self.device, self.dtype
+        self.k_cache = [torch.zeros((B, self.n_kv, self.max_length, self.head_dim), dtype=dt, device=dev) for _ in plans]
+        self.v_cache = [torch.zeros_like(k) for k in self.k_cache]
+        self._pos = torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
+        self._ids = torch.zeros(B, dtype=torch.int64, device=dev)
+        self._arange = torch.arange(self.max_length, device=dev)
+        self._length = 0                                                    # host copy of the position
+
+        # chain_0 = [input_layernorm_0 -> q|k|v_0]
+        self.chains = []
+        ch = DecodeChain(M=B, dtype=dt, device=dev)
+        self._x0 = ch.input(H)
+        w, eps = plans[0][2]
+        qkv = ch.stage([attn0.q_proj, attn0.k_proj, attn0.v_proj], self._x0, x_mode="rmsnorm", norm_weight=w, norm_eps=eps)
+        self.chains.append(ch.build())
+        self._qkv = [qkv]              # q, k, v of block i
+        self._attn_in = []             # o_proj input of block i (written by the attention)
+        resid = self._x0
+        for i, (attn, mlp, _, (w2, eps2)) in enumerate(plans):
+            ch = DecodeChain(M=B, dtype=dt, device=dev)
+            a_in = ch.input(attn.o_proj.infeatures)
+            (o,) = ch.stage([attn.o_proj], a_in)
+            gate, up, h1 = ch.stage([mlp.gate_proj, mlp.up_proj], o, x2=resid, x_mode="add_rmsnorm", norm_weight=w2,
+                                    norm_eps=eps2)
+            (down,) = ch.stage([mlp.down_proj], gate, x2=up, x_mode="silu_mul")
+            if i + 1 < L:
+                na = plans[i + 1][0]
+                w1, eps1 = plans[i + 1][2]
+                q, k, v, resid = ch.stage([na.q_proj, na.k_proj, na.v_proj], down, x2=h1, x_mode="add_rmsnorm",
+                                          norm_weight=w1, norm_eps=eps1)
+                self._qkv.append((q, k, v))
+            else:
+                self._last = (h1, down)
+            self._attn_in.append(a_in)
+            self.chains.append(ch.build())
+        self._final_norm = inner.norm
+        self._graph = None
+        self._logits = None
+
+    # ------------------------------------------------------------------ state
+    @property
+    def position(self) -> int:
+        """Tokens in the cache: the position the next step writes."""
+        return self._length
+
+    @position.setter
+    def position(self, p: int):
+        if not 0 <= p <= self.max_length:
+            raise ValueError(f"position {p} outside 0..{self.max_length}")
+        self._pos.fill_(p)
+        self._length = int(p)
+
+    @torch.no_grad()
+    def prefill(self, input_ids: torch.Tensor) -> torch.Tensor:
+        """Run the prompt [batch, T] through the HF model (its own prefill kernels), copy its cache into the static one
+        and return the logits of the last position [batch, vocab]."""
+        from transformers import DynamicCache
+
+        ids = input_ids.to(self.device)
+        if ids.dim() != 2 or ids.shape[0] != self.batch:
+            raise ValueError(f"input_ids must be [{self.batch}, T] (sequences in lockstep), got {tuple(ids.shape)}")
+        T = ids.shape[1]
+        if not 1 <= T < self.max_length:
+            raise ValueError(f"prompt length {T} must be in 1..{self.max_length - 1}")
+        cache = DynamicCache(config=self.model.config)
+        out = self.model(input_ids=ids, past_key_values=cache, use_cache=True)
+        for i, lay in enumerate(cache.layers):
+            self.k_cache[i][:, :, :T].copy_(lay.keys)
+            self.v_cache[i][:, :, :T].copy_(lay.values)
+        self.position = T
+        return out.logits[:, -1]
+
+    # ------------------------------------------------------------------ one token
+    def _attention(self, i: int, cos, sin, mask):
+        from transformers.models.llama.modeling_llama import apply_rotary_pos_emb
+
+        B, hd = self.batch, self.head_dim
+        q, k, v = self._qkv[i]
+        q = q.view(B, 1, self.n_heads, hd).transpose(1, 2)
+        k = k.view(B, 1, self.n_kv, hd).transpose(1, 2)
+        v = v.view(B, 1, self.n_kv, hd).transpose(1, 2)
+        q, k = apply_rotary_pos_emb(q, k, cos, sin)
+        self.k_cache[i].index_copy_(2, self._pos, k)
+        self.v_cache[i].index_copy_(2, self._pos, v)
+        o = F.scaled_dot_product_attention(q, self.k_cache[i], self.v_cache[i], attn_mask=mask, scale=self.scaling,
+                                           enable_gqa=self.n_kv != self.n_heads)
+        self._attn_in[i].copy_(o.transpose(1, 2).reshape(B, -1))
+
+    def _step_body(self) -> torch.Tensor:
+        inner = self.model.model
+        self._x0.copy_(inner.embed_tokens(self._ids))
+        pos_ids = self._pos.view(1, 1).expand(self.batch, 1)
+        cos, sin = inner.rotary_emb(self._x0.view(self.batch, 1, -1), pos_ids)
+        mask = (self._arange <= self._pos).view(1, 1, 1, -1)
+        self.chains[0].run()
+        for i in range(len(self._attn_in)):
+            self._attention(i, cos, sin, mask)
+            self.chains[i + 1].run()
+        h1, down = self._last
+        n = self._final_norm(h1 + down)
+        logits = self.model.lm_head(n)
+        self._pos.add_(1)
+        return logits
+
+    @torch.no_grad()
+    def step(self, ids: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
+        """Decode one token per sequence: ``ids`` [batch] -> logits [batch, vocab] (a buffer the next step overwrites
+        when ``use_graph``).  The first graph step captures the whole step in one CUDA graph; later steps replay it."""
+        if self._length >= self.max_length:
+            raise RuntimeError(f"the static cache is full ({self.max_length} tokens)")
+        self._ids.copy_(ids.reshape(-1).to(self._ids.device))
+        if not use_graph:
+            logits = self._step_body()
+        else:
+            if self._graph is None:
+                p = self._length
+                side = torch.cuda.Stream(self.device)
+                side.wait_stream(torch.cuda.current_stream(self.device))
+                with torch.cuda.stream(side):                 # warm-up outside the graph (library workspaces)
+                    self._step_body()
+                torch.cuda.current_stream(self.device).wait_stream(side)
+                self.position = p
+                g = torch.cuda.CUDAGraph()
+                with torch.cuda.graph(g):
+                    self._logits = self._step_body()
+                self._graph = g
+                self.position = p
+            self._graph.replay()
+            logits = self._logits
+        self._length += 1
+        return logits
+
+    @torch.no_grad()
+    def generate(self, input_ids: torch.Tensor, max_new_tokens: int) -> torch.Tensor:
+        """Greedy decoding: prompt [batch, T] -> [batch, T + max_new_tokens]."""
+        if input_ids.shape[1] + max_new_tokens > self.max_length:
+            raise ValueError(f"prompt + {max_new_tokens} new tokens exceed max_length={self.max_length}")
+        logits = self.prefill(input_ids)
+        out = [input_ids.to(self.device)]
+        for t in range(max_new_tokens):
+            tok = logits.argmax(-1)
+            out.append(tok.view(-1, 1))
+            if t + 1 < max_new_tokens:
+                logits = self.step(tok)
+        return torch.cat(out, dim=1)
+
+
+__all__ = ["ChainDecoder"]

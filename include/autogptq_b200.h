@@ -191,6 +191,19 @@ int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const
  *                             part r inside that rank's buffer (peer memory, e.g. cudaIpcOpenMemHandle), and its epilogue
  *                             stores the tagged words there - a one-shot all-reduce with one NVLink one-way latency.  All
  *                             ranks must run the same number of launches of their chains (the tag is the launch count).
+ *   AGB200_CHAIN_X_RMSNORM    n = RMSNorm_w(x): the input_layernorm in front of a block's q|k|v
+ *   AGB200_CHAIN_X_ADD_RMSNORM h = x + x2 (x2: the residual), n = RMSNorm_w(h); h is written to the norm entry's
+ *                             `residual_out` and is an output of this stage that later stages of the chain may read as
+ *                             their x or x2 (matched by pointer, like a layer's y): the residual add and the
+ *                             post_attention_layernorm (or the next block's input_layernorm) of a decoder layer.
+ *                             Rounding, as transformers' LlamaDecoderLayer / LlamaRMSNorm: h = rnd(x + x2);
+ *                             var = mean(h^2) and r = 1 / sqrt(var + eps) in fp32 (sqrt and division correctly rounded);
+ *                             n = rnd(rnd(h r) w) with w the norm weight of the chain's dtype.  The fp32 sum of h^2 runs
+ *                             in a fixed order (the same bits from launch to launch), not in torch's order, so n may be
+ *                             the neighbour of torch's value where h r lies next to a rounding midpoint.  Each of x and
+ *                             x2 may be a chain output or an external buffer that is ready at launch.  Norm stages take
+ *                             K <= AGB200_CHAIN_NORM_MAX_K; the normalised x is staged in shared memory (M * K * 2 bytes
+ *                             that the weight ring gives up).  Norm stages need agb200_chain_create_norm.
  * Act-order layers: pass the matrix produced by agb200_w4_make_sequential as qweight and `perm` (shared by the stage).
  * Constraints: K % 128 == 0, K <= 32768, group_size % 128 == 0 (pass K for -1), N % 32 == 0,
  * 16-byte aligned pointers.
@@ -205,6 +218,9 @@ int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const
 #define AGB200_CHAIN_X_PLAIN 0
 #define AGB200_CHAIN_X_SILU_MUL 1
 #define AGB200_CHAIN_X_SUM_PARTS 2
+#define AGB200_CHAIN_X_RMSNORM 3
+#define AGB200_CHAIN_X_ADD_RMSNORM 4
+#define AGB200_CHAIN_NORM_MAX_K 16384
 #define AGB200_CHAIN_DEBUG_NO_DEPS 1   /* measurement aid: do not wait for x (results are garbage) */
 #define AGB200_CHAIN_DEBUG_NO_MATH 2   /* measurement aid: consumers only free ring slots (results are garbage) */
 #define AGB200_CHAIN_DEBUG_NO_CONVERT 4 /* measurement aid: x is not re-read per stage (results are garbage) */
@@ -235,11 +251,27 @@ typedef struct agb200_chain_stage {
   agb200_chain_layer layer[4];
 } agb200_chain_stage;
 
+/* Parameters of the norm stage inputs (X_RMSNORM / X_ADD_RMSNORM), one entry per stage, parallel to the stage array of
+ * agb200_chain_plan_bytes_norm / agb200_chain_create_norm; entries of other stages are ignored.  A separate array keeps
+ * agb200_chain_stage, and so every existing caller, binary compatible. */
+typedef struct agb200_chain_norm {
+  const void* weight;       /* [K] of the chain's dtype */
+  void* residual_out;       /* X_ADD_RMSNORM: [M, K] of the chain's dtype that h is written to; X_RMSNORM: NULL */
+  float eps;                /* the variance epsilon, > 0 */
+  int32_t reserved;
+} agb200_chain_norm;
+
 size_t agb200_chain_plan_bytes(const agb200_chain_stage* stages, int n_stages, int M);
 /* Bytes of one X_SUM_PARTS buffer: parts * M * K / 2 words of 8 bytes. */
 size_t agb200_chain_parts_bytes(int parts, int M, int K);
 int agb200_chain_create(const agb200_chain_stage* stages, int n_stages, int M, int dtype, void* plan, size_t plan_bytes,
                         void** handle_out);
+/* The same with norm stage inputs: `norms` is NULL (then these are agb200_chain_plan_bytes / agb200_chain_create) or
+ * holds n_stages entries.  AGB200_EINVAL names a missing weight or residual_out, eps <= 0, or a misaligned pointer;
+ * AGB200_ENOSUP a norm stage with K > AGB200_CHAIN_NORM_MAX_K. */
+size_t agb200_chain_plan_bytes_norm(const agb200_chain_stage* stages, const agb200_chain_norm* norms, int n_stages, int M);
+int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chain_norm* norms, int n_stages, int M,
+                             int dtype, void* plan, size_t plan_bytes, void** handle_out);
 /* flags: 0, or AGB200_CHAIN_DEBUG_* bits (benchmarks only). */
 int agb200_chain_forward(void* handle, int flags, void* stream);
 int agb200_chain_destroy(void* handle);
