@@ -10,6 +10,7 @@ Only what the path needs lives here:
   mlp.py           forward_gate_up / FusedQuantMLP / inject_fused_mlp: a dense MLP's gate, up and silu * mul in one launch
   chain.py         DecodeChain: dependent QuantLinear stages (with residual adds and RMSNorms) in one persistent launch
   decoder.py       ChainDecoder: greedy decoding of a Llama / Mistral / Qwen2 model, one chain launch per decoder block
+  attention.py     decode_attention: rotary embedding, KV-cache write and split-KV attention of one layer in one launch
   gptq.py          GPTQ: the quantiser (Hessian accumulation + blocked quantisation) writing packed 4-bit layers
   awq.py           AWQ GEMM packed layers -> the GPTQ layout (exact integer re-layout, used by the loader)
   checkpoint.py    safetensors GPTQ / AWQ checkpoint -> QuantLinear modules, TP-aware (SURVEY.md 8f rank 1; `from autogptq_b200 import checkpoint`)

@@ -29,6 +29,9 @@ MOE_MAX_EXPERTS = 256
 MOE_INDEX_I32, MOE_INDEX_I64, MOE_WEIGHTS_F32 = 0, 1, 2
 GATE_UP_AUTO, GATE_UP_DECODE, GATE_UP_GEMM = 0, 1, 2
 DGRAD_AUTO, DGRAD_CUDA_CORE, DGRAD_WGMMA = 0, 1, 2
+ATTN_HEAD_DIMS = (64, 128)
+ATTN_MAX_G = 8
+ATTN_MAX_B = 2
 
 _lib = None
 
@@ -97,6 +100,8 @@ def _declare(lib):
         "agb200_gptq_hessian_update": (I, [P, P, I, I, I, c_float, c_float, P]),
         "agb200_gptq_quantize": (I, [P, P, P, P, I, I, I, I, I, P, P, P, P, P, P, P, I, P, S, P]),
         "agb200_gptq_workspace_bytes": (S, [I, I, I]),
+        "agb200_decode_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
+        "agb200_decode_attention_workspace_bytes": (S, [I, I, I, I, I]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

@@ -1,0 +1,117 @@
+// Host side of the decode attention (include/autogptq_b200.h: agb200_decode_attention*): argument checking, the split
+// count, workspace layout and the launch on the caller's stream.  Kernel: attention.cuh.
+#include <cuda_runtime.h>
+
+#include <cstdarg>
+#include <cstdio>
+
+#include "../../include/autogptq_b200.h"
+#include "attention.cuh"
+#include "internal.h"
+
+namespace {
+
+int failf(int code, const char* fmt, ...) {
+  char buf[400];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  return agb_internal_fail(code, buf);
+}
+
+#define AT_CUDA(expr)                                                                           \
+  do {                                                                                          \
+    cudaError_t e_ = (expr);                                                                    \
+    if (e_ != cudaSuccess) return failf(AGB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
+  } while (0)
+
+size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
+bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+// Splits of the sequence per (b, kv head): about four CTAs per SM over the whole grid, at most one per tile of the cache.
+// Depends only on the shape and the device, so one launch configuration serves every position (graph capture).
+int attn_splits(int B, int n_kv, int max_length) {
+  int dev = 0, sms = 132;
+  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
+    sms = 132;
+  const int want = (4 * sms + B * n_kv - 1) / (B * n_kv);
+  const int tiles = (max_length + agb::kAttnTile - 1) / agb::kAttnTile;
+  int s = want < tiles ? want : tiles;
+  if (s > agb::kAttnMaxSplits) s = agb::kAttnMaxSplits;
+  return s < 1 ? 1 : s;
+}
+
+size_t counter_bytes(int B, int n_kv) { return align_up(size_t(B) * n_kv * sizeof(unsigned), 256); }
+
+}  // namespace
+
+extern "C" {
+
+size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int head_dim, int max_length) {
+  if (B <= 0 || n_heads <= 0 || n_kv <= 0 || head_dim <= 0 || max_length <= 0 || n_heads % n_kv != 0) return 0;
+  const int S = attn_splits(B, n_kv, max_length);
+  return counter_bytes(B, n_kv) +
+         align_up(size_t(B) * n_kv * S * agb::attn_part_floats(n_heads / n_kv, head_dim) * sizeof(float), 256);
+}
+
+int agb200_decode_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int64_t* pos,
+                            const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
+                            int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  if (!q || !k || !v || !k_cache || !v_cache || !pos || !inv_freq || !out || !workspace)
+    return failf(AGB200_EINVAL, "decode_attention: null pointer argument");
+  if (B <= 0 || n_heads <= 0 || n_kv <= 0 || head_dim <= 0 || max_length <= 0 || n_heads % n_kv != 0)
+    return failf(AGB200_EINVAL, "decode_attention: need positive B, n_heads, n_kv, head_dim, max_length and "
+                 "n_heads %% n_kv == 0 (got B=%d, n_heads=%d, n_kv=%d, head_dim=%d, max_length=%d)",
+                 B, n_heads, n_kv, head_dim, max_length);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16)
+    return failf(AGB200_ENOSUP, "decode_attention: dtype %d; only AGB200_F16 and AGB200_BF16 are supported", dtype);
+  if (head_dim != 64 && head_dim != 128)
+    return failf(AGB200_ENOSUP, "decode_attention: head_dim %d; supported: 64, 128", head_dim);
+  if (n_heads / n_kv > agb::kAttnMaxG)
+    return failf(AGB200_ENOSUP, "decode_attention: %d query heads per kv head; at most %d", n_heads / n_kv, agb::kAttnMaxG);
+  if (B > agb::kAttnMaxB) return failf(AGB200_ENOSUP, "decode_attention: batch %d; at most %d", B, agb::kAttnMaxB);
+  if (static_cast<long long>(B) * n_kv * max_length * head_dim >= (1ll << 31))
+    return failf(AGB200_ENOSUP, "decode_attention: the cache holds %lld elements; at most 2^31 - 1",
+                 static_cast<long long>(B) * n_kv * max_length * head_dim);
+  if (!aligned(q, 16) || !aligned(k, 16) || !aligned(v, 16) || !aligned(k_cache, 16) || !aligned(v_cache, 16) ||
+      !aligned(out, 16) || !aligned(pos, 8) || !aligned(inv_freq, 4) || !aligned(workspace, 256))
+    return failf(AGB200_EINVAL, "decode_attention: q, k, v, the caches and out must be 16-byte aligned, the workspace "
+                 "256-byte aligned");
+  const size_t need = agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, head_dim, max_length);
+  if (workspace_bytes < need)
+    return failf(AGB200_EWORKSPACE, "decode_attention: workspace needs %zu bytes (got %zu)", need, workspace_bytes);
+
+  agb::DecodeAttnParams p{};
+  p.q = static_cast<const uint16_t*>(q);
+  p.k = static_cast<const uint16_t*>(k);
+  p.v = static_cast<const uint16_t*>(v);
+  p.k_cache = static_cast<uint16_t*>(k_cache);
+  p.v_cache = static_cast<uint16_t*>(v_cache);
+  p.pos = reinterpret_cast<const long long*>(pos);
+  p.inv_freq = inv_freq;
+  p.attn_scaling = attention_scaling;
+  p.scaling = scaling;
+  p.out = static_cast<uint16_t*>(out);
+  p.counter = static_cast<unsigned*>(workspace);
+  p.part = reinterpret_cast<float*>(static_cast<unsigned char*>(workspace) + counter_bytes(B, n_kv));
+  p.n_heads = n_heads;
+  p.n_kv = n_kv;
+  p.max_length = max_length;
+  p.splits = attn_splits(B, n_kv, max_length);
+  const dim3 grid(p.splits, n_kv, B);
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  const bool bf16 = dtype == AGB200_BF16;
+  if (head_dim == 128) {
+    if (bf16) agb::decode_attention_kernel<true, 128><<<grid, agb::kAttnThreads, 0, s>>>(p);
+    else agb::decode_attention_kernel<false, 128><<<grid, agb::kAttnThreads, 0, s>>>(p);
+  } else {
+    if (bf16) agb::decode_attention_kernel<true, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
+    else agb::decode_attention_kernel<false, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
+  }
+  AT_CUDA(cudaGetLastError());
+  return 0;
+}
+
+}  // extern "C"

@@ -1,0 +1,281 @@
+// Decode attention of one layer in one launch: rotary embedding of q and k, the KV-cache write at a device-side
+// position, and split-KV attention over positions [0, pos] with a last-arriving-CTA combine (DESIGN §3.16).
+#pragma once
+#include <math.h>
+
+#include "common.cuh"
+
+namespace agb {
+
+constexpr int kAttnThreads = 128;      // 4 warps
+constexpr int kAttnTile = 32;          // positions per shared-memory tile (one per lane in the score phase)
+constexpr int kAttnMaxG = 8;           // query heads per kv head
+constexpr int kAttnMaxSplits = 64;
+constexpr int kAttnMaxB = 2;
+
+// Floats of one split's partials: acc[G][hd], then m and l of up to kAttnMaxG heads (keeps every split 16-byte aligned)
+__host__ __device__ constexpr int attn_part_floats(int G, int hd) { return G * hd + 2 * kAttnMaxG; }
+
+struct DecodeAttnParams {
+  const uint16_t* q;        // [B, n_heads·hd]
+  const uint16_t* k;        // [B, n_kv·hd]
+  const uint16_t* v;        // [B, n_kv·hd]
+  uint16_t* k_cache;        // [B, n_kv, max_length, hd]
+  uint16_t* v_cache;
+  const long long* pos;     // device scalar
+  const float* inv_freq;    // [hd/2]
+  float attn_scaling;       // the rotary embedding's attention_scaling
+  float scaling;            // softmax scale σ
+  uint16_t* out;            // [B, n_heads·hd]
+  float* part;              // [B, n_kv, splits, attn_part_floats(G, hd)]: acc[G][hd], m[8], l[8] of each split
+  unsigned* counter;        // [B·n_kv] arrivals; zero between launches
+  int n_heads, n_kv, max_length, splits;
+};
+
+template <int kHd>
+struct AttnSmem {
+  static constexpr int kKRow = kHd + 8;   // padded K row: 32 lanes reading 16 B of 32 different rows hit distinct banks
+  uint16_t k[2][kAttnTile * kKRow];
+  uint16_t v[2][kAttnTile * kHd];
+  float q[kAttnMaxG][kHd];                // q̂ (already rounded to the dtype), widened
+  float p[kAttnMaxG][kAttnTile];          // softmax weights of the current tile
+  float scale[kAttnMaxG];                 // rescale of the running sums at this tile
+  float wt[kAttnMaxSplits][kAttnMaxG];    // combine weights
+  float lsum[kAttnMaxG];
+  uint16_t knew[kHd], vnew[kHd];          // k̂ and v of the new token
+  int last;
+};
+
+template <bool kBf16>
+__device__ __forceinline__ float rnd_elt(float x) { return elt_to_float<kBf16>(float_to_elt<kBf16>(x)); }
+
+// transformers' rotary embedding, rounding step by step as torch does:
+//   f = fp32(inv_freq[j mod hd/2] · pos), c = rnd(fp32(cosf(f) · a)), s = rnd(fp32(sinf(f) · a)),
+//   x̂[j] = rnd(rnd(x[j]·c) + rnd(rotate_half(x)[j]·s))
+template <bool kBf16, int kHd>
+__device__ __forceinline__ float rope_elt(const uint16_t* x, int j, const float* inv_freq, float fpos, float a) {
+  constexpr int kH2 = kHd / 2;
+  const float f = __fmul_rn(inv_freq[j % kH2], fpos);
+  const float c = rnd_elt<kBf16>(__fmul_rn(cosf(f), a));
+  const float s = rnd_elt<kBf16>(__fmul_rn(sinf(f), a));
+  const float xj = elt_to_float<kBf16>(x[j]);
+  const float r = j < kH2 ? -elt_to_float<kBf16>(x[j + kH2]) : elt_to_float<kBf16>(x[j - kH2]);
+  return rnd_elt<kBf16>(__fadd_rn(rnd_elt<kBf16>(__fmul_rn(xj, c)), rnd_elt<kBf16>(__fmul_rn(r, s))));
+}
+
+__device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem))),
+               "l"(gmem) : "memory");
+}
+
+template <int kN>
+__device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(kN) : "memory"); }
+__device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
+
+__device__ __forceinline__ float warp_max(float x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x = fmaxf(x, __shfl_xor_sync(0xffffffffu, x, o));
+  return x;
+}
+// Tree sum in a fixed order; every lane gets lane 0's result.
+__device__ __forceinline__ float warp_sum(float x) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) x = __fadd_rn(x, __shfl_down_sync(0xffffffffu, x, o));
+  return __shfl_sync(0xffffffffu, x, 0);
+}
+
+// Grid (splits, n_kv, B), kAttnThreads threads.  CTA (b, kv head, split i) owns positions [i·C, min((i+1)·C, pos+1)),
+// C = ceil((pos+1) / splits), for the G query heads of its kv head.
+template <bool kBf16, int kHd>
+__global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const DecodeAttnParams p) {
+  using Smem = AttnSmem<kHd>;
+  constexpr int kKRow = Smem::kKRow;
+  constexpr int kChunks = kHd / 8;                     // 16-byte chunks of a row
+  constexpr int kDimThreads = kHd / 4;                 // PV: 4 output dims per thread
+  constexpr int kHeadsPerPass = kAttnThreads / kDimThreads;
+  constexpr int kHpt = (kAttnMaxG + kHeadsPerPass - 1) / kHeadsPerPass;
+  __shared__ __align__(16) Smem sm;
+
+  const int split = blockIdx.x, kvh = blockIdx.y, b = blockIdx.z;
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  const int G = p.n_heads / p.n_kv;
+  const int S = p.splits;
+  const long long pos64 = *p.pos;
+  const int head0 = kvh * G;
+  uint16_t* out = p.out + (size_t(b) * p.n_heads + head0) * kHd;
+  if (pos64 < 0 || pos64 >= p.max_length) {            // nothing to attend to: a NaN output, caches untouched
+    for (int i = tid; i < G * kHd; i += kAttnThreads) out[i] = float_to_elt<kBf16>(__int_as_float(0x7fffffff));
+    return;
+  }
+  const int pos = static_cast<int>(pos64);
+  const int n = pos + 1;
+  const int C = (n + S - 1) / S;
+  const int t0 = min(split * C, n), t1 = min(t0 + C, n);
+  const unsigned cache0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) * kHd;   // < 2^31 (host check)
+  const float fpos = __int2float_rn(pos);
+
+  const uint16_t* qrow = p.q + (size_t(b) * p.n_heads + head0) * kHd;
+  for (int i = tid; i < G * kHd; i += kAttnThreads)
+    sm.q[i / kHd][i % kHd] = rope_elt<kBf16, kHd>(qrow + (i / kHd) * kHd, i % kHd, p.inv_freq, fpos, p.attn_scaling);
+  const bool owner = t0 <= pos && pos < t1;           // exactly one split per (b, kv head) holds the new token
+  if (owner) {
+    const uint16_t* krow = p.k + (size_t(b) * p.n_kv + kvh) * kHd;
+    const uint16_t* vrow = p.v + (size_t(b) * p.n_kv + kvh) * kHd;
+    for (int j = tid; j < kHd; j += kAttnThreads) {
+      const uint16_t kn = float_to_elt<kBf16>(rope_elt<kBf16, kHd>(krow, j, p.inv_freq, fpos, p.attn_scaling));
+      sm.knew[j] = kn;
+      sm.vnew[j] = vrow[j];
+      p.k_cache[cache0 + unsigned(pos) * kHd + j] = kn;
+      p.v_cache[cache0 + unsigned(pos) * kHd + j] = vrow[j];
+    }
+  }
+  __syncthreads();
+
+  const int n_tiles = (t1 - t0 + kAttnTile - 1) / kAttnTile;
+  // K and V rows of one tile into buffer `buf`; the new token's row comes from knew / vnew, never from the cache.
+  auto load_tile = [&](int it, int buf) {
+    const int ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
+    for (int i = tid; i < nv * kChunks; i += kAttnThreads) {
+      const int r = i / kChunks, c = i % kChunks, t = ts + r;
+      uint16_t* ks = &sm.k[buf][r * kKRow + c * 8];
+      uint16_t* vs = &sm.v[buf][r * kHd + c * 8];
+      if (t == pos) {
+        *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 8]);
+        *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 8]);
+      } else {
+        const unsigned g = cache0 + unsigned(t) * kHd + c * 8;
+        cp_async16(ks, p.k_cache + g);
+        cp_async16(vs, p.v_cache + g);
+      }
+    }
+    cp_async_commit();
+  };
+  if (n_tiles > 0) load_tile(0, 0);
+  if (n_tiles > 1) load_tile(1, 1);
+
+  float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // score role: heads warp, warp + 4
+  float acc[kHpt][4];
+#pragma unroll
+  for (int k = 0; k < kHpt; ++k)
+#pragma unroll
+    for (int e = 0; e < 4; ++e) acc[k][e] = 0.f;
+  const int dgrp = tid % kDimThreads, hbase = tid / kDimThreads;
+
+  for (int it = 0; it < n_tiles; ++it) {
+    if (it + 1 < n_tiles) cp_async_wait<1>();
+    else cp_async_wait<0>();
+    __syncthreads();
+    const int buf = it & 1, ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
+
+    // scores: lane = position of the tile, warp = heads {warp, warp + 4}; one fp32 FMA chain over d per head
+    float s[2] = {0.f, 0.f};
+    const uint16_t* krow = &sm.k[buf][lane * kKRow];
+#pragma unroll 4
+    for (int c = 0; c < kChunks; ++c) {
+      const uint4 kv = *reinterpret_cast<const uint4*>(krow + c * 8);
+      const uint32_t w[4] = {kv.x, kv.y, kv.z, kv.w};
+      float kf[8];
+#pragma unroll
+      for (int e = 0; e < 4; ++e) {
+        kf[2 * e] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] & 0xffffu));
+        kf[2 * e + 1] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] >> 16));
+      }
+#pragma unroll
+      for (int hh = 0; hh < 2; ++hh) {
+        const int h = warp + 4 * hh;
+        if (h < G) {
+          const float4 qa = *reinterpret_cast<const float4*>(&sm.q[h][c * 8]);
+          const float4 qb = *reinterpret_cast<const float4*>(&sm.q[h][c * 8 + 4]);
+          s[hh] = fmaf(qa.x, kf[0], s[hh]); s[hh] = fmaf(qa.y, kf[1], s[hh]);
+          s[hh] = fmaf(qa.z, kf[2], s[hh]); s[hh] = fmaf(qa.w, kf[3], s[hh]);
+          s[hh] = fmaf(qb.x, kf[4], s[hh]); s[hh] = fmaf(qb.y, kf[5], s[hh]);
+          s[hh] = fmaf(qb.z, kf[6], s[hh]); s[hh] = fmaf(qb.w, kf[7], s[hh]);
+        }
+      }
+    }
+#pragma unroll
+    for (int hh = 0; hh < 2; ++hh) {
+      const int h = warp + 4 * hh;
+      if (h < G) {
+        const float sc = lane < nv ? __fmul_rn(s[hh], p.scaling) : -INFINITY;
+        const float mn = fmaxf(m_run[hh], warp_max(sc));        // finite: the tile holds at least one position
+        const float e = expf(__fsub_rn(sc, mn));
+        const float rescale = expf(__fsub_rn(m_run[hh], mn));  // 0 at the first tile
+        l_run[hh] = fmaf(l_run[hh], rescale, warp_sum(e));
+        m_run[hh] = mn;
+        sm.p[h][lane] = e;
+        if (lane == 0) sm.scale[h] = rescale;
+      }
+    }
+    __syncthreads();
+
+    // Σ p·v: thread = 4 dims of heads hbase + k·kHeadsPerPass; rows past nv are never read
+#pragma unroll
+    for (int k = 0; k < kHpt; ++k) {
+      const int h = hbase + k * kHeadsPerPass;
+      if (h < G) {
+        const float r = sm.scale[h];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) acc[k][e] = __fmul_rn(acc[k][e], r);
+        for (int t = 0; t < nv; ++t) {
+          const float pt = sm.p[h][t];
+          const uint2 vv = *reinterpret_cast<const uint2*>(&sm.v[buf][t * kHd + dgrp * 4]);
+          acc[k][0] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x & 0xffffu)), acc[k][0]);
+          acc[k][1] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x >> 16)), acc[k][1]);
+          acc[k][2] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y & 0xffffu)), acc[k][2]);
+          acc[k][3] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y >> 16)), acc[k][3]);
+        }
+      }
+    }
+    __syncthreads();
+    if (it + 2 < n_tiles) load_tile(it + 2, buf);
+  }
+
+  // partials of this split (an empty split stores m = -inf, l = 0, acc = 0)
+  const int stride = attn_part_floats(G, kHd);
+  const unsigned bk = unsigned(b * p.n_kv + kvh);
+  float* part = p.part + (size_t(bk) * S + split) * stride;
+#pragma unroll
+  for (int k = 0; k < kHpt; ++k) {
+    const int h = hbase + k * kHeadsPerPass;
+    if (h < G) *reinterpret_cast<float4*>(&part[h * kHd + dgrp * 4]) = make_float4(acc[k][0], acc[k][1], acc[k][2], acc[k][3]);
+  }
+#pragma unroll
+  for (int hh = 0; hh < 2; ++hh) {
+    const int h = warp + 4 * hh;
+    if (h < G && lane == 0) {
+      part[G * kHd + h] = m_run[hh];
+      part[G * kHd + kAttnMaxG + h] = l_run[hh];
+    }
+  }
+  __threadfence();
+  __syncthreads();
+  if (tid == 0) sm.last = atomicAdd(&p.counter[bk], 1u) == unsigned(S - 1);
+  __syncthreads();
+  if (!sm.last) return;
+  __threadfence();
+
+  // last CTA of (b, kv head): combine the splits in split order
+  const float* parts = p.part + size_t(bk) * S * stride;
+  if (tid < G) {
+    float M = -INFINITY;
+    for (int i = 0; i < S; ++i) M = fmaxf(M, __ldcg(&parts[i * stride + G * kHd + tid]));
+    float L = 0.f;
+    for (int i = 0; i < S; ++i) {
+      const float w = expf(__fsub_rn(__ldcg(&parts[i * stride + G * kHd + tid]), M));   // empty split: 0
+      sm.wt[i][tid] = w;
+      L = fmaf(__ldcg(&parts[i * stride + G * kHd + kAttnMaxG + tid]), w, L);
+    }
+    sm.lsum[tid] = L;
+  }
+  __syncthreads();
+  for (int i = tid; i < G * kHd; i += kAttnThreads) {
+    const int h = i / kHd;
+    float o = 0.f;
+    for (int j = 0; j < S; ++j) o = fmaf(__ldcg(&parts[j * stride + i]), sm.wt[j][h], o);
+    out[i] = float_to_elt<kBf16>(__fdiv_rn(o, sm.lsum[h]));
+  }
+  if (tid == 0) p.counter[bk] = 0u;                   // ready for the next launch (graph replays)
+}
+
+}  // namespace agb

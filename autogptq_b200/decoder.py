@@ -19,6 +19,11 @@ device-side position, and ``F.scaled_dot_product_attention`` with GQA and a leng
 the next chain's o_proj input buffer.  The final add, ``model.model.norm`` and ``lm_head`` run in torch.  One token is
 then n_layers + 1 chain launches and n_layers attentions, captured together in one CUDA graph.
 
+``fused_attention=True`` runs each attention as one ``agb200_decode_attention`` launch instead (rotary embedding, cache
+write and split-KV attention, ``autogptq_b200.attention``): a token is then 2·n_layers + 1 launches of the project's own
+kernels plus the embedding, final norm and lm_head.  It rounds differently from SDPA (fp32 online softmax), so it is
+opt-in.
+
 Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  What does not fit raises
 NotImplementedError naming the module.
 """
@@ -28,6 +33,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
+from .attention import attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
 from .mlp import FusedQuantMLP, _is_silu
 from .qlinear import QuantLinear
@@ -83,6 +89,21 @@ def _plan_layer(i: int, layer, batch: int, dtype):
     return attn, mlp, ln1, ln2
 
 
+def _rotary_params(rotary, head_dim: int):
+    """(inv_freq fp32 [head_dim/2], attention_scaling) of a rotary embedding whose frequencies do not depend on the
+    sequence length; default, linear, llama3 and yarn all reduce to these two."""
+    rope_type = getattr(rotary, "rope_type", "default")
+    if rope_type in ("dynamic", "longrope"):
+        raise NotImplementedError(f"ChainDecoder(fused_attention=True): model.model.rotary_emb is {rope_type!r} rope, "
+                                  "whose inv_freq changes with the sequence length; a captured graph cannot follow it")
+    inv_freq = getattr(rotary, "inv_freq", None)
+    if inv_freq is None or inv_freq.dim() != 1 or inv_freq.numel() != head_dim // 2:
+        n = None if inv_freq is None else tuple(inv_freq.shape)
+        raise NotImplementedError(f"ChainDecoder(fused_attention=True): model.model.rotary_emb.inv_freq has shape {n}, "
+                                  f"not [{head_dim // 2}] (partial rotary is not supported)")
+    return inv_freq.detach().to(torch.float32).contiguous(), float(getattr(rotary, "attention_scaling", 1.0))
+
+
 def _check_window(config, max_length: int):
     sw = getattr(config, "sliding_window", None)
     if getattr(config, "use_sliding_window", True) is False:
@@ -94,9 +115,10 @@ def _check_window(config, max_length: int):
 
 class ChainDecoder:
     """Greedy decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
-    projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too)."""
+    projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too).  ``fused_attention``:
+    run each layer's attention as one CUDA launch (``autogptq_b200.attention.decode_attention``) instead of torch."""
 
-    def __init__(self, model, batch: int = 1, max_length: int = 2048):
+    def __init__(self, model, batch: int = 1, max_length: int = 2048, fused_attention: bool = False):
         if not 1 <= batch <= _lib.CHAIN_MAX_M:
             raise NotImplementedError(f"ChainDecoder: batch {batch}; the decode chain runs 1..{_lib.CHAIN_MAX_M} rows")
         inner = getattr(model, "model", None)
@@ -112,6 +134,14 @@ class ChainDecoder:
         self.dtype = inner.embed_tokens.weight.dtype
         if self.dtype not in (torch.float16, torch.bfloat16):
             raise NotImplementedError(f"ChainDecoder: activations are {self.dtype}; the chain computes in fp16 / bf16")
+        self.fused_attention = bool(fused_attention)
+        if self.fused_attention:
+            hd = getattr(cfg, "head_dim", None) or cfg.hidden_size // cfg.num_attention_heads
+            n_kv = getattr(cfg, "num_key_value_heads", None) or cfg.num_attention_heads
+            why = attention_supported(cfg.num_attention_heads, n_kv, hd, batch, self.max_length, self.dtype)
+            if why is not None:
+                raise NotImplementedError(f"ChainDecoder(fused_attention=True): model.layers.*.self_attn: {why}")
+            self._inv_freq, self._attn_scaling = _rotary_params(inner.rotary_emb, hd)
         self.device = inner.embed_tokens.weight.device
         if self.device.type != "cuda":
             raise RuntimeError("ChainDecoder needs the model on a CUDA device")
@@ -133,6 +163,8 @@ class ChainDecoder:
         self._ids = torch.zeros(B, dtype=torch.int64, device=dev)
         self._arange = torch.arange(self.max_length, device=dev)
         self._length = 0                                                    # host copy of the position
+        if self.fused_attention:                                            # shared by the layers (one stream)
+            self._attn_ws = decode_attention_workspace(B, self.n_heads, self.n_kv, self.head_dim, self.max_length, dev)
 
         # chain_0 = [input_layernorm_0 -> q|k|v_0]
         self.chains = []
@@ -214,16 +246,27 @@ class ChainDecoder:
                                            enable_gqa=self.n_kv != self.n_heads)
         self._attn_in[i].copy_(o.transpose(1, 2).reshape(B, -1))
 
+    def _fused_attention(self, i: int):
+        q, k, v = self._qkv[i]
+        decode_attention(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq, self._attn_scaling,
+                         self.scaling, self._attn_in[i], self._attn_ws)
+
     def _step_body(self) -> torch.Tensor:
         inner = self.model.model
         self._x0.copy_(inner.embed_tokens(self._ids))
-        pos_ids = self._pos.view(1, 1).expand(self.batch, 1)
-        cos, sin = inner.rotary_emb(self._x0.view(self.batch, 1, -1), pos_ids)
-        mask = (self._arange <= self._pos).view(1, 1, 1, -1)
-        self.chains[0].run()
-        for i in range(len(self._attn_in)):
-            self._attention(i, cos, sin, mask)
-            self.chains[i + 1].run()
+        if self.fused_attention:
+            self.chains[0].run()
+            for i in range(len(self._attn_in)):
+                self._fused_attention(i)
+                self.chains[i + 1].run()
+        else:
+            pos_ids = self._pos.view(1, 1).expand(self.batch, 1)
+            cos, sin = inner.rotary_emb(self._x0.view(self.batch, 1, -1), pos_ids)
+            mask = (self._arange <= self._pos).view(1, 1, 1, -1)
+            self.chains[0].run()
+            for i in range(len(self._attn_in)):
+                self._attention(i, cos, sin, mask)
+                self.chains[i + 1].run()
         h1, down = self._last
         n = self._final_norm(h1 + down)
         logits = self.model.lm_head(n)

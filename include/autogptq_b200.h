@@ -575,6 +575,33 @@ int agb200_w4_dequantize(const int32_t* qweight, const int32_t* qzeros, const vo
 int agb200_permute_columns(const void* x, const int32_t* perm, void* x_out, int M, int K, int dtype,
                            void* stream);
 
+/*
+ * One decode step of one attention layer (a Llama / Mistral / Qwen2 block at batch B <= 2, sequences in lockstep), in
+ * one launch on `stream`, all pointers DEVICE memory:
+ *   q [B, n_heads*head_dim], k and v [B, n_kv*head_dim]   the projections' outputs (bias included), dtype
+ *   k_cache, v_cache [B, n_kv, max_length, head_dim]       contiguous static caches, dtype
+ *   pos                                                     int64 scalar: the position this token is written to
+ *   inv_freq [head_dim/2] (fp32), attention_scaling         the rotary embedding (transformers' rotary_emb)
+ *   scaling                                                 the softmax scale
+ *   out [B, n_heads*head_dim]                               attention output (before o_proj), dtype
+ * The kernel applies the rotary embedding to q and k with transformers' roundings (every step rounds to the dtype as
+ * torch does, cosf / sinf of fp32(inv_freq*pos)), writes k-hat and v to position pos of the caches, and attends query
+ * head h (kv head h / (n_heads/n_kv)) over positions 0..pos: fp32 scores, a running-max fp32 softmax and fp32 sums,
+ * the output rounded once.  No position above pos is read or written; a pos outside [0, max_length) writes NaN to out
+ * and leaves the caches untouched.  Two calls on the same input are bit-identical (no atomics in any sum).
+ * `workspace` holds agb200_decode_attention_workspace_bytes(...) bytes (the value depends on the current device), is
+ * 256-byte aligned, and must be zero before the first call; every call leaves its counter words zero again, so one
+ * workspace serves any number of calls of the same shape on one stream, captured in a CUDA graph or not.
+ * Constraints (else AGB200_ENOSUP): dtype AGB200_F16 / AGB200_BF16, head_dim 64 or 128, n_heads/n_kv <= 8, B <= 2,
+ * B*n_kv*max_length*head_dim < 2^31.  q, k, v, the caches and out 16-byte aligned (else AGB200_EINVAL).
+ * The reference runs this step in torch (auto_gptq/nn_modules/fused_llama_attn.py:59-98).
+ */
+int agb200_decode_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int64_t* pos,
+                            const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
+                            int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                            void* stream);
+size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int head_dim, int max_length);
+
 /* Static facts about the build, for logs: returns e.g. "autogptq_b200 sm_90a: ... gemm=wgmma ...". */
 const char* agb200_build_info(void);
 

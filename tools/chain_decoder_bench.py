@@ -2,7 +2,12 @@
 decoder block, attention in torch between them) against the HF model's own eager decode step with the same QuantLinears,
 with and without inject_fused_mlp.
 
-    python tools/chain_decoder_bench.py [--layers 32] [--prompt 512] [--steps 128] [--batch 1]
+    python tools/chain_decoder_bench.py [--layers 32] [--prompt 512] [--steps 128] [--batch 1] [--attention torch]
+
+``--attention`` picks ChainDecoder's attention: ``torch`` (the default path; the HF baselines run too), ``fused``
+(``fused_attention=True``) or ``both`` (the two decoders alternated, torch / fused / torch / fused, in one run; no HF
+baselines).  Each ChainDecoder record has tokens/s and the split of a token between the chain launches, the attentions
+and the rest.
 
 Weights are synthetic, packed like bench.py's (uniform nibbles, unit-gain signed scales), with random norm weights, an
 fp16 lm_head and embedding.  Prints one JSON line: tokens/s of each path, the split of a ChainDecoder token between the
@@ -90,6 +95,7 @@ def main():
     ap.add_argument("--prompt", type=int, default=512)
     ap.add_argument("--steps", type=int, default=128)
     ap.add_argument("--batch", type=int, default=1)
+    ap.add_argument("--attention", choices=("torch", "fused", "both"), default="torch")
     args = ap.parse_args()
     from transformers import DynamicCache
 
@@ -104,41 +110,61 @@ def main():
     prompt = torch.randint(0, 32000, (B, T), device=dev, generator=torch.Generator(device=dev).manual_seed(1))
     rec = {"gpu": name, "power_limit": power, "layers": args.layers, "batch": B, "prompt": T, "steps": S}
 
-    # ChainDecoder: graph per token
-    dec = ChainDecoder(model, batch=B, max_length=T + S + 8)
-    rec["block_chain_info"] = dec.chains[1].info()
-    rec["first_chain_info"] = dec.chains[0].info()
-    logits = dec.prefill(prompt)
-    tok = logits.argmax(-1)
-    for _ in range(3):                                   # capture + warm replays
-        tok = dec.step(tok).argmax(-1)
-    dec.position = T
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(S):
-        tok = dec.step(tok).argmax(-1)
-    e1.record()
-    torch.cuda.synchronize()
-    ms = e0.elapsed_time(e1) / S
-    rec["chain_decoder_ms_per_token"] = ms
-    rec["chain_decoder_tokens_per_s"] = 1000.0 * B / ms
-
-    # split: the chains alone and the attentions alone, each as one graph, at the middle of the timed window
-    dec.position = T + S // 2
-    chains_ms = time_graph(lambda: [c.run() for c in dec.chains], 20)
     inner = model.model
 
-    def attn_only():
-        pos_ids = dec._pos.view(1, 1).expand(B, 1)
-        cos, sin = inner.rotary_emb(dec._x0.view(B, 1, -1), pos_ids)
-        mask = (dec._arange <= dec._pos).view(1, 1, 1, -1)
-        for i in range(len(dec._attn_in)):
-            dec._attention(i, cos, sin, mask)
+    def chain_decoder(fused):
+        """One ChainDecoder run: (ms per token, split) with one CUDA graph per token."""
+        dec = ChainDecoder(model, batch=B, max_length=T + S + 8, fused_attention=fused)
+        info = dec.chains[1].info(), dec.chains[0].info()
+        logits = dec.prefill(prompt)
+        tok = logits.argmax(-1)
+        for _ in range(3):                                   # capture + warm replays
+            tok = dec.step(tok).argmax(-1)
+        dec.position = T
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        for _ in range(S):
+            tok = dec.step(tok).argmax(-1)
+        e1.record()
+        torch.cuda.synchronize()
+        ms = e0.elapsed_time(e1) / S
 
-    attn_ms = time_graph(attn_only, 20)
-    rec["split_ms"] = {"chains": chains_ms, "attention": attn_ms, "rest": ms - chains_ms - attn_ms}
-    del dec
-    torch.cuda.empty_cache()
+        # split: the chains alone and the attentions alone, each as one graph, at the middle of the timed window
+        dec.position = T + S // 2
+        chains_ms = time_graph(lambda: [c.run() for c in dec.chains], 20)
+
+        def attn_only():
+            if fused:
+                for i in range(len(dec._attn_in)):
+                    dec._fused_attention(i)
+                return
+            pos_ids = dec._pos.view(1, 1).expand(B, 1)
+            cos, sin = inner.rotary_emb(dec._x0.view(B, 1, -1), pos_ids)
+            mask = (dec._arange <= dec._pos).view(1, 1, 1, -1)
+            for i in range(len(dec._attn_in)):
+                dec._attention(i, cos, sin, mask)
+
+        attn_ms = time_graph(attn_only, 20)
+        del dec
+        torch.cuda.empty_cache()
+        return ms, {"chains": chains_ms, "attention": attn_ms, "rest": ms - chains_ms - attn_ms}, info
+
+    if args.attention == "torch":
+        ms, split, info = chain_decoder(False)
+        rec["block_chain_info"], rec["first_chain_info"] = info
+        rec["chain_decoder_ms_per_token"] = ms
+        rec["chain_decoder_tokens_per_s"] = 1000.0 * B / ms
+        rec["split_ms"] = split
+    else:
+        order = ["torch", "fused", "torch", "fused"] if args.attention == "both" else ["fused"]
+        runs = {m: [] for m in order}
+        for m in order:
+            ms, split, info = chain_decoder(m == "fused")
+            runs[m].append({"ms_per_token": ms, "tokens_per_s": 1000.0 * B / ms, "split_ms": split})
+        rec["block_chain_info"], rec["first_chain_info"] = info
+        rec["chain_decoder"] = runs
+        print(json.dumps(rec))
+        return
 
     def hf_decode(what):
         cache = DynamicCache(config=model.config)
