@@ -6,10 +6,11 @@ Only what the path needs lives here:
   import_utils.py  mirror of ``dynamically_import_QuantLinear`` + the patch that installs it into auto_gptq
   sharding.py      column/row tensor-parallel slicing of packed layers (SURVEY.md 8e)
   tp.py            column/row parallel modules: one NCCL all-reduce per row-parallel layer
-  moe.py           QuantExperts: the routed experts of a Mixtral-style block as one grouped forward
+  moe.py           QuantExperts: the routed experts of a Mixtral-style block as one grouped forward; moe_router: its
+                   residual add, RMSNorm and top-k router for decode rows in one launch
   mlp.py           forward_gate_up / FusedQuantMLP / inject_fused_mlp: a dense MLP's gate, up and silu * mul in one launch
   chain.py         DecodeChain: dependent QuantLinear stages (with residual adds and RMSNorms) in one persistent launch
-  decoder.py       ChainDecoder: greedy decoding of a Llama / Mistral / Qwen2 model, one chain launch per decoder block
+  decoder.py       ChainDecoder: greedy decoding of a Llama / Mistral / Qwen2 / Mixtral model, one CUDA graph per token
   attention.py     decode_attention: rotary embedding, KV-cache write and split-KV attention of one layer in one launch
   gptq.py          GPTQ: the quantiser (Hessian accumulation + blocked quantisation) writing packed 4-bit layers
   awq.py           AWQ GEMM packed layers -> the GPTQ layout (exact integer re-layout, used by the loader)

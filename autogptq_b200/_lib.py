@@ -27,6 +27,7 @@ IMMA_MAX_M = 8
 MOE_DECODE_MAX_T = 8
 MOE_MAX_EXPERTS = 256
 MOE_INDEX_I32, MOE_INDEX_I64, MOE_WEIGHTS_F32 = 0, 1, 2
+MOE_ROUTER_MAX_TOP_K = 8
 GATE_UP_AUTO, GATE_UP_DECODE, GATE_UP_GEMM = 0, 1, 2
 DGRAD_AUTO, DGRAD_CUDA_CORE, DGRAD_WGMMA = 0, 1, 2
 ATTN_HEAD_DIMS = (64, 128)
@@ -102,6 +103,7 @@ def _declare(lib):
         "agb200_gptq_workspace_bytes": (S, [I, I, I]),
         "agb200_decode_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
         "agb200_decode_attention_workspace_bytes": (S, [I, I, I, I, I]),
+        "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

@@ -1,0 +1,76 @@
+// Host side of the MoE router (include/autogptq_b200.h: agb200_moe_router): argument checking and the launch on the
+// caller's stream.  Kernel: moe_router.cuh.
+#include <cuda_runtime.h>
+
+#include <cstdarg>
+#include <cstdio>
+
+#include "../../include/autogptq_b200.h"
+#include "internal.h"
+#include "moe_router.cuh"
+
+static_assert(agb::kRouterMaxH == AGB200_CHAIN_NORM_MAX_K, "router and chain norm share the hidden-size limit");
+static_assert(agb::kRouterMaxE == AGB200_MOE_MAX_EXPERTS, "router and grouped experts share the expert limit");
+static_assert(agb::kRouterMaxTopK == AGB200_MOE_ROUTER_MAX_TOP_K, "router top-k limit");
+
+namespace {
+
+int failf(int code, const char* fmt, ...) {
+  char buf[400];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  return agb_internal_fail(code, buf);
+}
+
+bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
+
+}  // namespace
+
+extern "C" {
+
+int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, int T,
+                      int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
+                      void* logits, void* stream) {
+  if (!x || !norm_weight || !gate_weight || !n || !top_k_index || !top_k_weights)
+    return failf(AGB200_EINVAL, "moe_router: null pointer argument");
+  if ((x2 == nullptr) != (h == nullptr)) return failf(AGB200_EINVAL, "moe_router: h is written exactly when x2 is given");
+  if (T < 0 || H <= 0 || E <= 0 || k <= 0)
+    return failf(AGB200_EINVAL, "moe_router: need T >= 0 and positive H, E, k (got T=%d, H=%d, E=%d, k=%d)", T, H, E, k);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16)
+    return failf(AGB200_ENOSUP, "moe_router: dtype %d; only AGB200_F16 and AGB200_BF16 are supported", dtype);
+  if (T > AGB200_MOE_DECODE_MAX_T) return failf(AGB200_ENOSUP, "moe_router: T=%d rows; at most %d", T, AGB200_MOE_DECODE_MAX_T);
+  if (H % 128 != 0 || H > AGB200_CHAIN_NORM_MAX_K)
+    return failf(AGB200_ENOSUP, "moe_router: H=%d must be a multiple of 128, at most %d", H, AGB200_CHAIN_NORM_MAX_K);
+  if (k > AGB200_MOE_ROUTER_MAX_TOP_K) return failf(AGB200_ENOSUP, "moe_router: k=%d; at most %d", k, AGB200_MOE_ROUTER_MAX_TOP_K);
+  if (E < k || E > AGB200_MOE_MAX_EXPERTS)
+    return failf(AGB200_ENOSUP, "moe_router: E=%d experts; need k=%d <= E <= %d", E, k, AGB200_MOE_MAX_EXPERTS);
+  if (!aligned(x, 16) || (x2 && !aligned(x2, 16)) || !aligned(norm_weight, 16) || !aligned(gate_weight, 16) ||
+      (h && !aligned(h, 16)) || !aligned(n, 16) || !aligned(top_k_index, 4) || !aligned(top_k_weights, 4) ||
+      (logits && !aligned(logits, 2)))
+    return failf(AGB200_EINVAL, "moe_router: x, x2, norm_weight, gate_weight, h and n must be 16-byte aligned");
+  if (T == 0) return 0;
+  agb::MoeRouterParams p{};
+  p.x = static_cast<const uint16_t*>(x);
+  p.x2 = static_cast<const uint16_t*>(x2);
+  p.norm_w = static_cast<const uint16_t*>(norm_weight);
+  p.gate = static_cast<const uint16_t*>(gate_weight);
+  p.h = static_cast<uint16_t*>(h);
+  p.n = static_cast<uint16_t*>(n);
+  p.idx = top_k_index;
+  p.wts = top_k_weights;
+  p.logits = static_cast<uint16_t*>(logits);
+  p.eps = eps;
+  p.H = H;
+  p.E = E;
+  p.k = k;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == AGB200_BF16) agb::moe_router_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
+  else agb::moe_router_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
+  const cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return failf(AGB200_ECUDA, "moe_router: launch: %s", cudaGetErrorString(e));
+  return 0;
+}
+
+}  // extern "C"

@@ -24,6 +24,19 @@ write and split-KV attention, ``autogptq_b200.attention``): a token is then 2·n
 kernels plus the embedding, final norm and lm_head.  It rounds differently from SDPA (fp32 online softmax), so it is
 opt-in.
 
+Mixtral-style models (``MixtralSparseMoeBlock`` MLPs whose ``experts`` are an ``autogptq_b200.QuantExperts``, see
+``autogptq_b200.moe``) decode through the same graph with a different block (DESIGN §3.17):
+
+    chain [o_i] -> moe_router: h1 = x + o, n2 = post_attention_layernorm(h1), logits, softmax, top-k, renormalise
+                -> QuantExperts on (n2, top_k_index, top_k_weights)
+                -> chain [add_rmsnorm(moe_i, h1; input_layernorm_i+1) -> q|k|v_i+1]
+
+so a token is 5 to 8 launches per layer (the experts' forward is several), all in one graph.  Every buffer, the experts'
+plans and their workspaces are allocated when the decoder is built.  ``prefill`` runs the HF model: a prompt of more
+than 8 tokens (``MOE_DECODE_MAX_T``) makes each ``QuantExperts`` build its tensor-core weight copies on first use, K·N/2
+bytes per layer, about 22 GB more for Mixtral-8x7B.  Router variants other than Mixtral's (Qwen2-MoE's shared expert,
+DeepSeek, no renormalisation), experts that are not grouped, and models that mix dense and MoE layers are refused.
+
 Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  What does not fit raises
 NotImplementedError naming the module.
 """
@@ -36,9 +49,12 @@ from . import _lib
 from .attention import attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
 from .mlp import FusedQuantMLP, _is_silu
+from .moe import QuantExperts, moe_router, router_supported
 from .qlinear import QuantLinear
 
-_RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm")
+_RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm", "MixtralRMSNorm")
+_MOE_BLOCKS = ("MixtralSparseMoeBlock",)
+_ROUTERS = ("MixtralTopKRouter",)
 
 
 def _norm_of(mod, name: str):
@@ -49,8 +65,38 @@ def _norm_of(mod, name: str):
     return mod.weight, float(mod.variance_epsilon)
 
 
+def _plan_moe(i: int, mlp, H: int, batch: int, dtype):
+    """(router weight [E, H], top_k, QuantExperts) of a Mixtral sparse MoE block, after checking that they fit."""
+    where = f"model.layers.{i}.mlp"
+    gate, experts = getattr(mlp, "gate", None), getattr(mlp, "experts", None)
+    if type(gate).__name__ not in _ROUTERS:
+        raise NotImplementedError(f"ChainDecoder: {where}.gate is {type(gate).__name__}; only {', '.join(_ROUTERS)} "
+                                  "(softmax, top-k, renormalised weights) runs in the router kernel")
+    w = getattr(gate, "weight", None)
+    if getattr(gate, "bias", None) is not None:
+        raise NotImplementedError(f"ChainDecoder: {where}.gate has a bias; the router kernel is bias-free")
+    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[1] != H:
+        raise NotImplementedError(f"ChainDecoder: {where}.gate.weight has shape "
+                                  f"{None if w is None else tuple(w.shape)}, not [num_experts, {H}]")
+    if w.dtype != dtype:
+        raise NotImplementedError(f"ChainDecoder: {where}.gate.weight is {w.dtype}, the activations {dtype}")
+    if not isinstance(experts, QuantExperts):
+        raise NotImplementedError(f"ChainDecoder: {where}.experts is {type(experts).__name__}, not "
+                                  "autogptq_b200.QuantExperts (build one from the experts' QuantLinear layers with "
+                                  "autogptq_b200.group_experts)")
+    E, k = w.shape[0], int(getattr(gate, "top_k", 0))
+    if experts.hidden_size != H or experts.num_experts != E:
+        raise NotImplementedError(f"ChainDecoder: {where}.experts has {experts.num_experts} experts of hidden size "
+                                  f"{experts.hidden_size}; the router has {E} of {H}")
+    why = router_supported(batch, H, E, k, dtype)
+    if why is not None:
+        raise NotImplementedError(f"ChainDecoder: {where}.gate: {why}")
+    return w.detach().contiguous(), k, experts
+
+
 def _plan_layer(i: int, layer, batch: int, dtype):
-    """The modules of decoder layer i that the chains read, after checking that they fit."""
+    """The modules of decoder layer i that the chains read, after checking that they fit: (attn, mlp, ln1, ln2, moe)
+    with moe = (router weight, top_k, QuantExperts) for a Mixtral sparse MoE block and None for a dense MLP."""
     attn, mlp = getattr(layer, "self_attn", None), getattr(layer, "mlp", None)
     if attn is None or mlp is None:
         raise NotImplementedError(f"ChainDecoder: model.layers.{i} has no self_attn / mlp")
@@ -59,19 +105,29 @@ def _plan_layer(i: int, layer, batch: int, dtype):
         if not isinstance(getattr(attn, n, None), QuantLinear):
             raise NotImplementedError(f"ChainDecoder: model.layers.{i}.self_attn.{n} is "
                                       f"{type(getattr(attn, n, None)).__name__}, not autogptq_b200.QuantLinear")
-    if not isinstance(mlp, FusedQuantMLP):
+    moe = None
+    if type(mlp).__name__ in _MOE_BLOCKS:
+        moe = _plan_moe(i, mlp, attn.q_proj.infeatures, batch, dtype)
+        groups = {"self_attn.q_proj|k_proj|v_proj": [attn.q_proj, attn.k_proj, attn.v_proj],
+                  "self_attn.o_proj": [attn.o_proj]}
+    elif hasattr(mlp, "experts") or (hasattr(mlp, "gate") and not hasattr(mlp, "gate_proj")):
+        raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp is {type(mlp).__name__}; the only "
+                                  f"mixture-of-experts block ChainDecoder runs is {', '.join(_MOE_BLOCKS)}")
+    elif not isinstance(mlp, FusedQuantMLP):
         if not all(hasattr(mlp, n) for n in ("gate_proj", "up_proj", "down_proj")):
             raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp ({type(mlp).__name__}) is not a "
                                       "gate/up/down MLP")
         if not _is_silu(getattr(mlp, "act_fn", None)):
             raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp.act_fn is "
                                       f"{type(getattr(mlp, 'act_fn', None)).__name__}, not SiLU")
-    for n in ("gate_proj", "up_proj", "down_proj"):
-        if not isinstance(getattr(mlp, n), QuantLinear):
-            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp.{n} is {type(getattr(mlp, n)).__name__}, "
-                                      "not autogptq_b200.QuantLinear")
-    groups = {"self_attn.q_proj|k_proj|v_proj": [attn.q_proj, attn.k_proj, attn.v_proj], "self_attn.o_proj": [attn.o_proj],
-              "mlp.gate_proj|up_proj": [mlp.gate_proj, mlp.up_proj], "mlp.down_proj": [mlp.down_proj]}
+    if moe is None:
+        for n in ("gate_proj", "up_proj", "down_proj"):
+            if not isinstance(getattr(mlp, n), QuantLinear):
+                raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp.{n} is "
+                                          f"{type(getattr(mlp, n)).__name__}, not autogptq_b200.QuantLinear")
+        groups = {"self_attn.q_proj|k_proj|v_proj": [attn.q_proj, attn.k_proj, attn.v_proj],
+                  "self_attn.o_proj": [attn.o_proj], "mlp.gate_proj|up_proj": [mlp.gate_proj, mlp.up_proj],
+                  "mlp.down_proj": [mlp.down_proj]}
     for n, ls in groups.items():
         if not chain_supported(ls, batch):
             raise NotImplementedError(f"ChainDecoder: model.layers.{i}.{n} cannot run in a decode chain (needs "
@@ -86,7 +142,18 @@ def _plan_layer(i: int, layer, batch: int, dtype):
     if attn.q_proj.infeatures > _lib.CHAIN_NORM_MAX_K:
         raise NotImplementedError(f"ChainDecoder: model.layers.{i}: hidden size {attn.q_proj.infeatures} > "
                                   f"{_lib.CHAIN_NORM_MAX_K}, the largest a chain norm stage takes")
-    return attn, mlp, ln1, ln2
+    return attn, mlp, ln1, ln2, moe
+
+
+def _is_moe(plans) -> bool:
+    """Whether the layers of ``_plan_layer`` are all mixture-of-experts blocks (else all dense)."""
+    moe = plans[0][4] is not None
+    for i, p in enumerate(plans):
+        if (p[4] is not None) != moe:
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp is {type(p[1]).__name__} but "
+                                      f"model.layers.0.mlp is {type(plans[0][1]).__name__}; a model that mixes dense "
+                                      "and mixture-of-experts layers is not supported")
+    return moe
 
 
 def _rotary_params(rotary, head_dim: int):
@@ -115,7 +182,8 @@ def _check_window(config, max_length: int):
 
 class ChainDecoder:
     """Greedy decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
-    projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too).  ``fused_attention``:
+    projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too), or a
+    ``MixtralForCausalLM`` whose experts are ``autogptq_b200.QuantExperts``.  ``fused_attention``:
     run each layer's attention as one CUDA launch (``autogptq_b200.attention.decode_attention``) instead of torch."""
 
     def __init__(self, model, batch: int = 1, max_length: int = 2048, fused_attention: bool = False):
@@ -148,6 +216,7 @@ class ChainDecoder:
         plans = [_plan_layer(i, layer, batch, self.dtype) for i, layer in enumerate(inner.layers)]
         if not plans:
             raise NotImplementedError("ChainDecoder: the model has no decoder layers")
+        self.moe = _is_moe(plans)
         fw, feps = _norm_of(inner.norm, "model.norm")
         attn0 = plans[0][0]
         self.head_dim = attn0.head_dim
@@ -175,8 +244,19 @@ class ChainDecoder:
         self.chains.append(ch.build())
         self._qkv = [qkv]              # q, k, v of block i
         self._attn_in = []             # o_proj input of block i (written by the attention)
+        if self.moe:
+            self._build_moe(plans, H)
+        else:
+            self._build_dense(plans)
+        self._final_norm = inner.norm
+        self._graph = None
+        self._logits = None
+
+    def _build_dense(self, plans):
+        """chain_i = [o_i, add_rmsnorm -> gate|up_i, silu_mul -> down_i, add_rmsnorm(input_layernorm_i+1) -> q|k|v_i+1]"""
+        B, L, dev, dt = self.batch, len(plans), self.device, self.dtype
         resid = self._x0
-        for i, (attn, mlp, _, (w2, eps2)) in enumerate(plans):
+        for i, (attn, mlp, _, (w2, eps2), _) in enumerate(plans):
             ch = DecodeChain(M=B, dtype=dt, device=dev)
             a_in = ch.input(attn.o_proj.infeatures)
             (o,) = ch.stage([attn.o_proj], a_in)
@@ -193,9 +273,46 @@ class ChainDecoder:
                 self._last = (h1, down)
             self._attn_in.append(a_in)
             self.chains.append(ch.build())
-        self._final_norm = inner.norm
-        self._graph = None
-        self._logits = None
+
+    def _build_moe(self, plans, H: int):
+        """Per block i: chain [o_i]; the router (h1 = x + o, n2 = post_attention_layernorm(h1), top-k); the grouped
+        experts on n2; then chain [add_rmsnorm(moe_i, h1; input_layernorm_i+1) -> q|k|v_i+1], which publishes the next
+        residual.  Every buffer, the experts' plans and their workspaces are allocated here, once."""
+        B, L, dev, dt = self.batch, len(plans), self.device, self.dtype
+        self._o_chains, self._qkv_chains, self._moe_layers = [], [], []
+        resid = self._x0
+        for i, (attn, _, _, (w2, eps2), (gate_w, k, experts)) in enumerate(plans):
+            ch = DecodeChain(M=B, dtype=dt, device=dev)
+            a_in = ch.input(attn.o_proj.infeatures)
+            (o,) = ch.stage([attn.o_proj], a_in)
+            self._o_chains.append(ch.build())
+            self._attn_in.append(a_in)
+            h1, n2, out = (torch.zeros((B, H), dtype=dt, device=dev) for _ in range(3))
+            idx = torch.zeros((B, k), dtype=torch.int32, device=dev)
+            wts = torch.zeros((B, k), dtype=torch.float32, device=dev)
+            plan, ws = experts._static_buffers(B, k, dt, dev)
+            self._moe_layers.append(dict(o=o, resid=resid, w2=w2, eps2=eps2, gate=gate_w, k=k, experts=experts,
+                                         h1=h1, n2=n2, idx=idx, w=wts, out=out, plan=plan, ws=ws))
+            if i + 1 < L:
+                na = plans[i + 1][0]
+                w1, eps1 = plans[i + 1][2]
+                ch = DecodeChain(M=B, dtype=dt, device=dev)
+                q, kk, v, resid = ch.stage([na.q_proj, na.k_proj, na.v_proj], out, x2=h1, x_mode="add_rmsnorm",
+                                           norm_weight=w1, norm_eps=eps1)
+                self._qkv.append((q, kk, v))
+                self._qkv_chains.append(ch.build())
+            else:
+                self._last = (h1, out)
+
+    def _moe_block(self, i: int):
+        """Block i after its attention: o_proj, the router and the experts, then the next block's q|k|v."""
+        m = self._moe_layers[i]
+        self._o_chains[i].run()
+        moe_router(m["o"], m["resid"], m["w2"], m["eps2"], m["gate"], m["k"], h=m["h1"], n=m["n2"], idx=m["idx"],
+                   w=m["w"])
+        m["experts"]._forward(m["n2"], m["idx"], m["w"], out=m["out"], plan=m["plan"], ws=m["ws"])
+        if i < len(self._qkv_chains):
+            self._qkv_chains[i].run()
 
     # ------------------------------------------------------------------ state
     @property
@@ -254,11 +371,12 @@ class ChainDecoder:
     def _step_body(self) -> torch.Tensor:
         inner = self.model.model
         self._x0.copy_(inner.embed_tokens(self._ids))
+        tail = self._moe_block if self.moe else (lambda i: self.chains[i + 1].run())
         if self.fused_attention:
             self.chains[0].run()
             for i in range(len(self._attn_in)):
                 self._fused_attention(i)
-                self.chains[i + 1].run()
+                tail(i)
         else:
             pos_ids = self._pos.view(1, 1).expand(self.batch, 1)
             cos, sin = inner.rotary_emb(self._x0.view(self.batch, 1, -1), pos_ids)
@@ -266,7 +384,7 @@ class ChainDecoder:
             self.chains[0].run()
             for i in range(len(self._attn_in)):
                 self._attention(i, cos, sin, mask)
-                self.chains[i + 1].run()
+                tail(i)
         h1, down = self._last
         n = self._final_norm(h1 + down)
         logits = self.model.lm_head(n)

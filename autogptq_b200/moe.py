@@ -214,22 +214,41 @@ class QuantExperts(nn.Module):
         out = out.reshape(out_shape)
         return out if x_dtype == cdtype else out.to(x_dtype)
 
-    def _forward(self, x: torch.Tensor, idx: torch.Tensor, w: torch.Tensor, save: bool = False):
+    def _static_buffers(self, T: int, k: int, dtype, device):
+        """(plan, workspace) for ``_forward(..., out=, plan=, ws=)`` of up to T <= MOE_DECODE_MAX_T rows with k experts
+        each: a caller that captures the forward in a CUDA graph owns both instead of the per-stream workspace cache."""
+        if not 1 <= T <= _lib.MOE_DECODE_MAX_T:
+            raise ValueError(f"static buffers are for decode rows, 1..{_lib.MOE_DECODE_MAX_T} (got {T})")
+        device = torch.device(device)
+        with torch.cuda.device(device):
+            plan = self._plan(dtype, device)
+            n = int(_lib.load().agb200_moe_workspace_bytes(T, k, self.num_experts, self.hidden_size,
+                                                            self.intermediate_size))
+        return plan, torch.empty(n, dtype=torch.uint8, device=device)
+
+    def _forward(self, x: torch.Tensor, idx: torch.Tensor, w: torch.Tensor, save: bool = False, *, out=None,
+                 plan: _Plan | None = None, ws: torch.Tensor | None = None):
         """(out [T, H], saved or None) of the grouped forward on prepared inputs (x [T, H] of the compute dtype,
         contiguous and 16-byte aligned; idx [T, k] int32 / int64; w [T, k] fp32 or the compute dtype).  ``save``: also
-        keep what the backward reads (``agb200_moe_forward_saving``)."""
+        keep what the backward reads (``agb200_moe_forward_saving``).  ``out``, ``plan`` and ``ws`` (from
+        ``_static_buffers``): write into ``out`` with that plan and workspace, allocating nothing."""
         device, cdtype = x.device, x.dtype
         T, k = idx.shape
         H, E, I = self.hidden_size, self.num_experts, self.intermediate_size
-        out = torch.empty((T, H), dtype=cdtype, device=device)
+        if out is None:
+            out = torch.empty((T, H), dtype=cdtype, device=device)
         if T == 0:
             return out, (torch.empty(0, dtype=torch.uint8, device=device) if save else None)
-        if T > _lib.MOE_DECODE_MAX_T and not self._tc:
-            self._tc = True                          # same lazy rule as QuantLinear: tensor-core copies on first need
-        plan = self._plan(cdtype, device)
+        if plan is None:
+            if T > _lib.MOE_DECODE_MAX_T and not self._tc:
+                self._tc = True                      # same lazy rule as QuantLinear: tensor-core copies on first need
+            plan = self._plan(cdtype, device)
         lib = _lib.load()
         ws_bytes = int(lib.agb200_moe_workspace_bytes(T, k, E, H, I))
-        ws = _workspace(device, ws_bytes)
+        if ws is None:
+            ws = _workspace(device, ws_bytes)
+        elif ws.numel() < ws_bytes:
+            raise ValueError(f"the workspace holds {ws.numel()} bytes, the forward needs {ws_bytes}")
         args = (plan.handle, x.data_ptr(), idx.data_ptr(),
                 _lib.MOE_INDEX_I64 if idx.dtype == torch.int64 else _lib.MOE_INDEX_I32, w.data_ptr(),
                 _lib.MOE_WEIGHTS_F32 if w.dtype == torch.float32 else _DTYPE_CODE[cdtype], T, k, out.data_ptr())
@@ -295,6 +314,74 @@ class _QuantExpertsFunction(torch.autograd.Function):
         return dx, dw, None, None
 
 
+def router_supported(T: int, H: int, E: int, k: int, dtype) -> str | None:
+    """None when ``moe_router`` takes this shape, else the reason it does not."""
+    if dtype not in _DTYPE_CODE:
+        return f"dtype {dtype}; the router kernel computes in fp16 / bf16"
+    if not 0 <= T <= _lib.MOE_DECODE_MAX_T:
+        return f"{T} rows; the router kernel takes 0..{_lib.MOE_DECODE_MAX_T}"
+    if H <= 0 or H % 128 or H > _lib.CHAIN_NORM_MAX_K:
+        return f"hidden size {H}; the router kernel needs a multiple of 128 up to {_lib.CHAIN_NORM_MAX_K}"
+    if not 1 <= k <= _lib.MOE_ROUTER_MAX_TOP_K:
+        return f"top_k {k}; the router kernel takes 1..{_lib.MOE_ROUTER_MAX_TOP_K}"
+    if not k <= E <= _lib.MOE_MAX_EXPERTS:
+        return f"{E} experts; the router kernel takes top_k..{_lib.MOE_MAX_EXPERTS}"
+    return None
+
+
+def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n=None, idx=None, w=None, logits=None):
+    """The routing of a Mixtral-style block for decode rows in one launch (``agb200_moe_router``, DESIGN §3.17):
+
+        h = x + x2 (skipped when x2 is None)   n = RMSNorm(h; norm_weight, eps)   logits = n · gate_weightᵀ
+        p = softmax(fp32 logits)               idx = top-k of p (an exact tie to the lower expert)   w = p_idx / Σ p_idx
+
+    with the roundings of transformers' MixtralDecoderLayer / MixtralRMSNorm / MixtralTopKRouter.  x, x2 [T, H] and
+    norm_weight [H], gate_weight [E, H] of one 16-bit dtype.  Returns (h or None, n [T, H], idx int32 [T, k],
+    w fp32 [T, k], logits [T, E] or None); ``h``, ``n``, ``idx`` and ``w`` are written in place when given (a decoder
+    preallocates them), ``logits`` only when a buffer is given.  No host synchronisation."""
+    if x.dim() != 2:
+        raise ValueError(f"x must be [T, H], got {tuple(x.shape)}")
+    T, H = x.shape
+    dev, dt = x.device, x.dtype
+    if dev.type != "cuda":
+        raise RuntimeError("moe_router needs CUDA tensors (there is no CPU fallback)")
+    if gate_weight.dim() != 2 or gate_weight.shape[1] != H:
+        raise ValueError(f"gate_weight must be [E, {H}], got {tuple(gate_weight.shape)}")
+    E = gate_weight.shape[0]
+    why = router_supported(T, H, E, k, dt)
+    if why is not None:
+        raise NotImplementedError(f"moe_router: {why}")
+    if h is None and x2 is not None:
+        h = torch.empty((T, H), dtype=dt, device=dev)
+    n = torch.empty((T, H), dtype=dt, device=dev) if n is None else n
+    idx = torch.empty((T, k), dtype=torch.int32, device=dev) if idx is None else idx
+    w = torch.empty((T, k), dtype=torch.float32, device=dev) if w is None else w
+    checks = [("x", x, (T, H), dt), ("norm_weight", norm_weight, (H,), dt), ("gate_weight", gate_weight, (E, H), dt),
+              ("n", n, (T, H), dt), ("idx", idx, (T, k), torch.int32), ("w", w, (T, k), torch.float32)]
+    if x2 is not None:
+        checks += [("x2", x2, (T, H), dt), ("h", h, (T, H), dt)]
+    elif h is not None:
+        raise ValueError("h is the residual x + x2; pass x2 or leave h out")
+    if logits is not None:
+        checks.append(("logits", logits, (T, E), dt))
+    for name, t, shape, tdt in checks:
+        if tuple(t.shape) != shape or t.dtype != tdt:
+            raise ValueError(f"{name} must be {tdt} {list(shape)}, got {t.dtype} {list(t.shape)}")
+        if t.device != dev:
+            raise ValueError(f"{name} is on {t.device}, x on {dev}")
+        if not t.is_contiguous():
+            raise ValueError(f"{name} must be contiguous")
+        if t.dtype != torch.float32 and t.dtype != torch.int32 and name != "logits" and t.data_ptr() % 16:
+            raise ValueError(f"{name} must be 16-byte aligned")
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.agb200_moe_router(x.data_ptr(), _ptr(x2), norm_weight.data_ptr(), float(eps), gate_weight.data_ptr(),
+                                   T, H, E, k, _DTYPE_CODE[dt], _ptr(h), n.data_ptr(), idx.data_ptr(), w.data_ptr(),
+                                   _ptr(logits), torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, "agb200_moe_router")
+    return h, n, idx, w, logits
+
+
 def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTERN, *,
                   input_grad: bool = False) -> Dict[str, nn.Module]:
     """``{prefix: QuantLinear}`` (e.g. from ``checkpoint.load_quant_linears``) -> the same mapping with every
@@ -324,4 +411,4 @@ def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTE
     return out
 
 
-__all__ = ["QuantExperts", "group_experts", "EXPERT_PATTERN"]
+__all__ = ["QuantExperts", "group_experts", "EXPERT_PATTERN", "moe_router", "router_supported"]

@@ -602,6 +602,31 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
                             void* stream);
 size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int head_dim, int max_length);
 
+/*
+ * Router of a Mixtral-style block for T decode rows (addition to ABI v10), one launch on `stream`, all pointers DEVICE
+ * memory of `dtype` unless stated:
+ *   x [T, H], x2 [T, H] or NULL   h = x + x2 (the residual add; x2 NULL: h = x)
+ *   norm_weight [H], eps          n = RMSNorm(h) (post_attention_layernorm)
+ *   gate_weight [E, H]            the router's bias-free linear layer (not quantised)
+ *   h [T, H]                      written exactly when x2 is given (else NULL)
+ *   n [T, H]                      the experts' input
+ *   top_k_index int32 [T, k], top_k_weights fp32 [T, k]   the routing of agb200_moe_forward (AGB200_MOE_INDEX_I32,
+ *                                 AGB200_MOE_WEIGHTS_F32)
+ *   logits [T, E] or NULL         the rounded router logits
+ * Rounding (transformers 5.5 MixtralDecoderLayer / MixtralRMSNorm / MixtralTopKRouter): h = rnd(x + x2);
+ * n = rnd(rnd(h·r)·w) with r = 1/sqrt(Σh²/H + eps) in fp32, Σh² summed as the decode chain's norm stage sums it;
+ * logit_e = rnd(Σ n·G[e]) with an fp32 sum; p = softmax(fp32 logits) (maximum subtracted, expf); the k largest p,
+ * largest first, an exact tie going to the lower expert index; top_k_weights = p_j / Σ_j p_j in fp32.  Every sum runs
+ * in a fixed order and nothing synchronises with the host: two calls are bit-identical and the call can be captured in
+ * a CUDA graph.  Constraints (else AGB200_ENOSUP): dtype AGB200_F16 / AGB200_BF16, T <= AGB200_MOE_DECODE_MAX_T,
+ * H % 128 == 0, H <= AGB200_CHAIN_NORM_MAX_K, 1 <= k <= AGB200_MOE_ROUTER_MAX_TOP_K, k <= E <= AGB200_MOE_MAX_EXPERTS.
+ * x, x2, norm_weight, gate_weight, h and n 16-byte aligned (else AGB200_EINVAL).  T = 0 does nothing.
+ */
+#define AGB200_MOE_ROUTER_MAX_TOP_K 8
+int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, int T,
+                      int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
+                      void* logits, void* stream);
+
 /* Static facts about the build, for logs: returns e.g. "autogptq_b200 sm_90a: ... gemm=wgmma ...". */
 const char* agb200_build_info(void);
 
