@@ -6,11 +6,9 @@
 #include <cstdarg>
 #include <cstdio>
 #include <cstdlib>
-#include <cstring>
 #include <mutex>
 
-#include "../../include/autogptq_b200.h"
-#include "internal.h"
+#include "host.h"
 #include "aux_kernels.cuh"
 #include "gemm_tcgen05.cuh"   // the wgmma GEMM (file name kept from the first target)
 #include "dgrad.cuh"
@@ -35,22 +33,6 @@ agb::PrefetchHint take_prefetch_hint() {
   return h;
 }
 
-int fail(int code, const char* fmt, ...) {
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(g_err, sizeof(g_err), fmt, ap);
-  va_end(ap);
-  return code;
-}
-
-#define AGB_CUDA(expr)                                                                         \
-  do {                                                                                         \
-    cudaError_t e_ = (expr);                                                                   \
-    if (e_ != cudaSuccess) return fail(AGB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
-  } while (0)
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
 // Debug switch: AGB200_NO_PDL=1 launches without programmatic stream serialization (measurement aid).
 int pdl_allowed() {
   static int v = -1;
@@ -61,28 +43,35 @@ int pdl_allowed() {
   return v;
 }
 
-struct DeviceInfo {
-  int sms = 0;
-  int smem_optin = 0;
-  bool ok = false;
-};
+}  // namespace
 
-int get_device_info(DeviceInfo& out) {
+int failf(int code, const char* fmt, ...) {
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(g_err, sizeof(g_err), fmt, ap);
+  va_end(ap);
+  return code;
+}
+
+int device_info(DeviceInfo& out) {
   static DeviceInfo cache[64];
   static std::atomic<bool> ready[64];
   static std::mutex mu;
   int dev = 0;
   AGB_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return fail(AGB200_EINVAL, "device index %d out of range", dev);
+  if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "device index %d out of range", dev);
   if (!ready[dev].load(std::memory_order_acquire)) {
     std::lock_guard<std::mutex> lock(mu);
     DeviceInfo d;
+    d.device = dev;
     AGB_CUDA(cudaDeviceGetAttribute(&d.sms, cudaDevAttrMultiProcessorCount, dev));
     AGB_CUDA(cudaDeviceGetAttribute(&d.smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-    int major = 0;
+    AGB_CUDA(cudaDeviceGetAttribute(&d.l2_bytes, cudaDevAttrL2CacheSize, dev));
+    int major = 0, coop = 0;
+    AGB_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
     AGB_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-    if (major != 9) return fail(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
-    d.ok = true;
+    if (major != 9) return failf(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
+    d.coop = coop != 0;
     cache[dev] = d;
     ready[dev].store(true, std::memory_order_release);
   }
@@ -90,44 +79,21 @@ int get_device_info(DeviceInfo& out) {
   return 0;
 }
 
+namespace {
+
 // ------------------------------------------------------------------------------------------ GEMV
 using agb::GemvParams;
 
 template <int kM, int kLN, bool kBf16, bool kBiased, int kOcc = 2>
 int launch_gemv_inst(const GemvParams& p, int n_tiles, cudaStream_t stream, int smem_optin) {
-  auto kern = agb::w4a16_gemv_kernel<kM, kLN, kBf16, kBiased, (kM == 1 ? kOcc : (kM <= 2 ? 2 : 1))>;
+  constexpr auto kern = &agb::w4a16_gemv_kernel<kM, kLN, kBf16, kBiased, (kM == 1 ? kOcc : (kM <= 2 ? 2 : 1))>;
   const size_t smem = agb::GemvSmem<kM, kLN, kBiased>::total(p.rows_per_split);
   if (smem > static_cast<size_t>(smem_optin))
-    return fail(AGB200_ENOSUP, "gemv: K chunk of %d rows needs %zu B shared memory (> %d)", p.rows_per_split, smem, smem_optin);
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    AGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-    attr_set_dev[attr_dev] = true;
-  }
+    return failf(AGB200_ENOSUP, "gemv: K chunk of %d rows needs %zu B shared memory (> %d)", p.rows_per_split, smem, smem_optin);
+  if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
   GemvParams pp = p;
   agb::prefetch_set_grid(pp.pf, static_cast<unsigned>(n_tiles) * p.split);
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(n_tiles, p.split, 1);
-  cfg.blockDim = dim3(agb::kGemvThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[na].val.programmaticStreamSerializationAllowed = pdl_allowed();
-  ++na;
-  if (p.split > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = 1;
-    attrs[na].val.clusterDim.y = p.split;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  AGB_CUDA(cudaLaunchKernelEx(&cfg, kern, pp));
-  return 0;
+  return launch(kern, dim3(n_tiles, p.split), dim3(agb::kGemvThreads), smem, stream, pdl_allowed(), dim3(1, p.split, 1), false, pp);
 }
 
 template <int kM, int kLN>
@@ -150,7 +116,7 @@ int launch_gemv_m(const GemvParams& p, int ln, bool bf16, bool biased, cudaStrea
     case 16: return launch_gemv_mln<kM, 16>(p, n_tiles, bf16, biased, s, so);
     case 32: return launch_gemv_mln<kM, 32>(p, n_tiles, bf16, biased, s, so);
   }
-  return fail(AGB200_EINVAL, "gemv: lanes-along-N must be 8, 16 or 32 (got %d)", ln);
+  return failf(AGB200_EINVAL, "gemv: lanes-along-N must be 8, 16 or 32 (got %d)", ln);
 }
 
 // One GEMV pass over m <= 4 rows.
@@ -185,7 +151,7 @@ int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, cons
     while (split < 8 && n_tiles * split < 2 * di.sms && (p.rows / (split * 2)) >= row_lanes * 4) split *= 2;
   }
   if (split != 1 && split != 2 && split != 4 && split != 8)
-    return fail(AGB200_EINVAL, "gemv: split-K must be 1, 2, 4 or 8 (got %d)", split);
+    return failf(AGB200_EINVAL, "gemv: split-K must be 1, 2, 4 or 8 (got %d)", split);
   // shared-memory bound on the K chunk: grow the split until it fits
   auto chunk_smem = [&](int sp) {
     const int rps = ((p.rows + sp - 1) / sp + 7) / 8 * 8;
@@ -200,50 +166,26 @@ int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, cons
     case 3: return launch_gemv_m<3>(p, ln, bf16, biased, stream, di.smem_optin);
     case 4: return launch_gemv_m<4>(p, ln, bf16, biased, stream, di.smem_optin);
   }
-  return fail(AGB200_EINVAL, "gemv pass with m=%d", m);
+  return failf(AGB200_EINVAL, "gemv pass with m=%d", m);
 }
 
 // ------------------------------------------------------------------------------------------ skinny (M <= 8)
 template <bool kBf16, bool kBiased>
 int launch_skinny_inst(const agb::SkinnyParams& p, cudaStream_t stream, int smem_optin) {
-  auto kern = agb::w4a16_skinny_kernel<kBf16, kBiased>;
+  constexpr auto kern = &agb::w4a16_skinny_kernel<kBf16, kBiased>;
   const size_t smem = agb::SkinnySmem::total(p.rows_per_split, p.M);
   if (smem > static_cast<size_t>(smem_optin))
-    return fail(AGB200_ENOSUP, "skinny: K chunk of %d rows x M=%d needs %zu B shared memory (> %d)", p.rows_per_split, p.M, smem, smem_optin);
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    AGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-    attr_set_dev[attr_dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((p.N + agb::kSkTN - 1) / agb::kSkTN, p.split, 1);
-  cfg.blockDim = dim3(agb::kSkThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[na].val.programmaticStreamSerializationAllowed = pdl_allowed();
-  ++na;
-  if (p.split > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = 1;
-    attrs[na].val.clusterDim.y = p.split;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  AGB_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-  return 0;
+    return failf(AGB200_ENOSUP, "skinny: K chunk of %d rows x M=%d needs %zu B shared memory (> %d)", p.rows_per_split, p.M, smem, smem_optin);
+  if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
+  return launch(kern, dim3((p.N + agb::kSkTN - 1) / agb::kSkTN, p.split), dim3(agb::kSkThreads), smem, stream, pdl_allowed(),
+                dim3(1, p.split, 1), false, p);
 }
 
 int skinny_launch(const void* x, const int32_t* qweight, const int32_t* qzeros, const void* scales, const int32_t* perm,
                   const void* bias, void* y, int M, int K, int N, int group_size, bool bf16, int split, bool biased,
                   cudaStream_t stream, const DeviceInfo& di) {
-  if (group_size % 32 != 0) return fail(AGB200_ENOSUP, "skinny kernel needs group_size %% 32 == 0 (got %d)", group_size);
-  if (M < 1 || M > AGB200_SKINNY_MAX_M) return fail(AGB200_EINVAL, "skinny kernel handles 1 <= M <= 8 (got %d)", M);
+  if (group_size % 32 != 0) return failf(AGB200_ENOSUP, "skinny kernel needs group_size %% 32 == 0 (got %d)", group_size);
+  if (M < 1 || M > AGB200_SKINNY_MAX_M) return failf(AGB200_EINVAL, "skinny kernel handles 1 <= M <= 8 (got %d)", M);
   agb::SkinnyParams p{};
   p.x = x; p.qweight = qweight; p.qzeros = qzeros; p.scales = scales; p.perm = perm; p.bias = bias; p.y = y;
   p.M = M; p.K = K; p.N = N; p.rows = K / 8; p.rows_per_group = group_size / 8;
@@ -253,7 +195,7 @@ int skinny_launch(const void* x, const int32_t* qweight, const int32_t* qzeros, 
     while (split < 8 && tiles * split < 2 * di.sms && p.rows / (split * 2) >= 64) split *= 2;
   }
   if (split != 1 && split != 2 && split != 4 && split != 8)
-    return fail(AGB200_EINVAL, "skinny: split-K must be 1, 2, 4 or 8 (got %d)", split);
+    return failf(AGB200_EINVAL, "skinny: split-K must be 1, 2, 4 or 8 (got %d)", split);
   auto rps_of = [&](int sp) { return ((p.rows + sp - 1) / sp + 31) / 32 * 32; };
   while (split < 8 && agb::SkinnySmem::total(rps_of(split), M) > static_cast<size_t>(di.smem_optin)) split *= 2;
   p.split = split;
@@ -266,37 +208,12 @@ int skinny_launch(const void* x, const int32_t* qweight, const int32_t* qzeros, 
 // ------------------------------------------------------------------------------------------ integer tensor-core decode (M <= 8)
 template <int kNG, int kWN, bool kBf16>
 int launch_imma_inst(const agb::ImmaParams& p, int n_tiles, cudaStream_t stream, int smem_optin) {
-  auto kern = agb::w4a16_imma_kernel<kNG, kWN, kBf16>;
+  constexpr auto kern = &agb::w4a16_imma_kernel<kNG, kWN, kBf16>;
   const size_t smem = agb::ImmaSmem::total(p.rows_per_split, p.M, 8 * kNG, 32 * kWN);
   if (smem > static_cast<size_t>(smem_optin))
-    return fail(AGB200_ENOSUP, "imma: K chunk of %d rows x M=%d needs %zu B shared memory (> %d)", p.rows_per_split, p.M, smem, smem_optin);
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    AGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-    attr_set_dev[attr_dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(n_tiles, p.split, 1);
-  cfg.blockDim = dim3(agb::kImThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[na].val.programmaticStreamSerializationAllowed = pdl_allowed();
-  ++na;
-  if (p.split > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = 1;
-    attrs[na].val.clusterDim.y = p.split;
-    attrs[na].val.clusterDim.z = 1;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  AGB_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-  return 0;
+    return failf(AGB200_ENOSUP, "imma: K chunk of %d rows x M=%d needs %zu B shared memory (> %d)", p.rows_per_split, p.M, smem, smem_optin);
+  if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
+  return launch(kern, dim3(n_tiles, p.split), dim3(agb::kImThreads), smem, stream, pdl_allowed(), dim3(1, p.split, 1), false, p);
 }
 
 template <int kNG>
@@ -307,25 +224,9 @@ int launch_imma_ng(const agb::ImmaParams& p, int wn, int n_tiles, bool bf16, cud
 
 template <int kNG, bool kBf16>
 int launch_imma_persistent_inst(const agb::ImmaPParams& p, int grid, size_t smem, cudaStream_t stream, int smem_optin) {
-  auto kern = agb::w4a16_imma_persistent_kernel<kNG, kBf16>;
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    AGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-    attr_set_dev[attr_dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(grid, 1, 1);
-  cfg.blockDim = dim3(agb::kIpThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[0].val.programmaticStreamSerializationAllowed = pdl_allowed();
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  AGB_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-  return 0;
+  constexpr auto kern = &agb::w4a16_imma_persistent_kernel<kNG, kBf16>;
+  if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
+  return launch(kern, dim3(grid), dim3(agb::kIpThreads), smem, stream, pdl_allowed(), dim3(1, 1, 1), false, p);
 }
 
 // flush block (k8-rows) of the integer kernel for this layer shape, or 0 when it cannot run it
@@ -340,9 +241,9 @@ int imma_rows_per_block(int K, int group_size) {
 int imma_launch(const void* x, int n_layers, const int32_t* const* qweight, const int32_t* const* qzeros, const void* const* scales,
                 const int32_t* const* perm, const void* const* bias, void* const* y, const int* N, int M, int K, int group_size,
                 bool bf16, int wn_req, int split_req, cudaStream_t stream, const DeviceInfo& di) {
-  if (M < 1 || M > agb::kImMaxM) return fail(AGB200_EINVAL, "imma kernel handles 1 <= M <= 8 (got %d)", M);
+  if (M < 1 || M > agb::kImMaxM) return failf(AGB200_EINVAL, "imma kernel handles 1 <= M <= 8 (got %d)", M);
   const int rpb = imma_rows_per_block(K, group_size);
-  if (rpb == 0) return fail(AGB200_ENOSUP, "imma kernel needs group_size %% 32 == 0 and K %% 32 == 0 (got %d, %d)", group_size, K);
+  if (rpb == 0) return failf(AGB200_ENOSUP, "imma kernel needs group_size %% 32 == 0 and K %% 32 == 0 (got %d, %d)", group_size, K);
   const int ng = M <= 2 ? 1 : (M <= 5 ? 2 : 3);
   const int max_chunk = ng == 1 ? agb::ImmaCfg<1>::kMaxChunkRows : agb::ImmaCfg<2>::kMaxChunkRows;
   agb::ImmaParams p{};
@@ -360,7 +261,7 @@ int imma_launch(const void* x, int n_layers, const int32_t* const* qweight, cons
     for (int i = 1; i < n_layers; ++i) same_perm = same_perm && (perm ? perm[i] : nullptr) == (perm ? perm[0] : nullptr);
     const bool eligible = rpb == 16 && same_perm;
     if (wn_req == 2 && !eligible)
-      return fail(AGB200_ENOSUP, "imma persistent form needs group_size %% 128 == 0 (or no groups with K %% 128 == 0) and one x permutation (K=%d, group_size=%d)", K, group_size);
+      return failf(AGB200_ENOSUP, "imma persistent form needs group_size %% 128 == 0 (or no groups with K %% 128 == 0) and one x permutation (K=%d, group_size=%d)", K, group_size);
     if ((wn_req == 0 || wn_req == 2) && eligible) {
       agb::ImmaPParams q{};
       q.x = x; q.M = M; q.K = K; q.rows = p.rows; q.blocks_per_group = p.rows_per_group / rpb; q.n_layers = n_layers;
@@ -397,7 +298,7 @@ int imma_launch(const void* x, int n_layers, const int32_t* const* qweight, cons
           }
         }
       }
-      if (wn_req == 2) return fail(AGB200_ENOSUP, "imma persistent form: M=%d does not fit in shared memory", M);
+      if (wn_req == 2) return failf(AGB200_ENOSUP, "imma persistent form: M=%d does not fit in shared memory", M);
     }
   }
   auto rps_of = [&](int sp) { return (nblocks + sp - 1) / sp * rpb; };
@@ -407,13 +308,13 @@ int imma_launch(const void* x, int n_layers, const int32_t* const* qweight, cons
     while (split < 8 && tiles32 * split < 2 * di.sms && p.rows / (split * 2) >= 128) split *= 2;
   }
   if (split != 1 && split != 2 && split != 4 && split != 8)
-    return fail(AGB200_EINVAL, "imma: split-K must be 1, 2, 4 or 8 (got %d)", split);
+    return failf(AGB200_EINVAL, "imma: split-K must be 1, 2, 4 or 8 (got %d)", split);
   while (split < 8 && rps_of(split) > max_chunk) split *= 2;
   if (rps_of(split) > max_chunk)
-    return fail(AGB200_ENOSUP, "imma: K=%d x M=%d exceeds the per-CTA chunk of %d rows at split 8", K, M, max_chunk * 8);
+    return failf(AGB200_ENOSUP, "imma: K=%d x M=%d exceeds the per-CTA chunk of %d rows at split 8", K, M, max_chunk * 8);
   int wn = wn_req;
   if (wn == 0) wn = (ng >= 2 && tiles32 * split >= 4 * di.sms) ? 4 : 1;
-  if (wn != 1 && wn != 4) return fail(AGB200_EINVAL, "imma: tune0 must be 0 (auto), 1 or 4 (warps along N of the tile-per-CTA kernel) or 2 (persistent); got %d", wn);
+  if (wn != 1 && wn != 4) return failf(AGB200_EINVAL, "imma: tune0 must be 0 (auto), 1 or 4 (warps along N of the tile-per-CTA kernel) or 2 (persistent); got %d", wn);
   p.split = split;
   p.rows_per_split = rps_of(split);
   int tiles = 0;
@@ -432,34 +333,27 @@ int imma_launch(const void* x, int n_layers, const int32_t* const* qweight, cons
 
 int check_common(const void* x, const int32_t* qweight, const int32_t* qzeros, const void* scales, const void* y,
                  int M, int K, int N, int group_size, int dtype) {
-  if (!x || !qweight || !qzeros || !scales || !y) return fail(AGB200_EINVAL, "null pointer argument");
-  if (M < 0 || K <= 0 || N <= 0) return fail(AGB200_EINVAL, "bad shape M=%d K=%d N=%d", M, K, N);
-  if (K % 8 != 0) return fail(AGB200_EINVAL, "infeatures K=%d must be a multiple of 8 (4-bit row packing)", K);
-  if (N % 8 != 0) return fail(AGB200_EINVAL, "outfeatures N=%d must be a multiple of 8 (qzeros packing)", N);
-  if (group_size <= 0) return fail(AGB200_EINVAL, "group_size must be > 0 (pass K for -1)");
-  if (group_size % 8 != 0) return fail(AGB200_ENOSUP, "group_size=%d is not a multiple of 8", group_size);
-  if (dtype != AGB200_F16 && dtype != AGB200_BF16) return fail(AGB200_EINVAL, "dtype must be AGB200_F16 or AGB200_BF16");
-  if (!aligned16(x) || !aligned16(qweight) || !aligned16(y) || !aligned16(scales) || (reinterpret_cast<uintptr_t>(qzeros) & 3u))
-    return fail(AGB200_EINVAL, "x, qweight, scales and y must be 16-byte aligned");
+  if (!x || !qweight || !qzeros || !scales || !y) return failf(AGB200_EINVAL, "null pointer argument");
+  if (M < 0 || K <= 0 || N <= 0) return failf(AGB200_EINVAL, "bad shape M=%d K=%d N=%d", M, K, N);
+  if (K % 8 != 0) return failf(AGB200_EINVAL, "infeatures K=%d must be a multiple of 8 (4-bit row packing)", K);
+  if (N % 8 != 0) return failf(AGB200_EINVAL, "outfeatures N=%d must be a multiple of 8 (qzeros packing)", N);
+  if (group_size <= 0) return failf(AGB200_EINVAL, "group_size must be > 0 (pass K for -1)");
+  if (group_size % 8 != 0) return failf(AGB200_ENOSUP, "group_size=%d is not a multiple of 8", group_size);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16) return failf(AGB200_EINVAL, "dtype must be AGB200_F16 or AGB200_BF16");
+  if (!aligned(x, 16) || !aligned(qweight, 16) || !aligned(y, 16) || !aligned(scales, 16) || !aligned(qzeros, 4))
+    return failf(AGB200_EINVAL, "x, qweight, scales and y must be 16-byte aligned");
   return 0;
 }
 
 }  // namespace
 
-int agb_internal_fail(int code, const char* msg) { return fail(code, "%s", msg); }
-
 int agb_internal_unpermute_columns(const void* in, const int* perm, void* out, int M, int K, void* stream) {
   DeviceInfo di;
-  if (int rc = get_device_info(di)) return rc;
+  if (int rc = device_info(di)) return rc;
   const size_t smem = static_cast<size_t>(K) * 2;
   if (smem > static_cast<size_t>(di.smem_optin))
-    return fail(AGB200_ENOSUP, "dgrad: act-order row of K=%d does not fit in shared memory", K);
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    AGB_CUDA(cudaFuncSetAttribute(agb::unpermute_columns_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, di.smem_optin));
-    attr_set_dev[attr_dev] = true;
-  }
+    return failf(AGB200_ENOSUP, "dgrad: act-order row of K=%d does not fit in shared memory", K);
+  if (int rc = opt_in_smem<agb::unpermute_columns_kernel>(di.smem_optin)) return rc;
   const int grid = M < 8 * di.sms ? M : 8 * di.sms;
   agb::unpermute_columns_kernel<<<grid, 256, smem, static_cast<cudaStream_t>(stream)>>>(static_cast<const uint16_t*>(in), perm,
                                                                                        static_cast<uint16_t*>(out), M, K);
@@ -480,12 +374,12 @@ const char* agb200_build_info(void) {
 }
 
 int agb200_w4_prefetch_hint(int n, const void* const* ptrs, const size_t* bytes) {
-  if (n < 0 || n > agb::kMaxPrefetchRanges) return fail(AGB200_EINVAL, "prefetch hint: 0 <= n <= %d ranges (got %d)", agb::kMaxPrefetchRanges, n);
-  if (n > 0 && (!ptrs || !bytes)) return fail(AGB200_EINVAL, "null pointer argument");
+  if (n < 0 || n > agb::kMaxPrefetchRanges) return failf(AGB200_EINVAL, "prefetch hint: 0 <= n <= %d ranges (got %d)", agb::kMaxPrefetchRanges, n);
+  if (n > 0 && (!ptrs || !bytes)) return failf(AGB200_EINVAL, "null pointer argument");
   g_pf.n = 0;
   for (int i = 0; i < n; ++i) {
     if (ptrs[i] == nullptr || bytes[i] == 0) continue;
-    if (!aligned16(ptrs[i])) return fail(AGB200_EINVAL, "prefetch ranges must be 16-byte aligned");
+    if (!aligned(ptrs[i], 16)) return failf(AGB200_EINVAL, "prefetch ranges must be 16-byte aligned");
     g_pf.ptr[g_pf.n] = static_cast<const char*>(ptrs[i]);
     g_pf.bytes[g_pf.n] = bytes[i];
     ++g_pf.n;
@@ -495,8 +389,7 @@ int agb200_w4_prefetch_hint(int n, const void* const* ptrs, const size_t* bytes)
 
 int agb200_device_count(void) {
   int n = 0;
-  cudaError_t e = cudaGetDeviceCount(&n);
-  if (e != cudaSuccess) return fail(AGB200_ECUDA, "cudaGetDeviceCount: %s", cudaGetErrorString(e));
+  AGB_CUDA(cudaGetDeviceCount(&n));
   return n;
 }
 
@@ -512,7 +405,7 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
   if (int rc = check_common(x, qweight, qzeros, scales, y, M, K, N, group_size, dtype)) return rc;
   if (M == 0) return 0;
   DeviceInfo di;
-  if (int rc = get_device_info(di)) return rc;
+  if (int rc = device_info(di)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool bf16 = dtype == AGB200_BF16;
   if (kernel == AGB200_KERNEL_AUTO) {
@@ -569,20 +462,17 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
   }
   if (kernel == AGB200_KERNEL_GEMM) {
     if (qweight_tc == nullptr)
-      return fail(AGB200_ENOSUP, "the tensor-core path (M=%d > 8) needs qweight_tc: run agb200_w4_prepare_tc once at load time", M);
-    if (!aligned16(qweight_tc)) return fail(AGB200_EINVAL, "qweight_tc must be 16-byte aligned");
-    if (N % 32 != 0) return fail(AGB200_ENOSUP, "the tensor-core path needs outfeatures %% 32 == 0 (got %d)", N);
+      return failf(AGB200_ENOSUP, "the tensor-core path (M=%d > 8) needs qweight_tc: run agb200_w4_prepare_tc once at load time", M);
+    if (!aligned(qweight_tc, 16)) return failf(AGB200_EINVAL, "qweight_tc must be 16-byte aligned");
+    if (N % 32 != 0) return failf(AGB200_ENOSUP, "the tensor-core path needs outfeatures %% 32 == 0 (got %d)", N);
     agb::GemmArgs a{};
     a.x = x; a.qweight = qweight_tc; a.qzeros = qzeros; a.scales = scales; a.perm = perm; a.bias = bias; a.y = y;
     a.M = M; a.K = K; a.N = N; a.group_size = group_size; a.bf16 = bf16;
     a.workspace = workspace; a.workspace_bytes = workspace_bytes;
-    a.tile_m = tune0; a.split_k = tune1; a.sms = di.sms; a.smem_optin = di.smem_optin;
-    char msg[400] = "";
-    const int rc = agb::launch_w4a16_gemm(a, stream, msg, sizeof(msg));
-    if (rc != 0) return fail(rc, "%s", msg);
-    return 0;
+    a.tile_m = tune0; a.split_k = tune1; a.sms = di.sms;
+    return agb::launch_w4a16_gemm(a, stream);
   }
-  return fail(AGB200_EINVAL, "unknown kernel selector %d", kernel);
+  return failf(AGB200_EINVAL, "unknown kernel selector %d", kernel);
 }
 
 int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const* qweight, const int32_t* const* qweight_tc,
@@ -590,13 +480,13 @@ int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const
                                const void* const* bias, void* const* y, const int* N, int M, int K, int group_size,
                                int dtype, void* workspace, size_t workspace_bytes, void* stream_) {
   activate_prefetch_hint();
-  if (n_layers < 1 || n_layers > agb::kGemvMaxGroup) return fail(AGB200_EINVAL, "forward_group: 1 <= n_layers <= 4 (got %d)", n_layers);
-  if (!qweight || !qzeros || !scales || !y || !N) return fail(AGB200_EINVAL, "null pointer argument");
+  if (n_layers < 1 || n_layers > agb::kGemvMaxGroup) return failf(AGB200_EINVAL, "forward_group: 1 <= n_layers <= 4 (got %d)", n_layers);
+  if (!qweight || !qzeros || !scales || !y || !N) return failf(AGB200_EINVAL, "null pointer argument");
   for (int i = 0; i < n_layers; ++i)
     if (int rc = check_common(x, qweight[i], qzeros[i], scales[i], y[i], M, K, N[i], group_size, dtype)) return rc;
   if (M == 0) return 0;
   DeviceInfo di;
-  if (int rc = get_device_info(di)) return rc;
+  if (int rc = device_info(di)) return rc;
   {
     bool same_perm = true;
     for (int i = 1; i < n_layers; ++i) same_perm = same_perm && (perm ? perm[i] : nullptr) == (perm ? perm[0] : nullptr);
@@ -644,7 +534,7 @@ int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const
     case 3: return launch_gemv_mln<3, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
     case 4: return launch_gemv_mln<4, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
   }
-  return fail(AGB200_EINVAL, "forward_group: M=%d", M);
+  return failf(AGB200_EINVAL, "forward_group: M=%d", M);
 }
 
 int agb200_w4a16_forward(const void* x, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros, const void* scales,
@@ -655,21 +545,20 @@ int agb200_w4a16_forward(const void* x, const int32_t* qweight, const int32_t* q
 }
 
 size_t agb200_w4a16_host_staging_bytes(int M, int K, int N) {
-  auto up = [](size_t v) { return (v + 255) / 256 * 256; };
-  return up(static_cast<size_t>(M) * K * 2) + up(static_cast<size_t>(M) * N * 2) + up(agb::gemm_workspace_bytes(M, K, N));
+  return align_up(static_cast<size_t>(M) * K * 2, 256) + align_up(static_cast<size_t>(M) * N * 2, 256) +
+         align_up(agb::gemm_workspace_bytes(M, K, N), 256);
 }
 
 int agb200_w4a16_forward_host(const void* x_host, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros, const void* scales,
                               const int32_t* perm, const void* bias, void* y_host, int M, int K, int N, int group_size,
                               int dtype, void* staging, size_t staging_bytes, void* stream_) {
-  if (!x_host || !y_host || !staging) return fail(AGB200_EINVAL, "null host/staging pointer");
+  if (!x_host || !y_host || !staging) return failf(AGB200_EINVAL, "null host/staging pointer");
   if (staging_bytes < agb200_w4a16_host_staging_bytes(M, K, N))
-    return fail(AGB200_EWORKSPACE, "staging buffer too small: %zu < %zu", staging_bytes, agb200_w4a16_host_staging_bytes(M, K, N));
-  auto up = [](size_t v) { return (v + 255) / 256 * 256; };
+    return failf(AGB200_EWORKSPACE, "staging buffer too small: %zu < %zu", staging_bytes, agb200_w4a16_host_staging_bytes(M, K, N));
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   char* xd = static_cast<char*>(staging);
-  char* yd = xd + up(static_cast<size_t>(M) * K * 2);
-  char* ws = yd + up(static_cast<size_t>(M) * N * 2);
+  char* yd = xd + align_up(static_cast<size_t>(M) * K * 2, 256);
+  char* ws = yd + align_up(static_cast<size_t>(M) * N * 2, 256);
   AGB_CUDA(cudaMemcpyAsync(xd, x_host, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, stream));
   if (int rc = agb200_w4a16_forward(xd, qweight, qweight_tc, qzeros, scales, perm, bias, yd, M, K, N, group_size, dtype, ws,
                                     agb::gemm_workspace_bytes(M, K, N), stream_))
@@ -680,9 +569,9 @@ int agb200_w4a16_forward_host(const void* x_host, const int32_t* qweight, const 
 
 int agb200_w4_make_sequential(const int32_t* qweight_in, const int32_t* perm, int32_t* qweight_out, int K, int N,
                               void* stream) {
-  if (!qweight_in || !perm || !qweight_out) return fail(AGB200_EINVAL, "null pointer argument");
-  if (K <= 0 || N <= 0 || K % 8 != 0) return fail(AGB200_EINVAL, "bad shape K=%d N=%d", K, N);
-  if (qweight_in == qweight_out) return fail(AGB200_EINVAL, "make_sequential is not in-place");
+  if (!qweight_in || !perm || !qweight_out) return failf(AGB200_EINVAL, "null pointer argument");
+  if (K <= 0 || N <= 0 || K % 8 != 0) return failf(AGB200_EINVAL, "bad shape K=%d N=%d", K, N);
+  if (qweight_in == qweight_out) return failf(AGB200_EINVAL, "make_sequential is not in-place");
   dim3 grid((N + 255) / 256, K / 8);
   agb::w4_make_sequential_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const uint32_t*>(qweight_in), perm, reinterpret_cast<uint32_t*>(qweight_out), K / 8, N);
@@ -691,8 +580,8 @@ int agb200_w4_make_sequential(const int32_t* qweight_in, const int32_t* perm, in
 }
 
 int agb200_w4_prepare_tc(const int32_t* qweight_in, int32_t* qweight_tc_out, int K, int N, void* stream) {
-  if (!qweight_in || !qweight_tc_out) return fail(AGB200_EINVAL, "null pointer argument");
-  if (K <= 0 || N <= 0 || K % 8 != 0) return fail(AGB200_EINVAL, "bad shape K=%d N=%d", K, N);
+  if (!qweight_in || !qweight_tc_out) return failf(AGB200_EINVAL, "null pointer argument");
+  if (K <= 0 || N <= 0 || K % 8 != 0) return failf(AGB200_EINVAL, "bad shape K=%d N=%d", K, N);
   const size_t nwords = static_cast<size_t>(K / 8) * N;
   agb::w4_prepare_tc_kernel<<<static_cast<unsigned>((nwords + 255) / 256), 256, 0, static_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<const uint32_t*>(qweight_in), reinterpret_cast<uint32_t*>(qweight_tc_out), nwords);
@@ -702,7 +591,7 @@ int agb200_w4_prepare_tc(const int32_t* qweight_in, int32_t* qweight_tc_out, int
 
 int agb200_w4_dequantize(const int32_t* qweight, const int32_t* qzeros, const void* scales, const int32_t* g_idx,
                          void* w_out, int K, int N, int group_size, int dtype, void* stream) {
-  if (!w_out) return fail(AGB200_EINVAL, "null output");
+  if (!w_out) return failf(AGB200_EINVAL, "null output");
   if (int rc = check_common(w_out, qweight, qzeros, scales, w_out, 1, K, N, group_size, dtype)) return rc;
   dim3 grid((N + 255) / 256, K / 8);
   auto s = static_cast<cudaStream_t>(stream);
@@ -729,10 +618,10 @@ int agb200_w4a16_dgrad_ex(const void* dy, const int32_t* qweight, const int32_t*
                           void* dx, int M, int K, int N, int group_size, int dtype, void* workspace, size_t workspace_bytes,
                           void* stream_, int kernel, int tile_m, int split_k) {
   if (int rc = check_common(dy, qweight, qzeros, scales, dx, M, K, N, group_size, dtype)) return rc;
-  if (dy == dx) return fail(AGB200_EINVAL, "dgrad: dy and dx must not alias");
+  if (dy == dx) return failf(AGB200_EINVAL, "dgrad: dy and dx must not alias");
   if (M == 0) return 0;
   DeviceInfo di;
-  if (int rc = get_device_info(di)) return rc;
+  if (int rc = device_info(di)) return rc;
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool bf16 = dtype == AGB200_BF16;
   const bool tc_ok = agb::dgrad_tc_supported(K, N, group_size);
@@ -750,24 +639,23 @@ int agb200_w4a16_dgrad_ex(const void* dy, const int32_t* qweight, const int32_t*
     AGB_CUDA(cudaGetLastError());
     return 0;
   }
-  if (kernel != AGB200_DGRAD_WGMMA) return fail(AGB200_EINVAL, "dgrad: unknown kernel selector %d", kernel);
+  if (kernel != AGB200_DGRAD_WGMMA) return failf(AGB200_EINVAL, "dgrad: unknown kernel selector %d", kernel);
   if (!tc_ok)
-    return fail(AGB200_ENOSUP, "dgrad: the tensor-core path needs N %% 32 == 0 and group_size >= 32 with group_size %% 16 == 0 "
+    return failf(AGB200_ENOSUP, "dgrad: the tensor-core path needs N %% 32 == 0 and group_size >= 32 with group_size %% 16 == 0 "
                                "(or one group); got K=%d N=%d group_size=%d", K, N, group_size);
   void* out = dx;
   if (perm != nullptr) {
     const size_t need = static_cast<size_t>(M) * K * 2;
     if (workspace == nullptr || workspace_bytes < need)
-      return fail(AGB200_EWORKSPACE, "dgrad: act-order needs a %zu-byte workspace for the row-sorted dx (got %zu)", need, workspace_bytes);
-    if (!aligned16(workspace)) return fail(AGB200_EINVAL, "dgrad: workspace must be 16-byte aligned");
+      return failf(AGB200_EWORKSPACE, "dgrad: act-order needs a %zu-byte workspace for the row-sorted dx (got %zu)", need, workspace_bytes);
+    if (!aligned(workspace, 16)) return failf(AGB200_EINVAL, "dgrad: workspace must be 16-byte aligned");
     out = workspace;
   }
   agb::DgradArgs a{};
   a.dy = dy; a.qweight = qweight; a.qzeros = qzeros; a.scales = scales; a.dx = out;
   a.M = M; a.K = K; a.N = N; a.group_size = group_size; a.bf16 = bf16;
   a.tile_m = tile_m; a.split_k = split_k; a.sms = di.sms;
-  char msg[400] = "";
-  if (int rc = agb::launch_w4a16_dgrad(a, stream, msg, sizeof(msg))) return fail(rc, "%s", msg);
+  if (int rc = agb::launch_w4a16_dgrad(a, stream)) return rc;
   if (perm != nullptr) return agb_internal_unpermute_columns(out, perm, dx, M, K, stream);
   return 0;
 }
@@ -781,8 +669,8 @@ int agb200_w4a16_dgrad(const void* dy, const int32_t* qweight, const int32_t* qz
 
 int agb200_permute_columns(const void* x, const int32_t* perm, void* x_out, int M, int K, int dtype, void* stream) {
   (void)dtype;
-  if (!x || !perm || !x_out) return fail(AGB200_EINVAL, "null pointer argument");
-  if (M <= 0 || K <= 0) return fail(AGB200_EINVAL, "bad shape M=%d K=%d", M, K);
+  if (!x || !perm || !x_out) return failf(AGB200_EINVAL, "null pointer argument");
+  if (M <= 0 || K <= 0) return failf(AGB200_EINVAL, "bad shape M=%d K=%d", M, K);
   dim3 grid((K + 255) / 256, M);
   agb::permute_columns_kernel<<<grid, 256, 0, static_cast<cudaStream_t>(stream)>>>(
       static_cast<const uint16_t*>(x), perm, static_cast<uint16_t*>(x_out), M, K);

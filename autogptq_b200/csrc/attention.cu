@@ -2,39 +2,17 @@
 // count, workspace layout and the launch on the caller's stream.  Kernel: attention.cuh.
 #include <cuda_runtime.h>
 
-#include <cstdarg>
-#include <cstdio>
-
-#include "../../include/autogptq_b200.h"
 #include "attention.cuh"
-#include "internal.h"
+#include "host.h"
 
 namespace {
 
-int failf(int code, const char* fmt, ...) {
-  char buf[400];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return agb_internal_fail(code, buf);
-}
-
-#define AT_CUDA(expr)                                                                           \
-  do {                                                                                          \
-    cudaError_t e_ = (expr);                                                                    \
-    if (e_ != cudaSuccess) return failf(AGB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
-  } while (0)
-
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
 // Splits of the sequence per (b, kv head): about four CTAs per SM over the whole grid, at most one per tile of the cache.
-// Depends only on the shape and the device, so one launch configuration serves every position (graph capture).
+// Depends only on the shape and the device, so one launch configuration serves every position (graph capture).  Without
+// a usable device (the workspace size query has no error channel) it plans for the 132 SMs of an H100 SXM.
 int attn_splits(int B, int n_kv, int max_length) {
-  int dev = 0, sms = 132;
-  if (cudaGetDevice(&dev) != cudaSuccess || cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess)
-    sms = 132;
+  DeviceInfo di;
+  const int sms = device_info(di) == 0 ? di.sms : 132;
   const int want = (4 * sms + B * n_kv - 1) / (B * n_kv);
   const int tiles = (max_length + agb::kAttnTile - 1) / agb::kAttnTile;
   int s = want < tiles ? want : tiles;
@@ -110,7 +88,7 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
     if (bf16) agb::decode_attention_kernel<true, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
     else agb::decode_attention_kernel<false, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
   }
-  AT_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 

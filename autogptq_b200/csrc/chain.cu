@@ -5,34 +5,16 @@
 
 #include <algorithm>
 #include <mutex>
-#include <cstdarg>
-#include <cstdio>
 #include <cstdlib>
 #include <cstring>
 #include <new>
 #include <vector>
 
-#include "../../include/autogptq_b200.h"
 #include "chain.cuh"
-#include "internal.h"
+#include "host.h"
 #include "tmap.cuh"
 
 namespace {
-
-int failf(int code, const char* fmt, ...) {
-  char buf[400];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return agb_internal_fail(code, buf);
-}
-
-#define CH_CUDA(expr)                                                                           \
-  do {                                                                                          \
-    cudaError_t e_ = (expr);                                                                    \
-    if (e_ != cudaSuccess) return failf(AGB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
-  } while (0)
 
 constexpr uint32_t kMagic = 0x43484e32u;   // "CHN2"
 // Measured on one H100 80GB HBM3 at a 400 W power limit, bench.py's Llama-2-7B token (tools/chain_lookahead_sweep.py,
@@ -53,7 +35,6 @@ struct Chain {
   agb::ChainParams params;
 };
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
 constexpr size_t kFlagsBytes = 256;
 constexpr size_t kProfBytes = 256 * agb::kChProfRows * agb::kChProfSlots * sizeof(long long);   // up to 256 CTAs
 size_t stages_bytes(int n) { return align_up(size_t(n) * sizeof(agb::ChainStage), 128); }
@@ -69,20 +50,6 @@ size_t ll_bytes(const agb200_chain_stage* stages, const agb200_chain_norm* norms
     if (norms && publishes_residual(stages[i], norms + i)) total += align_up(size_t(M) * stages[i].K * 4, 128);
   }
   return total;
-}
-
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
-
-int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType dt, const void* base, uint64_t inner,
-              uint64_t outer, uint64_t row_bytes, uint32_t box_inner, uint32_t box_outer, const char* what, bool swizzle128 = false) {
-  const cuuint64_t gdim[2] = {inner, outer};
-  const cuuint64_t gstride[1] = {row_bytes};
-  const cuuint32_t box[2] = {box_inner, box_outer};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult cr = encode(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return failf(AGB200_ECUDA, "chain: cuTensorMapEncodeTiled(%s) failed (CUresult %d)", what, static_cast<int>(cr));
-  return 0;
 }
 
 // Host-mapped diagnostic words shared by all chains of the process: a protocol timeout writes {site, stage, CTA, warp,
@@ -119,26 +86,12 @@ const char* site_name(int site) {
 
 template <int kM, bool kBf16, bool kProf>
 int launch_inst(const Chain& c, int flags, cudaStream_t stream) {
-  auto kern = agb::w4a16_chain_kernel<kM, kBf16, kProf>;
-  static bool attr_set[64] = {};
-  if (!attr_set[c.device]) {
-    CH_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, c.smem_optin));
-    attr_set[c.device] = true;
-  }
+  constexpr auto kern = &agb::w4a16_chain_kernel<kM, kBf16, kProf>;
+  if (int rc = opt_in_smem<kern>(c.smem_optin)) return rc;
   agb::ChainParams p = c.params;
   p.debug = flags;
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(c.grid, 1, 1);
-  cfg.blockDim = dim3(agb::kChThreads, 1, 1);
-  cfg.dynamicSmemBytes = c.smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[1];
-  attrs[0].id = cudaLaunchAttributeCooperative;      // every CTA must be resident: they wait for each other's outputs
-  attrs[0].val.cooperative = 1;
-  cfg.attrs = attrs;
-  cfg.numAttrs = 1;
-  CH_CUDA(cudaLaunchKernelEx(&cfg, kern, p));
-  return 0;
+  // cooperative: every CTA must be resident, they wait for each other's outputs
+  return launch(kern, dim3(c.grid), dim3(agb::kChThreads), c.smem, stream, false, dim3(1, 1, 1), true, p);
 }
 
 template <int kM>
@@ -182,22 +135,14 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
     if (stages[i].n_layers < 1 || stages[i].n_layers > agb::kChMaxGroup)
       return failf(AGB200_EINVAL, "chain stage %d: 1 <= n_layers <= 4 (got %d)", i, stages[i].n_layers);
   const size_t need = agb200_chain_plan_bytes_norm(stages, norms, n_stages, M);
-  if (plan_bytes < need || (reinterpret_cast<uintptr_t>(plan) & 255u))
+  if (plan_bytes < need || !aligned(plan, 256))
     return failf(AGB200_EWORKSPACE, "chain: plan buffer needs %zu bytes, 256-byte aligned (got %zu)", need, plan_bytes);
 
-  int dev = 0;
-  CH_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "chain: device index %d out of range", dev);
-  int major = 0, sms = 0, smem_optin = 0, coop = 0;
-  CH_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 9) return failf(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
-  CH_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  CH_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  CH_CUDA(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
-  if (!coop) return failf(AGB200_ECUDA, "chain: device %d does not support cooperative launches", dev);
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  const int dev = di.device, sms = di.sms, smem_optin = di.smem_optin;
+  if (!di.coop) return failf(AGB200_ECUDA, "chain: device %d does not support cooperative launches", dev);
   if (sms > 256) return failf(AGB200_ENOSUP, "chain: %d SMs (profile buffer holds 256)", sms);
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "chain: cuTensorMapEncodeTiled entry point not available");
 
   unsigned char* base = static_cast<unsigned char*>(plan);
   unsigned* d_flags = reinterpret_cast<unsigned*>(base);
@@ -225,18 +170,18 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
     const int K = in.K, g = in.group_size;
     if (K <= 0 || K % 128 != 0 || K > max_k) return failf(AGB200_ENOSUP, "chain stage %d: K=%d must be a multiple of 128, at most %d for M=%d", i, K, max_k, M);
     if (g <= 0 || g % 128 != 0) return failf(AGB200_ENOSUP, "chain stage %d: group_size=%d must be a multiple of 128 (pass K for -1)", i, g);
-    if (!in.x || !aligned16(in.x)) return failf(AGB200_EINVAL, "chain stage %d: x must be a 16-byte aligned device pointer", i);
+    if (!in.x || !aligned(in.x, 16)) return failf(AGB200_EINVAL, "chain stage %d: x must be a 16-byte aligned device pointer", i);
     if (in.x_mode < 0 || in.x_mode > AGB200_CHAIN_X_ADD_RMSNORM) return failf(AGB200_EINVAL, "chain stage %d: unknown x_mode %d", i, in.x_mode);
     const bool norm_stage = in.x_mode == AGB200_CHAIN_X_RMSNORM || in.x_mode == AGB200_CHAIN_X_ADD_RMSNORM;
     if (norm_stage) {
       const agb200_chain_norm* nm = norms ? norms + i : nullptr;
       if (!nm) return failf(AGB200_EINVAL, "chain stage %d: a norm stage needs agb200_chain_create_norm with a norm entry", i);
-      if (!nm->weight || !aligned16(nm->weight)) return failf(AGB200_EINVAL, "chain stage %d: the norm weight must be a 16-byte aligned device pointer", i);
+      if (!nm->weight || !aligned(nm->weight, 16)) return failf(AGB200_EINVAL, "chain stage %d: the norm weight must be a 16-byte aligned device pointer", i);
       if (!(nm->eps > 0.f)) return failf(AGB200_EINVAL, "chain stage %d: norm eps must be > 0", i);
       if (K > AGB200_CHAIN_NORM_MAX_K) return failf(AGB200_ENOSUP, "chain stage %d: norm stages take K <= %d (got %d)", i, AGB200_CHAIN_NORM_MAX_K, K);
       if (in.x_mode == AGB200_CHAIN_X_ADD_RMSNORM) {
-        if (!in.x2 || !aligned16(in.x2)) return failf(AGB200_EINVAL, "chain stage %d: X_ADD_RMSNORM needs the residual as x2", i);
-        if (!nm->residual_out || !aligned16(nm->residual_out))
+        if (!in.x2 || !aligned(in.x2, 16)) return failf(AGB200_EINVAL, "chain stage %d: X_ADD_RMSNORM needs the residual as x2", i);
+        if (!nm->residual_out || !aligned(nm->residual_out, 16))
           return failf(AGB200_EINVAL, "chain stage %d: X_ADD_RMSNORM needs a 16-byte aligned residual_out", i);
       } else if (nm->residual_out) {
         return failf(AGB200_EINVAL, "chain stage %d: X_RMSNORM publishes no residual (residual_out must be NULL)", i);
@@ -273,7 +218,7 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
       if (src && src->N != K) return failf(AGB200_EINVAL, "chain stage %d: x is the output of a layer with N=%d but K=%d", i, src->N, K);
       st.x = in.x; st.x_ll = src ? src->ll : nullptr;
       if (in.x_mode == AGB200_CHAIN_X_SILU_MUL) {
-        if (!in.x2 || !aligned16(in.x2)) return failf(AGB200_EINVAL, "chain stage %d: X_SILU_MUL needs x2", i);
+        if (!in.x2 || !aligned(in.x2, 16)) return failf(AGB200_EINVAL, "chain stage %d: X_SILU_MUL needs x2", i);
         const Out* src2 = find(in.x2);
         if ((src2 != nullptr) != (src != nullptr)) return failf(AGB200_EINVAL, "chain stage %d: x and x2 must both be chain outputs or both be external", i);
         if (src2 && src2->N != K) return failf(AGB200_EINVAL, "chain stage %d: x2 is the output of a layer with N=%d but K=%d", i, src2->N, K);
@@ -289,7 +234,7 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
     if (norm_stage) xs_bytes = std::max(xs_bytes, static_cast<int>(align_up(size_t(M) * K * 2, 128)));
     rows_pad_max = std::max(rows_pad_max, st.chunks * agb::kChSlotRows);
     if (in.perm != nullptr) {
-      if (reinterpret_cast<uintptr_t>(in.perm) & 15u) return failf(AGB200_EINVAL, "chain stage %d: perm must be 16-byte aligned", i);
+      if (!aligned(in.perm, 16)) return failf(AGB200_EINVAL, "chain stage %d: perm must be 16-byte aligned", i);
       xs_bytes = std::max(xs_bytes, static_cast<int>(align_up(size_t(M) * K * 2, 128)));
     }
     const int G = (K + g - 1) / g;
@@ -301,7 +246,7 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
       if (L.n_peers < 0 || L.n_peers > AGB200_CHAIN_MAX_PEERS || (L.n_peers > 0 && !L.y_peers))
         return failf(AGB200_EINVAL, "chain stage %d layer %d: 0 <= n_peers <= %d with a device table", i, l, AGB200_CHAIN_MAX_PEERS);
       if (L.N <= 0 || L.N % 32 != 0) return failf(AGB200_ENOSUP, "chain stage %d layer %d: N=%d must be a positive multiple of 32", i, l, L.N);
-      if (!aligned16(L.qweight) || !aligned16(L.qzeros) || !aligned16(L.scales) || (reinterpret_cast<uintptr_t>(L.y) & 3u))
+      if (!aligned(L.qweight, 16) || !aligned(L.qzeros, 16) || !aligned(L.scales, 16) || !aligned(L.y, 4))
         return failf(AGB200_EINVAL, "chain stage %d layer %d: qweight, qzeros and scales must be 16-byte aligned (y: 4)", i, l);
       agb::ChainLayer& D = st.layer[l];
       D.bias = L.bias; D.y = L.y; D.N = L.N; D.tile_begin = tiles;
@@ -314,10 +259,14 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
       }
       tiles += L.N / 32;
       CUtensorMap mw, ms, mz;
-      if (int rc = encode_2d(encode, &mw, CU_TENSOR_MAP_DATA_TYPE_INT32, L.qweight, L.N, K / 8, size_t(L.N) * 4, 32, agb::kChSlotRows, "qweight", true)) return rc;   // 128 B rows, bank-conflict-free fragment loads
-      if (int rc = encode_2d(encode, &ms, dtype == AGB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
-                             L.scales, L.N, G, size_t(L.N) * elt, 32, 8, "scales")) return rc;
-      if (int rc = encode_2d(encode, &mz, CU_TENSOR_MAP_DATA_TYPE_INT32, L.qzeros, L.N / 8, G, size_t(L.N / 8) * 4, 4, 8, "qzeros")) return rc;
+      // qweight: 128 B rows, bank-conflict-free fragment loads
+      if (int rc = agb::encode_2d(&mw, CU_TENSOR_MAP_DATA_TYPE_INT32, L.qweight, L.N, K / 8, size_t(L.N) * 4, 32, agb::kChSlotRows,
+                                  CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "chain qweight")) return rc;
+      if (int rc = agb::encode_2d(&ms, dtype == AGB200_BF16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16,
+                                  L.scales, L.N, G, size_t(L.N) * elt, 32, 8, CU_TENSOR_MAP_SWIZZLE_NONE,
+                                  CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "chain scales")) return rc;
+      if (int rc = agb::encode_2d(&mz, CU_TENSOR_MAP_DATA_TYPE_INT32, L.qzeros, L.N / 8, G, size_t(L.N / 8) * 4, 4, 8,
+                                  CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "chain qzeros")) return rc;
       hm.push_back(mw); hm.push_back(ms); hm.push_back(mz);
     }
     st.total_tiles = tiles;
@@ -359,19 +308,17 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
   // L2 lookahead (chain.cuh, producer): the slots prefetched into L2 while the ring is full must still be there when the
   // consumers resume, next to the weights every other SM is streaming through L2 at the same time: all CTAs together keep
   // at most a third of the L2 in lookahead slots (H100: 7 slots)
-  int l2_bytes = 0;
-  CH_CUDA(cudaDeviceGetAttribute(&l2_bytes, cudaDevAttrL2CacheSize, dev));
-  const int lookahead_max = static_cast<int>(static_cast<size_t>(l2_bytes) / 3 / (size_t(agb::kChSlotBytes) * sms));
+  const int lookahead_max = static_cast<int>(static_cast<size_t>(di.l2_bytes) / 3 / (size_t(agb::kChSlotBytes) * sms));
   int lookahead = std::min(kDefaultLookahead, lookahead_max);
   if (const char* e = getenv("AGB200_CHAIN_L2_LOOKAHEAD")) { const int v = atoi(e); if (v >= 0) lookahead = std::min(v, lookahead_max); }
 
   // the plan is caller memory a stream-ordered allocator may have just recycled from a tensor that kernels queued on a
   // non-blocking stream still write; the legacy-stream copies below are not ordered after them (create time only)
-  CH_CUDA(cudaDeviceSynchronize());
-  CH_CUDA(cudaMemset(d_flags, 0, kFlagsBytes + kProfBytes));
-  if (ll_total > 0) CH_CUDA(cudaMemset(d_ll, 0, ll_total));
-  CH_CUDA(cudaMemcpy(d_stages, hs.data(), size_t(n_stages) * sizeof(agb::ChainStage), cudaMemcpyHostToDevice));
-  CH_CUDA(cudaMemcpy(d_maps, hm.data(), hm.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
+  AGB_CUDA(cudaDeviceSynchronize());
+  AGB_CUDA(cudaMemset(d_flags, 0, kFlagsBytes + kProfBytes));
+  if (ll_total > 0) AGB_CUDA(cudaMemset(d_ll, 0, ll_total));
+  AGB_CUDA(cudaMemcpy(d_stages, hs.data(), size_t(n_stages) * sizeof(agb::ChainStage), cudaMemcpyHostToDevice));
+  AGB_CUDA(cudaMemcpy(d_maps, hm.data(), hm.size() * sizeof(CUtensorMap), cudaMemcpyHostToDevice));
 
   Chain* c = new (std::nothrow) Chain();
   if (!c) return failf(AGB200_EINVAL, "chain: out of host memory");
@@ -396,7 +343,7 @@ int agb200_chain_forward(void* handle, int flags, void* stream) {
   Chain* c = static_cast<Chain*>(handle);
   if (!c || c->magic != kMagic) return failf(AGB200_EINVAL, "chain: bad handle");
   int dev = 0;
-  CH_CUDA(cudaGetDevice(&dev));
+  AGB_CUDA(cudaGetDevice(&dev));
   if (dev != c->device) return failf(AGB200_EINVAL, "chain: created on device %d, current device is %d", c->device, dev);
   if (g_diag_host != nullptr && g_diag_host[0] != 0)
     return failf(AGB200_ECUDA, "chain: an earlier launch timed out (%s; stage %d, CTA %d, warp %d, detail %d)", site_name(g_diag_host[0]),
@@ -434,23 +381,23 @@ int agb200_chain_profile(void* handle, long long* out_host, int max_entries) {
   if (!c || c->magic != kMagic || !out_host) return failf(AGB200_EINVAL, "chain: bad handle");
   const int n = c->grid * agb::kChProfRows * agb::kChProfSlots;
   if (max_entries < n) return failf(AGB200_EWORKSPACE, "chain profile: need room for %d entries", n);
-  CH_CUDA(cudaMemcpy(out_host, c->params.prof, size_t(n) * sizeof(long long), cudaMemcpyDeviceToHost));
+  AGB_CUDA(cudaMemcpy(out_host, c->params.prof, size_t(n) * sizeof(long long), cudaMemcpyDeviceToHost));
   return n;
 }
 
 int agb200_peer_alloc(size_t bytes, void** ptr_out) {
   if (!ptr_out || bytes == 0) return failf(AGB200_EINVAL, "peer_alloc: bad argument");
   void* p = nullptr;
-  CH_CUDA(cudaMalloc(&p, bytes));
+  AGB_CUDA(cudaMalloc(&p, bytes));
   cudaError_t e = cudaMemset(p, 0, bytes);
   if (e != cudaSuccess) { cudaFree(p); return failf(AGB200_ECUDA, "cudaMemset: %s", cudaGetErrorString(e)); }
-  CH_CUDA(cudaDeviceSynchronize());
+  AGB_CUDA(cudaDeviceSynchronize());
   *ptr_out = p;
   return 0;
 }
 
 int agb200_peer_free(void* ptr) {
-  if (ptr) CH_CUDA(cudaFree(ptr));
+  if (ptr) AGB_CUDA(cudaFree(ptr));
   return 0;
 }
 
@@ -458,7 +405,7 @@ int agb200_peer_export(const void* ptr, void* handle_out) {
   if (!ptr || !handle_out) return failf(AGB200_EINVAL, "peer_export: null pointer argument");
   static_assert(sizeof(cudaIpcMemHandle_t) == AGB200_PEER_HANDLE_BYTES, "IPC handle size");
   cudaIpcMemHandle_t h;
-  CH_CUDA(cudaIpcGetMemHandle(&h, const_cast<void*>(ptr)));
+  AGB_CUDA(cudaIpcGetMemHandle(&h, const_cast<void*>(ptr)));
   memcpy(handle_out, &h, sizeof(h));
   return 0;
 }
@@ -468,13 +415,13 @@ int agb200_peer_open(const void* handle, void** ptr_out) {
   cudaIpcMemHandle_t h;
   memcpy(&h, handle, sizeof(h));
   void* p = nullptr;
-  CH_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
+  AGB_CUDA(cudaIpcOpenMemHandle(&p, h, cudaIpcMemLazyEnablePeerAccess));
   *ptr_out = p;
   return 0;
 }
 
 int agb200_peer_close(void* ptr) {
-  if (ptr) CH_CUDA(cudaIpcCloseMemHandle(ptr));
+  if (ptr) AGB_CUDA(cudaIpcCloseMemHandle(ptr));
   return 0;
 }
 

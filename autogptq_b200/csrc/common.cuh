@@ -9,14 +9,6 @@ namespace agb {
 
 constexpr int kPack = 8;  // nibbles per int32 word of qweight / qzeros
 
-// Index into the per-device "function attribute already set" tables of the launchers (the opt-in to > 48 KB of dynamic
-// shared memory is per device: a process that drives several GPUs must set it on each of them).
-inline int current_device_index() {
-  int d = 0;
-  if (cudaGetDevice(&d) != cudaSuccess || d < 0 || d >= 64) d = 0;
-  return d;
-}
-
 // ---------------------------------------------------------------- memory
 // Predicated loads: the destination keeps its old value when !pred.  Written as one asm block so the compiler
 // sees a plain read-modify-write of the destination registers (no control flow, no phi copies that would

@@ -12,12 +12,12 @@
 #include <cooperative_groups.h>
 #include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched through the runtime)
 
-#include <cstdio>
 #include <type_traits>
 
 #include "common.cuh"
 #include "dgrad_common.cuh"
 #include "gemm_common.cuh"
+#include "host.h"
 #include "ptx.cuh"
 #include "tmap.cuh"
 
@@ -248,103 +248,54 @@ struct DgradArgs {
 
 template <int kMT, bool kBf16>
 int launch_dgrad_inst(const DgradParams& p, const CUtensorMap& tmap_dy, const CUtensorMap& tmap_w, const CUtensorMap& tmap_s,
-                      const CUtensorMap& tmap_z, int k_tiles, int m_tiles, cudaStream_t stream, char* msg, size_t msg_n) {
-  auto kern = w4a16_dgrad_kernel<kMT, kBf16>;
+                      const CUtensorMap& tmap_z, int k_tiles, int m_tiles, cudaStream_t stream) {
+  constexpr auto kern = &w4a16_dgrad_kernel<kMT, kBf16>;
   constexpr int smem = DgradSmem<kMT>::kTotal;
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { snprintf(msg, msg_n, "dgrad: cudaFuncSetAttribute(%d B): %s", smem, cudaGetErrorString(e)); return -2; }
-    attr_set_dev[attr_dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(k_tiles, m_tiles, p.split);
-  cfg.blockDim = dim3(kGemmThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[na].val.programmaticStreamSerializationAllowed = 1;
-  ++na;
-  if (p.split > 1) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = 1;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = p.split;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p, tmap_dy, tmap_w, tmap_s, tmap_z);
-  if (e != cudaSuccess) { snprintf(msg, msg_n, "dgrad launch (MT=%d split=%d): %s", kMT, p.split, cudaGetErrorString(e)); return -2; }
-  return 0;
+  if (int rc = opt_in_smem<kern>(smem)) return rc;
+  return launch(kern, dim3(k_tiles, m_tiles, p.split), dim3(kGemmThreads), smem, stream, true, dim3(1, 1, p.split), false,
+                p, tmap_dy, tmap_w, tmap_s, tmap_z);
 }
 
 // dx (row-sorted order for act-order layers) = dy * W^T on the tensor cores; the caller has checked dgrad_tc_supported
-inline int launch_w4a16_dgrad(const DgradArgs& a, cudaStream_t stream, char* msg, size_t msg_n) {
+inline int launch_w4a16_dgrad(const DgradArgs& a, cudaStream_t stream) {
   const int k_tiles = (a.K + kDgBK - 1) / kDgBK;
   int mt = a.tile_m;
   if (mt == 0) mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
-  if (mt != 32 && mt != 64 && mt != 128) { snprintf(msg, msg_n, "dgrad: dy-row tile must be 32/64/128 (got %d)", mt); return -1; }
+  if (mt != 32 && mt != 64 && mt != 128) return failf(AGB200_EINVAL, "dgrad: dy-row tile must be 32/64/128 (got %d)", mt);
   const int m_tiles = (a.M + mt - 1) / mt;
-  if (m_tiles > 65535) { snprintf(msg, msg_n, "dgrad: M=%d needs more than 65535 row tiles of %d", a.M, mt); return -1; }
+  if (m_tiles > 65535) return failf(AGB200_EINVAL, "dgrad: M=%d needs more than 65535 row tiles of %d", a.M, mt);
   DgradParams p{};
   p.dx = a.dx; p.M = a.M; p.K = a.K; p.N = a.N; p.group_size = a.group_size;
   p.num_nb = (a.N + kDgBN - 1) / kDgBN;
   int split = a.split_k;
   if (split == 0) split = gemm_auto_split(mt, k_tiles * m_tiles, p.num_nb, a.sms);
-  if (split != 1 && split != 2 && split != 4 && split != 8) { snprintf(msg, msg_n, "dgrad: split must be 1/2/4/8 (got %d)", split); return -1; }
+  if (split != 1 && split != 2 && split != 4 && split != 8) return failf(AGB200_EINVAL, "dgrad: split must be 1/2/4/8 (got %d)", split);
   while (split > 1 && split > p.num_nb) split /= 2;
   p.split = split;
   p.nb_per_split = (p.num_nb + split - 1) / split;
 
-  EncodeTiledFn encode = get_encode_fn();
-  if (encode == nullptr) { snprintf(msg, msg_n, "dgrad: cuTensorMapEncodeTiled entry point not available"); return -2; }
-  if (cudaError_t e = ensure_context()) { snprintf(msg, msg_n, "dgrad: no CUDA context: %s", cudaGetErrorString(e)); return -2; }
   const CUtensorMapDataType t16 = a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
-  const cuuint32_t one[2] = {1, 1};
   const int G = (a.K + a.group_size - 1) / a.group_size;
   CUtensorMap tmap_dy, tmap_w, tmap_s, tmap_z;
-  const cuuint64_t ddim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.M)};
-  const cuuint64_t dstride[1] = {static_cast<cuuint64_t>(a.N) * 2};
-  const cuuint32_t dbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(mt)};
-  const cuuint64_t wdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.K / 8)};
-  const cuuint64_t wstride[1] = {static_cast<cuuint64_t>(a.N) * 4};
-  const cuuint32_t wbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(kDgBK / 8)};
-  const cuuint64_t sdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(G)};
-  const cuuint64_t sstride[1] = {static_cast<cuuint64_t>(a.N) * 2};
-  const cuuint32_t sbox[2] = {static_cast<cuuint32_t>(kDgBN), static_cast<cuuint32_t>(kDgGroups)};
-  const cuuint64_t zdim[2] = {static_cast<cuuint64_t>(a.N / 8), static_cast<cuuint64_t>(G)};
-  const cuuint64_t zstride[1] = {static_cast<cuuint64_t>(a.N / 8) * 4};
-  const cuuint32_t zbox[2] = {static_cast<cuuint32_t>(kDgBN / 8), static_cast<cuuint32_t>(kDgGroups)};
-  const CUresult r0 = encode(&tmap_dy, t16, 2, const_cast<void*>(a.dy), ddim, dstride, dbox, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  const CUresult r1 = encode(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qweight), wdim, wstride, wbox, one,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  const CUresult r2 = encode(&tmap_s, t16, 2, const_cast<void*>(a.scales), sdim, sstride, sbox, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                             CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  const CUresult r3 = encode(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qzeros), zdim, zstride, zbox, one,
-                             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (r0 != CUDA_SUCCESS || r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS || r3 != CUDA_SUCCESS) {
-    snprintf(msg, msg_n, "dgrad: cuTensorMapEncodeTiled failed (dy %d, qweight %d, scales %d, qzeros %d)", static_cast<int>(r0),
-             static_cast<int>(r1), static_cast<int>(r2), static_cast<int>(r3));
-    return -2;
-  }
+  if (int rc = encode_2d(&tmap_dy, t16, a.dy, a.N, a.M, size_t(a.N) * 2, kDgBN, mt, CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "dgrad dy")) return rc;
+  if (int rc = encode_2d(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qweight, a.N, a.K / 8, size_t(a.N) * 4, kDgBN, kDgBK / 8,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "dgrad qweight")) return rc;
+  if (int rc = encode_2d(&tmap_s, t16, a.scales, a.N, G, size_t(a.N) * 2, kDgBN, kDgGroups, CU_TENSOR_MAP_SWIZZLE_NONE,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "dgrad scales")) return rc;
+  if (int rc = encode_2d(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qzeros, a.N / 8, G, size_t(a.N / 8) * 4, kDgBN / 8, kDgGroups,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "dgrad qzeros")) return rc;
 #define AGB_DGRAD_CASE(MT)                                                                                         \
   case MT:                                                                                                         \
-    return a.bf16 ? launch_dgrad_inst<MT, true>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream, msg, msg_n) \
-                  : launch_dgrad_inst<MT, false>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream, msg, msg_n);
+    return a.bf16 ? launch_dgrad_inst<MT, true>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream) \
+                  : launch_dgrad_inst<MT, false>(p, tmap_dy, tmap_w, tmap_s, tmap_z, k_tiles, m_tiles, stream);
   switch (mt) {
     AGB_DGRAD_CASE(32)
     AGB_DGRAD_CASE(64)
     AGB_DGRAD_CASE(128)
   }
 #undef AGB_DGRAD_CASE
-  return -1;
+  return AGB200_EINVAL;
 }
 
 }  // namespace agb

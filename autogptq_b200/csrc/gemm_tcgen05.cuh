@@ -8,12 +8,12 @@
 #include <cooperative_groups.h>
 #include <cuda.h>  // CUtensorMap (types only; the encode entry point is fetched through the runtime)
 
-#include <cstdio>
 #include <type_traits>
 
 #include "aux_kernels.cuh"
 #include "common.cuh"
 #include "gemm_common.cuh"
+#include "host.h"
 #include "ptx.cuh"
 #include "tmap.cuh"
 
@@ -23,7 +23,7 @@ namespace cg = cooperative_groups;
 struct GemmArgs {
   const void* x; const int32_t* qweight; const int32_t* qzeros; const void* scales; const int32_t* perm;
   const void* bias; void* y; int M, K, N, group_size; bool bf16; void* workspace; size_t workspace_bytes;
-  int tile_m, split_k, sms, smem_optin;
+  int tile_m, split_k, sms;
 };
 
 struct GemmParams {
@@ -265,49 +265,23 @@ inline size_t gemm_workspace_bytes(int M, int K, int) {
 
 template <int kMT, bool kBf16, bool kMcast>
 int launch_gemm_inst(const GemmParams& p, const CUtensorMap& tmap, const CUtensorMap& tmap_w, const CUtensorMap& tmap_s,
-                     const CUtensorMap& tmap_z, int m_tiles, cudaStream_t stream, char* msg, size_t msg_n) {
-  auto kern = w4a16_gemm_kernel<kMT, kBf16, kMcast>;
+                     const CUtensorMap& tmap_z, int m_tiles, cudaStream_t stream) {
+  constexpr auto kern = &w4a16_gemm_kernel<kMT, kBf16, kMcast>;
   constexpr int smem = GemmSmem<kMT>::kTotal;
-  static bool attr_set_dev[64] = {};   // cudaFuncSetAttribute is per device; benign race: idempotent
-  const int attr_dev = agb::current_device_index();
-  if (!attr_set_dev[attr_dev]) {
-    cudaError_t e = cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem);
-    if (e != cudaSuccess) { snprintf(msg, msg_n, "gemm: cudaFuncSetAttribute(%d B): %s", smem, cudaGetErrorString(e)); return -2; }
-    attr_set_dev[attr_dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3((p.N + kGemmBN - 1) / kGemmBN, m_tiles, p.split);
-  cfg.blockDim = dim3(kGemmThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attrs[2];
-  int na = 0;
-  attrs[na].id = cudaLaunchAttributeProgrammaticStreamSerialization;
-  attrs[na].val.programmaticStreamSerializationAllowed = 1;
-  ++na;
-  if (p.split > 1 || kMcast) {
-    attrs[na].id = cudaLaunchAttributeClusterDimension;
-    attrs[na].val.clusterDim.x = kMcast ? 2 : 1;
-    attrs[na].val.clusterDim.y = 1;
-    attrs[na].val.clusterDim.z = kMcast ? 1 : p.split;
-    ++na;
-  }
-  cfg.attrs = attrs;
-  cfg.numAttrs = na;
-  cudaError_t e = cudaLaunchKernelEx(&cfg, kern, p, tmap, tmap_w, tmap_s, tmap_z);
-  if (e != cudaSuccess) { snprintf(msg, msg_n, "gemm launch (MT=%d split=%d): %s", kMT, p.split, cudaGetErrorString(e)); return -2; }
-  return 0;
+  if (int rc = opt_in_smem<kern>(smem)) return rc;
+  const dim3 cluster = kMcast ? dim3(2, 1, 1) : dim3(1, 1, p.split);
+  return launch(kern, dim3((p.N + kGemmBN - 1) / kGemmBN, m_tiles, p.split), dim3(kGemmThreads), smem, stream, true, cluster,
+                false, p, tmap, tmap_w, tmap_s, tmap_z);
 }
 
-inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, size_t msg_n) {
-  if (a.group_size != 32 && a.group_size % 64 != 0) { snprintf(msg, msg_n, "gemm: group_size=%d must be 32 or a multiple of 64 (a 64-k stage carries one scale row)", a.group_size); return -3; }
+inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream) {
+  if (a.group_size != 32 && a.group_size % 64 != 0)
+    return failf(AGB200_ENOSUP, "gemm: group_size=%d must be 32 or a multiple of 64 (a 64-k stage carries one scale row)", a.group_size);
   const void* x = a.x;
   if (a.perm != nullptr) {
     const size_t need = static_cast<size_t>(a.M) * a.K * 2;
-    if (a.workspace == nullptr || a.workspace_bytes < need) {
-      snprintf(msg, msg_n, "gemm: act-order needs a %zu-byte workspace for the gathered x (got %zu)", need, a.workspace_bytes);
-      return -4;
-    }
+    if (a.workspace == nullptr || a.workspace_bytes < need)
+      return failf(AGB200_EWORKSPACE, "gemm: act-order needs a %zu-byte workspace for the gathered x (got %zu)", need, a.workspace_bytes);
     dim3 grid((a.K + 255) / 256, a.M);
     permute_columns_kernel<<<grid, 256, 0, stream>>>(static_cast<const uint16_t*>(a.x), a.perm,
                                                      static_cast<uint16_t*>(a.workspace), a.M, a.K);
@@ -320,7 +294,7 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
     // asynchronous, and a 128 x 128 tile already keeps the tensor cores busier than the weight expansion
     mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
   }
-  if (mt != 32 && mt != 64 && mt != 128 && mt != 256) { snprintf(msg, msg_n, "gemm: x-row tile must be 32/64/128/256 (got %d)", mt); return -1; }
+  if (mt != 32 && mt != 64 && mt != 128 && mt != 256) return failf(AGB200_EINVAL, "gemm: x-row tile must be 32/64/128/256 (got %d)", mt);
   const int m_tiles = (a.M + mt - 1) / mt;
   GemmParams p{};
   p.qweight = a.qweight; p.qzeros = a.qzeros; p.scales = a.scales; p.bias = a.bias; p.y = a.y;
@@ -332,73 +306,38 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
   int split = a.split_k & 0xff;
   const int mcast_req = (a.split_k >> 8) & 3;          // tests: 1 = force off, 2 = force on
   if (split == 0) split = gemm_auto_split(mt, n_tiles * m_tiles, p.num_kb, a.sms);
-  if (split != 1 && split != 2 && split != 4 && split != 8) { snprintf(msg, msg_n, "gemm: split-K must be 1/2/4/8 (got %d)", split); return -1; }
+  if (split != 1 && split != 2 && split != 4 && split != 8) return failf(AGB200_EINVAL, "gemm: split-K must be 1/2/4/8 (got %d)", split);
   while (split > 1 && split > p.num_kb) split /= 2;
   p.split = split;
   p.kb_per_split = (p.num_kb + split - 1) / split;
   bool mcast = false;   // pair-multicast of x: only on request
   if (mcast_req == 1) mcast = false;
   if (mcast_req == 2) {
-    if (split != 1 || n_tiles % 2 != 0 || mt < 128) { snprintf(msg, msg_n, "gemm: multicast needs split=1, an even number of N tiles and MT>=128"); return -1; }
+    if (split != 1 || n_tiles % 2 != 0 || mt < 128)
+      return failf(AGB200_EINVAL, "gemm: multicast needs split=1, an even number of N tiles and MT>=128");
     mcast = true;
   }
 
-  EncodeTiledFn encode = get_encode_fn();
-  if (encode == nullptr) { snprintf(msg, msg_n, "gemm: cuTensorMapEncodeTiled entry point not available"); return -2; }
-  if (cudaError_t e = ensure_context()) { snprintf(msg, msg_n, "gemm: no CUDA context: %s", cudaGetErrorString(e)); return -2; }
-  CUtensorMap tmap;
-  const cuuint64_t gdim[2] = {static_cast<cuuint64_t>(a.K), static_cast<cuuint64_t>(a.M)};
-  const cuuint64_t gstride[1] = {static_cast<cuuint64_t>(a.K) * 2};
-  const cuuint32_t box[2] = {static_cast<cuuint32_t>(kGemmBK), static_cast<cuuint32_t>(mcast ? mt / 2 : mt)};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult cr = encode(&tmap, a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                       const_cast<void*>(x), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) { snprintf(msg, msg_n, "gemm: cuTensorMapEncodeTiled failed (CUresult %d)", static_cast<int>(cr)); return -2; }
-
-  CUtensorMap tmap_w;
-  {
-    const cuuint64_t wdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(a.K / 8)};
-    const cuuint64_t wstride[1] = {static_cast<cuuint64_t>(a.N) * 4};
-    const cuuint32_t wbox[2] = {static_cast<cuuint32_t>(kGemmBN), static_cast<cuuint32_t>(kGemmBK / 8)};
-    const cuuint32_t westr[2] = {1, 1};
-    CUresult wr = encode(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qweight), wdim, wstride, wbox,
-                         westr, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (wr != CUDA_SUCCESS) { snprintf(msg, msg_n, "gemm: cuTensorMapEncodeTiled(qweight) failed (CUresult %d)", static_cast<int>(wr)); return -2; }
-  }
-
-  CUtensorMap tmap_s, tmap_z;
-  {
-    const int G = (a.K + a.group_size - 1) / a.group_size;
-    const cuuint32_t ngr = a.group_size == 32 ? 2 : 1;
-    const cuuint64_t sdim[2] = {static_cast<cuuint64_t>(a.N), static_cast<cuuint64_t>(G)};
-    const cuuint64_t sstride[1] = {static_cast<cuuint64_t>(a.N) * 2};
-    const cuuint32_t sbox[2] = {static_cast<cuuint32_t>(kGemmBN), ngr};
-    const cuuint32_t one[2] = {1, 1};
-    CUresult r1 = encode(&tmap_s, a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16, 2,
-                         const_cast<void*>(a.scales), sdim, sstride, sbox, one, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    const cuuint64_t zdim[2] = {static_cast<cuuint64_t>(a.N / 8), static_cast<cuuint64_t>(G)};
-    const cuuint64_t zstride[1] = {static_cast<cuuint64_t>(a.N / 8) * 4};
-    const cuuint32_t zbox[2] = {static_cast<cuuint32_t>(kGemmBN / 8), ngr};
-    CUresult r2 = encode(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, 2, const_cast<int32_t*>(a.qzeros), zdim, zstride, zbox, one,
-                         CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                         CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    if (r1 != CUDA_SUCCESS || r2 != CUDA_SUCCESS) {
-      snprintf(msg, msg_n, "gemm: cuTensorMapEncodeTiled(scales/qzeros) failed (CUresult %d / %d; N/8*4 = %d bytes must be a multiple of 16)",
-               static_cast<int>(r1), static_cast<int>(r2), a.N / 8 * 4);
-      return -2;
-    }
-  }
+  const CUtensorMapDataType t16 = a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
+  const int G = (a.K + a.group_size - 1) / a.group_size;
+  const uint32_t ngr = a.group_size == 32 ? 2 : 1;
+  CUtensorMap tmap, tmap_w, tmap_s, tmap_z;
+  if (int rc = encode_2d(&tmap, t16, x, a.K, a.M, size_t(a.K) * 2, kGemmBK, mcast ? mt / 2 : mt, CU_TENSOR_MAP_SWIZZLE_128B,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "gemm x")) return rc;
+  if (int rc = encode_2d(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qweight, a.N, a.K / 8, size_t(a.N) * 4, kGemmBN, kGemmBK / 8,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "gemm qweight")) return rc;
+  if (int rc = encode_2d(&tmap_s, t16, a.scales, a.N, G, size_t(a.N) * 2, kGemmBN, ngr, CU_TENSOR_MAP_SWIZZLE_NONE,
+                         CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "gemm scales")) return rc;
+  if (int rc = encode_2d(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qzeros, a.N / 8, G, size_t(a.N / 8) * 4, kGemmBN / 8, ngr,
+                         CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "gemm qzeros")) return rc;
 
 #define AGB_GEMM_CASE(MT)                                                                                       \
   case MT:                                                                                                      \
     if (MT >= 128 && mcast)                                                                                     \
-      return a.bf16 ? launch_gemm_inst<(MT >= 128 ? MT : 128), true, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream, msg, msg_n)  \
-                    : launch_gemm_inst<(MT >= 128 ? MT : 128), false, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream, msg, msg_n); \
-    return a.bf16 ? launch_gemm_inst<MT, true, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream, msg, msg_n)                     \
-                  : launch_gemm_inst<MT, false, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream, msg, msg_n);
+      return a.bf16 ? launch_gemm_inst<(MT >= 128 ? MT : 128), true, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream)  \
+                    : launch_gemm_inst<(MT >= 128 ? MT : 128), false, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream); \
+    return a.bf16 ? launch_gemm_inst<MT, true, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream)                     \
+                  : launch_gemm_inst<MT, false, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream);
   switch (mt) {
     AGB_GEMM_CASE(32)
     AGB_GEMM_CASE(64)
@@ -406,7 +345,7 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream, char* msg, 
     AGB_GEMM_CASE(256)
   }
 #undef AGB_GEMM_CASE
-  return -1;
+  return AGB200_EINVAL;
 }
 
 }  // namespace agb

@@ -9,40 +9,20 @@
 #include <cuda_runtime.h>
 
 #include <algorithm>
-#include <cstdarg>
-#include <cstdio>
 #include <cstring>
 #include <new>
 #include <vector>
 
-#include "../../include/autogptq_b200.h"
-#include "internal.h"
+#include "host.h"
 #include "moe.cuh"
 #include "moe_dgrad.cuh"
 #include "tmap.cuh"
 
 namespace {
 
-int failf(int code, const char* fmt, ...) {
-  char buf[400];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return agb_internal_fail(code, buf);
-}
-
-#define MOE_CUDA(expr)                                                                          \
-  do {                                                                                          \
-    cudaError_t e_ = (expr);                                                                    \
-    if (e_ != cudaSuccess) return failf(AGB200_ECUDA, "%s: %s", #expr, cudaGetErrorString(e_)); \
-  } while (0)
-
 constexpr uint32_t kMagic = 0x4d4f4531u;   // "MOE1"
 constexpr size_t kDownXsCap = 64 * 1024;     // x bytes per down-stage work item: <= 64 KB keeps 3 CTAs per SM
 
-size_t align_up(size_t v, size_t a) { return (v + a - 1) / a * a; }
-bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15u) == 0; }
 int round_up(int v, int a) { return (v + a - 1) / a * a; }
 
 struct Moe {
@@ -99,17 +79,12 @@ agb::MoeRoute route_views(void* ws, int E, const WsLayout& w) {
   return r;
 }
 
-int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType dt, const void* base, uint64_t inner,
-              uint64_t outer, uint64_t row_bytes, uint32_t box_inner, uint32_t box_outer, bool swizzle128, const char* what) {
-  const cuuint64_t gdim[2] = {inner, outer};
-  const cuuint64_t gstride[1] = {row_bytes};
-  const cuuint32_t box[2] = {box_inner, box_outer};
-  const cuuint32_t estr[2] = {1, 1};
-  CUresult cr = encode(out, dt, 2, const_cast<void*>(base), gdim, gstride, box, estr, CU_TENSOR_MAP_INTERLEAVE_NONE,
-                       swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
-                       CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-  if (cr != CUDA_SUCCESS) return failf(AGB200_ECUDA, "moe: cuTensorMapEncodeTiled(%s) failed (CUresult %d)", what, static_cast<int>(cr));
-  return 0;
+// agb::encode_2d with the policy of every map of this unit: L2 promotion in 256-byte lines, 128-byte swizzle for the
+// activation tiles, none for the weights.
+int encode_map(CUtensorMap* out, CUtensorMapDataType dt, const void* base, uint64_t inner, uint64_t outer, uint64_t row_bytes,
+               uint32_t box_inner, uint32_t box_outer, bool swizzle128, const char* what) {
+  return agb::encode_2d(out, dt, base, inner, outer, row_bytes, box_inner, box_outer,
+                        swizzle128 ? CU_TENSOR_MAP_SWIZZLE_128B : CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, what);
 }
 
 // The attribute is the kernel's, shared by every plan in the process: it is raised to the device's opt-in limit, never
@@ -117,8 +92,8 @@ int encode_2d(agb::EncodeTiledFn encode, CUtensorMap* out, CUtensorMapDataType d
 template <bool kBf16, bool kGateUp, class Src = agb::MoeRouted>
 int decode_setup(size_t smem, int smem_optin, int& occ) {
   auto kern = agb::moe_decode_kernel<kBf16, kGateUp, Src>;
-  MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-  MOE_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, agb::kMdThreads, smem));
+  AGB_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
+  AGB_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, kern, agb::kMdThreads, smem));
   if (occ < 1) return failf(AGB200_ENOSUP, "moe: decode kernel with %zu B of shared memory does not fit an SM", smem);
   return 0;
 }
@@ -130,7 +105,7 @@ int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, const Src& src, i
   const int grid = std::max(1, std::min(max_items, m.sms * occ));
   if (m.dtype == AGB200_BF16) agb::moe_decode_kernel<true, kGateUp, Src><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
   else agb::moe_decode_kernel<false, kGateUp, Src><<<grid, agb::kMdThreads, smem, stream>>>(p, src);
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -138,33 +113,11 @@ int launch_decode(const Moe& m, const agb::MoeDecodeParams& p, const Src& src, i
 template <int kMT, bool kBf16, bool kGateUp, class Src>
 int launch_gemm_inst(const agb::MoeGemmParams& p, const CUtensorMap& tmap_x, const Src& src, int n_tiles, int m_tiles,
                      cudaStream_t stream) {
-  auto kern = agb::moe_gemm_kernel<kMT, kBf16, kGateUp, Src>;
+  constexpr auto kern = &agb::moe_gemm_kernel<kMT, kBf16, kGateUp, Src>;
   constexpr int smem = agb::MoeGemmSmem<kMT>::kTotal;
-  static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
-  const int dev = agb::current_device_index();
-  if (!attr_set_dev[dev]) {
-    MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set_dev[dev] = true;
-  }
-  if (p.split == 1) {
-    kern<<<dim3(n_tiles, m_tiles, 1), agb::kGemmThreads, smem, stream>>>(p, tmap_x, src);
-  } else {
-    cudaLaunchConfig_t cfg{};
-    cfg.gridDim = dim3(n_tiles, m_tiles, p.split);
-    cfg.blockDim = dim3(agb::kGemmThreads, 1, 1);
-    cfg.dynamicSmemBytes = smem;
-    cfg.stream = stream;
-    cudaLaunchAttribute attr;
-    attr.id = cudaLaunchAttributeClusterDimension;
-    attr.val.clusterDim.x = 1;
-    attr.val.clusterDim.y = 1;
-    attr.val.clusterDim.z = p.split;
-    cfg.attrs = &attr;
-    cfg.numAttrs = 1;
-    MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tmap_x, src));
-  }
-  MOE_CUDA(cudaGetLastError());
-  return 0;
+  if (int rc = opt_in_smem<kern>(smem)) return rc;
+  return launch(kern, dim3(n_tiles, m_tiles, p.split), dim3(agb::kGemmThreads), smem, stream, false, dim3(1, 1, p.split), false,
+                p, tmap_x, src);
 }
 
 template <bool kGateUp, class Src>
@@ -210,16 +163,12 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
     if (gs <= 0 || (gs != 32 && gs % 64 != 0))
       return failf(AGB200_ENOSUP, "moe: group_size=%d must be 32, a multiple of 64, or -1", group_size);
   const size_t need = agb200_moe_plan_bytes(E, H, I, group_size);
-  if (plan_bytes < need || (reinterpret_cast<uintptr_t>(plan) & 255u))
+  if (plan_bytes < need || !aligned(plan, 256))
     return failf(AGB200_EWORKSPACE, "moe: plan buffer needs %zu bytes, 256-byte aligned (got %zu)", need, plan_bytes);
 
-  int dev = 0, major = 0, sms = 0, smem_optin = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "moe: device index %d out of range", dev);
-  MOE_CUDA(cudaDeviceGetAttribute(&major, cudaDevAttrComputeCapabilityMajor, dev));
-  if (major != 9) return failf(AGB200_ECUDA, "device %d is sm_%dx; this library is built for sm_90a only", dev, major);
-  MOE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  MOE_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  const int dev = di.device, sms = di.sms, smem_optin = di.smem_optin;
 
   // decode path: the gate/up stage keeps all H of x for its rows in shared memory (h needs the full K); the down stage
   // splits I so that a work item's x stays within kDownXsCap
@@ -237,8 +186,6 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
   bool has_tc = experts[0].w1.qweight_tc != nullptr;
   std::vector<agb::MoeExpertDev> table(E);
   std::vector<CUtensorMap> maps;
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (has_tc && encode == nullptr) return failf(AGB200_ECUDA, "moe: cuTensorMapEncodeTiled entry point not available");
   unsigned char* base = static_cast<unsigned char*>(plan);
   CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base);
   agb::MoeExpertDev* d_ex = reinterpret_cast<agb::MoeExpertDev*>(base + maps_bytes(E));
@@ -251,7 +198,7 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
     for (int l = 0; l < 3; ++l) {
       const agb200_moe_layer& X = *L[l];
       if (!X.qweight || !X.qzeros || !X.scales) return failf(AGB200_EINVAL, "moe expert %d layer %d: null qweight/qzeros/scales", e, l);
-      if (!aligned16(X.qweight) || !aligned16(X.qzeros) || !aligned16(X.scales) || !aligned16(X.bias) || !aligned16(X.qweight_tc))
+      if (!aligned(X.qweight, 16) || !aligned(X.qzeros, 16) || !aligned(X.scales, 16) || !aligned(X.bias, 16) || !aligned(X.qweight_tc, 16))
         return failf(AGB200_EINVAL, "moe expert %d layer %d: buffers must be 16-byte aligned", e, l);
       if ((X.qweight_tc != nullptr) != has_tc)
         return failf(AGB200_EINVAL, "moe expert %d layer %d: qweight_tc must be given for every layer or for none", e, l);
@@ -261,15 +208,15 @@ int agb200_moe_create(const agb200_moe_expert* experts, int E, int H, int I, int
         const int G = (K + gs - 1) / gs;
         const uint32_t ngr = gs == 32 ? 2 : 1;
         CUtensorMap mw, ms, mz;
-        if (int rc = encode_2d(encode, &mw, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qweight_tc, N, K / 8, size_t(N) * 4, 64, 8, false, "qweight_tc")) return rc;
-        if (int rc = encode_2d(encode, &ms, sdt, X.scales, N, G, size_t(N) * 2, 64, ngr, false, "scales")) return rc;
-        if (int rc = encode_2d(encode, &mz, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qzeros, N / 8, G, size_t(N / 8) * 4, 8, ngr, false, "qzeros")) return rc;
+        if (int rc = encode_map(&mw, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qweight_tc, N, K / 8, size_t(N) * 4, 64, 8, false, "moe qweight_tc")) return rc;
+        if (int rc = encode_map(&ms, sdt, X.scales, N, G, size_t(N) * 2, 64, ngr, false, "moe scales")) return rc;
+        if (int rc = encode_map(&mz, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qzeros, N / 8, G, size_t(N / 8) * 4, 8, ngr, false, "moe qzeros")) return rc;
         maps.push_back(mw); maps.push_back(ms); maps.push_back(mz);
       }
     }
     if (experts[e].w1.perm != experts[e].w3.perm)
       return failf(AGB200_ENOSUP, "moe expert %d: w1 and w3 must share one act-order permutation of x (same pointer, or both NULL)", e);
-    if (experts[e].w2.perm != nullptr && !aligned16(experts[e].w2.perm)) return failf(AGB200_EINVAL, "moe expert %d: perm must be 16-byte aligned", e);
+    if (experts[e].w2.perm != nullptr && !aligned(experts[e].w2.perm, 16)) return failf(AGB200_EINVAL, "moe expert %d: perm must be 16-byte aligned", e);
     D.perm13 = experts[e].w1.perm;
     D.inv2 = experts[e].w2.perm != nullptr ? d_inv + size_t(e) * I : nullptr;
   }
@@ -330,10 +277,10 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
   if (T == 0) return 0;
   if (static_cast<long long>(T) * k > (1ll << 30)) return failf(AGB200_ENOSUP, "moe: T*k=%lld pairs is too many", static_cast<long long>(T) * k);
   int dev = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
+  AGB_CUDA(cudaGetDevice(&dev));
   if (dev != m->device) return failf(AGB200_EINVAL, "moe: created on device %d, current device is %d", m->device, dev);
   if (!x || !top_k_index || !top_k_weights || !out || !workspace) return failf(AGB200_EINVAL, "moe: null pointer argument");
-  if (!aligned16(x) || !aligned16(out) || (reinterpret_cast<uintptr_t>(workspace) & 255u))
+  if (!aligned(x, 16) || !aligned(out, 16) || !aligned(workspace, 256))
     return failf(AGB200_EINVAL, "moe: x and out must be 16-byte aligned, the workspace 256-byte aligned");
   if (index_dtype != AGB200_MOE_INDEX_I32 && index_dtype != AGB200_MOE_INDEX_I64) return failf(AGB200_EINVAL, "moe: unknown index dtype %d", index_dtype);
   if (weights_dtype != m->dtype && weights_dtype != AGB200_MOE_WEIGHTS_F32)
@@ -346,7 +293,7 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
   uint16_t* sv_y = nullptr;
   if (saved != nullptr) {
     const size_t need = saved_bytes(T, k, H, I);
-    if (saved_bytes_given < need || (reinterpret_cast<uintptr_t>(saved) & 255u))
+    if (saved_bytes_given < need || !aligned(saved, 256))
       return failf(AGB200_EWORKSPACE, "moe: saved buffer needs %zu bytes, 256-byte aligned (got %zu)", need, saved_bytes_given);
     const size_t gu = align_up(size_t(T) * k * I * 2, 256);
     sv_g = static_cast<uint16_t*>(saved);
@@ -368,7 +315,7 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
     mt = avg <= 32 ? 32 : avg <= 64 ? 64 : 128;
   }
   agb::moe_route_kernel<<<1, agb::kMoeRouteThreads, 0, s>>>(top_k_index, ids64, P, E, mt, r);
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
 
   uint16_t* hs = reinterpret_cast<uint16_t*>(ws + w.hs);
   const bool bf = m->dtype == AGB200_BF16;
@@ -399,7 +346,7 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
     } else {
       agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, wf32, k, E, H, P, nullptr, part, m->down_split, m->d_ex, o16);
     }
-    MOE_CUDA(cudaGetLastError());
+    AGB_CUDA(cudaGetLastError());
     return 0;
   }
 
@@ -408,13 +355,11 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
   const int m_tiles = (P + mt - 1) / mt + E;
   if (m_tiles > 65535) return failf(AGB200_ENOSUP, "moe: %d row tiles exceed the grid limit", m_tiles);
   agb::moe_gather_x_kernel<<<P, 128, 0, s>>>(static_cast<const uint16_t*>(x), top_k_index, ids64, k, H, E, r, m->d_ex, xs);
-  MOE_CUDA(cudaGetLastError());
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "moe: cuTensorMapEncodeTiled entry point not available");
+  AGB_CUDA(cudaGetLastError());
   const CUtensorMapDataType xdt = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tx, th;
-  if (int rc = encode_2d(encode, &tx, xdt, xs, H, w.rows, size_t(H) * 2, agb::kGemmBK, mt, true, "gathered x")) return rc;
-  if (int rc = encode_2d(encode, &th, xdt, hs, I, w.rows, size_t(I) * 2, agb::kGemmBK, mt, true, "h")) return rc;
+  if (int rc = encode_map(&tx, xdt, xs, H, w.rows, size_t(H) * 2, agb::kGemmBK, mt, true, "moe gathered x")) return rc;
+  if (int rc = encode_map(&th, xdt, hs, I, w.rows, size_t(I) * 2, agb::kGemmBK, mt, true, "moe h")) return rc;
   agb::MoeGemmParams p{};
   p.split = 1;
   p.out = hs; p.K = H; p.N = I; p.group_size = m->gs13; p.gs_log2 = gs_log2(m->gs13); p.num_kb = (H + agb::kGemmBK - 1) / agb::kGemmBK;
@@ -428,7 +373,7 @@ int moe_forward(void* handle, const void* x, const void* top_k_index, int index_
                                                               ys, nullptr, 0, m->d_ex, static_cast<uint16_t*>(out));
   else agb::moe_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, top_k_weights, weights_dtype == AGB200_MOE_WEIGHTS_F32, k, E, H, P,
                                                             ys, nullptr, 0, m->d_ex, static_cast<uint16_t*>(out));
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -494,28 +439,11 @@ BwdLayout bwd_layout(int T, int k, int E, int H, int I) {
 template <int kMT, bool kBf16, bool kDown, class Rows>
 int launch_moe_dgrad_inst(const agb::MoeDgradParams& p, const CUtensorMap& tb, const Rows& rows, int k_tiles, int m_tiles,
                           cudaStream_t stream) {
-  auto kern = agb::moe_dgrad_kernel<kMT, kBf16, kDown, Rows>;
+  constexpr auto kern = &agb::moe_dgrad_kernel<kMT, kBf16, kDown, Rows>;
   constexpr int smem = agb::DgradSmem<kMT>::kTotal;
-  static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
-  const int dev = agb::current_device_index();
-  if (!attr_set_dev[dev]) {
-    MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
-    attr_set_dev[dev] = true;
-  }
-  cudaLaunchConfig_t cfg{};
-  cfg.gridDim = dim3(k_tiles, m_tiles, p.split);
-  cfg.blockDim = dim3(agb::kGemmThreads, 1, 1);
-  cfg.dynamicSmemBytes = smem;
-  cfg.stream = stream;
-  cudaLaunchAttribute attr;
-  attr.id = cudaLaunchAttributeClusterDimension;
-  attr.val.clusterDim.x = 1;
-  attr.val.clusterDim.y = 1;
-  attr.val.clusterDim.z = p.split;
-  cfg.attrs = &attr;
-  cfg.numAttrs = p.split > 1 ? 1 : 0;
-  MOE_CUDA(cudaLaunchKernelEx(&cfg, kern, p, tb, rows));
-  return 0;
+  if (int rc = opt_in_smem<kern>(smem)) return rc;
+  return launch(kern, dim3(k_tiles, m_tiles, p.split), dim3(agb::kGemmThreads), smem, stream, false, dim3(1, 1, p.split), false,
+                p, tb, rows);
 }
 
 // One moe_dgrad_kernel launch with row tile mt (32 / 64 / 128)
@@ -568,18 +496,15 @@ int agb200_moe_grad_attach(void* handle, const agb200_moe_expert* experts, void*
   if (!experts || !grad_plan) return failf(AGB200_EINVAL, "moe grad: null pointer argument");
   const int E = m->E, H = m->H, I = m->I;
   const size_t need = agb200_moe_grad_plan_bytes(E, H, I, 0);
-  if (grad_plan_bytes < need || (reinterpret_cast<uintptr_t>(grad_plan) & 255u))
+  if (grad_plan_bytes < need || !aligned(grad_plan, 256))
     return failf(AGB200_EWORKSPACE, "moe grad: plan buffer needs %zu bytes, 256-byte aligned (got %zu)", need, grad_plan_bytes);
   int dev = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
+  AGB_CUDA(cudaGetDevice(&dev));
   if (dev != m->device) return failf(AGB200_EINVAL, "moe grad: created on device %d, current device is %d", m->device, dev);
   // every configuration agb200_moe_create accepts (H, I multiples of 128; group 32, a multiple of 64, or one group)
   // has whole 16-row groups: the tensor-core dgrad takes all three layers
   if (!agb::dgrad_tc_supported(H, I, m->gs13) || !agb::dgrad_tc_supported(I, H, m->gs2))
     return failf(AGB200_ENOSUP, "moe grad: H=%d, I=%d, group sizes %d / %d are outside the tensor-core dgrad", H, I, m->gs13, m->gs2);
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "moe grad: cuTensorMapEncodeTiled entry point not available");
-  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "moe grad: no CUDA context: %s", cudaGetErrorString(e));
   unsigned char* base = static_cast<unsigned char*>(grad_plan);
   CUtensorMap* d_maps = reinterpret_cast<CUtensorMap*>(base);
   agb::MoeGradExpertDev* d_ex = reinterpret_cast<agb::MoeGradExpertDev*>(base + maps_bytes(E));
@@ -592,14 +517,14 @@ int agb200_moe_grad_attach(void* handle, const agb200_moe_expert* experts, void*
     for (int l = 0; l < 3; ++l) {
       const agb200_moe_layer& X = *L[l];
       if (!X.qweight || !X.qzeros || !X.scales) return failf(AGB200_EINVAL, "moe grad expert %d layer %d: null qweight/qzeros/scales", e, l);
-      if (!aligned16(X.qweight) || !aligned16(X.qzeros) || !aligned16(X.scales))
+      if (!aligned(X.qweight, 16) || !aligned(X.qzeros, 16) || !aligned(X.scales, 16))
         return failf(AGB200_EINVAL, "moe grad expert %d layer %d: buffers must be 16-byte aligned", e, l);
       const int K = l == 2 ? I : H, N = l == 2 ? H : I, gs = l == 2 ? m->gs2 : m->gs13;
       const int G = (K + gs - 1) / gs;
       CUtensorMap mw, ms, mz;   // the dgrad kernel's boxes: [16 word rows][64 n], [5 groups][64 n], [5 groups][8 words]
-      if (int rc = encode_2d(encode, &mw, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "qweight")) return rc;
-      if (int rc = encode_2d(encode, &ms, sdt, X.scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "scales")) return rc;
-      if (int rc = encode_2d(encode, &mz, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "qzeros")) return rc;
+      if (int rc = encode_map(&mw, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "moe grad qweight")) return rc;
+      if (int rc = encode_map(&ms, sdt, X.scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "moe grad scales")) return rc;
+      if (int rc = encode_map(&mz, CU_TENSOR_MAP_DATA_TYPE_INT32, X.qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "moe grad qzeros")) return rc;
       maps.push_back(mw); maps.push_back(ms); maps.push_back(mz);
     }
     if (experts[e].w1.perm != experts[e].w3.perm)
@@ -638,11 +563,10 @@ int agb200_moe_backward(void* handle, const void* dy, const void* top_k_index, i
   if (static_cast<long long>(T) * k > (1ll << 30)) return failf(AGB200_ENOSUP, "moe backward: T*k=%lld pairs is too many", static_cast<long long>(T) * k);
   if (m->g_maps == nullptr) return failf(AGB200_EINVAL, "moe backward: no grad plan (call agb200_moe_grad_attach first)");
   int dev = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
+  AGB_CUDA(cudaGetDevice(&dev));
   if (dev != m->device) return failf(AGB200_EINVAL, "moe backward: created on device %d, current device is %d", m->device, dev);
   if (!dy || !top_k_index || !top_k_weights || !saved || !workspace) return failf(AGB200_EINVAL, "moe backward: null pointer argument");
-  if (!aligned16(dy) || !aligned16(dx) || !aligned16(dw) || (reinterpret_cast<uintptr_t>(saved) & 255u) ||
-      (reinterpret_cast<uintptr_t>(workspace) & 255u))
+  if (!aligned(dy, 16) || !aligned(dx, 16) || !aligned(dw, 16) || !aligned(saved, 256) || !aligned(workspace, 256))
     return failf(AGB200_EINVAL, "moe backward: dy, dx and dw must be 16-byte aligned, saved and the workspace 256-byte aligned");
   if (index_dtype != AGB200_MOE_INDEX_I32 && index_dtype != AGB200_MOE_INDEX_I64) return failf(AGB200_EINVAL, "moe backward: unknown index dtype %d", index_dtype);
   if (weights_dtype != m->dtype && weights_dtype != AGB200_MOE_WEIGHTS_F32)
@@ -667,22 +591,19 @@ int agb200_moe_backward(void* handle, const void* dy, const void* top_k_index, i
   uint16_t* dyp = dx != nullptr ? reinterpret_cast<uint16_t*>(ws + b.dyp) : nullptr;
 
   agb::moe_route_kernel<<<1, agb::kMoeRouteThreads, 0, s>>>(top_k_index, ids64, P, E, b.mt, r);
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   const uint16_t* dy16 = static_cast<const uint16_t*>(dy);
   if (bf) agb::moe_combine_bwd_kernel<true><<<P, 256, 0, s>>>(dy16, top_k_index, ids64, top_k_weights, wf32, k, E, H, r, sv_y, prow, dyp, dw);
   else agb::moe_combine_bwd_kernel<false><<<P, 256, 0, s>>>(dy16, top_k_index, ids64, top_k_weights, wf32, k, E, H, r, sv_y, prow, dyp, dw);
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   if (dx == nullptr) return 0;
 
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "moe backward: cuTensorMapEncodeTiled entry point not available");
-  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "moe backward: no CUDA context: %s", cudaGetErrorString(e));
   const CUtensorMapDataType t16 = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   uint16_t* dgu = reinterpret_cast<uint16_t*>(ws + b.dgu);
   float* dxp = reinterpret_cast<float*>(ws + b.dxp);
   CUtensorMap t_dyp, t_dgu;
-  if (int rc = encode_2d(encode, &t_dyp, t16, dyp, H, b.rows, size_t(H) * 2, agb::kDgBN, b.mt, true, "dy_pair")) return rc;
-  if (int rc = encode_2d(encode, &t_dgu, t16, dgu, 2 * I, b.rows, size_t(2 * I) * 2, agb::kDgBN, b.mt, true, "dg | du")) return rc;
+  if (int rc = encode_map(&t_dyp, t16, dyp, H, b.rows, size_t(H) * 2, agb::kDgBN, b.mt, true, "moe backward dy_pair")) return rc;
+  if (int rc = encode_map(&t_dgu, t16, dgu, 2 * I, b.rows, size_t(2 * I) * 2, agb::kDgBN, b.mt, true, "moe backward dg | du")) return rc;
   agb::MoeDgradParams p{};
   p.out = dgu; p.K = I; p.N = H; p.I = I; p.group_size = m->gs2; p.num_nb = H / agb::kDgBN; p.g = sv_g; p.u = sv_u;
   if (int rc = launch_moe_dgrad<true>(*m, b.mt, P, p, t_dyp, r, s)) return rc;
@@ -691,7 +612,7 @@ int agb200_moe_backward(void* handle, const void* dy, const void* top_k_index, i
   const dim3 cgrid(T, (H + 255) / 256, 1);
   if (bf) agb::moe_dx_combine_kernel<true><<<cgrid, 256, 0, s>>>(top_k_index, ids64, k, E, H, prow, dxp, m->g_ex, static_cast<uint16_t*>(dx));
   else agb::moe_dx_combine_kernel<false><<<cgrid, 256, 0, s>>>(top_k_index, ids64, k, E, H, prow, dxp, m->g_ex, static_cast<uint16_t*>(dx));
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -715,15 +636,10 @@ size_t gate_up_decode_smem(int K) { return size_t(round_up(K / 8, 32)) * agb::kM
 
 template <bool kBf16, class Src>
 int launch_gate_up_decode(const Src& src, const agb::MoeDecodeParams& p, size_t smem, int smem_optin, cudaStream_t stream) {
-  auto kern = agb::moe_decode_kernel<kBf16, true, Src>;
-  static bool attr_set_dev[64] = {};   // per device; benign race: idempotent
-  const int dev = agb::current_device_index();
-  if (!attr_set_dev[dev]) {
-    MOE_CUDA(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, smem_optin));
-    attr_set_dev[dev] = true;
-  }
+  constexpr auto kern = &agb::moe_decode_kernel<kBf16, true, Src>;
+  if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
   kern<<<p.tiles, agb::kMdThreads, smem, stream>>>(p, src);   // one CTA per 32-column tile
-  MOE_CUDA(cudaGetLastError());
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
@@ -754,24 +670,22 @@ int gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer*
   if (!x || !h) return failf(AGB200_EINVAL, "gate_up: null x or h");
   for (const agb200_moe_layer* L : {gate, up}) {
     if (!L->qweight || !L->qzeros || !L->scales) return failf(AGB200_EINVAL, "gate_up: null qweight/qzeros/scales");
-    if (!aligned16(L->qweight) || !aligned16(L->qzeros) || !aligned16(L->scales) || !aligned16(L->bias) ||
-        !aligned16(L->qweight_tc) || !aligned16(L->perm))
+    if (!aligned(L->qweight, 16) || !aligned(L->qzeros, 16) || !aligned(L->scales, 16) || !aligned(L->bias, 16) ||
+        !aligned(L->qweight_tc, 16) || !aligned(L->perm, 16))
       return failf(AGB200_EINVAL, "gate_up: layer buffers must be 16-byte aligned");
   }
-  if (!aligned16(x) || !aligned16(h)) return failf(AGB200_EINVAL, "gate_up: x and h must be 16-byte aligned");
+  if (!aligned(x, 16) || !aligned(h, 16)) return failf(AGB200_EINVAL, "gate_up: x and h must be 16-byte aligned");
   const bool save = g != nullptr;
-  if (save && (u == nullptr || !aligned16(g) || !aligned16(u)))
+  if (save && (u == nullptr || !aligned(g, 16) || !aligned(u, 16)))
     return failf(AGB200_EINVAL, "gate_up: the saved g and u must both be given, 16-byte aligned");
   if (K % 8 != 0 || I % 32 != 0) return failf(AGB200_ENOSUP, "gate_up: K %% 8 == 0 and I %% 32 == 0 (got K=%d, I=%d)", K, I);
   if (gate->perm != up->perm)
     return failf(AGB200_ENOSUP, "gate_up: gate and up must share one act-order permutation of x (same pointer, or both NULL)");
   const int gs = group_size == -1 ? K : group_size;
   if (gs <= 0) return failf(AGB200_EINVAL, "gate_up: group_size must be positive or -1 (got %d)", group_size);
-  int dev = 0, smem_optin = 0, sms = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
-  if (dev < 0 || dev >= 64) return failf(AGB200_EINVAL, "gate_up: device index %d out of range", dev);
-  MOE_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  MOE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  const int smem_optin = di.smem_optin, sms = di.sms;
   const bool bf = dtype == AGB200_BF16;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
 
@@ -810,7 +724,7 @@ int gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer*
     const size_t need = size_t(M) * K * 2;
     if (!workspace || workspace_bytes < need)
       return failf(AGB200_EWORKSPACE, "gate_up: act-order needs a %zu-byte workspace for the gathered x (got %zu)", need, workspace_bytes);
-    if (!aligned16(workspace)) return failf(AGB200_EINVAL, "gate_up: the workspace must be 16-byte aligned");
+    if (!aligned(workspace, 16)) return failf(AGB200_EINVAL, "gate_up: the workspace must be 16-byte aligned");
     if (int rc = agb200_permute_columns(x, gate->perm, workspace, M, K, dtype, stream)) return rc;
     xa = workspace;
   }
@@ -828,11 +742,9 @@ int gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer*
   p.split = split;
   p.kb_per_split = (p.num_kb + split - 1) / split;
 
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "gate_up: cuTensorMapEncodeTiled entry point not available");
   const CUtensorMapDataType xdt = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   CUtensorMap tx;
-  if (int rc = encode_2d(encode, &tx, xdt, xa, K, M, size_t(K) * 2, agb::kGemmBK, mt, true, "x")) return rc;
+  if (int rc = encode_map(&tx, xdt, xa, K, M, size_t(K) * 2, agb::kGemmBK, mt, true, "gate_up x")) return rc;
   agb::DenseGemmRows src{};
   src.M = M;
   src.lay.bias[0] = gate->bias;
@@ -842,9 +754,9 @@ int gate_up(const void* x, const agb200_moe_layer* gate, const agb200_moe_layer*
   const agb200_moe_layer* L[2] = {gate, up};
   for (int l = 0; l < 2; ++l) {
     CUtensorMap* mp = src.maps + 3 * l;
-    if (int rc = encode_2d(encode, mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qweight_tc, I, K / 8, size_t(I) * 4, 64, 8, false, "qweight_tc")) return rc;
-    if (int rc = encode_2d(encode, mp + 1, xdt, L[l]->scales, I, G, size_t(I) * 2, 64, ngr, false, "scales")) return rc;
-    if (int rc = encode_2d(encode, mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qzeros, I / 8, G, size_t(I / 8) * 4, 8, ngr, false, "qzeros")) return rc;
+    if (int rc = encode_map(mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qweight_tc, I, K / 8, size_t(I) * 4, 64, 8, false, "gate_up qweight_tc")) return rc;
+    if (int rc = encode_map(mp + 1, xdt, L[l]->scales, I, G, size_t(I) * 2, 64, ngr, false, "gate_up scales")) return rc;
+    if (int rc = encode_map(mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L[l]->qzeros, I / 8, G, size_t(I / 8) * 4, 8, ngr, false, "gate_up qzeros")) return rc;
   }
   if (save) {
     agb::DenseGemmRowsSave ss{};
@@ -914,12 +826,11 @@ MlpBwdLayout mlp_bwd_layout(int M, int H, int I) {
 }
 
 // the dgrad tensor maps of one layer (K rows, N columns) at mp[0..2]: packed words, scales, zeros
-int encode_dgrad_layer(agb::EncodeTiledFn encode, CUtensorMap* mp, const agb200_moe_layer* L, int K, int N, int gs,
-                       CUtensorMapDataType sdt) {
+int encode_dgrad_layer(CUtensorMap* mp, const agb200_moe_layer* L, int K, int N, int gs, CUtensorMapDataType sdt) {
   const int G = (K + gs - 1) / gs;
-  if (int rc = encode_2d(encode, mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "qweight")) return rc;
-  if (int rc = encode_2d(encode, mp + 1, sdt, L->scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "scales")) return rc;
-  return encode_2d(encode, mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "qzeros");
+  if (int rc = encode_map(mp + 0, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qweight, N, K / 8, size_t(N) * 4, agb::kDgBN, agb::kDgBK / 8, false, "mlp_backward qweight")) return rc;
+  if (int rc = encode_map(mp + 1, sdt, L->scales, N, G, size_t(N) * 2, agb::kDgBN, agb::kDgGroups, false, "mlp_backward scales")) return rc;
+  return encode_map(mp + 2, CU_TENSOR_MAP_DATA_TYPE_INT32, L->qzeros, N / 8, G, size_t(N / 8) * 4, agb::kDgBN / 8, agb::kDgGroups, false, "mlp_backward qzeros");
 }
 
 }  // namespace
@@ -942,10 +853,10 @@ int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, c
   if (!dy || !g || !u || !dx || !workspace) return failf(AGB200_EINVAL, "mlp_backward: null pointer argument");
   for (const agb200_moe_layer* L : {gate, up, down}) {
     if (!L->qweight || !L->qzeros || !L->scales) return failf(AGB200_EINVAL, "mlp_backward: null qweight/qzeros/scales");
-    if (!aligned16(L->qweight) || !aligned16(L->qzeros) || !aligned16(L->scales))
+    if (!aligned(L->qweight, 16) || !aligned(L->qzeros, 16) || !aligned(L->scales, 16))
       return failf(AGB200_EINVAL, "mlp_backward: layer buffers must be 16-byte aligned");
   }
-  if (!aligned16(dy) || !aligned16(g) || !aligned16(u) || !aligned16(dx) || (reinterpret_cast<uintptr_t>(workspace) & 255u))
+  if (!aligned(dy, 16) || !aligned(g, 16) || !aligned(u, 16) || !aligned(dx, 16) || !aligned(workspace, 256))
     return failf(AGB200_EINVAL, "mlp_backward: dy, g, u and dx must be 16-byte aligned, the workspace 256-byte aligned");
   if (dy == dx) return failf(AGB200_EINVAL, "mlp_backward: dy and dx must not alias");
   if (gate->perm != up->perm)
@@ -965,15 +876,11 @@ int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, c
     return failf(AGB200_EINVAL, "mlp_backward: split must be 1/2/4/8 (got %d)", split_k);
   const int m_tiles = (M + mt - 1) / mt;
   if (m_tiles > 65535) return failf(AGB200_ENOSUP, "mlp_backward: %d row tiles exceed the grid limit", m_tiles);
-  int dev = 0, sms = 0, smem_optin = 0;
-  MOE_CUDA(cudaGetDevice(&dev));
-  MOE_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-  MOE_CUDA(cudaDeviceGetAttribute(&smem_optin, cudaDevAttrMaxSharedMemoryPerBlockOptin, dev));
-  if (gate->perm != nullptr && size_t(H) * 2 > static_cast<size_t>(smem_optin))
+  DeviceInfo di;
+  if (int rc = device_info(di)) return rc;
+  const int sms = di.sms;
+  if (gate->perm != nullptr && size_t(H) * 2 > static_cast<size_t>(di.smem_optin))
     return failf(AGB200_ENOSUP, "mlp_backward: act-order row of H=%d does not fit in shared memory", H);
-  agb::EncodeTiledFn encode = agb::get_encode_fn();
-  if (encode == nullptr) return failf(AGB200_ECUDA, "mlp_backward: cuTensorMapEncodeTiled entry point not available");
-  if (cudaError_t e = agb::ensure_context()) return failf(AGB200_ECUDA, "mlp_backward: no CUDA context: %s", cudaGetErrorString(e));
   const bool bf = dtype == AGB200_BF16;
   const CUtensorMapDataType t16 = bf ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
@@ -985,12 +892,12 @@ int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, c
   agb::DenseGradRows rows{};
   rows.M = M;
   rows.perm2_ = down->perm;
-  if (int rc = encode_dgrad_layer(encode, rows.maps + 0, gate, H, I, gs13, t16)) return rc;
-  if (int rc = encode_dgrad_layer(encode, rows.maps + 3, up, H, I, gs13, t16)) return rc;
-  if (int rc = encode_dgrad_layer(encode, rows.maps + 6, down, I, H, gs2, t16)) return rc;
+  if (int rc = encode_dgrad_layer(rows.maps + 0, gate, H, I, gs13, t16)) return rc;
+  if (int rc = encode_dgrad_layer(rows.maps + 3, up, H, I, gs13, t16)) return rc;
+  if (int rc = encode_dgrad_layer(rows.maps + 6, down, I, H, gs2, t16)) return rc;
   CUtensorMap t_dy, t_dgu;
-  if (int rc = encode_2d(encode, &t_dy, t16, dy, H, M, size_t(H) * 2, agb::kDgBN, mt, true, "dy")) return rc;
-  if (int rc = encode_2d(encode, &t_dgu, t16, dgu, 2 * I, M, size_t(2 * I) * 2, agb::kDgBN, mt, true, "dg | du")) return rc;
+  if (int rc = encode_map(&t_dy, t16, dy, H, M, size_t(H) * 2, agb::kDgBN, mt, true, "mlp_backward dy")) return rc;
+  if (int rc = encode_map(&t_dgu, t16, dgu, 2 * I, M, size_t(2 * I) * 2, agb::kDgBN, mt, true, "mlp_backward dg | du")) return rc;
 
   // split over n by the wave model of the dense dgrad (no host synchronisation, no atomics)
   auto plan = [&](agb::MoeDgradParams& p, int k_tiles) {

@@ -2,31 +2,12 @@
 // caller's stream.  Kernel: moe_router.cuh.
 #include <cuda_runtime.h>
 
-#include <cstdarg>
-#include <cstdio>
-
-#include "../../include/autogptq_b200.h"
-#include "internal.h"
+#include "host.h"
 #include "moe_router.cuh"
 
 static_assert(agb::kRouterMaxH == AGB200_CHAIN_NORM_MAX_K, "router and chain norm share the hidden-size limit");
 static_assert(agb::kRouterMaxE == AGB200_MOE_MAX_EXPERTS, "router and grouped experts share the expert limit");
 static_assert(agb::kRouterMaxTopK == AGB200_MOE_ROUTER_MAX_TOP_K, "router top-k limit");
-
-namespace {
-
-int failf(int code, const char* fmt, ...) {
-  char buf[400];
-  va_list ap;
-  va_start(ap, fmt);
-  vsnprintf(buf, sizeof(buf), fmt, ap);
-  va_end(ap);
-  return agb_internal_fail(code, buf);
-}
-
-bool aligned(const void* p, uintptr_t a) { return (reinterpret_cast<uintptr_t>(p) & (a - 1)) == 0; }
-
-}  // namespace
 
 extern "C" {
 
@@ -68,8 +49,7 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == AGB200_BF16) agb::moe_router_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
   else agb::moe_router_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
-  const cudaError_t e = cudaGetLastError();
-  if (e != cudaSuccess) return failf(AGB200_ECUDA, "moe_router: launch: %s", cudaGetErrorString(e));
+  AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
