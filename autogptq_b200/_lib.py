@@ -33,6 +33,7 @@ DGRAD_AUTO, DGRAD_CUDA_CORE, DGRAD_WGMMA = 0, 1, 2
 ATTN_HEAD_DIMS = (64, 128)
 ATTN_MAX_G = 8
 ATTN_MAX_B = 2
+ATTN_ROWS_MAX_B = 8            # AGB200_ATTN_ROWS_MAX_B
 
 _lib = None
 
@@ -103,7 +104,9 @@ def _declare(lib):
         "agb200_gptq_workspace_bytes": (S, [I, I, I]),
         "agb200_decode_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
         "agb200_decode_attention_workspace_bytes": (S, [I, I, I, I, I]),
+        "agb200_decode_attention_rows": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
+        "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

@@ -7,6 +7,10 @@ applies transformers' rotary embedding to q and k (the same roundings as ``apply
 position ``pos`` of the static caches, and attends every query head over positions 0..pos (GQA: query head h reads kv
 head h // (n_heads / n_kv)).  ``pos`` is an int64 device scalar, so the call can be captured once in a CUDA graph and
 replayed as the position advances.  No host synchronisation.
+
+``decode_attention_rows`` (``agb200_decode_attention_rows``, DESIGN §3.18) runs the same kernel for up to
+``ATTN_ROWS_MAX_B`` = 8 independent sequences: ``pos`` is an int64 device tensor [B], row b attends over 0..pos[b], and a
+row with pos[b] = -1 is idle (zeros out, its cache row untouched).  The workspace is ``decode_attention_workspace``'s.
 """
 from __future__ import annotations
 
@@ -34,6 +38,16 @@ def attention_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, max_
     return None
 
 
+def attention_rows_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, max_length: int, dtype) -> str | None:
+    """None when ``decode_attention_rows`` takes this shape, else the reason it does not."""
+    why = attention_supported(n_heads, n_kv, head_dim, 1, max_length, dtype)
+    if why is None and not 1 <= batch <= _lib.ATTN_ROWS_MAX_B:
+        why = f"batch {batch}; the kernel takes 1..{_lib.ATTN_ROWS_MAX_B} independent rows"
+    if why is None and batch * n_kv * max_length * head_dim >= 2 ** 31:
+        why = "the cache has 2^31 elements or more"
+    return why
+
+
 def decode_attention_workspace(batch: int, n_heads: int, n_kv: int, head_dim: int, max_length: int,
                                device) -> torch.Tensor:
     """A zeroed workspace for ``decode_attention`` of this shape on ``device``.  Calls leave it ready for the next
@@ -51,19 +65,34 @@ def decode_attention(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling
                      workspace=None):
     """q [B, n_heads·hd], k / v [B, n_kv·hd], caches [B, n_kv, max_length, hd], pos int64 [1] (device), inv_freq fp32
     [hd/2], out [B, n_heads·hd] written in place and returned.  Raises NotImplementedError outside the kernel's limits."""
+    return _launch("decode_attention", attention_supported, 1, q, k, v, k_cache, v_cache, pos, inv_freq,
+                   attention_scaling, scaling, out, workspace)
+
+
+def decode_attention_rows(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling: float, scaling: float, out,
+                          workspace=None):
+    """``decode_attention`` for independent sequences: pos int64 [B] (device), one position per row, -1 for an idle
+    row (zeros out, cache row untouched).  B <= ``ATTN_ROWS_MAX_B``."""
+    return _launch("decode_attention_rows", attention_rows_supported, None, q, k, v, k_cache, v_cache, pos, inv_freq,
+                   attention_scaling, scaling, out, workspace)
+
+
+def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out,
+            workspace):
+    """Checks and the call of agb200_<entry>; ``n_pos`` elements of pos (None: one per row)."""
     if k_cache.dim() != 4:
         raise ValueError(f"k_cache must be [B, n_kv, max_length, head_dim], got {tuple(k_cache.shape)}")
     B, n_kv, L, hd = k_cache.shape
     dev = k_cache.device
     if dev.type != "cuda":
-        raise RuntimeError("decode_attention needs CUDA tensors (there is no CPU fallback)")
+        raise RuntimeError(f"{entry} needs CUDA tensors (there is no CPU fallback)")
     dt = k_cache.dtype
     if q.dim() != 2 or q.shape[0] != B or q.shape[1] % hd != 0:
         raise ValueError(f"q must be [{B}, n_heads·{hd}], got {tuple(q.shape)}")
     n_heads = q.shape[1] // hd
-    why = attention_supported(n_heads, n_kv, hd, B, L, dt)
+    why = supported(n_heads, n_kv, hd, B, L, dt)
     if why is not None:
-        raise NotImplementedError(f"decode_attention: {why}")
+        raise NotImplementedError(f"{entry}: {why}")
     for name, t, shape in (("q", q, (B, n_heads * hd)), ("k", k, (B, n_kv * hd)), ("v", v, (B, n_kv * hd)),
                            ("v_cache", v_cache, (B, n_kv, L, hd)), ("out", out, (B, n_heads * hd))):
         if tuple(t.shape) != shape:
@@ -76,8 +105,9 @@ def decode_attention(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling
             raise ValueError(f"{name} is on {t.device}, the cache on {dev}")
         if not t.is_contiguous():
             raise ValueError(f"{name} must be contiguous")
-    if pos.dtype != torch.int64 or pos.numel() != 1:
-        raise ValueError(f"pos must be one int64 element, got {pos.dtype} with {pos.numel()} elements")
+    n_pos = B if n_pos is None else n_pos
+    if pos.dtype != torch.int64 or pos.numel() != n_pos:
+        raise ValueError(f"pos must be {n_pos} int64 element(s), got {pos.dtype} with {pos.numel()} elements")
     if inv_freq.dtype != torch.float32 or tuple(inv_freq.shape) != (hd // 2,):
         raise ValueError(f"inv_freq must be float32 [{hd // 2}], got {inv_freq.dtype} {list(inv_freq.shape)}")
     lib = _lib.load()
@@ -87,13 +117,14 @@ def decode_attention(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling
             workspace = decode_attention_workspace(B, n_heads, n_kv, hd, L, dev)
         elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
             raise ValueError(f"workspace must hold {need} bytes on {dev}")
-        rc = lib.agb200_decode_attention(
+        rc = getattr(lib, f"agb200_{entry}")(
             q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), pos.data_ptr(),
             inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads, n_kv, hd, L,
             _DT[dt], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
             torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(rc, "agb200_decode_attention")
+    _lib.check(rc, f"agb200_{entry}")
     return out
 
 
-__all__ = ["decode_attention", "decode_attention_workspace", "attention_supported"]
+__all__ = ["decode_attention", "decode_attention_rows", "decode_attention_workspace", "attention_supported",
+           "attention_rows_supported"]

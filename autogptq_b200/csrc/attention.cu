@@ -5,6 +5,8 @@
 #include "attention.cuh"
 #include "host.h"
 
+static_assert(agb::kAttnRowsMaxB == AGB200_ATTN_ROWS_MAX_B, "per-row decode attention batch limit");
+
 namespace {
 
 // Splits of the sequence per (b, kv head): about four CTAs per SM over the whole grid, at most one per tile of the cache.
@@ -33,33 +35,38 @@ size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int
          align_up(size_t(B) * n_kv * S * agb::attn_part_floats(n_heads / n_kv, head_dim) * sizeof(float), 256);
 }
 
-int agb200_decode_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int64_t* pos,
-                            const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
-                            int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
-                            void* stream) {
+}  // extern "C"
+
+namespace {
+
+// Both entries: `what` names the entry in errors, `pos_stride` 0 (one position) or 1 (a position per row).
+int decode_attention(const char* what, int max_b, int pos_stride, const void* q, const void* k, const void* v,
+                     void* k_cache, void* v_cache, const int64_t* pos, const float* inv_freq, float attention_scaling,
+                     float scaling, void* out, int B, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
+                     void* workspace, size_t workspace_bytes, void* stream) {
   if (!q || !k || !v || !k_cache || !v_cache || !pos || !inv_freq || !out || !workspace)
-    return failf(AGB200_EINVAL, "decode_attention: null pointer argument");
+    return failf(AGB200_EINVAL, "%s: null pointer argument", what);
   if (B <= 0 || n_heads <= 0 || n_kv <= 0 || head_dim <= 0 || max_length <= 0 || n_heads % n_kv != 0)
-    return failf(AGB200_EINVAL, "decode_attention: need positive B, n_heads, n_kv, head_dim, max_length and "
-                 "n_heads %% n_kv == 0 (got B=%d, n_heads=%d, n_kv=%d, head_dim=%d, max_length=%d)",
+    return failf(AGB200_EINVAL, "%s: need positive B, n_heads, n_kv, head_dim, max_length and "
+                 "n_heads %% n_kv == 0 (got B=%d, n_heads=%d, n_kv=%d, head_dim=%d, max_length=%d)", what,
                  B, n_heads, n_kv, head_dim, max_length);
   if (dtype != AGB200_F16 && dtype != AGB200_BF16)
-    return failf(AGB200_ENOSUP, "decode_attention: dtype %d; only AGB200_F16 and AGB200_BF16 are supported", dtype);
+    return failf(AGB200_ENOSUP, "%s: dtype %d; only AGB200_F16 and AGB200_BF16 are supported", what, dtype);
   if (head_dim != 64 && head_dim != 128)
-    return failf(AGB200_ENOSUP, "decode_attention: head_dim %d; supported: 64, 128", head_dim);
+    return failf(AGB200_ENOSUP, "%s: head_dim %d; supported: 64, 128", what, head_dim);
   if (n_heads / n_kv > agb::kAttnMaxG)
-    return failf(AGB200_ENOSUP, "decode_attention: %d query heads per kv head; at most %d", n_heads / n_kv, agb::kAttnMaxG);
-  if (B > agb::kAttnMaxB) return failf(AGB200_ENOSUP, "decode_attention: batch %d; at most %d", B, agb::kAttnMaxB);
+    return failf(AGB200_ENOSUP, "%s: %d query heads per kv head; at most %d", what, n_heads / n_kv, agb::kAttnMaxG);
+  if (B > max_b) return failf(AGB200_ENOSUP, "%s: batch %d; at most %d", what, B, max_b);
   if (static_cast<long long>(B) * n_kv * max_length * head_dim >= (1ll << 31))
-    return failf(AGB200_ENOSUP, "decode_attention: the cache holds %lld elements; at most 2^31 - 1",
+    return failf(AGB200_ENOSUP, "%s: the cache holds %lld elements; at most 2^31 - 1", what,
                  static_cast<long long>(B) * n_kv * max_length * head_dim);
   if (!aligned(q, 16) || !aligned(k, 16) || !aligned(v, 16) || !aligned(k_cache, 16) || !aligned(v_cache, 16) ||
       !aligned(out, 16) || !aligned(pos, 8) || !aligned(inv_freq, 4) || !aligned(workspace, 256))
-    return failf(AGB200_EINVAL, "decode_attention: q, k, v, the caches and out must be 16-byte aligned, the workspace "
-                 "256-byte aligned");
+    return failf(AGB200_EINVAL, "%s: q, k, v, the caches and out must be 16-byte aligned, the workspace "
+                 "256-byte aligned", what);
   const size_t need = agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, head_dim, max_length);
   if (workspace_bytes < need)
-    return failf(AGB200_EWORKSPACE, "decode_attention: workspace needs %zu bytes (got %zu)", need, workspace_bytes);
+    return failf(AGB200_EWORKSPACE, "%s: workspace needs %zu bytes (got %zu)", what, need, workspace_bytes);
 
   agb::DecodeAttnParams p{};
   p.q = static_cast<const uint16_t*>(q);
@@ -68,6 +75,7 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
   p.k_cache = static_cast<uint16_t*>(k_cache);
   p.v_cache = static_cast<uint16_t*>(v_cache);
   p.pos = reinterpret_cast<const long long*>(pos);
+  p.pos_stride = pos_stride;
   p.inv_freq = inv_freq;
   p.attn_scaling = attention_scaling;
   p.scaling = scaling;
@@ -90,6 +98,28 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
   }
   AGB_CUDA(cudaGetLastError());
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int agb200_decode_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache, const int64_t* pos,
+                            const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
+                            int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                            void* stream) {
+  return decode_attention("decode_attention", agb::kAttnMaxB, 0, q, k, v, k_cache, v_cache, pos, inv_freq,
+                          attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype, workspace,
+                          workspace_bytes, stream);
+}
+
+int agb200_decode_attention_rows(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                 const int64_t* pos, const float* inv_freq, float attention_scaling, float scaling,
+                                 void* out, int B, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
+                                 void* workspace, size_t workspace_bytes, void* stream) {
+  return decode_attention("decode_attention_rows", agb::kAttnRowsMaxB, 1, q, k, v, k_cache, v_cache, pos, inv_freq,
+                          attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype, workspace,
+                          workspace_bytes, stream);
 }
 
 }  // extern "C"

@@ -1,5 +1,6 @@
 // Decode attention of one layer in one launch: rotary embedding of q and k, the KV-cache write at a device-side
-// position, and split-KV attention over positions [0, pos] with a last-arriving-CTA combine (DESIGN §3.16).
+// position, and split-KV attention over positions [0, pos] with a last-arriving-CTA combine (DESIGN §3.16).  The
+// position is one for every row (sequences in lockstep) or one per row (independent sequences, DESIGN §3.18).
 #pragma once
 #include <math.h>
 
@@ -11,7 +12,8 @@ constexpr int kAttnThreads = 128;      // 4 warps
 constexpr int kAttnTile = 32;          // positions per shared-memory tile (one per lane in the score phase)
 constexpr int kAttnMaxG = 8;           // query heads per kv head
 constexpr int kAttnMaxSplits = 64;
-constexpr int kAttnMaxB = 2;
+constexpr int kAttnMaxB = 2;            // agb200_decode_attention (one position)
+constexpr int kAttnRowsMaxB = 8;        // agb200_decode_attention_rows (a position per row)
 
 // Floats of one split's partials: acc[G][hd], then m and l of up to kAttnMaxG heads (keeps every split 16-byte aligned)
 __host__ __device__ constexpr int attn_part_floats(int G, int hd) { return G * hd + 2 * kAttnMaxG; }
@@ -22,7 +24,8 @@ struct DecodeAttnParams {
   const uint16_t* v;        // [B, n_kv·hd]
   uint16_t* k_cache;        // [B, n_kv, max_length, hd]
   uint16_t* v_cache;
-  const long long* pos;     // device scalar
+  const long long* pos;     // row b reads pos[b * pos_stride]
+  int pos_stride;           // 0: one position for every row; 1: one per row, and -1 marks an idle row
   const float* inv_freq;    // [hd/2]
   float attn_scaling;       // the rotary embedding's attention_scaling
   float scaling;            // softmax scale σ
@@ -85,7 +88,8 @@ __device__ __forceinline__ float warp_sum(float x) {
 }
 
 // Grid (splits, n_kv, B), kAttnThreads threads.  CTA (b, kv head, split i) owns positions [i·C, min((i+1)·C, pos+1)),
-// C = ceil((pos+1) / splits), for the G query heads of its kv head.
+// C = ceil((pos+1) / splits) with pos row b's position, for the G query heads of its kv head.  Rows share nothing but
+// the launch: every CTA of row b reads only row b's q, k, v, position, cache rows, partials and counter words.
 template <bool kBf16, int kHd>
 __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const DecodeAttnParams p) {
   using Smem = AttnSmem<kHd>;
@@ -100,11 +104,12 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int G = p.n_heads / p.n_kv;
   const int S = p.splits;
-  const long long pos64 = *p.pos;
+  const long long pos64 = p.pos[b * p.pos_stride];
   const int head0 = kvh * G;
   uint16_t* out = p.out + (size_t(b) * p.n_heads + head0) * kHd;
-  if (pos64 < 0 || pos64 >= p.max_length) {            // nothing to attend to: a NaN output, caches untouched
-    for (int i = tid; i < G * kHd; i += kAttnThreads) out[i] = float_to_elt<kBf16>(__int_as_float(0x7fffffff));
+  if (pos64 < 0 || pos64 >= p.max_length) {            // an idle row: zeros; else nothing to attend to: NaN; caches untouched
+    const float fill = p.pos_stride != 0 && pos64 == -1 ? 0.f : __int_as_float(0x7fffffff);
+    for (int i = tid; i < G * kHd; i += kAttnThreads) out[i] = float_to_elt<kBf16>(fill);
     return;
   }
   const int pos = static_cast<int>(pos64);

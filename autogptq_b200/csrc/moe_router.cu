@@ -1,5 +1,5 @@
-// Host side of the MoE router (include/autogptq_b200.h: agb200_moe_router): argument checking and the launch on the
-// caller's stream.  Kernel: moe_router.cuh.
+// Host side of the MoE router and of its residual add + RMSNorm alone (include/autogptq_b200.h: agb200_moe_router,
+// agb200_add_rmsnorm): argument checking and the launch on the caller's stream.  Kernels: moe_router.cuh.
 #include <cuda_runtime.h>
 
 #include "host.h"
@@ -49,6 +49,34 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   if (dtype == AGB200_BF16) agb::moe_router_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
   else agb::moe_router_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
+  AGB_CUDA(cudaGetLastError());
+  return 0;
+}
+
+int agb200_add_rmsnorm(const void* x, const void* x2, const void* norm_weight, float eps, int T, int H, int dtype,
+                       void* h, void* n, void* stream) {
+  if (!x || !norm_weight || !n) return failf(AGB200_EINVAL, "add_rmsnorm: null pointer argument");
+  if ((x2 == nullptr) != (h == nullptr)) return failf(AGB200_EINVAL, "add_rmsnorm: h is written exactly when x2 is given");
+  if (T < 0 || H <= 0) return failf(AGB200_EINVAL, "add_rmsnorm: need T >= 0 and H > 0 (got T=%d, H=%d)", T, H);
+  if (dtype != AGB200_F16 && dtype != AGB200_BF16)
+    return failf(AGB200_ENOSUP, "add_rmsnorm: dtype %d; only AGB200_F16 and AGB200_BF16 are supported", dtype);
+  if (T > AGB200_MOE_DECODE_MAX_T) return failf(AGB200_ENOSUP, "add_rmsnorm: T=%d rows; at most %d", T, AGB200_MOE_DECODE_MAX_T);
+  if (H % 128 != 0 || H > AGB200_CHAIN_NORM_MAX_K)
+    return failf(AGB200_ENOSUP, "add_rmsnorm: H=%d must be a multiple of 128, at most %d", H, AGB200_CHAIN_NORM_MAX_K);
+  if (!aligned(x, 16) || (x2 && !aligned(x2, 16)) || !aligned(norm_weight, 16) || (h && !aligned(h, 16)) || !aligned(n, 16))
+    return failf(AGB200_EINVAL, "add_rmsnorm: x, x2, norm_weight, h and n must be 16-byte aligned");
+  if (T == 0) return 0;
+  agb::AddRmsnormParams p{};
+  p.x = static_cast<const uint16_t*>(x);
+  p.x2 = static_cast<const uint16_t*>(x2);
+  p.norm_w = static_cast<const uint16_t*>(norm_weight);
+  p.h = static_cast<uint16_t*>(h);
+  p.n = static_cast<uint16_t*>(n);
+  p.eps = eps;
+  p.H = H;
+  cudaStream_t s = static_cast<cudaStream_t>(stream);
+  if (dtype == AGB200_BF16) agb::add_rmsnorm_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
+  else agb::add_rmsnorm_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
   AGB_CUDA(cudaGetLastError());
   return 0;
 }

@@ -1,5 +1,6 @@
 // Router of a Mixtral-style block for decode rows (DESIGN §3.17): residual add, RMSNorm, router logits, fp32 softmax,
-// top-k and renormalised weights, one CTA per row in one launch.
+// top-k and renormalised weights, one CTA per row in one launch.  Its residual add and RMSNorm also run alone, for the
+// decode rows of dense blocks (add_rmsnorm_kernel, DESIGN §3.18).
 #pragma once
 #include <math.h>
 
@@ -36,28 +37,34 @@ struct RouterSmem {
   float tv[kRouterMaxTopK];
 };
 
-// One CTA per row t.  Rounding points (transformers 5.5 MixtralDecoderLayer, MixtralRMSNorm, MixtralTopKRouter):
-//   h = rnd(x + x2)                              n = rnd(rnd(h·r)·w),  r = 1/sqrt(Σh²/H + eps)  (the chain's pre-pass)
-//   logit_e = rnd(Σ_k n_k·G[e,k])                fp32 sum, rounded once as F.linear's output
-//   p = softmax(fp32 logits)                     max subtracted, expf, fp32 sum
-//   top-k of p, largest first, an exact tie to the lower expert index;  w_j = p_j / Σ_j p_j  (fp32, j in order)
-// Every sum runs in a fixed order (per thread in index order, a xor-shuffle tree per warp, the warps in order), so two
-// launches on the same input are bit-identical.  Σh² is summed exactly as ch_norm_prepass sums it for one row.
-template <bool kBf16>
-__global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRouterParams p) {
-  __shared__ __align__(16) RouterSmem sm;
-  const int ctid = threadIdx.x, lane = ctid & 31, warp = ctid >> 5;
-  const int H = p.H, E = p.E, rows = H / kPack;
-  const size_t base = static_cast<size_t>(blockIdx.x) * H;
+struct AddRmsnormParams {
+  const uint16_t* x;        // [T, H]
+  const uint16_t* x2;       // [T, H] or null (then h = x)
+  const uint16_t* norm_w;   // [H]
+  uint16_t* h;              // [T, H] or null
+  uint16_t* n;              // [T, H]
+  float eps;
+  int H;
+};
 
+// h = rnd(x + x2) (x2 null: h = x; written to h_out when both are given), Σh², r and n = rnd(rnd(h·r)·w) of row `row0`
+// by one CTA of kRouterThreads threads.  n goes to n_out and to `xs`; each thread writes n over the same 8-element rows of
+// `xs` it staged h in, so a caller that reads back only those rows needs no barrier.  `red` holds kRouterWarps floats.
+template <bool kBf16>
+__device__ __forceinline__ void add_rmsnorm_row(const uint16_t* x, const uint16_t* x2, const uint16_t* norm_w,
+                                                uint16_t* h_out, uint16_t* n_out, float eps, int H, int row0, uint16_t* xs,
+                                                float* red) {
+  const int ctid = threadIdx.x, lane = ctid & 31, warp = ctid >> 5;
+  const int rows = H / kPack;
+  const size_t base = static_cast<size_t>(row0) * H;
   // h and Σh²
   float ss = 0.f;
   for (int row = ctid; row < rows; row += kRouterThreads) {
     const size_t off = base + static_cast<size_t>(row) * kPack;
-    const uint4 a = __ldg(reinterpret_cast<const uint4*>(p.x + off));
+    const uint4 a = __ldg(reinterpret_cast<const uint4*>(x + off));
     uint32_t hw[4] = {a.x, a.y, a.z, a.w};
-    if (p.x2 != nullptr) {
-      const uint4 b = __ldg(reinterpret_cast<const uint4*>(p.x2 + off));
+    if (x2 != nullptr) {
+      const uint4 b = __ldg(reinterpret_cast<const uint4*>(x2 + off));
       const uint32_t bw[4] = {b.x, b.y, b.z, b.w};
 #pragma unroll
       for (int i = 0; i < 4; ++i) {
@@ -67,7 +74,7 @@ __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRou
                                                 elt_to_float<kBf16>(static_cast<uint16_t>(bw[i] >> 16)));
         hw[i] = lo | (hi << 16);
       }
-      if (p.h != nullptr) *reinterpret_cast<uint4*>(p.h + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+      if (h_out != nullptr) *reinterpret_cast<uint4*>(h_out + off) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
     }
 #pragma unroll
     for (int i = 0; i < 4; ++i) {
@@ -76,20 +83,20 @@ __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRou
       ss = fmaf(f0, f0, ss);
       ss = fmaf(f1, f1, ss);
     }
-    *reinterpret_cast<uint4*>(sm.xs + row * kPack) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
+    *reinterpret_cast<uint4*>(xs + row * kPack) = make_uint4(hw[0], hw[1], hw[2], hw[3]);
   }
 #pragma unroll
   for (int o = 16; o > 0; o >>= 1) ss += __shfl_xor_sync(0xffffffffu, ss, o);
-  if (lane == 0) sm.red[warp] = ss;
+  if (lane == 0) red[warp] = ss;
   __syncthreads();
   float tot = 0.f;
-  for (int w = 0; w < kRouterWarps; ++w) tot += sm.red[w];
-  const float r = __frsqrt_rn(__fadd_rn(__fdiv_rn(tot, static_cast<float>(H)), p.eps));
+  for (int w = 0; w < kRouterWarps; ++w) tot += red[w];
+  const float r = __frsqrt_rn(__fadd_rn(__fdiv_rn(tot, static_cast<float>(H)), eps));
 
-  // n = rnd(rnd(h·r)·w): each thread rewrites the rows it staged, so no barrier is needed before the logit loop reads them
+  // n = rnd(rnd(h·r)·w): each thread rewrites the rows it staged
   for (int row = ctid; row < rows; row += kRouterThreads) {
-    const uint4 hv = *reinterpret_cast<const uint4*>(sm.xs + row * kPack);
-    const uint4 wv = __ldg(reinterpret_cast<const uint4*>(p.norm_w + static_cast<size_t>(row) * kPack));
+    const uint4 hv = *reinterpret_cast<const uint4*>(xs + row * kPack);
+    const uint4 wv = __ldg(reinterpret_cast<const uint4*>(norm_w + static_cast<size_t>(row) * kPack));
     const uint32_t hw[4] = {hv.x, hv.y, hv.z, hv.w}, ww[4] = {wv.x, wv.y, wv.z, wv.w};
     uint32_t nv[4];
 #pragma unroll
@@ -105,9 +112,26 @@ __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRou
       nv[i] = o[0] | (o[1] << 16);
     }
     const uint4 n4 = make_uint4(nv[0], nv[1], nv[2], nv[3]);
-    *reinterpret_cast<uint4*>(sm.xs + row * kPack) = n4;
-    *reinterpret_cast<uint4*>(p.n + base + static_cast<size_t>(row) * kPack) = n4;
+    *reinterpret_cast<uint4*>(xs + row * kPack) = n4;
+    *reinterpret_cast<uint4*>(n_out + base + static_cast<size_t>(row) * kPack) = n4;
   }
+}
+
+// One CTA per row t.  Rounding points (transformers 5.5 MixtralDecoderLayer, MixtralRMSNorm, MixtralTopKRouter):
+//   h = rnd(x + x2)                              n = rnd(rnd(h·r)·w),  r = 1/sqrt(Σh²/H + eps)  (the chain's pre-pass)
+//   logit_e = rnd(Σ_k n_k·G[e,k])                fp32 sum, rounded once as F.linear's output
+//   p = softmax(fp32 logits)                     max subtracted, expf, fp32 sum
+//   top-k of p, largest first, an exact tie to the lower expert index;  w_j = p_j / Σ_j p_j  (fp32, j in order)
+// Every sum runs in a fixed order (per thread in index order, a xor-shuffle tree per warp, the warps in order), so two
+// launches on the same input are bit-identical.  Σh² is summed exactly as ch_norm_prepass sums it for one row.
+template <bool kBf16>
+__global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRouterParams p) {
+  __shared__ __align__(16) RouterSmem sm;
+  const int ctid = threadIdx.x, lane = ctid & 31, warp = ctid >> 5;
+  const int H = p.H, E = p.E, rows = H / kPack;
+
+  // h, n (into sm.xs, each thread over its own rows: no barrier is needed before the logit loop reads them)
+  add_rmsnorm_row<kBf16>(p.x, p.x2, p.norm_w, p.h, p.n, p.eps, H, blockIdx.x, sm.xs, sm.red);
 
   // logits: thread ctid owns the same 8-element rows of every expert's G row; per-warp partials, then the warps in order
   for (int eb = 0; eb < E; eb += kRouterEB) {
@@ -210,6 +234,14 @@ __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRou
     for (int j = 0; j < p.k; ++j) tsum = __fadd_rn(tsum, sm.tv[j]);
     p.wts[static_cast<size_t>(blockIdx.x) * p.k + lane] = __fdiv_rn(sm.tv[lane], tsum);
   }
+}
+
+// The residual add and RMSNorm of a dense block's decode rows: the router's first phase alone, one CTA per row.
+template <bool kBf16>
+__global__ void __launch_bounds__(kRouterThreads) add_rmsnorm_kernel(const AddRmsnormParams p) {
+  __shared__ __align__(16) uint16_t xs[kRouterMaxH];
+  __shared__ float red[kRouterWarps];
+  add_rmsnorm_row<kBf16>(p.x, p.x2, p.norm_w, p.h, p.n, p.eps, p.H, blockIdx.x, xs, red);
 }
 
 }  // namespace agb

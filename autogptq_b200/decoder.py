@@ -38,7 +38,8 @@ bytes per layer, about 22 GB more for Mixtral-8x7B.  Router variants other than 
 DeepSeek, no renormalisation), experts that are not grouped, and models that mix dense and MoE layers are refused.
 
 Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  What does not fit raises
-NotImplementedError naming the module.
+NotImplementedError naming the module.  Up to eight independent sequences of any lengths, admitted and retired between
+steps: ``autogptq_b200.batch_decoder.BatchDecoder``.
 """
 from __future__ import annotations
 
@@ -57,10 +58,10 @@ _MOE_BLOCKS = ("MixtralSparseMoeBlock",)
 _ROUTERS = ("MixtralTopKRouter",)
 
 
-def _norm_of(mod, name: str):
+def _norm_of(mod, name: str, who: str = "ChainDecoder"):
     """(weight, eps) of an RMSNorm with transformers' Llama rounding: weight · rnd(h · rsqrt(mean(h²) + eps))."""
     if type(mod).__name__ not in _RMSNORMS or not hasattr(mod, "weight") or not hasattr(mod, "variance_epsilon"):
-        raise NotImplementedError(f"ChainDecoder: {name} is {type(mod).__name__}; only Llama-style RMSNorm "
+        raise NotImplementedError(f"{who}: {name} is {type(mod).__name__}; only Llama-style RMSNorm "
                                   f"({', '.join(_RMSNORMS)}) runs inside the decode chain")
     return mod.weight, float(mod.variance_epsilon)
 
@@ -156,27 +157,27 @@ def _is_moe(plans) -> bool:
     return moe
 
 
-def _rotary_params(rotary, head_dim: int):
+def _rotary_params(rotary, head_dim: int, who: str = "ChainDecoder(fused_attention=True)"):
     """(inv_freq fp32 [head_dim/2], attention_scaling) of a rotary embedding whose frequencies do not depend on the
     sequence length; default, linear, llama3 and yarn all reduce to these two."""
     rope_type = getattr(rotary, "rope_type", "default")
     if rope_type in ("dynamic", "longrope"):
-        raise NotImplementedError(f"ChainDecoder(fused_attention=True): model.model.rotary_emb is {rope_type!r} rope, "
+        raise NotImplementedError(f"{who}: model.model.rotary_emb is {rope_type!r} rope, "
                                   "whose inv_freq changes with the sequence length; a captured graph cannot follow it")
     inv_freq = getattr(rotary, "inv_freq", None)
     if inv_freq is None or inv_freq.dim() != 1 or inv_freq.numel() != head_dim // 2:
         n = None if inv_freq is None else tuple(inv_freq.shape)
-        raise NotImplementedError(f"ChainDecoder(fused_attention=True): model.model.rotary_emb.inv_freq has shape {n}, "
+        raise NotImplementedError(f"{who}: model.model.rotary_emb.inv_freq has shape {n}, "
                                   f"not [{head_dim // 2}] (partial rotary is not supported)")
     return inv_freq.detach().to(torch.float32).contiguous(), float(getattr(rotary, "attention_scaling", 1.0))
 
 
-def _check_window(config, max_length: int):
+def _check_window(config, max_length: int, who: str = "ChainDecoder"):
     sw = getattr(config, "sliding_window", None)
     if getattr(config, "use_sliding_window", True) is False:
         sw = None
     if sw is not None and sw < max_length:
-        raise NotImplementedError(f"ChainDecoder: the model attends through a sliding window of {sw} tokens, below "
+        raise NotImplementedError(f"{who}: the model attends through a sliding window of {sw} tokens, below "
                                   f"max_length={max_length}; the static cache holds full attention only")
 
 

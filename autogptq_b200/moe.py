@@ -382,6 +382,57 @@ def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n
     return h, n, idx, w, logits
 
 
+def add_rmsnorm_supported(T: int, H: int, dtype) -> str | None:
+    """None when ``add_rmsnorm`` takes this shape, else the reason it does not."""
+    if dtype not in _DTYPE_CODE:
+        return f"dtype {dtype}; the norm kernel computes in fp16 / bf16"
+    if not 0 <= T <= _lib.MOE_DECODE_MAX_T:
+        return f"{T} rows; the norm kernel takes 0..{_lib.MOE_DECODE_MAX_T}"
+    if H <= 0 or H % 128 or H > _lib.CHAIN_NORM_MAX_K:
+        return f"hidden size {H}; the norm kernel needs a multiple of 128 up to {_lib.CHAIN_NORM_MAX_K}"
+    return None
+
+
+def add_rmsnorm(x, x2, weight, eps: float, h=None, n=None):
+    """The residual add and RMSNorm of decode rows in one launch (``agb200_add_rmsnorm``, DESIGN §3.18): the first
+    phase of ``moe_router`` alone, so ``h`` and ``n`` are bit-equal to the router's on the same input.
+
+        h = x + x2 (skipped when x2 is None)   n = RMSNorm(h; weight, eps)
+
+    x, x2 [T, H] (T <= 8) and weight [H] of one 16-bit dtype.  Returns (h or None, n); ``h`` and ``n`` are written in
+    place when given.  No host synchronisation."""
+    if x.dim() != 2:
+        raise ValueError(f"x must be [T, H], got {tuple(x.shape)}")
+    T, H = x.shape
+    dev, dt = x.device, x.dtype
+    if dev.type != "cuda":
+        raise RuntimeError("add_rmsnorm needs CUDA tensors (there is no CPU fallback)")
+    why = add_rmsnorm_supported(T, H, dt)
+    if why is not None:
+        raise NotImplementedError(f"add_rmsnorm: {why}")
+    if x2 is None and h is not None:
+        raise ValueError("h is the residual x + x2; pass x2 or leave h out")
+    if x2 is not None and h is None:
+        h = torch.empty((T, H), dtype=dt, device=dev)
+    n = torch.empty((T, H), dtype=dt, device=dev) if n is None else n
+    checks = [("x", x, (T, H)), ("weight", weight, (H,)), ("n", n, (T, H))]
+    if x2 is not None:
+        checks += [("x2", x2, (T, H)), ("h", h, (T, H))]
+    for name, t, shape in checks:
+        if tuple(t.shape) != shape or t.dtype != dt:
+            raise ValueError(f"{name} must be {dt} {list(shape)}, got {t.dtype} {list(t.shape)}")
+        if t.device != dev:
+            raise ValueError(f"{name} is on {t.device}, x on {dev}")
+        if not t.is_contiguous() or t.data_ptr() % 16:
+            raise ValueError(f"{name} must be contiguous and 16-byte aligned")
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = lib.agb200_add_rmsnorm(x.data_ptr(), _ptr(x2), weight.data_ptr(), float(eps), T, H, _DTYPE_CODE[dt],
+                                    _ptr(h), n.data_ptr(), torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, "agb200_add_rmsnorm")
+    return h, n
+
+
 def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTERN, *,
                   input_grad: bool = False) -> Dict[str, nn.Module]:
     """``{prefix: QuantLinear}`` (e.g. from ``checkpoint.load_quant_linears``) -> the same mapping with every
@@ -411,4 +462,5 @@ def group_experts(layers: Mapping[str, QuantLinear], pattern: str = EXPERT_PATTE
     return out
 
 
-__all__ = ["QuantExperts", "group_experts", "EXPERT_PATTERN", "moe_router", "router_supported"]
+__all__ = ["QuantExperts", "group_experts", "EXPERT_PATTERN", "moe_router", "router_supported", "add_rmsnorm",
+           "add_rmsnorm_supported"]

@@ -603,6 +603,24 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
 size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int head_dim, int max_length);
 
 /*
+ * The same step for B <= AGB200_ATTN_ROWS_MAX_B independent sequences (addition to ABI v10): as
+ * agb200_decode_attention, with the same kernel, but
+ *   pos int64 [B]              row b's position: its rotary angle, its cache write and its range 0..pos[b]
+ * A row with pos[b] == -1 is idle: its output row is written as zeros and its cache row is neither read nor written.
+ * Any other pos[b] outside [0, max_length) writes NaN to its output row and leaves its cache row untouched.  Rows are
+ * independent: row b's output and cache row depend on row b's q, k, v, cache row and position only, bit for bit.  The
+ * split count depends on the shape and the device only (each row splits its own pos[b] + 1 positions into that many
+ * chunks), so the call can be captured once in a CUDA graph and replayed as the positions change.  The workspace is
+ * agb200_decode_attention_workspace_bytes(B, ...) bytes with the same rules.  Constraints as agb200_decode_attention
+ * except B <= AGB200_ATTN_ROWS_MAX_B; pos 8-byte aligned.
+ */
+#define AGB200_ATTN_ROWS_MAX_B 8
+int agb200_decode_attention_rows(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                 const int64_t* pos, const float* inv_freq, float attention_scaling, float scaling,
+                                 void* out, int B, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
+                                 void* workspace, size_t workspace_bytes, void* stream);
+
+/*
  * Router of a Mixtral-style block for T decode rows (addition to ABI v10), one launch on `stream`, all pointers DEVICE
  * memory of `dtype` unless stated:
  *   x [T, H], x2 [T, H] or NULL   h = x + x2 (the residual add; x2 NULL: h = x)
@@ -626,6 +644,21 @@ size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int
 int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, int T,
                       int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
                       void* logits, void* stream);
+
+/*
+ * The residual add and RMSNorm of agb200_moe_router without the router (addition to ABI v10): for T decode rows of a
+ * dense block, one launch on `stream`, all pointers DEVICE memory of `dtype`:
+ *   x [T, H], x2 [T, H] or NULL   h = x + x2 (x2 NULL: h = x)
+ *   norm_weight [H], eps          n = RMSNorm(h)
+ *   h [T, H]                      written exactly when x2 is given (else NULL)
+ *   n [T, H]
+ * The same code as the router's first phase: h and n are bit-equal to agb200_moe_router's on the same input.  Rows
+ * are independent; two calls are bit-identical; no host synchronisation.  Constraints (else AGB200_ENOSUP): dtype
+ * AGB200_F16 / AGB200_BF16, T <= AGB200_MOE_DECODE_MAX_T, H % 128 == 0, H <= AGB200_CHAIN_NORM_MAX_K.  x, x2,
+ * norm_weight, h and n 16-byte aligned (else AGB200_EINVAL).  T = 0 does nothing.
+ */
+int agb200_add_rmsnorm(const void* x, const void* x2, const void* norm_weight, float eps, int T, int H, int dtype,
+                       void* h, void* n, void* stream);
 
 /* Static facts about the build, for logs: returns e.g. "autogptq_b200 sm_90a: ... gemm=wgmma ...". */
 const char* agb200_build_info(void);
