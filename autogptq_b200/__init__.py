@@ -15,7 +15,8 @@ Only what the path needs lives here:
   batch_decoder.py BatchDecoder: up to eight independent sequences of a Llama / Mistral / Qwen2 model, admitted and
                    retired between steps, one CUDA graph per step
   attention.py     decode_attention: rotary embedding, KV-cache write and split-KV attention of one layer in one launch;
-                   decode_attention_rows: the same with one position per row
+                   decode_attention_rows: the same with one position per row; both over a 16-bit or an FP8 cache
+                   (quantize_kv: E4M3 codes with a power-of-two scale per row)
   gptq.py          GPTQ: the quantiser (Hessian accumulation + blocked quantisation) writing packed 4-bit layers
   awq.py           AWQ GEMM packed layers -> the GPTQ layout (exact integer re-layout, used by the loader)
   checkpoint.py    safetensors GPTQ / AWQ checkpoint -> QuantLinear modules, TP-aware (SURVEY.md 8f rank 1; `from autogptq_b200 import checkpoint`)

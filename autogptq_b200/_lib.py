@@ -105,6 +105,10 @@ def _declare(lib):
         "agb200_decode_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
         "agb200_decode_attention_workspace_bytes": (S, [I, I, I, I, I]),
         "agb200_decode_attention_rows": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S, P]),
+        "agb200_decode_attention_fp8": (I, [P, P, P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P, S,
+                                             P]),
+        "agb200_decode_attention_rows_fp8": (I, [P, P, P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P,
+                                                  S, P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
         "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
     }

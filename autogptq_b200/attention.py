@@ -11,6 +11,12 @@ replayed as the position advances.  No host synchronisation.
 ``decode_attention_rows`` (``agb200_decode_attention_rows``, DESIGN §3.18) runs the same kernel for up to
 ``ATTN_ROWS_MAX_B`` = 8 independent sequences: ``pos`` is an int64 device tensor [B], row b attends over 0..pos[b], and a
 row with pos[b] = -1 is idle (zeros out, its cache row untouched).  The workspace is ``decode_attention_workspace``'s.
+
+FP8 cache (``agb200_decode_attention_fp8`` / ``agb200_decode_attention_rows_fp8``, DESIGN §3.19): caches of
+``torch.float8_e4m3fn`` codes [B, n_kv, max_length, head_dim] with ``k_scale=`` / ``v_scale=`` fp32
+[B, n_kv, max_length], one power-of-two scale per cached row, select the FP8 entries.  The step quantises the new k̂ and v with
+``quantize_kv``'s rule, writes codes and scales at the position and attends through them.  q, k, v and out stay in
+the activation dtype.  Half the cache bytes (hd + 4 per row instead of 2·hd).
 """
 from __future__ import annotations
 
@@ -19,6 +25,30 @@ import torch
 from . import _lib
 
 _DT = {torch.float16: _lib.F16, torch.bfloat16: _lib.BF16}
+FP8 = torch.float8_e4m3fn
+E4M3_MAX = 448.0
+
+
+def quantize_kv(x: torch.Tensor):
+    """Rows x [..., hd] (fp16 / bf16) -> (codes float8_e4m3fn [..., hd], scale fp32 [...]), the FP8 cache's format:
+    scale = 2^e with e the smallest integer such that max|x| <= 448·2^e (at least -126), codes = e4m3(x·2^-e) rounded
+    to nearest even; a row of zeros gets scale 1 and codes 0.  Every code·scale is exact in fp32 (and in the dtype for
+    bf16, and for fp16 when 448·2^-16 < max|x| <= 448·2^7).  The kernel quantises the new token by the same rule."""
+    if x.dtype not in _DT:
+        raise ValueError(f"quantize_kv: x is {x.dtype}; the cache rows are fp16 / bf16")
+    a = x.abs().amax(dim=-1).float()                  # exact
+    f, E = torch.frexp(a)                             # a = f·2^E, f in [0.5, 1)
+    e = torch.where(f <= E4M3_MAX / 512, E - 9, E - 8).clamp(min=-126)
+    e = torch.where(a == 0, torch.zeros_like(e), e).to(torch.int32)
+    pow2 = lambda n: ((n + 127) << 23).view(torch.float32)                 # 2^n for -126 <= n <= 127, exactly
+    codes = (x.float() * pow2(-e).unsqueeze(-1)).to(FP8)                  # exact scaling, then one rounding
+    codes.view(torch.uint8).masked_fill_((a == 0).unsqueeze(-1), 0)
+    return codes, pow2(e)
+
+
+def dequantize_kv(codes: torch.Tensor, scale: torch.Tensor) -> torch.Tensor:
+    """codes [..., hd], scale [...] -> the fp32 values the FP8 cache holds (exact)."""
+    return codes.float() * scale.unsqueeze(-1)
 
 
 def attention_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, max_length: int, dtype) -> str | None:
@@ -62,45 +92,59 @@ def decode_attention_workspace(batch: int, n_heads: int, n_kv: int, head_dim: in
 
 
 def decode_attention(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling: float, scaling: float, out,
-                     workspace=None):
+                     workspace=None, *, k_scale=None, v_scale=None):
     """q [B, n_heads·hd], k / v [B, n_kv·hd], caches [B, n_kv, max_length, hd], pos int64 [1] (device), inv_freq fp32
-    [hd/2], out [B, n_heads·hd] written in place and returned.  Raises NotImplementedError outside the kernel's limits."""
+    [hd/2], out [B, n_heads·hd] written in place and returned.  Raises NotImplementedError outside the kernel's limits.
+    float8_e4m3fn caches with ``k_scale`` / ``v_scale`` fp32 [B, n_kv, max_length]: the FP8 cache (module docstring)."""
     return _launch("decode_attention", attention_supported, 1, q, k, v, k_cache, v_cache, pos, inv_freq,
-                   attention_scaling, scaling, out, workspace)
+                   attention_scaling, scaling, out, workspace, k_scale, v_scale)
 
 
 def decode_attention_rows(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling: float, scaling: float, out,
-                          workspace=None):
+                          workspace=None, *, k_scale=None, v_scale=None):
     """``decode_attention`` for independent sequences: pos int64 [B] (device), one position per row, -1 for an idle
-    row (zeros out, cache row untouched).  B <= ``ATTN_ROWS_MAX_B``."""
+    row (zeros out, cache row untouched).  B <= ``ATTN_ROWS_MAX_B``.  FP8 caches as ``decode_attention``."""
     return _launch("decode_attention_rows", attention_rows_supported, None, q, k, v, k_cache, v_cache, pos, inv_freq,
-                   attention_scaling, scaling, out, workspace)
+                   attention_scaling, scaling, out, workspace, k_scale, v_scale)
 
 
 def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out,
-            workspace):
-    """Checks and the call of agb200_<entry>; ``n_pos`` elements of pos (None: one per row)."""
+            workspace, k_scale=None, v_scale=None):
+    """Checks and the call of agb200_<entry> (agb200_<entry>_fp8 for a float8_e4m3fn cache); ``n_pos`` elements of pos
+    (None: one per row).  The activation dtype is the 16-bit cache's, or q's for an FP8 cache."""
     if k_cache.dim() != 4:
         raise ValueError(f"k_cache must be [B, n_kv, max_length, head_dim], got {tuple(k_cache.shape)}")
     B, n_kv, L, hd = k_cache.shape
     dev = k_cache.device
     if dev.type != "cuda":
         raise RuntimeError(f"{entry} needs CUDA tensors (there is no CPU fallback)")
-    dt = k_cache.dtype
+    fp8 = k_cache.dtype == FP8
+    if not fp8 and (k_scale is not None or v_scale is not None):
+        raise ValueError(f"{entry}: k_scale / v_scale go with a {FP8} cache, not {k_cache.dtype}")
+    if fp8 and (k_scale is None or v_scale is None):
+        raise ValueError(f"{entry}: a {FP8} cache needs k_scale and v_scale (fp32 [B, n_kv, max_length])")
+    dt = q.dtype if fp8 else k_cache.dtype
     if q.dim() != 2 or q.shape[0] != B or q.shape[1] % hd != 0:
         raise ValueError(f"q must be [{B}, n_heads·{hd}], got {tuple(q.shape)}")
     n_heads = q.shape[1] // hd
     why = supported(n_heads, n_kv, hd, B, L, dt)
     if why is not None:
         raise NotImplementedError(f"{entry}: {why}")
-    for name, t, shape in (("q", q, (B, n_heads * hd)), ("k", k, (B, n_kv * hd)), ("v", v, (B, n_kv * hd)),
-                           ("v_cache", v_cache, (B, n_kv, L, hd)), ("out", out, (B, n_heads * hd))):
+    checks = [("q", q, (B, n_heads * hd), dt), ("k", k, (B, n_kv * hd), dt), ("v", v, (B, n_kv * hd), dt),
+              ("v_cache", v_cache, (B, n_kv, L, hd), k_cache.dtype), ("out", out, (B, n_heads * hd), dt)]
+    if fp8:
+        checks += [("k_scale", k_scale, (B, n_kv, L), torch.float32), ("v_scale", v_scale, (B, n_kv, L), torch.float32)]
+    for name, t, shape, want in checks:
         if tuple(t.shape) != shape:
             raise ValueError(f"{name} must be {list(shape)}, got {list(t.shape)}")
-        if t.dtype != dt:
-            raise ValueError(f"{name} is {t.dtype}, the cache {dt}")
-    for name, t in (("q", q), ("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out),
-                    ("pos", pos), ("inv_freq", inv_freq)):
+        if t.dtype != want:
+            if not fp8:
+                raise ValueError(f"{name} is {t.dtype}, the cache {dt}")
+            raise ValueError(f"{name} is {t.dtype}, the activations (q) {dt}" if want == dt else
+                             f"{name} is {t.dtype}, not {want}")
+    tensors = [("q", q), ("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out), ("pos", pos),
+               ("inv_freq", inv_freq)] + ([("k_scale", k_scale), ("v_scale", v_scale)] if fp8 else [])
+    for name, t in tensors:
         if t.device != dev:
             raise ValueError(f"{name} is on {t.device}, the cache on {dev}")
         if not t.is_contiguous():
@@ -110,6 +154,18 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
         raise ValueError(f"pos must be {n_pos} int64 element(s), got {pos.dtype} with {pos.numel()} elements")
     if inv_freq.dtype != torch.float32 or tuple(inv_freq.shape) != (hd // 2,):
         raise ValueError(f"inv_freq must be float32 [{hd // 2}], got {inv_freq.dtype} {list(inv_freq.shape)}")
+    caches = (k_cache.data_ptr(), v_cache.data_ptr())
+    if fp8:
+        entry, caches = entry + "_fp8", caches + (k_scale.data_ptr(), v_scale.data_ptr())
+    return _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace,
+                 n_heads, dt)
+
+
+def _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace, n_heads,
+          dt):
+    """agb200_<entry> after the checks: ``caches`` the cache pointers the entry takes after v."""
+    B, n_kv, L, hd = k_cache.shape
+    dev = k_cache.device
     lib = _lib.load()
     with torch.cuda.device(dev):
         need = int(lib.agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, hd, L))
@@ -118,8 +174,8 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
         elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
             raise ValueError(f"workspace must hold {need} bytes on {dev}")
         rc = getattr(lib, f"agb200_{entry}")(
-            q.data_ptr(), k.data_ptr(), v.data_ptr(), k_cache.data_ptr(), v_cache.data_ptr(), pos.data_ptr(),
-            inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads, n_kv, hd, L,
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, pos.data_ptr(), inv_freq.data_ptr(),
+            float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads, n_kv, hd, L,
             _DT[dt], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
             torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(rc, f"agb200_{entry}")
@@ -127,4 +183,4 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
 
 
 __all__ = ["decode_attention", "decode_attention_rows", "decode_attention_workspace", "attention_supported",
-           "attention_rows_supported"]
+           "attention_rows_supported", "quantize_kv", "dequantize_kv"]

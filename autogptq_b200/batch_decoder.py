@@ -22,7 +22,10 @@ writes the row's cache entry and attends over the row's positions only; an idle 
 Every kernel computes a row from that row's inputs alone, so what one slot holds never changes another slot's logits.
 
 ``prefill`` runs the HF model at batch 1 with a ``DynamicCache`` and copies its keys and values into the slot's row of
-the static caches.  Scope: Llama, Mistral and Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too),
+the static caches.  ``kv_cache_dtype=torch.float8_e4m3fn`` keeps the caches as E4M3 codes with a power-of-two scale per
+cached row (``k_scale`` / ``v_scale``, DESIGN §3.19): half the cache bytes, so twice the positions in the same memory;
+prefill quantises the prompt's rows with ``autogptq_b200.attention.quantize_kv``, each step the kernel its own.
+Scope: Llama, Mistral and Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too),
 greedy.  Mixture-of-experts blocks, dynamic / longrope rope, a sliding window below max_length and attention shapes the
 kernel does not take raise NotImplementedError naming the module.  For batch <= 2 sequences in lockstep,
 ``ChainDecoder`` runs each block as one decode-chain launch.
@@ -35,7 +38,7 @@ import torch
 
 from . import _lib
 from .attention import attention_rows_supported, decode_attention_rows, decode_attention_workspace
-from .decoder import _MOE_BLOCKS, _check_window, _norm_of, _rotary_params
+from .decoder import _MOE_BLOCKS, _check_window, _kv_caches, _kv_fp8, _norm_of, _rotary_params, _store_kv
 from .mlp import FusedQuantMLP, _is_silu, forward_gate_up
 from .moe import add_rmsnorm, add_rmsnorm_supported
 from .qlinear import QuantLinear, forward_group
@@ -76,12 +79,14 @@ def _plan_layer(i: int, layer, dtype):
 
 class BatchDecoder:
     """Greedy decoder of up to ``max_batch`` <= 8 independent sequences over a transformers ``LlamaForCausalLM`` /
-    ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose projections are ``autogptq_b200.QuantLinear``."""
+    ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose projections are ``autogptq_b200.QuantLinear``.
+    ``kv_cache_dtype``: None (the activation dtype) or ``torch.float8_e4m3fn``."""
 
-    def __init__(self, model, max_batch: int = 8, max_length: int = 4096):
+    def __init__(self, model, max_batch: int = 8, max_length: int = 4096, kv_cache_dtype=None):
         if not 1 <= max_batch <= _lib.ATTN_ROWS_MAX_B:
             raise NotImplementedError(f"{_WHO}: max_batch {max_batch}; the decode kernels run 1..{_lib.ATTN_ROWS_MAX_B} "
                                       "rows")
+        fp8 = _kv_fp8(kv_cache_dtype, _WHO)
         inner = getattr(model, "model", None)
         if inner is None or not hasattr(inner, "layers") or not hasattr(model, "lm_head"):
             raise NotImplementedError(f"{_WHO}: {type(model).__name__} is not a *ForCausalLM with model.layers and "
@@ -118,8 +123,7 @@ class BatchDecoder:
         self._plans = plans
 
         B, L, dev, dt = self.max_batch, self.max_length, self.device, self.dtype
-        self.k_cache = [torch.zeros((B, n_kv, L, hd), dtype=dt, device=dev) for _ in plans]
-        self.v_cache = [torch.zeros_like(k) for k in self.k_cache]
+        self.k_cache, self.v_cache, self.k_scale, self.v_scale = _kv_caches(len(plans), (B, n_kv, L, hd), dt, dev, fp8)
         self._pos = torch.full((B,), -1, dtype=torch.int64, device=dev)   # next position of each slot, -1 idle
         self._host_pos = [-1] * B                                           # its host mirror
         self._ids = torch.zeros(B, dtype=torch.int64, device=dev)
@@ -167,8 +171,7 @@ class BatchDecoder:
         cache = DynamicCache(config=self.model.config)
         out = self.model(input_ids=ids, past_key_values=cache, use_cache=True)
         for i, lay in enumerate(cache.layers):
-            self.k_cache[i][slot, :, :T].copy_(lay.keys[0])
-            self.v_cache[i][slot, :, :T].copy_(lay.values[0])
+            _store_kv(self, i, (slot, slice(None), slice(0, T)), lay.keys[0], lay.values[0])
         self._pos[slot] = T
         self._host_pos[slot] = T
         return out.logits[0, -1]
@@ -188,8 +191,9 @@ class BatchDecoder:
         resid = self._x
         for i, (attn, mlp, _, (w2, eps2)) in enumerate(self._plans):
             q, k, v = forward_group([attn.q_proj, attn.k_proj, attn.v_proj], self._n1)
+            fp8 = {} if self.k_scale is None else dict(k_scale=self.k_scale[i], v_scale=self.v_scale[i])
             decode_attention_rows(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq,
-                                  self._attn_scaling, self.scaling, self._attn_out, self._attn_ws)
+                                  self._attn_scaling, self.scaling, self._attn_out, self._attn_ws, **fp8)
             o = attn.o_proj(self._attn_out)
             add_rmsnorm(o, resid, w2, eps2, h=self._h1, n=self._n2)
             down = mlp.down_proj(forward_gate_up(mlp.gate_proj, mlp.up_proj, self._n2))

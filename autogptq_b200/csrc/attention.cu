@@ -1,5 +1,5 @@
-// Host side of the decode attention (include/autogptq_b200.h: agb200_decode_attention*): argument checking, the split
-// count, workspace layout and the launch on the caller's stream.  Kernel: attention.cuh.
+// Host side of the decode attention (include/autogptq_b200.h: agb200_decode_attention*, 16-bit and FP8 caches): argument
+// checking, the split count, workspace layout and the launch on the caller's stream.  Kernel: attention.cuh.
 #include <cuda_runtime.h>
 
 #include "attention.cuh"
@@ -39,12 +39,21 @@ size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int
 
 namespace {
 
-// Both entries: `what` names the entry in errors, `pos_stride` 0 (one position) or 1 (a position per row).
+template <bool kBf16, int kHd>
+void launch_attention(bool fp8, dim3 grid, cudaStream_t s, const agb::DecodeAttnParams& p) {
+  if (fp8) agb::decode_attention_kernel<kBf16, kHd, true><<<grid, agb::kAttnThreads, 0, s>>>(p);
+  else agb::decode_attention_kernel<kBf16, kHd><<<grid, agb::kAttnThreads, 0, s>>>(p);
+}
+
+// Every entry: `what` names the entry in errors, `pos_stride` 0 (one position) or 1 (a position per row); k_scale and
+// v_scale are given exactly for an FP8 cache (E4M3 codes in k_cache / v_cache) and null for a 16-bit one.
 int decode_attention(const char* what, int max_b, int pos_stride, const void* q, const void* k, const void* v,
-                     void* k_cache, void* v_cache, const int64_t* pos, const float* inv_freq, float attention_scaling,
-                     float scaling, void* out, int B, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
-                     void* workspace, size_t workspace_bytes, void* stream) {
-  if (!q || !k || !v || !k_cache || !v_cache || !pos || !inv_freq || !out || !workspace)
+                     void* k_cache, void* v_cache, float* k_scale, float* v_scale, bool fp8, const int64_t* pos,
+                     const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
+                     int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                     void* stream) {
+  if (!q || !k || !v || !k_cache || !v_cache || !pos || !inv_freq || !out || !workspace ||
+      (fp8 && (!k_scale || !v_scale)))
     return failf(AGB200_EINVAL, "%s: null pointer argument", what);
   if (B <= 0 || n_heads <= 0 || n_kv <= 0 || head_dim <= 0 || max_length <= 0 || n_heads % n_kv != 0)
     return failf(AGB200_EINVAL, "%s: need positive B, n_heads, n_kv, head_dim, max_length and "
@@ -64,6 +73,8 @@ int decode_attention(const char* what, int max_b, int pos_stride, const void* q,
       !aligned(out, 16) || !aligned(pos, 8) || !aligned(inv_freq, 4) || !aligned(workspace, 256))
     return failf(AGB200_EINVAL, "%s: q, k, v, the caches and out must be 16-byte aligned, the workspace "
                  "256-byte aligned", what);
+  if (fp8 && (!aligned(k_scale, 4) || !aligned(v_scale, 4)))
+    return failf(AGB200_EINVAL, "%s: k_scale and v_scale must be 4-byte aligned", what);
   const size_t need = agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, head_dim, max_length);
   if (workspace_bytes < need)
     return failf(AGB200_EWORKSPACE, "%s: workspace needs %zu bytes (got %zu)", what, need, workspace_bytes);
@@ -86,15 +97,17 @@ int decode_attention(const char* what, int max_b, int pos_stride, const void* q,
   p.n_kv = n_kv;
   p.max_length = max_length;
   p.splits = attn_splits(B, n_kv, max_length);
+  p.k_scale = k_scale;
+  p.v_scale = v_scale;
   const dim3 grid(p.splits, n_kv, B);
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == AGB200_BF16;
   if (head_dim == 128) {
-    if (bf16) agb::decode_attention_kernel<true, 128><<<grid, agb::kAttnThreads, 0, s>>>(p);
-    else agb::decode_attention_kernel<false, 128><<<grid, agb::kAttnThreads, 0, s>>>(p);
+    if (bf16) launch_attention<true, 128>(fp8, grid, s, p);
+    else launch_attention<false, 128>(fp8, grid, s, p);
   } else {
-    if (bf16) agb::decode_attention_kernel<true, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
-    else agb::decode_attention_kernel<false, 64><<<grid, agb::kAttnThreads, 0, s>>>(p);
+    if (bf16) launch_attention<true, 64>(fp8, grid, s, p);
+    else launch_attention<false, 64>(fp8, grid, s, p);
   }
   AGB_CUDA(cudaGetLastError());
   return 0;
@@ -108,18 +121,38 @@ int agb200_decode_attention(const void* q, const void* k, const void* v, void* k
                             const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
                             int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
                             void* stream) {
-  return decode_attention("decode_attention", agb::kAttnMaxB, 0, q, k, v, k_cache, v_cache, pos, inv_freq,
-                          attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype, workspace,
-                          workspace_bytes, stream);
+  return decode_attention("decode_attention", agb::kAttnMaxB, 0, q, k, v, k_cache, v_cache, nullptr, nullptr, false,
+                          pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype,
+                          workspace, workspace_bytes, stream);
 }
 
 int agb200_decode_attention_rows(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
                                  const int64_t* pos, const float* inv_freq, float attention_scaling, float scaling,
                                  void* out, int B, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
                                  void* workspace, size_t workspace_bytes, void* stream) {
-  return decode_attention("decode_attention_rows", agb::kAttnRowsMaxB, 1, q, k, v, k_cache, v_cache, pos, inv_freq,
-                          attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype, workspace,
-                          workspace_bytes, stream);
+  return decode_attention("decode_attention_rows", agb::kAttnRowsMaxB, 1, q, k, v, k_cache, v_cache, nullptr, nullptr,
+                          false, pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length,
+                          dtype, workspace, workspace_bytes, stream);
+}
+
+int agb200_decode_attention_fp8(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                float* k_scale, float* v_scale, const int64_t* pos, const float* inv_freq,
+                                float attention_scaling, float scaling, void* out, int B, int n_heads, int n_kv,
+                                int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                                void* stream) {
+  return decode_attention("decode_attention_fp8", agb::kAttnMaxB, 0, q, k, v, k_cache, v_cache, k_scale, v_scale, true,
+                          pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim, max_length, dtype,
+                          workspace, workspace_bytes, stream);
+}
+
+int agb200_decode_attention_rows_fp8(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                     float* k_scale, float* v_scale, const int64_t* pos, const float* inv_freq,
+                                     float attention_scaling, float scaling, void* out, int B, int n_heads, int n_kv,
+                                     int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                                     void* stream) {
+  return decode_attention("decode_attention_rows_fp8", agb::kAttnRowsMaxB, 1, q, k, v, k_cache, v_cache, k_scale,
+                          v_scale, true, pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim,
+                          max_length, dtype, workspace, workspace_bytes, stream);
 }
 
 }  // extern "C"

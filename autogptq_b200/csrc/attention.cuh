@@ -1,8 +1,11 @@
 // Decode attention of one layer in one launch: rotary embedding of q and k, the KV-cache write at a device-side
 // position, and split-KV attention over positions [0, pos] with a last-arriving-CTA combine (DESIGN §3.16).  The
-// position is one for every row (sequences in lockstep) or one per row (independent sequences, DESIGN §3.18).
+// position is one for every row (sequences in lockstep) or one per row (independent sequences, DESIGN §3.18).  The
+// cache holds the activation dtype, or E4M3 codes with a power-of-two fp32 scale per row (DESIGN §3.19).
 #pragma once
 #include <math.h>
+
+#include <type_traits>
 
 #include "common.cuh"
 
@@ -14,6 +17,7 @@ constexpr int kAttnMaxG = 8;           // query heads per kv head
 constexpr int kAttnMaxSplits = 64;
 constexpr int kAttnMaxB = 2;            // agb200_decode_attention (one position)
 constexpr int kAttnRowsMaxB = 8;        // agb200_decode_attention_rows (a position per row)
+constexpr int kAttnFp8Stages = 3;       // FP8 cache: tiles in the ring (measured against 2 and 4, DESIGN §3.19)
 
 // Floats of one split's partials: acc[G][hd], then m and l of up to kAttnMaxG heads (keeps every split 16-byte aligned)
 __host__ __device__ constexpr int attn_part_floats(int G, int hd) { return G * hd + 2 * kAttnMaxG; }
@@ -33,6 +37,8 @@ struct DecodeAttnParams {
   float* part;              // [B, n_kv, splits, attn_part_floats(G, hd)]: acc[G][hd], m[8], l[8] of each split
   unsigned* counter;        // [B·n_kv] arrivals; zero between launches
   int n_heads, n_kv, max_length, splits;
+  float* k_scale;           // FP8 cache only: [B, n_kv, max_length] power-of-two scale of each cached row
+  float* v_scale;           //   (k_cache / v_cache then hold E4M3 codes, one byte per element)
 };
 
 template <int kHd>
@@ -46,6 +52,25 @@ struct AttnSmem {
   float wt[kAttnMaxSplits][kAttnMaxG];    // combine weights
   float lsum[kAttnMaxG];
   uint16_t knew[kHd], vnew[kHd];          // k̂ and v of the new token
+  int last;
+};
+
+// The same for an FP8 cache: E4M3 codes and the scale of each row, in a ring of kAttnFp8Stages tiles.
+template <int kHd>
+struct AttnSmemFp8 {
+  static constexpr int kKRow = kHd + 16;  // padded K row (bytes): 32 lanes reading 16 B of 32 rows hit distinct banks
+  uint8_t k[kAttnFp8Stages][kAttnTile * kKRow];
+  uint8_t v[kAttnFp8Stages][kAttnTile * kHd];
+  float ks[kAttnFp8Stages][kAttnTile], vs[kAttnFp8Stages][kAttnTile];
+  float q[kAttnMaxG][kHd];
+  float p[kAttnMaxG][kAttnTile];          // softmax weights of the current tile, times the row's v scale
+  float scale[kAttnMaxG];
+  float wt[kAttnMaxSplits][kAttnMaxG];
+  float lsum[kAttnMaxG];
+  float red[2][kAttnThreads / 32];        // per-warp max |k̂|, max |v| of the new token
+  alignas(16) uint8_t knew[kHd];          // codes of the new token (read as 16-byte chunks)
+  alignas(16) uint8_t vnew[kHd];
+  float ksnew, vsnew;                     // and its scales
   int last;
 };
 
@@ -70,6 +95,40 @@ __device__ __forceinline__ void cp_async16(void* smem, const void* gmem) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem))),
                "l"(gmem) : "memory");
 }
+__device__ __forceinline__ void cp_async4(void* smem, const void* gmem) {
+  asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(static_cast<uint32_t>(__cvta_generic_to_shared(smem))),
+               "l"(gmem) : "memory");
+}
+
+// The exponent e of a row's scale 2^e: the smallest integer with a <= 448·2^e, a = max |x| >= 0 (DESIGN §3.19).  With
+// a = f·2^E, f in [0.5, 1): e = E - 9 when f <= 0.875 (448 = 0.875·2^9), else E - 8; at least -126; 0 for a = 0.
+__device__ __forceinline__ int kv_scale_exp(float a) {
+  const int bits = __float_as_int(a);
+  if (bits == 0) return 0;
+  const int eb = bits >> 23;                          // biased exponent (0: fp32 subnormal, below 2^-126)
+  if (eb == 0) return -126;
+  const int E = eb - 126;
+  const int e = (bits & 0x7fffff) <= 0x600000 ? E - 9 : E - 8;   // 1.m <= 1.75  <=>  f <= 0.875
+  return max(e, -126);
+}
+__device__ __forceinline__ float exp2_int(int e) { return __int_as_float((e + 127) << 23); }   // 2^e, -126 <= e <= 127
+
+// Two fp32 values (exact multiples of a power of two, |x| <= 448) to E4M3 with round-to-nearest-even: x0 -> low byte.
+__device__ __forceinline__ uint16_t e4m3x2_rn(float x0, float x1) {
+  uint16_t r;
+  asm("cvt.rn.satfinite.e4m3x2.f32 %0, %1, %2;" : "=h"(r) : "f"(x1), "f"(x0));
+  return r;
+}
+// Four E4M3 codes (byte i = element i) widened to fp32, exactly, through f16x2.
+__device__ __forceinline__ void e4m3x4_to_float(uint32_t w, float* f) {
+  uint32_t h0, h1;
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h0) : "h"(static_cast<uint16_t>(w & 0xffffu)));
+  asm("cvt.rn.f16x2.e4m3x2 %0, %1;" : "=r"(h1) : "h"(static_cast<uint16_t>(w >> 16)));
+  f[0] = __half2float(__ushort_as_half(static_cast<unsigned short>(h0 & 0xffffu)));
+  f[1] = __half2float(__ushort_as_half(static_cast<unsigned short>(h0 >> 16)));
+  f[2] = __half2float(__ushort_as_half(static_cast<unsigned short>(h1 & 0xffffu)));
+  f[3] = __half2float(__ushort_as_half(static_cast<unsigned short>(h1 >> 16)));
+}
 
 template <int kN>
 __device__ __forceinline__ void cp_async_wait() { asm volatile("cp.async.wait_group %0;" ::"n"(kN) : "memory"); }
@@ -90,9 +149,10 @@ __device__ __forceinline__ float warp_sum(float x) {
 // Grid (splits, n_kv, B), kAttnThreads threads.  CTA (b, kv head, split i) owns positions [i·C, min((i+1)·C, pos+1)),
 // C = ceil((pos+1) / splits) with pos row b's position, for the G query heads of its kv head.  Rows share nothing but
 // the launch: every CTA of row b reads only row b's q, k, v, position, cache rows, partials and counter words.
-template <bool kBf16, int kHd>
+// kFp8: the caches hold E4M3 codes and p.k_scale / p.v_scale a power-of-two scale per row (DESIGN §3.19).
+template <bool kBf16, int kHd, bool kFp8 = false>
 __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const DecodeAttnParams p) {
-  using Smem = AttnSmem<kHd>;
+  using Smem = std::conditional_t<kFp8, AttnSmemFp8<kHd>, AttnSmem<kHd>>;
   constexpr int kKRow = Smem::kKRow;
   constexpr int kChunks = kHd / 8;                     // 16-byte chunks of a row
   constexpr int kDimThreads = kHd / 4;                 // PV: 4 output dims per thread
@@ -123,40 +183,122 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
   for (int i = tid; i < G * kHd; i += kAttnThreads)
     sm.q[i / kHd][i % kHd] = rope_elt<kBf16, kHd>(qrow + (i / kHd) * kHd, i % kHd, p.inv_freq, fpos, p.attn_scaling);
   const bool owner = t0 <= pos && pos < t1;           // exactly one split per (b, kv head) holds the new token
-  if (owner) {
-    const uint16_t* krow = p.k + (size_t(b) * p.n_kv + kvh) * kHd;
-    const uint16_t* vrow = p.v + (size_t(b) * p.n_kv + kvh) * kHd;
-    for (int j = tid; j < kHd; j += kAttnThreads) {
-      const uint16_t kn = float_to_elt<kBf16>(rope_elt<kBf16, kHd>(krow, j, p.inv_freq, fpos, p.attn_scaling));
-      sm.knew[j] = kn;
-      sm.vnew[j] = vrow[j];
-      p.k_cache[cache0 + unsigned(pos) * kHd + j] = kn;
-      p.v_cache[cache0 + unsigned(pos) * kHd + j] = vrow[j];
+  if constexpr (kFp8) {
+    static_assert(kHd <= kAttnThreads, "one element of the new row per thread");
+    if (owner) {                                       // uniform over the CTA
+      // k̂ and v of the new token, rounded to the dtype; their row maxima; then codes and scales by the rule
+      const uint16_t* krow = p.k + (size_t(b) * p.n_kv + kvh) * kHd;
+      const uint16_t* vrow = p.v + (size_t(b) * p.n_kv + kvh) * kHd;
+      float kx = 0.f, vx = 0.f;
+      if (tid < kHd) {
+        kx = rope_elt<kBf16, kHd>(krow, tid, p.inv_freq, fpos, p.attn_scaling);
+        vx = elt_to_float<kBf16>(vrow[tid]);
+      }
+      const float mk = warp_max(fabsf(kx)), mv = warp_max(fabsf(vx));
+      if (lane == 0) {
+        sm.red[0][warp] = mk;
+        sm.red[1][warp] = mv;
+      }
+      __syncthreads();
+      float ak = sm.red[0][0], av = sm.red[1][0];
+#pragma unroll
+      for (int w = 1; w < kAttnThreads / 32; ++w) {
+        ak = fmaxf(ak, sm.red[0][w]);
+        av = fmaxf(av, sm.red[1][w]);
+      }
+      const int ek = kv_scale_exp(ak), ev = kv_scale_exp(av);
+      const float kq = __fmul_rn(kx, exp2_int(-ek)), vq = __fmul_rn(vx, exp2_int(-ev));   // exact
+      const float kq1 = __shfl_down_sync(0xffffffffu, kq, 1), vq1 = __shfl_down_sync(0xffffffffu, vq, 1);
+      if (tid < kHd && (tid & 1) == 0) {
+        const uint16_t kc = ak == 0.f ? uint16_t(0) : e4m3x2_rn(kq, kq1);   // a zero row: codes 0, scale 1
+        const uint16_t vc = av == 0.f ? uint16_t(0) : e4m3x2_rn(vq, vq1);
+        *reinterpret_cast<uint16_t*>(&sm.knew[tid]) = kc;
+        *reinterpret_cast<uint16_t*>(&sm.vnew[tid]) = vc;
+        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.k_cache) + cache0 + unsigned(pos) * kHd + tid) = kc;
+        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.v_cache) + cache0 + unsigned(pos) * kHd + tid) = vc;
+      }
+      if (tid == 0) {
+        const unsigned srow = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) + unsigned(pos);
+        sm.ksnew = p.k_scale[srow] = exp2_int(ek);
+        sm.vsnew = p.v_scale[srow] = exp2_int(ev);
+      }
+    }
+  } else {
+    if (owner) {
+      const uint16_t* krow = p.k + (size_t(b) * p.n_kv + kvh) * kHd;
+      const uint16_t* vrow = p.v + (size_t(b) * p.n_kv + kvh) * kHd;
+      for (int j = tid; j < kHd; j += kAttnThreads) {
+        const uint16_t kn = float_to_elt<kBf16>(rope_elt<kBf16, kHd>(krow, j, p.inv_freq, fpos, p.attn_scaling));
+        sm.knew[j] = kn;
+        sm.vnew[j] = vrow[j];
+        p.k_cache[cache0 + unsigned(pos) * kHd + j] = kn;
+        p.v_cache[cache0 + unsigned(pos) * kHd + j] = vrow[j];
+      }
     }
   }
   __syncthreads();
 
   const int n_tiles = (t1 - t0 + kAttnTile - 1) / kAttnTile;
-  // K and V rows of one tile into buffer `buf`; the new token's row comes from knew / vnew, never from the cache.
+  [[maybe_unused]] const unsigned srow0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length);   // FP8: row scales
+  // K and V rows of one tile into buffer `buf`; the new token's row comes from knew / vnew, never from the cache.  FP8:
+  // E4M3 codes and the scale of each position, in a ring of kAttnFp8Stages tiles with one cp.async group per tile
+  // index (empty past the last tile).
   auto load_tile = [&](int it, int buf) {
-    const int ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
-    for (int i = tid; i < nv * kChunks; i += kAttnThreads) {
-      const int r = i / kChunks, c = i % kChunks, t = ts + r;
-      uint16_t* ks = &sm.k[buf][r * kKRow + c * 8];
-      uint16_t* vs = &sm.v[buf][r * kHd + c * 8];
-      if (t == pos) {
-        *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 8]);
-        *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 8]);
-      } else {
-        const unsigned g = cache0 + unsigned(t) * kHd + c * 8;
-        cp_async16(ks, p.k_cache + g);
-        cp_async16(vs, p.v_cache + g);
+    if constexpr (kFp8) {
+      if (it < n_tiles) {
+        constexpr int kChunks8 = kHd / 16;
+        const int ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
+        for (int i = tid; i < nv * kChunks8; i += kAttnThreads) {
+          const int r = i / kChunks8, c = i % kChunks8, t = ts + r;
+          uint8_t* ks = &sm.k[buf][r * kKRow + c * 16];
+          uint8_t* vs = &sm.v[buf][r * kHd + c * 16];
+          if (t == pos) {
+            *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 16]);
+            *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 16]);
+          } else {
+            const unsigned g = cache0 + unsigned(t) * kHd + c * 16;
+            cp_async16(ks, reinterpret_cast<const uint8_t*>(p.k_cache) + g);
+            cp_async16(vs, reinterpret_cast<const uint8_t*>(p.v_cache) + g);
+          }
+        }
+        const int r = tid - (kAttnThreads - kAttnTile);   // the last warp: one scale pair per position
+        if (r >= 0 && r < nv) {
+          const int t = ts + r;
+          if (t == pos) {
+            sm.ks[buf][r] = sm.ksnew;
+            sm.vs[buf][r] = sm.vsnew;
+          } else {
+            cp_async4(&sm.ks[buf][r], p.k_scale + srow0 + t);
+            cp_async4(&sm.vs[buf][r], p.v_scale + srow0 + t);
+          }
+        }
       }
+      cp_async_commit();
+    } else {
+      const int ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
+      for (int i = tid; i < nv * kChunks; i += kAttnThreads) {
+        const int r = i / kChunks, c = i % kChunks, t = ts + r;
+        uint16_t* ks = &sm.k[buf][r * kKRow + c * 8];
+        uint16_t* vs = &sm.v[buf][r * kHd + c * 8];
+        if (t == pos) {
+          *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 8]);
+          *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 8]);
+        } else {
+          const unsigned g = cache0 + unsigned(t) * kHd + c * 8;
+          cp_async16(ks, p.k_cache + g);
+          cp_async16(vs, p.v_cache + g);
+        }
+      }
+      cp_async_commit();
     }
-    cp_async_commit();
   };
-  if (n_tiles > 0) load_tile(0, 0);
-  if (n_tiles > 1) load_tile(1, 1);
+  if constexpr (kFp8) {
+#pragma unroll
+    for (int it = 0; it < kAttnFp8Stages - 1; ++it) load_tile(it, it);
+  } else {
+    if (n_tiles > 0) load_tile(0, 0);
+    if (n_tiles > 1) load_tile(1, 1);
+  }
 
   float m_run[2] = {-INFINITY, -INFINITY}, l_run[2] = {0.f, 0.f};   // score role: heads warp, warp + 4
   float acc[kHpt][4];
@@ -167,34 +309,68 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
   const int dgrp = tid % kDimThreads, hbase = tid / kDimThreads;
 
   for (int it = 0; it < n_tiles; ++it) {
-    if (it + 1 < n_tiles) cp_async_wait<1>();
-    else cp_async_wait<0>();
+    if constexpr (kFp8) {
+      load_tile(it + kAttnFp8Stages - 1, (it + kAttnFp8Stages - 1) % kAttnFp8Stages);   // the buffer freed last round
+      cp_async_wait<kAttnFp8Stages - 1>();
+    } else {
+      if (it + 1 < n_tiles) cp_async_wait<1>();
+      else cp_async_wait<0>();
+    }
     __syncthreads();
-    const int buf = it & 1, ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
+    const int buf = kFp8 ? it % kAttnFp8Stages : it & 1, ts = t0 + it * kAttnTile, nv = min(kAttnTile, t1 - ts);
 
-    // scores: lane = position of the tile, warp = heads {warp, warp + 4}; one fp32 FMA chain over d per head
+    // scores: lane = position of the tile, warp = heads {warp, warp + 4}; one fp32 FMA chain over d per head.  FP8: the
+    // same chain on the codes, then times the row's k scale (a power of two: exact) before σ.
     float s[2] = {0.f, 0.f};
-    const uint16_t* krow = &sm.k[buf][lane * kKRow];
-#pragma unroll 4
-    for (int c = 0; c < kChunks; ++c) {
-      const uint4 kv = *reinterpret_cast<const uint4*>(krow + c * 8);
-      const uint32_t w[4] = {kv.x, kv.y, kv.z, kv.w};
-      float kf[8];
+    if constexpr (kFp8) {
+      const uint8_t* krow = &sm.k[buf][lane * kKRow];
+#pragma unroll 2
+      for (int c = 0; c < kHd / 16; ++c) {
+        const uint4 kv = *reinterpret_cast<const uint4*>(krow + c * 16);
+        float kf[16];
+        e4m3x4_to_float(kv.x, kf);
+        e4m3x4_to_float(kv.y, kf + 4);
+        e4m3x4_to_float(kv.z, kf + 8);
+        e4m3x4_to_float(kv.w, kf + 12);
 #pragma unroll
-      for (int e = 0; e < 4; ++e) {
-        kf[2 * e] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] & 0xffffu));
-        kf[2 * e + 1] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] >> 16));
+        for (int hh = 0; hh < 2; ++hh) {
+          const int h = warp + 4 * hh;
+          if (h < G) {
+#pragma unroll
+            for (int qi = 0; qi < 4; ++qi) {
+              const float4 qa = *reinterpret_cast<const float4*>(&sm.q[h][c * 16 + qi * 4]);
+              s[hh] = fmaf(qa.x, kf[4 * qi], s[hh]); s[hh] = fmaf(qa.y, kf[4 * qi + 1], s[hh]);
+              s[hh] = fmaf(qa.z, kf[4 * qi + 2], s[hh]); s[hh] = fmaf(qa.w, kf[4 * qi + 3], s[hh]);
+            }
+          }
+        }
       }
+      const float ksc = sm.ks[buf][lane];
 #pragma unroll
-      for (int hh = 0; hh < 2; ++hh) {
-        const int h = warp + 4 * hh;
-        if (h < G) {
-          const float4 qa = *reinterpret_cast<const float4*>(&sm.q[h][c * 8]);
-          const float4 qb = *reinterpret_cast<const float4*>(&sm.q[h][c * 8 + 4]);
-          s[hh] = fmaf(qa.x, kf[0], s[hh]); s[hh] = fmaf(qa.y, kf[1], s[hh]);
-          s[hh] = fmaf(qa.z, kf[2], s[hh]); s[hh] = fmaf(qa.w, kf[3], s[hh]);
-          s[hh] = fmaf(qb.x, kf[4], s[hh]); s[hh] = fmaf(qb.y, kf[5], s[hh]);
-          s[hh] = fmaf(qb.z, kf[6], s[hh]); s[hh] = fmaf(qb.w, kf[7], s[hh]);
+      for (int hh = 0; hh < 2; ++hh) s[hh] = __fmul_rn(s[hh], ksc);
+    } else {
+      const uint16_t* krow = &sm.k[buf][lane * kKRow];
+#pragma unroll 4
+      for (int c = 0; c < kChunks; ++c) {
+        const uint4 kv = *reinterpret_cast<const uint4*>(krow + c * 8);
+        const uint32_t w[4] = {kv.x, kv.y, kv.z, kv.w};
+        float kf[8];
+#pragma unroll
+        for (int e = 0; e < 4; ++e) {
+          kf[2 * e] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] & 0xffffu));
+          kf[2 * e + 1] = elt_to_float<kBf16>(static_cast<uint16_t>(w[e] >> 16));
+        }
+#pragma unroll
+        for (int hh = 0; hh < 2; ++hh) {
+          const int h = warp + 4 * hh;
+          if (h < G) {
+            const float4 qa = *reinterpret_cast<const float4*>(&sm.q[h][c * 8]);
+            const float4 qb = *reinterpret_cast<const float4*>(&sm.q[h][c * 8 + 4]);
+            s[hh] = fmaf(qa.x, kf[0], s[hh]); s[hh] = fmaf(qa.y, kf[1], s[hh]);
+            s[hh] = fmaf(qa.z, kf[2], s[hh]); s[hh] = fmaf(qa.w, kf[3], s[hh]);
+            s[hh] = fmaf(qb.x, kf[4], s[hh]); s[hh] = fmaf(qb.y, kf[5], s[hh]);
+            s[hh] = fmaf(qb.z, kf[6], s[hh]); s[hh] = fmaf(qb.w, kf[7], s[hh]);
+          }
         }
       }
     }
@@ -208,13 +384,15 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
         const float rescale = expf(__fsub_rn(m_run[hh], mn));  // 0 at the first tile
         l_run[hh] = fmaf(l_run[hh], rescale, warp_sum(e));
         m_run[hh] = mn;
-        sm.p[h][lane] = e;
+        if constexpr (kFp8) sm.p[h][lane] = lane < nv ? __fmul_rn(e, sm.vs[buf][lane]) : 0.f;   // l keeps e alone
+        else sm.p[h][lane] = e;
         if (lane == 0) sm.scale[h] = rescale;
       }
     }
     __syncthreads();
 
-    // Σ p·v: thread = 4 dims of heads hbase + k·kHeadsPerPass; rows past nv are never read
+    // Σ p·v: thread = 4 dims of heads hbase + k·kHeadsPerPass; rows past nv are never read.  FP8: p carries the row's
+    // v scale, so the products are the 16-bit kernel's on the dequantised values.
 #pragma unroll
     for (int k = 0; k < kHpt; ++k) {
       const int h = hbase + k * kHeadsPerPass;
@@ -224,17 +402,27 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
         for (int e = 0; e < 4; ++e) acc[k][e] = __fmul_rn(acc[k][e], r);
         for (int t = 0; t < nv; ++t) {
           const float pt = sm.p[h][t];
-          const uint2 vv = *reinterpret_cast<const uint2*>(&sm.v[buf][t * kHd + dgrp * 4]);
-          acc[k][0] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x & 0xffffu)), acc[k][0]);
-          acc[k][1] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x >> 16)), acc[k][1]);
-          acc[k][2] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y & 0xffffu)), acc[k][2]);
-          acc[k][3] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y >> 16)), acc[k][3]);
+          if constexpr (kFp8) {
+            float vf[4];
+            e4m3x4_to_float(*reinterpret_cast<const uint32_t*>(&sm.v[buf][t * kHd + dgrp * 4]), vf);
+#pragma unroll
+            for (int e = 0; e < 4; ++e) acc[k][e] = fmaf(pt, vf[e], acc[k][e]);
+          } else {
+            const uint2 vv = *reinterpret_cast<const uint2*>(&sm.v[buf][t * kHd + dgrp * 4]);
+            acc[k][0] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x & 0xffffu)), acc[k][0]);
+            acc[k][1] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.x >> 16)), acc[k][1]);
+            acc[k][2] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y & 0xffffu)), acc[k][2]);
+            acc[k][3] = fmaf(pt, elt_to_float<kBf16>(static_cast<uint16_t>(vv.y >> 16)), acc[k][3]);
+          }
         }
       }
     }
     __syncthreads();
-    if (it + 2 < n_tiles) load_tile(it + 2, buf);
+    if constexpr (!kFp8) {
+      if (it + 2 < n_tiles) load_tile(it + 2, buf);
+    }
   }
+  if constexpr (kFp8) cp_async_wait<0>();              // nothing in flight at exit (the groups past the end are empty)
 
   // partials of this split (an empty split stores m = -inf, l = 0, acc = 0)
   const int stride = attn_part_floats(G, kHd);

@@ -22,7 +22,9 @@ then n_layers + 1 chain launches and n_layers attentions, captured together in o
 ``fused_attention=True`` runs each attention as one ``agb200_decode_attention`` launch instead (rotary embedding, cache
 write and split-KV attention, ``autogptq_b200.attention``): a token is then 2·n_layers + 1 launches of the project's own
 kernels plus the embedding, final norm and lm_head.  It rounds differently from SDPA (fp32 online softmax), so it is
-opt-in.
+opt-in.  With it, ``kv_cache_dtype=torch.float8_e4m3fn`` keeps the caches as E4M3 codes with a power-of-two scale per
+cached row (``autogptq_b200.attention.quantize_kv``, DESIGN §3.19): half the cache bytes; the prompt's keys and values
+are quantised at prefill, each step's by the attention kernel.
 
 Mixtral-style models (``MixtralSparseMoeBlock`` MLPs whose ``experts`` are an ``autogptq_b200.QuantExperts``, see
 ``autogptq_b200.moe``) decode through the same graph with a different block (DESIGN §3.17):
@@ -47,7 +49,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from .attention import attention_supported, decode_attention, decode_attention_workspace
+from .attention import FP8, attention_supported, decode_attention, decode_attention_workspace, quantize_kv
 from .chain import DecodeChain, chain_supported
 from .mlp import FusedQuantMLP, _is_silu
 from .moe import QuantExperts, moe_router, router_supported
@@ -181,15 +183,54 @@ def _check_window(config, max_length: int, who: str = "ChainDecoder"):
                                   f"max_length={max_length}; the static cache holds full attention only")
 
 
+def _kv_fp8(kv_cache_dtype, who: str) -> bool:
+    """Whether the KV cache is FP8 (torch.float8_e4m3fn); None keeps it in the activation dtype.  Refuses the rest."""
+    if kv_cache_dtype is None:
+        return False
+    if kv_cache_dtype == FP8:
+        return True
+    raise NotImplementedError(f"{who}: kv_cache_dtype {kv_cache_dtype}; supported: None (the activation dtype) or "
+                              f"{FP8}")
+
+
+def _kv_caches(n_layers: int, shape, dtype, device, fp8: bool):
+    """(k_cache, v_cache, k_scale, v_scale): per-layer static caches of ``shape`` [B, n_kv, max_length, hd] in
+    ``dtype``, or E4M3 codes with fp32 scales [B, n_kv, max_length] for ``fp8`` (else the scales are None)."""
+    k = [torch.zeros(shape, dtype=FP8 if fp8 else dtype, device=device) for _ in range(n_layers)]
+    v = [torch.zeros_like(c) for c in k]
+    if not fp8:
+        return k, v, None, None
+    ks = [torch.ones(shape[:-1], dtype=torch.float32, device=device) for _ in range(n_layers)]
+    return k, v, ks, [torch.ones_like(s) for s in ks]
+
+
+def _store_kv(dec, i: int, index, keys, values):
+    """The prompt's keys and values [.., n_kv, T, hd] into layer i's caches at ``index`` (quantised for FP8)."""
+    if dec.k_scale is None:
+        dec.k_cache[i][index].copy_(keys)
+        dec.v_cache[i][index].copy_(values)
+        return
+    for cache, scale, x in ((dec.k_cache[i], dec.k_scale[i], keys), (dec.v_cache[i], dec.v_scale[i], values)):
+        codes, sc = quantize_kv(x)
+        cache.view(torch.uint8)[index].copy_(codes.view(torch.uint8))
+        scale[index].copy_(sc)
+
+
 class ChainDecoder:
     """Greedy decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
     projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too), or a
     ``MixtralForCausalLM`` whose experts are ``autogptq_b200.QuantExperts``.  ``fused_attention``:
-    run each layer's attention as one CUDA launch (``autogptq_b200.attention.decode_attention``) instead of torch."""
+    run each layer's attention as one CUDA launch (``autogptq_b200.attention.decode_attention``) instead of torch.
+    ``kv_cache_dtype``: None (the activation dtype) or ``torch.float8_e4m3fn`` (needs ``fused_attention``)."""
 
-    def __init__(self, model, batch: int = 1, max_length: int = 2048, fused_attention: bool = False):
+    def __init__(self, model, batch: int = 1, max_length: int = 2048, fused_attention: bool = False,
+                 kv_cache_dtype=None):
         if not 1 <= batch <= _lib.CHAIN_MAX_M:
             raise NotImplementedError(f"ChainDecoder: batch {batch}; the decode chain runs 1..{_lib.CHAIN_MAX_M} rows")
+        fp8 = _kv_fp8(kv_cache_dtype, "ChainDecoder")
+        if fp8 and not fused_attention:
+            raise NotImplementedError(f"ChainDecoder: kv_cache_dtype {FP8} needs fused_attention=True; the torch "
+                                      "attention reads a 16-bit cache")
         inner = getattr(model, "model", None)
         if inner is None or not hasattr(inner, "layers") or not hasattr(model, "lm_head"):
             raise NotImplementedError(f"ChainDecoder: {type(model).__name__} is not a *ForCausalLM with model.layers "
@@ -227,8 +268,8 @@ class ChainDecoder:
         H = attn0.q_proj.infeatures
 
         B, L, dev, dt = batch, len(plans), self.device, self.dtype
-        self.k_cache = [torch.zeros((B, self.n_kv, self.max_length, self.head_dim), dtype=dt, device=dev) for _ in plans]
-        self.v_cache = [torch.zeros_like(k) for k in self.k_cache]
+        self.k_cache, self.v_cache, self.k_scale, self.v_scale = _kv_caches(
+            len(plans), (B, self.n_kv, self.max_length, self.head_dim), dt, dev, fp8)
         self._pos = torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
         self._ids = torch.zeros(B, dtype=torch.int64, device=dev)
         self._arange = torch.arange(self.max_length, device=dev)
@@ -343,8 +384,7 @@ class ChainDecoder:
         cache = DynamicCache(config=self.model.config)
         out = self.model(input_ids=ids, past_key_values=cache, use_cache=True)
         for i, lay in enumerate(cache.layers):
-            self.k_cache[i][:, :, :T].copy_(lay.keys)
-            self.v_cache[i][:, :, :T].copy_(lay.values)
+            _store_kv(self, i, (slice(None), slice(None), slice(0, T)), lay.keys, lay.values)
         self.position = T
         return out.logits[:, -1]
 
@@ -366,8 +406,9 @@ class ChainDecoder:
 
     def _fused_attention(self, i: int):
         q, k, v = self._qkv[i]
+        fp8 = {} if self.k_scale is None else dict(k_scale=self.k_scale[i], v_scale=self.v_scale[i])
         decode_attention(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq, self._attn_scaling,
-                         self.scaling, self._attn_in[i], self._attn_ws)
+                         self.scaling, self._attn_in[i], self._attn_ws, **fp8)
 
     def _step_body(self) -> torch.Tensor:
         inner = self.model.model

@@ -621,6 +621,30 @@ int agb200_decode_attention_rows(const void* q, const void* k, const void* v, vo
                                  void* workspace, size_t workspace_bytes, void* stream);
 
 /*
+ * Both steps over an FP8 cache (addition to ABI v10): k_cache and v_cache [B, n_kv, max_length, head_dim] hold E4M3
+ * (float8_e4m3fn) codes, one byte per element, and k_scale, v_scale [B, n_kv, max_length] (fp32) the scale of each
+ * cached row; a row's value is code * scale.  The scale is a power of two, 2^e: with a = max_j |x_j| over the row (k-hat
+ * after the rotary embedding, rounded to dtype, or v), e is the smallest integer with a <= 448 * 2^e, at least -126, and
+ * code_j = e4m3(x_j * 2^-e) rounded to nearest even (subnormals included); a row of zeros has scale 1 and codes 0.
+ * The step writes the new token's codes and scales at pos (pos[b]) and attends through them, so its output is
+ * attention over the cache exactly as the next step reads it; every product of the 16-bit kernel is formed on the
+ * dequantised values, exactly.  dtype is the activation dtype of q, k, v and out; the workspace is
+ * agb200_decode_attention_workspace_bytes(B, ...) bytes with the same rules.  Constraints and idle rows as
+ * agb200_decode_attention (B <= 2, one position) and agb200_decode_attention_rows (B <= AGB200_ATTN_ROWS_MAX_B, a
+ * position per row); in addition k_scale and v_scale non-null and 4-byte aligned (else AGB200_EINVAL).
+ */
+int agb200_decode_attention_fp8(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                float* k_scale, float* v_scale, const int64_t* pos, const float* inv_freq,
+                                float attention_scaling, float scaling, void* out, int B, int n_heads, int n_kv,
+                                int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                                void* stream);
+int agb200_decode_attention_rows_fp8(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                     float* k_scale, float* v_scale, const int64_t* pos, const float* inv_freq,
+                                     float attention_scaling, float scaling, void* out, int B, int n_heads, int n_kv,
+                                     int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
+                                     void* stream);
+
+/*
  * Router of a Mixtral-style block for T decode rows (addition to ABI v10), one launch on `stream`, all pointers DEVICE
  * memory of `dtype` unless stated:
  *   x [T, H], x2 [T, H] or NULL   h = x + x2 (the residual add; x2 NULL: h = x)
