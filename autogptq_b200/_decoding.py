@@ -1,0 +1,216 @@
+"""The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules,
+the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, and the warm-up,
+capture and replay of a step's CUDA graph."""
+from __future__ import annotations
+
+import torch
+
+from .attention import FP8, quantize_kv
+from .mlp import FusedQuantMLP, _is_silu
+from .qlinear import QuantLinear
+
+_RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm", "MixtralRMSNorm")
+_MOE_BLOCKS = ("MixtralSparseMoeBlock",)
+
+
+def _is_moe_block(mlp) -> bool:
+    """Whether a layer's mlp is a mixture-of-experts block: a known one, or any with experts or a router gate."""
+    return (type(mlp).__name__ in _MOE_BLOCKS or hasattr(mlp, "experts")
+            or (hasattr(mlp, "gate") and not hasattr(mlp, "gate_proj")))
+
+
+def _norm_of(mod, name: str, who: str = "ChainDecoder"):
+    """(weight, eps) of an RMSNorm with transformers' Llama rounding: weight · rnd(h · rsqrt(mean(h²) + eps))."""
+    if type(mod).__name__ not in _RMSNORMS or not hasattr(mod, "weight") or not hasattr(mod, "variance_epsilon"):
+        raise NotImplementedError(f"{who}: {name} is {type(mod).__name__}; only Llama-style RMSNorm "
+                                  f"({', '.join(_RMSNORMS)}) runs inside the decode chain")
+    return mod.weight, float(mod.variance_epsilon)
+
+
+def _quant_linear(who: str, mod, where: str, name: str) -> QuantLinear:
+    lin = getattr(mod, name, None)
+    if not isinstance(lin, QuantLinear):
+        raise NotImplementedError(f"{who}: {where}.{name} is {type(lin).__name__}, not autogptq_b200.QuantLinear")
+    return lin
+
+
+def _rotary_params(rotary, head_dim: int, who: str):
+    """(inv_freq fp32 [head_dim/2], attention_scaling) of a rotary embedding whose frequencies do not depend on the
+    sequence length; default, linear, llama3 and yarn all reduce to these two."""
+    rope_type = getattr(rotary, "rope_type", "default")
+    if rope_type in ("dynamic", "longrope"):
+        raise NotImplementedError(f"{who}: model.model.rotary_emb is {rope_type!r} rope, "
+                                  "whose inv_freq changes with the sequence length; a captured graph cannot follow it")
+    inv_freq = getattr(rotary, "inv_freq", None)
+    if inv_freq is None or inv_freq.dim() != 1 or inv_freq.numel() != head_dim // 2:
+        n = None if inv_freq is None else tuple(inv_freq.shape)
+        raise NotImplementedError(f"{who}: model.model.rotary_emb.inv_freq has shape {n}, "
+                                  f"not [{head_dim // 2}] (partial rotary is not supported)")
+    return inv_freq.detach().to(torch.float32).contiguous(), float(getattr(rotary, "attention_scaling", 1.0))
+
+
+def _check_window(config, max_length: int, who: str = "ChainDecoder"):
+    sw = getattr(config, "sliding_window", None)
+    if getattr(config, "use_sliding_window", True) is False:
+        sw = None
+    if sw is not None and sw < max_length:
+        raise NotImplementedError(f"{who}: the model attends through a sliding window of {sw} tokens, below "
+                                  f"max_length={max_length}; the static cache holds full attention only")
+
+
+def _kv_fp8(kv_cache_dtype, who: str) -> bool:
+    """Whether the KV cache is FP8 (torch.float8_e4m3fn); None keeps it in the activation dtype.  Refuses the rest."""
+    if kv_cache_dtype is None:
+        return False
+    if kv_cache_dtype == FP8:
+        return True
+    raise NotImplementedError(f"{who}: kv_cache_dtype {kv_cache_dtype}; supported: None (the activation dtype) or "
+                              f"{FP8}")
+
+
+def _plan_common(i: int, layer, dtype, who: str):
+    """(attn, mlp, ln1, ln2) of decoder layer i after checking the rules every decoder shares: q/k/v/o
+    ``QuantLinear``, a SiLU gate/up/down MLP of ``QuantLinear`` (or ``FusedQuantMLP``), Llama-style norms in the
+    activation ``dtype``.  A mixture-of-experts mlp (``_is_moe_block``) is left to the caller to plan or refuse."""
+    where = f"model.layers.{i}"
+    attn, mlp = getattr(layer, "self_attn", None), getattr(layer, "mlp", None)
+    if attn is None or mlp is None:
+        raise NotImplementedError(f"{who}: {where} has no self_attn / mlp")
+    for n in ("q_proj", "k_proj", "v_proj", "o_proj"):
+        _quant_linear(who, attn, f"{where}.self_attn", n)
+    if not _is_moe_block(mlp):
+        if not isinstance(mlp, FusedQuantMLP):
+            if not all(hasattr(mlp, n) for n in ("gate_proj", "up_proj", "down_proj")):
+                raise NotImplementedError(f"{who}: {where}.mlp ({type(mlp).__name__}) is not a gate/up/down MLP")
+            if not _is_silu(getattr(mlp, "act_fn", None)):
+                raise NotImplementedError(f"{who}: {where}.mlp.act_fn is "
+                                          f"{type(getattr(mlp, 'act_fn', None)).__name__}, not SiLU")
+        for n in ("gate_proj", "up_proj", "down_proj"):
+            _quant_linear(who, mlp, f"{where}.mlp", n)
+    norms = [(n, _norm_of(getattr(layer, n, None), f"{where}.{n}", who))
+             for n in ("input_layernorm", "post_attention_layernorm")]
+    for n, (w, _) in norms:
+        if w.dtype != dtype:
+            raise NotImplementedError(f"{who}: {where}.{n}.weight is {w.dtype}, the activations {dtype}")
+    return attn, mlp, norms[0][1], norms[1][1]
+
+
+class StaticCacheDecoder:
+    """Base of a greedy decoder over a static KV cache whose step is one captured CUDA graph.  A subclass sets ``_who``
+    (the prefix of its refusals) and ``_plan`` (a layer's plan, starting from ``_plan_common``).  Its constructor calls
+    ``_read_model``, checks its kernels' limits on the geometry, calls ``_read_layers``, checks what spans the layers
+    and calls ``_allocate`` last, so every refusal comes before the device is needed.  It then sets ``_pos``, the device
+    positions its ``_step_body`` reads and advances."""
+
+    # ------------------------------------------------------------------ reading the model
+    def _read_model(self, model, max_length: int, kv_cache_dtype):
+        """The model's structure, activation dtype, sliding window and attention geometry (from the config)."""
+        who = self._who
+        self._fp8 = _kv_fp8(kv_cache_dtype, who)
+        inner = getattr(model, "model", None)
+        if inner is None or not hasattr(inner, "layers") or not hasattr(model, "lm_head"):
+            raise NotImplementedError(f"{who}: {type(model).__name__} is not a *ForCausalLM with model.layers and "
+                                      "lm_head")
+        for n in ("embed_tokens", "rotary_emb", "norm"):
+            if not hasattr(inner, n):
+                raise NotImplementedError(f"{who}: model.model has no {n}")
+        self.model, self.max_length = model, int(max_length)
+        cfg = model.config
+        _check_window(cfg, self.max_length, who)
+        self.dtype = inner.embed_tokens.weight.dtype
+        if self.dtype not in (torch.float16, torch.bfloat16):
+            raise NotImplementedError(f"{who}: activations are {self.dtype}; the kernels compute in fp16 / bf16")
+        self.hidden_size, self.n_heads = cfg.hidden_size, cfg.num_attention_heads
+        self.head_dim = getattr(cfg, "head_dim", None) or self.hidden_size // self.n_heads
+        self.n_kv = getattr(cfg, "num_key_value_heads", None) or self.n_heads
+
+    def _read_layers(self):
+        """``_plans`` (``_plan`` of each layer, whose q/k/v/o must have the config's geometry), ``scaling`` and
+        ``_final``: model.norm's (weight, eps)."""
+        inner, who = self.model.model, self._who
+        H, q, kv = self.hidden_size, self.n_heads * self.head_dim, self.n_kv * self.head_dim
+        self._plans = []
+        for i, layer in enumerate(inner.layers):
+            plan = self._plan(i, layer)
+            for n, shape in (("q_proj", (H, q)), ("k_proj", (H, kv)), ("v_proj", (H, kv)), ("o_proj", (q, H))):
+                lin = getattr(plan[0], n)
+                if (lin.infeatures, lin.outfeatures) != shape:
+                    raise NotImplementedError(
+                        f"{who}: model.layers.{i}.self_attn.{n} maps {lin.infeatures} -> {lin.outfeatures} features; "
+                        f"the config (hidden_size {H}, {self.n_heads} heads, {self.n_kv} kv heads, head_dim "
+                        f"{self.head_dim}) needs {shape[0]} -> {shape[1]}")
+            self._plans.append(plan)
+        if not self._plans:
+            raise NotImplementedError(f"{self._who}: the model has no decoder layers")
+        self.scaling = self._plans[0][0].scaling
+        self._final = _norm_of(inner.norm, "model.norm", self._who)
+
+    # ------------------------------------------------------------------ the KV cache
+    def _allocate(self, rows: int):
+        """After every refusal: the CUDA device, the static caches of ``rows`` rows and the step's token ids.  The
+        caches are per layer [rows, n_kv, max_length, head_dim] in the activation dtype, or E4M3 codes with fp32
+        scales ``k_scale`` / ``v_scale`` [rows, n_kv, max_length] for FP8 (else the scales are None)."""
+        self.device = self.model.model.embed_tokens.weight.device
+        if self.device.type != "cuda":
+            raise RuntimeError(f"{self._who} needs the model on a CUDA device")
+        shape, n, dev = (rows, self.n_kv, self.max_length, self.head_dim), len(self._plans), self.device
+        self.k_cache = [torch.zeros(shape, dtype=FP8 if self._fp8 else self.dtype, device=dev) for _ in range(n)]
+        self.v_cache = [torch.zeros_like(c) for c in self.k_cache]
+        self.k_scale = self.v_scale = None
+        if self._fp8:
+            self.k_scale = [torch.ones(shape[:-1], dtype=torch.float32, device=dev) for _ in range(n)]
+            self.v_scale = [torch.ones_like(s) for s in self.k_scale]
+        self._ids = torch.zeros(rows, dtype=torch.int64, device=dev)
+        self._graph = None
+        self._logits = None
+
+    def _store_kv(self, i: int, index, keys, values):
+        """Keys and values [.., n_kv, T, hd] into layer i's caches at ``index`` (quantised for FP8)."""
+        if self.k_scale is None:
+            self.k_cache[i][index].copy_(keys)
+            self.v_cache[i][index].copy_(values)
+            return
+        for cache, scale, x in ((self.k_cache[i], self.k_scale[i], keys), (self.v_cache[i], self.v_scale[i], values)):
+            codes, sc = quantize_kv(x)
+            cache.view(torch.uint8)[index].copy_(codes.view(torch.uint8))
+            scale[index].copy_(sc)
+
+    def _cache_kwargs(self, i: int) -> dict:
+        """Layer i's cache keyword arguments of ``decode_attention`` / ``decode_attention_rows`` beyond the caches."""
+        return {} if self.k_scale is None else dict(k_scale=self.k_scale[i], v_scale=self.v_scale[i])
+
+    def _prefill_cache(self, ids: torch.Tensor, rows: slice) -> torch.Tensor:
+        """Run ``ids`` [len(rows), T] through the HF model (its own prefill kernels) and store every layer's keys and
+        values into the static caches at ``rows``, positions :T.  Returns the model's logits [len(rows), T, vocab]."""
+        from transformers import DynamicCache
+
+        cache = DynamicCache(config=self.model.config)
+        out = self.model(input_ids=ids, past_key_values=cache, use_cache=True)
+        for i, lay in enumerate(cache.layers):
+            self._store_kv(i, (rows, slice(None), slice(0, ids.shape[1])), lay.keys, lay.values)
+        return out.logits
+
+    # ------------------------------------------------------------------ one step
+    def _run_step(self, ids: torch.Tensor, use_graph: bool) -> torch.Tensor:
+        """The subclass's ``_step_body`` (one step on ``_ids`` at the device positions ``_pos``, which it advances:
+        the logits) on ``ids``, eagerly or through the step's CUDA graph.  The first graph step warms up outside
+        the graph (library workspaces) and captures; both restore ``_pos`` after.  Later steps replay, and the logits
+        are a buffer the next step overwrites."""
+        self._ids.copy_(ids.reshape(-1).to(self._ids.device))
+        if not use_graph:
+            return self._step_body()
+        if self._graph is None:
+            saved = self._pos.clone()
+            side = torch.cuda.Stream(self.device)
+            side.wait_stream(torch.cuda.current_stream(self.device))
+            with torch.cuda.stream(side):
+                self._step_body()
+            torch.cuda.current_stream(self.device).wait_stream(side)
+            self._pos.copy_(saved)
+            g = torch.cuda.CUDAGraph()
+            with torch.cuda.graph(g):
+                self._logits = self._step_body()
+            self._graph = g
+            self._pos.copy_(saved)
+        self._graph.replay()
+        return self._logits

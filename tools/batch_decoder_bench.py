@@ -28,17 +28,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-from tools.chain_decoder_bench import build_model, gpu_facts, time_graph  # noqa: E402
-
-
-def timed_steps(step, tok, S):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(S):
-        tok = step(tok)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / S
+from tools.chain_decoder_bench import build_model, gpu_facts, time_graph, timed_steps  # noqa: E402
 
 
 def ragged(B, prompt, spread):
@@ -50,12 +40,10 @@ def ragged(B, prompt, spread):
 
 def _fill(dec, index, T, gen):
     """Synthetic keys and values N(0, 1) in positions :T of the decoder's caches at ``index`` (quantised for FP8)."""
-    from autogptq_b200.decoder import _store_kv
-
     for i, k in enumerate(dec.k_cache):
         shape = k[index][..., :T, :].shape
         x = [torch.randn(shape, generator=gen, device=k.device).half() for _ in range(2)]
-        _store_kv(dec, i, index + (slice(0, T),), *x)
+        dec._store_kv(i, index + (slice(0, T),), *x)
 
 
 def _kv_dtype(kv):
@@ -97,9 +85,8 @@ def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
 
     def attentions():
         for i, (qq, kk, vv) in enumerate(q):
-            fp8 = {} if dec.k_scale is None else dict(k_scale=dec.k_scale[i], v_scale=dec.v_scale[i])
             decode_attention_rows(qq, kk, vv, dec.k_cache[i], dec.v_cache[i], dec._pos, dec._inv_freq,
-                                  dec._attn_scaling, dec.scaling, dec._attn_out, dec._attn_ws, **fp8)
+                                  dec._attn_scaling, dec.scaling, dec._attn_out, dec._attn_ws, **dec._cache_kwargs(i))
 
     def norms():
         w, eps = plans[0][2]

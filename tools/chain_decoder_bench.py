@@ -88,6 +88,16 @@ def time_graph(fn, reps, warm=3):
     return e0.elapsed_time(e1) / reps
 
 
+def timed_steps(step, tok, S):
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    e0.record()
+    for _ in range(S):
+        tok = step(tok)
+    e1.record()
+    torch.cuda.synchronize()
+    return e0.elapsed_time(e1) / S
+
+
 @torch.no_grad()
 def main():
     ap = argparse.ArgumentParser()
@@ -121,13 +131,7 @@ def main():
         for _ in range(3):                                   # capture + warm replays
             tok = dec.step(tok).argmax(-1)
         dec.position = T
-        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        e0.record()
-        for _ in range(S):
-            tok = dec.step(tok).argmax(-1)
-        e1.record()
-        torch.cuda.synchronize()
-        ms = e0.elapsed_time(e1) / S
+        ms = timed_steps(lambda t: dec.step(t).argmax(-1), tok, S)
 
         # split: the chains alone and the attentions alone, each as one graph, at the middle of the timed window
         dec.position = T + S // 2

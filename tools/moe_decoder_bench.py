@@ -16,7 +16,6 @@ from __future__ import annotations
 import argparse
 import json
 import os
-import subprocess
 import sys
 
 import torch
@@ -24,15 +23,7 @@ import torch
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
-
-def gpu_facts():
-    name = torch.cuda.get_device_name()
-    try:
-        pl = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader", "-i",
-                             str(torch.cuda.current_device())], capture_output=True, text=True, timeout=30).stdout.strip()
-    except Exception as e:          # noqa: BLE001 - a missing nvidia-smi leaves the field empty
-        pl = f"unknown ({e})"
-    return name, pl
+from tools.chain_decoder_bench import gpu_facts, time_graph, timed_steps  # noqa: E402
 
 
 def build_model(layers, dev, seed=0):
@@ -73,36 +64,6 @@ def build_model(layers, dev, seed=0):
                 mod.weight.normal_(0, 2 * H ** -0.5, generator=gen)
     model.model.rotary_emb = MixtralRotaryEmbedding(cfg, device=dev)
     return model.eval()
-
-
-def time_graph(fn, reps, warm=3):
-    s = torch.cuda.Stream()
-    s.wait_stream(torch.cuda.current_stream())
-    with torch.cuda.stream(s):
-        for _ in range(warm):
-            fn()
-    torch.cuda.current_stream().wait_stream(s)
-    g = torch.cuda.CUDAGraph()
-    with torch.cuda.graph(g):
-        fn()
-    g.replay()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(reps):
-        g.replay()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / reps
-
-
-def timed_steps(step, tok, S):
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(S):
-        tok = step(tok)
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) / S
 
 
 @torch.no_grad()
