@@ -23,7 +23,8 @@ int launch_quantize(const agb::GptqQuantParams& p, cudaStream_t s) {
 extern "C" {
 
 int agb200_gptq_hessian_update(const void* x, float* H, int T, int K, int dtype, float alpha, float beta, void* stream) {
-  if (!x || !H) return failf(AGB200_EINVAL, "gptq_hessian_update: null pointer argument");
+  // an empty batch (T == 0) only rescales H; its x may be null, as torch gives an empty tensor no storage
+  if ((!x && T != 0) || !H) return failf(AGB200_EINVAL, "gptq_hessian_update: null pointer argument");
   if (T < 0 || K <= 0 || K % 8 != 0) return failf(AGB200_EINVAL, "gptq_hessian_update: need T >= 0 and K > 0, K %% 8 == 0 (got T=%d, K=%d)", T, K);
   if (dtype != AGB200_F16 && dtype != AGB200_BF16) return failf(AGB200_EINVAL, "gptq_hessian_update: x must be AGB200_F16 or AGB200_BF16");
   if (!aligned(x, 16) || !aligned(H, 16)) return failf(AGB200_EINVAL, "gptq_hessian_update: x and H must be 16-byte aligned");

@@ -133,17 +133,7 @@ class GPTQ:
 
         H = self.H
         del self.H
-        dead = torch.diag(H) == 0                                   # gptq.py:84-86
-        H[dead, dead] = 1
-        perm = None
-        if actorder:                                                # gptq.py:104-108, with a stable sort for ties
-            perm = torch.argsort(torch.diag(H), descending=True, stable=True)
-            H = H[perm][:, perm]
-        damp = percdamp * torch.mean(torch.diag(H))                 # gptq.py:113-119
-        H.diagonal().add_(damp)
-        H = torch.linalg.cholesky(H)
-        H = torch.cholesky_inverse(H)
-        Hinv = torch.linalg.cholesky(H, upper=True).contiguous()
+        Hinv, perm, dead = inverse_hessian_factor(H, percdamp, actorder)
         del H
 
         res = quantize_weight(W, Hinv, perm=perm, dead=dead if bool(dead.any()) else None, group_size=group_size,
@@ -168,6 +158,25 @@ class GPTQ:
         self.Losses = None
         self.Trace = None
         torch.cuda.empty_cache()
+
+
+def inverse_hessian_factor(H: torch.Tensor, percdamp=0.01, actorder=False):
+    """``(Hinv, perm, dead)`` for ``quantize_weight`` from the running-mean Hessian ``H`` [K, K] fp32, which is edited in
+    place: dead columns (``diag H = 0``) get a unit diagonal, act-order permutes H by descending diagonal (a stable sort
+    for ties), the damping adds ``percdamp`` times the mean diagonal, and three torch factorisations give the upper
+    Cholesky factor of the damped inverse in processing order (``gptq.py:84-119``).  ``perm`` is None without act-order;
+    ``dead`` is a bool [K] in original column order."""
+    dead = torch.diag(H) == 0                                       # gptq.py:84-86
+    H[dead, dead] = 1
+    perm = None
+    if actorder:                                                    # gptq.py:104-108
+        perm = torch.argsort(torch.diag(H), descending=True, stable=True)
+        H = H[perm][:, perm]
+    damp = percdamp * torch.mean(torch.diag(H))                     # gptq.py:113-119
+    H.diagonal().add_(damp)
+    H = torch.linalg.cholesky(H)
+    H = torch.cholesky_inverse(H)
+    return torch.linalg.cholesky(H, upper=True).contiguous(), perm, dead
 
 
 def quantize_weight(W: torch.Tensor, Hinv: torch.Tensor, perm=None, dead=None, group_size=-1, sym=True,
@@ -248,5 +257,5 @@ def patch_auto_gptq_quantizer() -> list:
     return patched
 
 
-__all__ = ["GPTQ", "Quantizer", "quantize_linear", "quantize_weight", "patch_auto_gptq_quantizer",
-           "running_mean_factors"]
+__all__ = ["GPTQ", "Quantizer", "inverse_hessian_factor", "quantize_linear", "quantize_weight",
+           "patch_auto_gptq_quantizer", "running_mean_factors"]

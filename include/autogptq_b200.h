@@ -491,7 +491,7 @@ int agb200_w4a16_mlp_backward_ex(const void* dy, const agb200_moe_layer* gate, c
  *   with fp32 accumulation (fp16 x fp16 and bf16 x bf16 products are exact in fp32).  The reference's running mean is
  *   alpha = n / (n + b), beta = 2 / (n + b) for a batch of b samples after n.  Only the tiles on or above the diagonal
  *   are computed; H must be symmetric on entry (it is read from its upper triangle) and is symmetric on return.
- *   T is arbitrary, K % 8 == 0; x and H 16-byte aligned.  The reduction over T runs in a fixed order without atomics:
+ *   T >= 0 (x may be null when T == 0: then H = alpha * H), K % 8 == 0; x and H 16-byte aligned.  The reduction over T runs in a fixed order without atomics:
  *   two calls on the same inputs give bit-identical H.
  */
 int agb200_gptq_hessian_update(const void* x, float* H, int T, int K, int dtype, float alpha, float beta, void* stream);
