@@ -12,7 +12,7 @@ from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
-ABI_VERSION = 10
+ABI_VERSION = 11
 F16, BF16 = 0, 1
 ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
@@ -51,15 +51,13 @@ def _declare(lib):
         "agb200_build_info": (c_char_p, []),
         "agb200_device_count": (I, []),
         "agb200_w4a16_forward": (I, fwd),
-        "agb200_w4a16_forward_ex": (I, fwd + [I, I, I, I]),
+        "agb200_w4a16_forward_ex": (I, fwd + [I, I, I]),
         "agb200_w4a16_workspace_bytes": (S, [I, I, I]),
         "agb200_w4a16_dgrad": (I, [P, P, P, P, P, P, I, I, I, I, I, P, S, P]),
         "agb200_w4a16_dgrad_ex": (I, [P, P, P, P, P, P, I, I, I, I, I, P, S, P, I, I, I]),
         "agb200_w4a16_dgrad_workspace_bytes": (S, [I, I, I]),
         "agb200_w4a16_forward_group":(I, [P, I, P, P, P, P, P, P, P, P, I, I, I, I, P, S, P]),
         "agb200_w4_prefetch_hint": (I, [I, P, P]),
-        "agb200_w4a16_forward_host": (I, fwd),
-        "agb200_w4a16_host_staging_bytes": (S, [I, I, I]),
         "agb200_w4_make_sequential": (I, [P, P, P, I, I, P]),
         "agb200_w4_prepare_tc": (I, [P, P, I, I, P]),
         "agb200_w4_dequantize": (I, [P, P, P, P, P, I, I, I, I, P]),

@@ -84,10 +84,10 @@ namespace {
 // ------------------------------------------------------------------------------------------ GEMV
 using agb::GemvParams;
 
-template <int kM, int kLN, bool kBf16, bool kBiased, int kOcc = 2>
+template <int kM, int kLN, bool kBf16, int kOcc = 2>
 int launch_gemv_inst(const GemvParams& p, int n_tiles, cudaStream_t stream, int smem_optin) {
-  constexpr auto kern = &agb::w4a16_gemv_kernel<kM, kLN, kBf16, kBiased, (kM == 1 ? kOcc : (kM <= 2 ? 2 : 1))>;
-  const size_t smem = agb::GemvSmem<kM, kLN, kBiased>::total(p.rows_per_split);
+  constexpr auto kern = &agb::w4a16_gemv_kernel<kM, kLN, kBf16, (kM == 1 ? kOcc : (kM <= 2 ? 2 : 1))>;
+  const size_t smem = agb::GemvSmem<kM, kLN>::total(p.rows_per_split);
   if (smem > static_cast<size_t>(smem_optin))
     return failf(AGB200_ENOSUP, "gemv: K chunk of %d rows needs %zu B shared memory (> %d)", p.rows_per_split, smem, smem_optin);
   if (int rc = opt_in_smem<kern>(smem_optin)) return rc;
@@ -97,24 +97,21 @@ int launch_gemv_inst(const GemvParams& p, int n_tiles, cudaStream_t stream, int 
 }
 
 template <int kM, int kLN>
-int launch_gemv_mln(const GemvParams& p, int n_tiles, bool bf16, bool biased, cudaStream_t s, int so) {
-  if constexpr (kM == 1 && kLN == 8) {
-    if (p.occ3 == 1 && !bf16 && !biased) return launch_gemv_inst<1, 8, false, false, 3>(p, n_tiles, s, so);
-    if (p.occ3 == 2 && !bf16 && !biased) return launch_gemv_inst<1, 8, false, false, 4>(p, n_tiles, s, so);
-  }
-  if (bf16) return launch_gemv_inst<kM, kLN, true, false>(p, n_tiles, s, so);
-  if (biased) return launch_gemv_inst<kM, kLN, false, true>(p, n_tiles, s, so);
-  return launch_gemv_inst<kM, kLN, false, false>(p, n_tiles, s, so);
+int launch_gemv_mln(const GemvParams& p, int n_tiles, bool bf16, cudaStream_t s, int so) {
+  if constexpr (kM == 1 && kLN == 8)
+    if (p.occ3 && !bf16) return launch_gemv_inst<1, 8, false, 3>(p, n_tiles, s, so);
+  if (bf16) return launch_gemv_inst<kM, kLN, true>(p, n_tiles, s, so);
+  return launch_gemv_inst<kM, kLN, false>(p, n_tiles, s, so);
 }
 
 template <int kM>
-int launch_gemv_m(const GemvParams& p, int ln, bool bf16, bool biased, cudaStream_t s, int so) {
+int launch_gemv_m(const GemvParams& p, int ln, bool bf16, cudaStream_t s, int so) {
   const int tn = ln * 4;
   const int n_tiles = (p.N + tn - 1) / tn;
   switch (ln) {
-    case 8: return launch_gemv_mln<kM, 8>(p, n_tiles, bf16, biased, s, so);
-    case 16: return launch_gemv_mln<kM, 16>(p, n_tiles, bf16, biased, s, so);
-    case 32: return launch_gemv_mln<kM, 32>(p, n_tiles, bf16, biased, s, so);
+    case 8: return launch_gemv_mln<kM, 8>(p, n_tiles, bf16, s, so);
+    case 16: return launch_gemv_mln<kM, 16>(p, n_tiles, bf16, s, so);
+    case 32: return launch_gemv_mln<kM, 32>(p, n_tiles, bf16, s, so);
   }
   return failf(AGB200_EINVAL, "gemv: lanes-along-N must be 8, 16 or 32 (got %d)", ln);
 }
@@ -122,7 +119,7 @@ int launch_gemv_m(const GemvParams& p, int ln, bool bf16, bool biased, cudaStrea
 // One GEMV pass over m <= 4 rows.
 int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, const void* scales,
               const int32_t* perm, const void* bias, void* y, int m, int K, int N, int group_size,
-              bool bf16, int ln, int split, bool biased, cudaStream_t stream, const DeviceInfo& di, int occ_req = 0) {
+              bool bf16, int ln, int split, cudaStream_t stream, const DeviceInfo& di) {
   GemvParams p{};
   p.x = x; p.qweight = qweight; p.qzeros = qzeros; p.scales = scales; p.perm = perm; p.bias = bias; p.y = y;
   p.K = K; p.N = N; p.rows = K / 8; p.rows_per_group = group_size / 8;
@@ -131,11 +128,9 @@ int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, cons
   // 128-column tiles with cluster split-K (tools/sweep_gemv.py sweeps the choices)
   p.occ3 = 0;
   if (ln == 0 && split == 0 && m == 1 && (N + 31) / 32 >= 2 * di.sms) { ln = 8; split = 1; p.occ3 = 1; }
-  if (occ_req == 3) p.occ3 = 1;        // tuning knob (flags bits 4-5): force the 3- / 4-CTAs-per-SM instantiation
-  if (occ_req == 4) p.occ3 = 2;
   // Everything else of Llama size: 32-column CTAs (128-byte row segments) as well.  Short K (q/k/v/o of a 7B model):
   // no clusters - half of the CTA slots stay free, so sibling layers launched on parallel graph branches overlap
-  // (tools/concurrency_probe.py).  Long K: 2-way cluster split-K (tools/sweep_occ.py).  Not re-tuned on H100.
+  // (tools/concurrency_probe.py).  Long K: 2-way cluster split-K (tools/sweep_gemv.py).  Not re-tuned on H100.
   if (ln == 0 && split == 0 && N >= 1024) {
     const int tiles32 = (N + 31) / 32;
     ln = 8;
@@ -161,18 +156,18 @@ int gemv_pass(const void* x, const int32_t* qweight, const int32_t* qzeros, cons
   p.split = split;
   p.rows_per_split = ((p.rows + split - 1) / split + 7) / 8 * 8;
   switch (m) {
-    case 1: return launch_gemv_m<1>(p, ln, bf16, biased, stream, di.smem_optin);
-    case 2: return launch_gemv_m<2>(p, ln, bf16, biased, stream, di.smem_optin);
-    case 3: return launch_gemv_m<3>(p, ln, bf16, biased, stream, di.smem_optin);
-    case 4: return launch_gemv_m<4>(p, ln, bf16, biased, stream, di.smem_optin);
+    case 1: return launch_gemv_m<1>(p, ln, bf16, stream, di.smem_optin);
+    case 2: return launch_gemv_m<2>(p, ln, bf16, stream, di.smem_optin);
+    case 3: return launch_gemv_m<3>(p, ln, bf16, stream, di.smem_optin);
+    case 4: return launch_gemv_m<4>(p, ln, bf16, stream, di.smem_optin);
   }
   return failf(AGB200_EINVAL, "gemv pass with m=%d", m);
 }
 
 // ------------------------------------------------------------------------------------------ skinny (M <= 8)
-template <bool kBf16, bool kBiased>
+template <bool kBf16>
 int launch_skinny_inst(const agb::SkinnyParams& p, cudaStream_t stream, int smem_optin) {
-  constexpr auto kern = &agb::w4a16_skinny_kernel<kBf16, kBiased>;
+  constexpr auto kern = &agb::w4a16_skinny_kernel<kBf16>;
   const size_t smem = agb::SkinnySmem::total(p.rows_per_split, p.M);
   if (smem > static_cast<size_t>(smem_optin))
     return failf(AGB200_ENOSUP, "skinny: K chunk of %d rows x M=%d needs %zu B shared memory (> %d)", p.rows_per_split, p.M, smem, smem_optin);
@@ -182,7 +177,7 @@ int launch_skinny_inst(const agb::SkinnyParams& p, cudaStream_t stream, int smem
 }
 
 int skinny_launch(const void* x, const int32_t* qweight, const int32_t* qzeros, const void* scales, const int32_t* perm,
-                  const void* bias, void* y, int M, int K, int N, int group_size, bool bf16, int split, bool biased,
+                  const void* bias, void* y, int M, int K, int N, int group_size, bool bf16, int split,
                   cudaStream_t stream, const DeviceInfo& di) {
   if (group_size % 32 != 0) return failf(AGB200_ENOSUP, "skinny kernel needs group_size %% 32 == 0 (got %d)", group_size);
   if (M < 1 || M > AGB200_SKINNY_MAX_M) return failf(AGB200_EINVAL, "skinny kernel handles 1 <= M <= 8 (got %d)", M);
@@ -200,9 +195,8 @@ int skinny_launch(const void* x, const int32_t* qweight, const int32_t* qzeros, 
   while (split < 8 && agb::SkinnySmem::total(rps_of(split), M) > static_cast<size_t>(di.smem_optin)) split *= 2;
   p.split = split;
   p.rows_per_split = rps_of(split);
-  if (bf16) return launch_skinny_inst<true, false>(p, stream, di.smem_optin);
-  if (biased) return launch_skinny_inst<false, true>(p, stream, di.smem_optin);
-  return launch_skinny_inst<false, false>(p, stream, di.smem_optin);
+  if (bf16) return launch_skinny_inst<true>(p, stream, di.smem_optin);
+  return launch_skinny_inst<false>(p, stream, di.smem_optin);
 }
 
 // ------------------------------------------------------------------------------------------ integer tensor-core decode (M <= 8)
@@ -400,7 +394,7 @@ size_t agb200_w4a16_workspace_bytes(int M, int K, int N) {
 int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros, const void* scales,
                             const int32_t* perm, const void* bias, void* y, int M, int K, int N, int group_size,
                             int dtype, void* workspace, size_t workspace_bytes, void* stream_, int kernel, int tune0,
-                            int tune1, int flags) {
+                            int tune1) {
   activate_prefetch_hint();
   if (int rc = check_common(x, qweight, qzeros, scales, y, M, K, N, group_size, dtype)) return rc;
   if (M == 0) return 0;
@@ -438,24 +432,22 @@ int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t
     return 0;
   }
   if (kernel == AGB200_KERNEL_SKINNY) {
-    const bool biased = (flags & 1) != 0 && !bf16;
     const size_t xs = static_cast<size_t>(K) * 2, ys = static_cast<size_t>(N) * 2;
     for (int m0 = 0; m0 < M; m0 += AGB200_SKINNY_MAX_M) {
       const int m = (M - m0 < AGB200_SKINNY_MAX_M) ? (M - m0) : AGB200_SKINNY_MAX_M;
       if (int rc = skinny_launch(static_cast<const char*>(x) + m0 * xs, qweight, qzeros, scales, perm, bias,
-                                 static_cast<char*>(y) + m0 * ys, m, K, N, group_size, bf16, tune1, biased, stream, di))
+                                 static_cast<char*>(y) + m0 * ys, m, K, N, group_size, bf16, tune1, stream, di))
         return rc;
     }
     return 0;
   }
 
   if (kernel == AGB200_KERNEL_GEMV) {
-    const bool biased = (flags & 1) != 0 && !bf16;
     const size_t xs = static_cast<size_t>(K) * 2, ys = static_cast<size_t>(N) * 2;
     for (int m0 = 0; m0 < M; m0 += AGB200_GEMV_MAX_M) {
       const int m = (M - m0 < AGB200_GEMV_MAX_M) ? (M - m0) : AGB200_GEMV_MAX_M;
       if (int rc = gemv_pass(static_cast<const char*>(x) + m0 * xs, qweight, qzeros, scales, perm, bias,
-                             static_cast<char*>(y) + m0 * ys, m, K, N, group_size, bf16, tune0, tune1, biased, stream, di, (flags >> 4) & 7))
+                             static_cast<char*>(y) + m0 * ys, m, K, N, group_size, bf16, tune0, tune1, stream, di))
         return rc;
     }
     return 0;
@@ -529,10 +521,10 @@ int agb200_w4a16_forward_group(const void* x, int n_layers, const int32_t* const
   cudaStream_t stream = static_cast<cudaStream_t>(stream_);
   const bool bf16 = dtype == AGB200_BF16;
   switch (M) {
-    case 1: return launch_gemv_mln<1, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
-    case 2: return launch_gemv_mln<2, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
-    case 3: return launch_gemv_mln<3, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
-    case 4: return launch_gemv_mln<4, kLN>(p, tiles, bf16, false, stream, di.smem_optin);
+    case 1: return launch_gemv_mln<1, kLN>(p, tiles, bf16, stream, di.smem_optin);
+    case 2: return launch_gemv_mln<2, kLN>(p, tiles, bf16, stream, di.smem_optin);
+    case 3: return launch_gemv_mln<3, kLN>(p, tiles, bf16, stream, di.smem_optin);
+    case 4: return launch_gemv_mln<4, kLN>(p, tiles, bf16, stream, di.smem_optin);
   }
   return failf(AGB200_EINVAL, "forward_group: M=%d", M);
 }
@@ -541,30 +533,7 @@ int agb200_w4a16_forward(const void* x, const int32_t* qweight, const int32_t* q
                          const int32_t* perm, const void* bias, void* y, int M, int K, int N, int group_size, int dtype,
                          void* workspace, size_t workspace_bytes, void* stream) {
   return agb200_w4a16_forward_ex(x, qweight, qweight_tc, qzeros, scales, perm, bias, y, M, K, N, group_size, dtype, workspace,
-                                 workspace_bytes, stream, AGB200_KERNEL_AUTO, 0, 0, 0);
-}
-
-size_t agb200_w4a16_host_staging_bytes(int M, int K, int N) {
-  return align_up(static_cast<size_t>(M) * K * 2, 256) + align_up(static_cast<size_t>(M) * N * 2, 256) +
-         align_up(agb::gemm_workspace_bytes(M, K, N), 256);
-}
-
-int agb200_w4a16_forward_host(const void* x_host, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros, const void* scales,
-                              const int32_t* perm, const void* bias, void* y_host, int M, int K, int N, int group_size,
-                              int dtype, void* staging, size_t staging_bytes, void* stream_) {
-  if (!x_host || !y_host || !staging) return failf(AGB200_EINVAL, "null host/staging pointer");
-  if (staging_bytes < agb200_w4a16_host_staging_bytes(M, K, N))
-    return failf(AGB200_EWORKSPACE, "staging buffer too small: %zu < %zu", staging_bytes, agb200_w4a16_host_staging_bytes(M, K, N));
-  cudaStream_t stream = static_cast<cudaStream_t>(stream_);
-  char* xd = static_cast<char*>(staging);
-  char* yd = xd + align_up(static_cast<size_t>(M) * K * 2, 256);
-  char* ws = yd + align_up(static_cast<size_t>(M) * N * 2, 256);
-  AGB_CUDA(cudaMemcpyAsync(xd, x_host, static_cast<size_t>(M) * K * 2, cudaMemcpyHostToDevice, stream));
-  if (int rc = agb200_w4a16_forward(xd, qweight, qweight_tc, qzeros, scales, perm, bias, yd, M, K, N, group_size, dtype, ws,
-                                    agb::gemm_workspace_bytes(M, K, N), stream_))
-    return rc;
-  AGB_CUDA(cudaMemcpyAsync(y_host, yd, static_cast<size_t>(M) * N * 2, cudaMemcpyDeviceToHost, stream));
-  return 0;
+                                 workspace_bytes, stream, AGB200_KERNEL_AUTO, 0, 0);
 }
 
 int agb200_w4_make_sequential(const int32_t* qweight_in, const int32_t* perm, int32_t* qweight_out, int K, int N,

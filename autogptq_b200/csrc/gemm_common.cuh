@@ -14,7 +14,6 @@ constexpr int kGemmConsumers = 256;
 constexpr int kGemmBN = 128;      // weight columns per CTA (two wgmma M = 64 slices)
 constexpr int kGemmBK = 64;       // k per pipeline stage   (one 128-byte swizzle row of 16-bit x)
 constexpr int kGemmLd = kGemmBN + 4;   // fp32 staging row pitch: conflict-free fragment stores
-__host__ __device__ constexpr int gemm_stages(int mt) { return mt == 256 ? 5 : 6; }
 
 // Reduction split over a thread-block cluster (DSMEM reduction) for `tiles` output tiles of `mt` rows and `num_kb`
 // 64-wide reduction stages: small tiles split while the grid is under one wave, 128-row tiles only while the doubled
@@ -36,7 +35,7 @@ __device__ __forceinline__ uint64_t make_b_desc(uint32_t smem_addr) {
 
 template <int kMT>
 struct GemmSmem {
-  static constexpr int kStages = gemm_stages(kMT);
+  static constexpr int kStages = 6;
   static constexpr int kBStage = kMT * 128;                       // bytes of one x stage
   static constexpr int kWStage = (kGemmBK / 8) * kGemmBN * 4;     // packed weight tile [8 k8-rows][128 cols] int32 = 4 KB
   static constexpr int kSStage = 2 * kGemmBN * 2;                 // scales of up to two groups x 128 columns (16-bit)
@@ -72,7 +71,6 @@ __device__ __forceinline__ void wgmma_tile(float (&d)[kMT / 2], const uint32_t* 
   if constexpr (kMT == 32) { if constexpr (kBf16) wgmma_m64n32k16_bf16(d, a, b_desc); else wgmma_m64n32k16_f16(d, a, b_desc); }
   if constexpr (kMT == 64) { if constexpr (kBf16) wgmma_m64n64k16_bf16(d, a, b_desc); else wgmma_m64n64k16_f16(d, a, b_desc); }
   if constexpr (kMT == 128) { if constexpr (kBf16) wgmma_m64n128k16_bf16(d, a, b_desc); else wgmma_m64n128k16_f16(d, a, b_desc); }
-  if constexpr (kMT == 256) { if constexpr (kBf16) wgmma_m64n256k16_bf16(d, a, b_desc); else wgmma_m64n256k16_f16(d, a, b_desc); }
 }
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, %0;" ::"n"(kGemmConsumers) : "memory"); }

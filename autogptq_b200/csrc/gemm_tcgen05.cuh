@@ -38,9 +38,7 @@ struct GemmParams {
   int debug;           // measurement aid: bit0 = no weight loads, bit1 = no x loads
 };
 
-// kMcast: clusters of two CTAs along N (adjacent weight-column tiles, same x rows).  Each CTA fetches HALF of the
-// x tile and TMA-multicasts it into both CTAs' shared memory, halving the L2->SM traffic of the B operand.
-template <int kMT, bool kBf16, bool kMcast>
+template <int kMT, bool kBf16>
 __global__ void __launch_bounds__(kGemmThreads, 1)
 w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x, const __grid_constant__ CUtensorMap tmap_w,
                   const __grid_constant__ CUtensorMap tmap_s, const __grid_constant__ CUtensorMap tmap_z) {
@@ -69,18 +67,11 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
     prefetch_tmap(&tmap_z);
     for (int s = 0; s < kGemmStages; ++s) {
       mbar_init(b_full(s), 2);                                   // x producer + weight producer
-      mbar_init(empty(s), (kMcast ? 2 : 1) * (kGemmConsumers / 32));
+      mbar_init(empty(s), kGemmConsumers / 32);
     }
     fence_mbar_init();
   }
-  uint32_t cta_rank = 0;
-  if constexpr (kMcast) {
-    cg::cluster_group cl = cg::this_cluster();
-    cl.sync();                                     // peer barriers are initialised before any remote arrive / multicast
-    cta_rank = cl.block_rank();
-  } else {
-    __syncthreads();
-  }
+  __syncthreads();
   float* stage_f32 = reinterpret_cast<float*>(smem_al);  // [kMT][kGemmLd], reuses the ring
 
   if (wg == 0) {
@@ -94,12 +85,7 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
         mbar_wait(empty(s), ph ^ 1u);
         if (p.debug & 2) { mbar_arrive(b_full(s)); continue; }
         mbar_arrive_expect_tx(b_full(s), Smem::kBStage);
-        if constexpr (kMcast) {
-          tma_load_2d_mcast(smem_base + s * Smem::kBStage + cta_rank * (Smem::kBStage / 2), &tmap_x,
-                            (kb_begin + it) * kGemmBK, m0 + static_cast<int>(cta_rank) * (kMT / 2), b_full(s), 0x3);
-        } else {
-          tma_load_2d(smem_base + s * Smem::kBStage, &tmap_x, (kb_begin + it) * kGemmBK, m0, b_full(s));
-        }
+        tma_load_2d(smem_base + s * Smem::kBStage, &tmap_x, (kb_begin + it) * kGemmBK, m0, b_full(s));
       }
     } else if (warp == 1 && lane == 0) {
       // ================= weight producer: packed int4 tile + scale / zero rows of its group(s) =================
@@ -139,8 +125,7 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
       zc = lo | (lo << 16);
     };
 
-    // 256-row tiles: no registers for a second A set, so every wgmma group retires before the next stage
-    constexpr int kInFlight = kMT == 256 ? 0 : 1;
+    constexpr int kInFlight = 1;   // one wgmma group stays in flight while the next stage's A is expanded
     float acc[kMT / 2];
 #pragma unroll
     for (int i = 0; i < kMT / 2; ++i) acc[i] = 0.f;
@@ -148,14 +133,7 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
 
     auto release = [&](int s) {
       __syncwarp();
-      if (lane == 0) {
-        if constexpr (kMcast) {
-          mbar_arrive_cluster(empty(s), 0);
-          mbar_arrive_cluster(empty(s), 1);
-        } else {
-          mbar_arrive(empty(s));
-        }
-      }
+      if (lane == 0) mbar_arrive(empty(s));
     };
 
     auto stage = [&](auto kb_tag, int it) {
@@ -200,7 +178,7 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
     if (it < num_it) stage(std::integral_constant<int, 0>{}, it);
     wgmma_wait<0>();
     wgmma_fence_operands(acc);
-    if (kInFlight > 0 && num_it > 0) release((num_it - 1) % kGemmStages);
+    if (num_it > 0) release((num_it - 1) % kGemmStages);
 
     // epilogue: d[4i + 2h + e] = (A row 16 w + g + 8 h, column 8 i + 2 t + e) -> fp32 staging [m][n]
     consumer_sync();  // both warpgroups are done with the ring
@@ -252,8 +230,6 @@ w4a16_gemm_kernel(const GemmParams p, const __grid_constant__ CUtensorMap tmap_x
       }
     }
     cluster.sync();
-  } else if constexpr (kMcast) {
-    cg::this_cluster().sync();                     // no CTA exits while its peer can still multicast / arrive into it
   }
 }
 
@@ -263,14 +239,13 @@ inline size_t gemm_workspace_bytes(int M, int K, int) {
   return (static_cast<size_t>(M) * K * 2 + 255) / 256 * 256;
 }
 
-template <int kMT, bool kBf16, bool kMcast>
+template <int kMT, bool kBf16>
 int launch_gemm_inst(const GemmParams& p, const CUtensorMap& tmap, const CUtensorMap& tmap_w, const CUtensorMap& tmap_s,
                      const CUtensorMap& tmap_z, int m_tiles, cudaStream_t stream) {
-  constexpr auto kern = &w4a16_gemm_kernel<kMT, kBf16, kMcast>;
+  constexpr auto kern = &w4a16_gemm_kernel<kMT, kBf16>;
   constexpr int smem = GemmSmem<kMT>::kTotal;
   if (int rc = opt_in_smem<kern>(smem)) return rc;
-  const dim3 cluster = kMcast ? dim3(2, 1, 1) : dim3(1, 1, p.split);
-  return launch(kern, dim3((p.N + kGemmBN - 1) / kGemmBN, m_tiles, p.split), dim3(kGemmThreads), smem, stream, true, cluster,
+  return launch(kern, dim3((p.N + kGemmBN - 1) / kGemmBN, m_tiles, p.split), dim3(kGemmThreads), smem, stream, true, dim3(1, 1, p.split),
                 false, p, tmap, tmap_w, tmap_s, tmap_z);
 }
 
@@ -289,12 +264,8 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream) {
   }
   const int n_tiles = (a.N + kGemmBN - 1) / kGemmBN;
   int mt = a.tile_m;
-  if (mt == 0) {
-    // 256-row tiles stay opt-in: their 128 accumulators per thread leave ptxas too few registers to keep wgmma
-    // asynchronous, and a 128 x 128 tile already keeps the tensor cores busier than the weight expansion
-    mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
-  }
-  if (mt != 32 && mt != 64 && mt != 128 && mt != 256) return failf(AGB200_EINVAL, "gemm: x-row tile must be 32/64/128/256 (got %d)", mt);
+  if (mt == 0) mt = a.M <= 32 ? 32 : a.M <= 64 ? 64 : 128;
+  if (mt != 32 && mt != 64 && mt != 128) return failf(AGB200_EINVAL, "gemm: x-row tile must be 32/64/128 (got %d)", mt);
   const int m_tiles = (a.M + mt - 1) / mt;
   GemmParams p{};
   p.qweight = a.qweight; p.qzeros = a.qzeros; p.scales = a.scales; p.bias = a.bias; p.y = a.y;
@@ -302,27 +273,21 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream) {
   p.num_kb = (a.K + kGemmBK - 1) / kGemmBK;
   p.gs_log2 = -1;
   for (int b = 5; b < 31; ++b) if (a.group_size == (1 << b)) p.gs_log2 = b;
+  if (a.split_k & ~0x30ff)
+    return failf(AGB200_EINVAL, "gemm: tune1 holds split-K in bits 0-7 and the debug bits 12-13 (got 0x%x)", a.split_k);
   p.debug = (a.split_k >> 12) & 3;
   int split = a.split_k & 0xff;
-  const int mcast_req = (a.split_k >> 8) & 3;          // tests: 1 = force off, 2 = force on
   if (split == 0) split = gemm_auto_split(mt, n_tiles * m_tiles, p.num_kb, a.sms);
   if (split != 1 && split != 2 && split != 4 && split != 8) return failf(AGB200_EINVAL, "gemm: split-K must be 1/2/4/8 (got %d)", split);
   while (split > 1 && split > p.num_kb) split /= 2;
   p.split = split;
   p.kb_per_split = (p.num_kb + split - 1) / split;
-  bool mcast = false;   // pair-multicast of x: only on request
-  if (mcast_req == 1) mcast = false;
-  if (mcast_req == 2) {
-    if (split != 1 || n_tiles % 2 != 0 || mt < 128)
-      return failf(AGB200_EINVAL, "gemm: multicast needs split=1, an even number of N tiles and MT>=128");
-    mcast = true;
-  }
 
   const CUtensorMapDataType t16 = a.bf16 ? CU_TENSOR_MAP_DATA_TYPE_BFLOAT16 : CU_TENSOR_MAP_DATA_TYPE_FLOAT16;
   const int G = (a.K + a.group_size - 1) / a.group_size;
   const uint32_t ngr = a.group_size == 32 ? 2 : 1;
   CUtensorMap tmap, tmap_w, tmap_s, tmap_z;
-  if (int rc = encode_2d(&tmap, t16, x, a.K, a.M, size_t(a.K) * 2, kGemmBK, mcast ? mt / 2 : mt, CU_TENSOR_MAP_SWIZZLE_128B,
+  if (int rc = encode_2d(&tmap, t16, x, a.K, a.M, size_t(a.K) * 2, kGemmBK, mt, CU_TENSOR_MAP_SWIZZLE_128B,
                          CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "gemm x")) return rc;
   if (int rc = encode_2d(&tmap_w, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qweight, a.N, a.K / 8, size_t(a.N) * 4, kGemmBN, kGemmBK / 8,
                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, "gemm qweight")) return rc;
@@ -331,18 +296,14 @@ inline int launch_w4a16_gemm(const GemmArgs& a, cudaStream_t stream) {
   if (int rc = encode_2d(&tmap_z, CU_TENSOR_MAP_DATA_TYPE_INT32, a.qzeros, a.N / 8, G, size_t(a.N / 8) * 4, kGemmBN / 8, ngr,
                          CU_TENSOR_MAP_SWIZZLE_NONE, CU_TENSOR_MAP_L2_PROMOTION_L2_128B, "gemm qzeros")) return rc;
 
-#define AGB_GEMM_CASE(MT)                                                                                       \
-  case MT:                                                                                                      \
-    if (MT >= 128 && mcast)                                                                                     \
-      return a.bf16 ? launch_gemm_inst<(MT >= 128 ? MT : 128), true, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream)  \
-                    : launch_gemm_inst<(MT >= 128 ? MT : 128), false, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream); \
-    return a.bf16 ? launch_gemm_inst<MT, true, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream)                     \
-                  : launch_gemm_inst<MT, false, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream);
+#define AGB_GEMM_CASE(MT)                                                                              \
+  case MT:                                                                                             \
+    return a.bf16 ? launch_gemm_inst<MT, true>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream)      \
+                  : launch_gemm_inst<MT, false>(p, tmap, tmap_w, tmap_s, tmap_z, m_tiles, stream);
   switch (mt) {
     AGB_GEMM_CASE(32)
     AGB_GEMM_CASE(64)
     AGB_GEMM_CASE(128)
-    AGB_GEMM_CASE(256)
   }
 #undef AGB_GEMM_CASE
   return AGB200_EINVAL;

@@ -26,7 +26,7 @@ namespace cg = cooperative_groups;
 
 constexpr int kGemvThreads = 256;
 constexpr int kGemvWarps = kGemvThreads / 32;
-constexpr int kGemvDepth = 8;  // 16-byte loads in flight per thread (kOcc <= 3); kOcc == 4 uses 4 (same bytes in flight per SM)
+constexpr int kGemvDepth = 8;  // 16-byte loads in flight per thread
 
 // One member of a grouped launch: sibling layers that read the same x (q|k|v, gate|up) share ONE kernel launch;
 // the CTAs of the grid are partitioned between them (tile_begin = first blockIdx.x of the layer).
@@ -56,11 +56,11 @@ struct GemvParams {
 };
 
 // shared memory carve-up (dynamic): xs | xsum | red | part
-template <int kM, int kLN, bool kBiased>
+template <int kM, int kLN>
 struct GemvSmem {
   static constexpr int kTN = kLN * 4;
   static __host__ __device__ size_t xs_bytes(int chunk_rows) { return size_t(chunk_rows) * kM * 16; }
-  static __host__ __device__ size_t xsum_bytes(int chunk_rows) { return size_t(chunk_rows) * kM * (kBiased ? 8 : 4); }
+  static __host__ __device__ size_t xsum_bytes(int chunk_rows) { return size_t(chunk_rows) * kM * 4; }
   static __host__ __device__ size_t red_bytes() { return size_t(kGemvWarps) * kM * kTN * 4; }
   static __host__ __device__ size_t part_bytes() { return size_t(kM) * kTN * 4; }
   static __host__ __device__ size_t total(int chunk_rows) {
@@ -68,19 +68,17 @@ struct GemvSmem {
   }
 };
 
-// kBiased selects the fp16 biased-exponent unpack (1024+q) instead of the subnormal unpack; bf16
-// (7 mantissa bits) always uses the biased form 128+q and ignores the flag (instantiate with false).
+// fp16 reads each nibble as a subnormal; bf16 (7 mantissa bits) reads it as 128 + q.
 // kOcc = CTAs per SM the register allocation is tuned for: 3 lets the 344-CTA grids of the wide (N = 11008)
 // layers run as a single wave; 2 keeps the full register ring for the narrower ones (measured: tools/sweep_gemv.py)
-template <int kM, int kLN, bool kBf16, bool kBiased, int kOcc = 2>
+template <int kM, int kLN, bool kBf16, int kOcc = 2>
 __global__ void __launch_bounds__(kGemvThreads, kOcc)
 w4a16_gemv_kernel(const GemvParams p) {
-  static_assert(!(kBf16 && kBiased), "bf16 has a single unpack mode");
   constexpr int kRS = 32 / kLN;              // row slots per warp
   constexpr int kRL = kGemvWarps * kRS;      // row lanes per CTA
   constexpr int kTN = kLN * 4;               // columns per CTA
-  constexpr int D = kOcc >= 4 ? 4 : kGemvDepth;
-  using Smem = GemvSmem<kM, kLN, kBiased>;
+  constexpr int D = kGemvDepth;
+  using Smem = GemvSmem<kM, kLN>;
 
   extern __shared__ __align__(16) unsigned char smem_raw[];
 
@@ -181,11 +179,7 @@ w4a16_gemv_kernel(const GemvParams p) {
       auto f = [](uint32_t w, int hi) { return elt_to_float<kBf16>(static_cast<uint16_t>(hi ? (w >> 16) : (w & 0xffff))); };
       const float even = (f(o.x, 0) + f(o.x, 1)) + (f(o.z, 0) + f(o.z, 1));   // k0,k4,k2,k6
       const float odd = (f(o.y, 0) + f(o.y, 1)) + (f(o.w, 0) + f(o.w, 1));    // k1,k5,k3,k7
-      if constexpr (kBiased) {
-        reinterpret_cast<float2*>(xsum)[m * p.rows_per_split + rc] = make_float2(even, odd);
-      } else {
-        xsum[m * p.rows_per_split + rc] = even + odd;
-      }
+      xsum[m * p.rows_per_split + rc] = even + odd;
     }
   }
   __syncthreads();
@@ -193,10 +187,10 @@ w4a16_gemv_kernel(const GemvParams p) {
   // ---- 4. main loop
   float yacc[kM][4];
   float a_lo[kM][4], a_hi[kM][4];
-  float sx_lo[kM], sx_hi[kM];
+  float sx[kM];
 #pragma unroll
   for (int m = 0; m < kM; ++m) {
-    sx_lo[m] = 0.f; sx_hi[m] = 0.f;
+    sx[m] = 0.f;
 #pragma unroll
     for (int c = 0; c < 4; ++c) { yacc[m][c] = 0.f; a_lo[m][c] = 0.f; a_hi[m][c] = 0.f; }
   }
@@ -212,24 +206,21 @@ w4a16_gemv_kernel(const GemvParams p) {
         float v;
         if constexpr (kBf16) {
           // every nibble was read as (128 + q): sum q x = a - 128 * sum x
-          v = (a_lo[m][c] + a_hi[m][c]) - (128.f + z) * sx_lo[m];
-        } else if constexpr (!kBiased) {
-          // a_lo holds sum q*x*2^-24, a_hi holds sum q*x*2^-20
-          v = fmaf(a_lo[m][c], 16.f, a_hi[m][c]) * 1048576.f - z * sx_lo[m];
+          v = (a_lo[m][c] + a_hi[m][c]) - (128.f + z) * sx[m];
         } else {
-          // a_lo = sum (1024+q) x over even nibbles, a_hi = sum (1024+16q) x over odd nibbles
-          v = (a_lo[m][c] - 1024.f * sx_lo[m]) + (a_hi[m][c] - 1024.f * sx_hi[m]) * 0.0625f - z * (sx_lo[m] + sx_hi[m]);
+          // a_lo holds sum q*x*2^-24, a_hi holds sum q*x*2^-20
+          v = fmaf(a_lo[m][c], 16.f, a_hi[m][c]) * 1048576.f - z * sx[m];
         }
         yacc[m][c] = fmaf(s, v, yacc[m][c]);
         a_lo[m][c] = 0.f; a_hi[m][c] = 0.f;
       }
     }
 #pragma unroll
-    for (int m = 0; m < kM; ++m) { sx_lo[m] = 0.f; sx_hi[m] = 0.f; }
+    for (int m = 0; m < kM; ++m) sx[m] = 0.f;
   };
 
   constexpr uint32_t kMaskLo = 0x000f000fu, kMaskHi = 0x00f000f0u;
-  constexpr uint32_t kMagic = kBf16 ? 0x43004300u : 0x64006400u;   // bf16: 128+q ; fp16: 1024+q
+  constexpr uint32_t kMagic = 0x43004300u;   // bf16: 128 + q
 
   auto process_row = [&](const uint4& w, int row) {
     if (row == next_boundary) {
@@ -244,18 +235,12 @@ w4a16_gemv_kernel(const GemvParams p) {
     uint32_t q0[4], q1[4], q2[4], q3[4];
 #pragma unroll
     for (int c = 0; c < 4; ++c) {
-      if constexpr (!kBf16 && !kBiased) {
+      if constexpr (!kBf16) {
         const uint32_t t = wq[c] >> 8;
         q0[c] = wq[c] & kMaskLo;   // (k0,k4) * 2^-24
         q1[c] = wq[c] & kMaskHi;   // (k1,k5) * 2^-20
         q2[c] = t & kMaskLo;       // (k2,k6) * 2^-24
         q3[c] = t & kMaskHi;       // (k3,k7) * 2^-20
-      } else if constexpr (!kBf16) {
-        const uint32_t t = wq[c] >> 8;
-        q0[c] = lop3_and_or(wq[c], kMaskLo, kMagic);   // 1024 + q
-        q1[c] = lop3_and_or(wq[c], kMaskHi, kMagic);   // 1024 + 16 q
-        q2[c] = lop3_and_or(t, kMaskLo, kMagic);
-        q3[c] = lop3_and_or(t, kMaskHi, kMagic);
       } else {
         // bf16 has 7 mantissa bits: every nibble is moved to bits 0..3 (128 + q)
         q0[c] = lop3_and_or(wq[c], kMaskLo, kMagic);
@@ -267,12 +252,7 @@ w4a16_gemv_kernel(const GemvParams p) {
 #pragma unroll
     for (int m = 0; m < kM; ++m) {
       const uint4 X = xs[m * p.rows_per_split + rc];
-      if constexpr (kBiased) {
-        const float2 sxy = reinterpret_cast<const float2*>(xsum)[m * p.rows_per_split + rc];
-        sx_lo[m] += sxy.x; sx_hi[m] += sxy.y;
-      } else {
-        sx_lo[m] += xsum[m * p.rows_per_split + rc];
-      }
+      sx[m] += xsum[m * p.rows_per_split + rc];
 #pragma unroll
       for (int c = 0; c < 4; ++c) {
         a_lo[m][c] = fma_mixed<kBf16, false>(q0[c], X.x, a_lo[m][c]);

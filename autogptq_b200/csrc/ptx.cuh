@@ -67,23 +67,12 @@ __device__ __forceinline__ uint64_t l2_policy_evict_first() {
   asm volatile("createpolicy.fractional.L2::evict_first.b64 %0, 1.0;" : "=l"(p));
   return p;
 }
-__device__ __forceinline__ void tma_load_2d_mcast(uint32_t smem_dst, const CUtensorMap* tmap, int c0, int c1, uint32_t bar, uint16_t mask) {
-  asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes.multicast::cluster [%0], [%1, {%4, %5}], [%2], %3;"
-               ::"r"(smem_dst), "l"(tmap), "r"(bar), "h"(mask), "r"(c0), "r"(c1) : "memory");
-}
 // Same box, fetched into L2 only: no shared memory, no barrier; a later load of the box hits L2
 __device__ __forceinline__ void tma_prefetch_l2_2d(const CUtensorMap* tmap, int c0, int c1) {
   asm volatile("cp.async.bulk.prefetch.tensor.2d.L2.global.tile [%0, {%1, %2}];" ::"l"(tmap), "r"(c0), "r"(c1) : "memory");
 }
 __device__ __forceinline__ void prefetch_tmap(const CUtensorMap* tmap) {
   asm volatile("prefetch.tensormap [%0];" ::"l"(tmap) : "memory");
-}
-
-// Arrive on the mbarrier at the same shared-memory offset in CTA `cta` of the cluster (release at cluster scope).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t bar, uint32_t cta) {
-  uint32_t remote;
-  asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(remote) : "r"(bar), "r"(cta));
-  asm volatile("mbarrier.arrive.release.cluster.shared::cluster.b64 _, [%0];" ::"r"(remote) : "memory");
 }
 
 // Register budget hand-over between warpgroups (all warps of a warpgroup execute it).
@@ -116,9 +105,6 @@ AGB_WGMMA_RS(64, bf16, AGB_R64, "{%32,%33,%34,%35}, %36", AGB_D8(0), AGB_D8(8), 
 #define AGB_R128 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63"
 AGB_WGMMA_RS(128, f16, AGB_R128, "{%64,%65,%66,%67}, %68", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56))
 AGB_WGMMA_RS(128, bf16, AGB_R128, "{%64,%65,%66,%67}, %68", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56))
-#define AGB_R256 "%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31,%32,%33,%34,%35,%36,%37,%38,%39,%40,%41,%42,%43,%44,%45,%46,%47,%48,%49,%50,%51,%52,%53,%54,%55,%56,%57,%58,%59,%60,%61,%62,%63,%64,%65,%66,%67,%68,%69,%70,%71,%72,%73,%74,%75,%76,%77,%78,%79,%80,%81,%82,%83,%84,%85,%86,%87,%88,%89,%90,%91,%92,%93,%94,%95,%96,%97,%98,%99,%100,%101,%102,%103,%104,%105,%106,%107,%108,%109,%110,%111,%112,%113,%114,%115,%116,%117,%118,%119,%120,%121,%122,%123,%124,%125,%126,%127"
-AGB_WGMMA_RS(256, f16, AGB_R256, "{%128,%129,%130,%131}, %132", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56), AGB_D8(64), AGB_D8(72), AGB_D8(80), AGB_D8(88), AGB_D8(96), AGB_D8(104), AGB_D8(112), AGB_D8(120))
-AGB_WGMMA_RS(256, bf16, AGB_R256, "{%128,%129,%130,%131}, %132", AGB_D8(0), AGB_D8(8), AGB_D8(16), AGB_D8(24), AGB_D8(32), AGB_D8(40), AGB_D8(48), AGB_D8(56), AGB_D8(64), AGB_D8(72), AGB_D8(80), AGB_D8(88), AGB_D8(96), AGB_D8(104), AGB_D8(112), AGB_D8(120))
 #undef AGB_WGMMA_RS
 #undef AGB_D8
 

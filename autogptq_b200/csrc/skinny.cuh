@@ -60,11 +60,9 @@ __device__ __forceinline__ void mma_16816(float (&d)[4], uint32_t a0, uint32_t a
                  : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]) : "r"(a0), "r"(a1), "r"(a2), "r"(a3), "r"(b0), "r"(b1));
 }
 
-// kBiased (fp16 only): operands are (1024 + q) / (1024 + 16 q) instead of subnormals.
-template <bool kBf16, bool kBiased>
+template <bool kBf16>
 __global__ void __launch_bounds__(kSkThreads)
 w4a16_skinny_kernel(const SkinnyParams p) {
-  static_assert(!(kBf16 && kBiased), "bf16 has a single unpack mode");
   constexpr int D = kSkDepth;
   extern __shared__ __align__(16) unsigned char smem_raw[];
   uint4* xs = reinterpret_cast<uint4*>(smem_raw);
@@ -163,7 +161,7 @@ w4a16_skinny_kernel(const SkinnyParams p) {
 
   constexpr uint32_t kOnes = kBf16 ? 0x3F803F80u : 0x3C003C00u;
   constexpr uint32_t kMaskLo = 0x000f000fu, kMaskHi = 0x00f000f0u;
-  constexpr uint32_t kMagic = kBf16 ? 0x43004300u : 0x64006400u;
+  constexpr uint32_t kMagic = 0x43004300u;   // bf16: 128 + q
 
   auto flush = [&]() {
     const uint16_t sh[4] = {uint16_t(s_cur.x & 0xffff), uint16_t(s_cur.x >> 16), uint16_t(s_cur.y & 0xffff), uint16_t(s_cur.y >> 16)};
@@ -178,8 +176,7 @@ w4a16_skinny_kernel(const SkinnyParams p) {
         const float s0 = sx[0][mm], s1 = sx[1][mm];
         float v;
         if constexpr (kBf16) v = (a0 + a1) - (128.f + z) * (s0 + s1);
-        else if constexpr (!kBiased) v = fmaf(a0, 16.f, a1) * 1048576.f - z * (s0 + s1);
-        else v = (a0 - 1024.f * s0) + (a1 - 1024.f * s1) * 0.0625f - z * (s0 + s1);
+        else v = fmaf(a0, 16.f, a1) * 1048576.f - z * (s0 + s1);
         yacc[j][mm] = fmaf(s, v, yacc[j][mm]);
       }
     }
@@ -211,13 +208,9 @@ w4a16_skinny_kernel(const SkinnyParams p) {
     uint32_t q0[4], q1[4], q2[4], q3[4];
 #pragma unroll
     for (int j = 0; j < 4; ++j) {
-      if constexpr (!kBf16 && !kBiased) {
+      if constexpr (!kBf16) {
         const uint32_t t8 = wq[j] >> 8;
         q0[j] = wq[j] & kMaskLo; q1[j] = wq[j] & kMaskHi; q2[j] = t8 & kMaskLo; q3[j] = t8 & kMaskHi;
-      } else if constexpr (!kBf16) {
-        const uint32_t t8 = wq[j] >> 8;
-        q0[j] = lop3_and_or(wq[j], kMaskLo, kMagic); q1[j] = lop3_and_or(wq[j], kMaskHi, kMagic);
-        q2[j] = lop3_and_or(t8, kMaskLo, kMagic);    q3[j] = lop3_and_or(t8, kMaskHi, kMagic);
       } else {
         q0[j] = lop3_and_or(wq[j], kMaskLo, kMagic);       q1[j] = lop3_and_or(wq[j] >> 4, kMaskLo, kMagic);
         q2[j] = lop3_and_or(wq[j] >> 8, kMaskLo, kMagic);  q3[j] = lop3_and_or(wq[j] >> 12, kMaskLo, kMagic);

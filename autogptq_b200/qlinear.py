@@ -104,7 +104,7 @@ class QuantLinear(nn.Module):
         self._run = {}             # per compute dtype: (scales, bias) tensors in that dtype
         self._plans = {}           # per compute dtype: constant part of the C-ABI call
         self.kernel = _lib.KERNEL_AUTO   # tests may force GEMV / GEMM
-        self.tune = (0, 0, 0)
+        self.tune = (0, 0)
 
     # ------------------------------------------------------------------ load-time preparation
     def post_init(self, temp_dq=None):
@@ -251,7 +251,7 @@ class QuantLinear(nn.Module):
             torch.cuda.set_device(dev_index)
         try:
             rc = fn(x2.data_ptr(), p_qw, p_tc, p_qz, p_sc, p_perm, p_bias, y.data_ptr(), M, K, N, self.group_size, code,
-                    ws_ptr, ws_bytes, _raw_stream(dev_index), self.kernel, self.tune[0], self.tune[1], self.tune[2])
+                    ws_ptr, ws_bytes, _raw_stream(dev_index), self.kernel, self.tune[0], self.tune[1])
         finally:
             if cur != dev_index:
                 torch.cuda.set_device(cur)

@@ -36,7 +36,7 @@
 extern "C" {
 #endif
 
-#define AGB200_ABI_VERSION 10
+#define AGB200_ABI_VERSION 11
 
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
@@ -101,18 +101,19 @@ int agb200_w4a16_forward(const void* x, const int32_t* qweight, const int32_t* q
 
 /* Same, with an explicit kernel choice and tuning knobs (tests / benchmarks).
  *   kernel   AGB200_KERNEL_*
- *   tune0/1  GEMV: tune0 = lanes along N per warp (8|16|32, 0=auto), tune1 = split-K (1|2|4|8, 0=auto),
- *            flags bit0 = biased-exponent unpack instead of the subnormal unpack.
- *            SKINNY: tune1 = split-K (1|2|4|8, 0=auto), flags bit0 as for GEMV.
+ *   tune0/1  GEMV: tune0 = lanes along N per warp (8|16|32, 0=auto), tune1 = split-K (1|2|4|8, 0=auto).
+ *            SKINNY: tune1 = split-K (1|2|4|8, 0=auto).
  *            IMMA: tune0 = 0 auto | 2 register-ring persistent form | 1, 4 tile-per-CTA form
  *                  with that many warps along N;
  *                  tune1 = split-K of the tile-per-CTA form (1|2|4|8, 0=auto).
- *            GEMM: tune0 = x-row tile (16..256, 0=auto), tune1 = split-K (0=auto). */
+ *            GEMM: tune0 = x-row tile (32|64|128, 0=auto), tune1 bits 0-7 = split-K (1|2|4|8, 0=auto),
+ *                  bits 12-13 = measurement aid (1 = skip the weight loads, 2 = skip the x loads; the result is
+ *                  garbage); any other tune1 bit is AGB200_EINVAL. */
 int agb200_w4a16_forward_ex(const void* x, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros,
                             const void* scales, const int32_t* perm, const void* bias, void* y,
                             int M, int K, int N, int group_size, int dtype,
                             void* workspace, size_t workspace_bytes, void* stream,
-                            int kernel, int tune0, int tune1, int flags);
+                            int kernel, int tune0, int tune1);
 
 size_t agb200_w4a16_workspace_bytes(int M, int K, int N);
 
@@ -532,18 +533,6 @@ size_t agb200_gptq_workspace_bytes(int N, int K, int act_order);
  * The reference has no counterpart (its kernels are launched one at a time on the legacy stream, q_gemm.cu:47,85).
  */
 int agb200_w4_prefetch_hint(int n, const void* const* ptrs, const size_t* bytes);
-
-/*
- * End-to-end variant with HOST activations: copies x_host -> device staging, runs the forward
- * and copies y back to y_host, all on `stream` (asynchronous when the host buffers are pinned).
- * `staging` is device scratch of agb200_w4a16_host_staging_bytes(M,K,N) bytes.
- * This is the call `bench.py` times for the "e2e" number.
- */
-int agb200_w4a16_forward_host(const void* x_host, const int32_t* qweight, const int32_t* qweight_tc, const int32_t* qzeros,
-                              const void* scales, const int32_t* perm, const void* bias, void* y_host,
-                              int M, int K, int N, int group_size, int dtype,
-                              void* staging, size_t staging_bytes, void* stream);
-size_t agb200_w4a16_host_staging_bytes(int M, int K, int N);
 
 /*
  * Load-time act-order transform (desc_act): gather packed rows so that groups become contiguous.

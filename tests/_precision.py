@@ -14,8 +14,8 @@ Per-element bound
       the other way (the other half).
     * A = Σ_k |x_k|·s·(q_k + z + o) + |b| is the uncancelled magnitude of what the kernel actually sums.  Every
       small-M kernel forms s·(Σ q·x − z·Σx) per group, so its partial sums are bounded by Σ|x|·s·(q + z); the bf16
-      unpack reads each nibble as 128 + q and the fp16 "biased" unpack as 1024 + q, which adds o = 128 / 1024 to the
-      summed terms (``gemv.cuh`` flush, ``skinny.cuh`` epilogue).  Near-zero outputs have a tiny ulp, so γ·A is what
+      unpack reads each nibble as 128 + q, which adds o = 128 to the summed terms (``gemv.cuh`` flush, ``skinny.cuh``
+      epilogue).  Near-zero outputs have a tiny ulp, so γ·A is what
       bounds them, and it is what a cancellation bug has to get past.
     * γ bounds the relative fp32 accumulation error.  Every product is exact in fp32 (two 16-bit significands, or an
       exact int32 dot product on the IMMA paths), so the error is that of an fp32 sum of n terms whose partial sums are
@@ -114,9 +114,7 @@ _BF = {"bfloat16": 128}
 _RATE = {"float16": 0.05, "bfloat16": 0.01}
 PATHS = {
     "gemv": Path("gemv", offset=_BF, rate=_RATE),
-    "gemv_biased": Path("gemv_biased", offset={"float16": 1024}, rate=_RATE),
     "skinny": Path("skinny", offset=_BF, tc=True, rate=_RATE),
-    "skinny_biased": Path("skinny_biased", offset={"float16": 1024}, tc=True, rate=_RATE),
     "imma": Path("imma", pe_max=126, rate=_RATE),
     "chain": Path("chain", pe_max=120, rate=_RATE),
     "gemm": Path("gemm", round_w=True, tc=True, rate=_RATE),

@@ -39,13 +39,13 @@ def fwd_args(x=A, qweight=A, qzeros=A, scales=A, y=A, M=1, K=128, N=128, group_s
 def test_w4a16_forward_errors(lib):
     assert call(lib, "agb200_w4a16_forward", *fwd_args(x=None, qweight=None, qzeros=None, scales=None, y=None)) == \
         (EINVAL, "null pointer argument")
-    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(dtype=7), 0, 0, 0, 0) == \
+    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(dtype=7), 0, 0, 0) == \
         (EINVAL, "dtype must be AGB200_F16 or AGB200_BF16")
-    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(x=MIS), 0, 0, 0, 0) == \
+    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(x=MIS), 0, 0, 0) == \
         (EINVAL, "x, qweight, scales and y must be 16-byte aligned")
-    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(K=12), 0, 0, 0, 0) == \
+    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(K=12), 0, 0, 0) == \
         (EINVAL, "infeatures K=12 must be a multiple of 8 (4-bit row packing)")
-    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(group_size=12), 0, 0, 0, 0) == \
+    assert call(lib, "agb200_w4a16_forward_ex", *fwd_args(group_size=12), 0, 0, 0) == \
         (ENOSUP, "group_size=12 is not a multiple of 8")
 
 

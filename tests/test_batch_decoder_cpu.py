@@ -21,7 +21,7 @@ def test_exports_declared_and_bound():
         assert name in _lib.declared_symbols(), f"{name} is not bound"
     m = re.search(r"#define AGB200_ATTN_ROWS_MAX_B (\d+)", hdr)
     assert m and int(m.group(1)) == _lib.ATTN_ROWS_MAX_B == 8
-    assert _lib.ABI_VERSION == 10
+    assert _lib.ABI_VERSION == 11
 
 
 def test_support_checks():

@@ -118,7 +118,7 @@ def test_exports_declared_and_bound():
     for name in ("agb200_decode_attention", "agb200_decode_attention_workspace_bytes"):
         assert re.search(rf"\b{name}\s*\(", hdr), f"{name} is not declared"
         assert name in _lib.declared_symbols(), f"{name} is not bound"
-    assert _lib.ABI_VERSION == 10
+    assert _lib.ABI_VERSION == 11
 
 
 def _cpu_llama(**kw):

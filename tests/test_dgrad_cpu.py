@@ -24,7 +24,7 @@ def test_library_exports_v10_dgrad():
     for name in ("agb200_w4a16_dgrad", "agb200_w4a16_dgrad_ex", "agb200_w4a16_dgrad_workspace_bytes"):
         assert hasattr(lib, name)
     L = _lib.load()
-    assert L.agb200_abi_version() == 10
+    assert L.agb200_abi_version() == 11
     assert L.agb200_w4a16_dgrad_workspace_bytes(3, 264, 64) == 1792       # 3 * 264 * 2 rounded up to 256 bytes
 
 

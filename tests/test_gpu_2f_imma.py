@@ -13,7 +13,7 @@ pytestmark = pytest.mark.gpu
 IMMA = 6
 
 
-def _run(d, x, tune=(0, 0, 0), dtype=torch.float16, kernel=IMMA):
+def _run(d, x, tune=(0, 0), dtype=torch.float16, kernel=IMMA):
     lin = make_layer(d, dtype=dtype)
     lin.kernel = kernel
     lin.tune = tune
@@ -38,7 +38,7 @@ def test_imma_shapes(M, K, N, g):
 def test_imma_variants(split, wn, M):
     K, N, g = 4096, 520, 128
     d = O.random_packed(K, N, g, seed=11, bias=True)
-    y, x = _run(d, rand_x(M, K, seed=2), tune=(wn, split, 0))
+    y, x = _run(d, rand_x(M, K, seed=2), tune=(wn, split))
     assert_parity(y, oracle_exact(d, x), atol_rms=6e-4, what=f"imma split={split} wn={wn} M={M}")
 
 
@@ -49,7 +49,7 @@ def test_imma_persistent_form(M, K, N, g):
     """tune0 = 2 forces the one-CTA-per-SM register-ring form (AUTO's choice for 2 <= M <= 4 and 128-k groups); large
     K x M convert x in several K chunks."""
     d = O.random_packed(K, N, g, seed=K + N + M, bias=(M % 2 == 1))
-    y, x = _run(d, rand_x(M, K, seed=M), tune=(2, 0, 0))
+    y, x = _run(d, rand_x(M, K, seed=M), tune=(2, 0))
     assert_parity(y, oracle_exact(d, x), atol_rms=6e-4, what=f"imma persistent M={M} K={K} N={N} g={g}")
 
 
@@ -57,7 +57,7 @@ def test_imma_persistent_is_deterministic_under_graph_replay():
     K, N, g, M = 4096, 5024, 128, 2
     d = O.random_packed(K, N, g, seed=5, bias=True)
     lin = make_layer(d)
-    lin.kernel, lin.tune = IMMA, (2, 0, 0)
+    lin.kernel, lin.tune = IMMA, (2, 0)
     x = torch.from_numpy(rand_x(M, K, seed=9)).cuda()
     y0 = lin(x).clone()
     for _ in range(5):
@@ -79,11 +79,11 @@ def test_imma_persistent_act_order_and_bf16():
     K, N, g = 2048, 392, 128
     d = O.random_packed(K, N, g, seed=77, desc_act=True, zero_max=15, bias=True)
     for M in (1, 7):
-        y, x = _run(d, rand_x(M, K, seed=5), tune=(2, 0, 0))
+        y, x = _run(d, rand_x(M, K, seed=5), tune=(2, 0))
         assert_parity(y, oracle_exact(d, x), atol_rms=6e-4, what="imma persistent act-order + wrap")
     d = O.random_packed(K, N, g, seed=78, scale_dtype=np.float32)
     d["scales"] = torch.from_numpy(d["scales"]).to(torch.bfloat16).float().numpy()
-    y, x = _run(d, rand_x(3, K, seed=3, dtype=np.float32), tune=(2, 0, 0), dtype=torch.bfloat16)
+    y, x = _run(d, rand_x(3, K, seed=3, dtype=np.float32), tune=(2, 0), dtype=torch.bfloat16)
     assert_parity(y, oracle_exact(d, x), rtol=8e-3, atol_rms=4e-3, what="imma persistent bf16")
 
 

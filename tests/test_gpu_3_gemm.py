@@ -9,7 +9,7 @@ from tests._util import assert_parity, make_layer, oracle_exact, oracle_fp16w, r
 pytestmark = pytest.mark.gpu
 
 
-def _run(d, x, tune=(0, 0, 0), dtype=torch.float16, kernel=2):
+def _run(d, x, tune=(0, 0), dtype=torch.float16, kernel=2):
     lin = make_layer(d, dtype=dtype)
     lin.kernel = kernel
     lin.tune = tune
@@ -42,12 +42,12 @@ def test_gemm_shapes(K, N, g):
     _check(d, y, x, f"gemm K={K} N={N} g={g}")
 
 
-@pytest.mark.parametrize("mt", [32, 64, 128, 256])
+@pytest.mark.parametrize("mt", [32, 64, 128])
 @pytest.mark.parametrize("split", [1, 2, 4, 8])
 def test_gemm_tiles_and_splitk(mt, split):
     K, N, g, M = 1024, 256, 128, 70
     d = O.random_packed(K, N, g, seed=7, bias=True)
-    y, x = _run(d, rand_x(M, K, seed=4), tune=(mt, split, 0))
+    y, x = _run(d, rand_x(M, K, seed=4), tune=(mt, split))
     _check(d, y, x, f"gemm mt={mt} split={split}")
 
 
@@ -76,14 +76,25 @@ def test_gemm_matches_gemv():
     assert_parity(y_gemm, y_gemv, rtol=1e-3, atol_rms=2e-3, what="gemm vs gemv")
 
 
-@pytest.mark.parametrize("mt", [128, 256])
-@pytest.mark.parametrize("mc", [1, 2], ids=["unicast", "multicast"])
-def test_gemm_tma_multicast_cluster(mt, mc):
-    """Clusters of two CTAs sharing the x tile through TMA multicast (tune1 bits 8-9: 1 = off, 2 = on)."""
+def test_gemm_tile128_ragged_m():
+    """AUTO's 128-row tile without split-K at an M that leaves the last tile partly filled."""
     K, N, g, M = 1024, 512, 128, 300
     d = O.random_packed(K, N, g, seed=17, bias=True)
-    y, x = _run(d, rand_x(M, K, seed=9), tune=(mt, 1 | (mc << 8), 0))
-    _check(d, y, x, f"gemm mt={mt} mcast={mc}")
+    y, x = _run(d, rand_x(M, K, seed=9), tune=(128, 1))
+    _check(d, y, x, "gemm mt=128 split=1")
+
+
+def test_gemm_rejects_unknown_tiles_and_tune1_bits():
+    """Only the 32/64/128-row tiles exist; tune1 carries split-K and the debug bits, nothing else."""
+    from autogptq_b200 import _lib
+
+    d = O.random_packed(1024, 512, 128, seed=17)
+    x = rand_x(300, 1024, seed=9)
+    with pytest.raises(_lib.B200KernelError, match=r"code -1\): gemm: x-row tile must be 32/64/128 \(got 256\)"):
+        _run(d, x, tune=(256, 1))
+    with pytest.raises(_lib.B200KernelError,
+                       match=r"code -1\): gemm: tune1 holds split-K in bits 0-7 and the debug bits 12-13 \(got 0x201\)"):
+        _run(d, x, tune=(128, 1 | (2 << 8)))
 
 
 def test_auto_handles_shapes_the_tensor_core_path_cannot():

@@ -140,8 +140,8 @@ def test_exports_declared_and_bound():
         assert re.search(rf"\b{name}\s*\(", hdr), f"{name} is not declared"
         assert name in _lib.declared_symbols(), f"{name} is not bound"
         assert hasattr(_lib.load(), name)
-    assert re.search(r"#define AGB200_ABI_VERSION 10\b", hdr)
-    assert _lib.ABI_VERSION == 10 == _lib.load().agb200_abi_version()
+    assert re.search(r"#define AGB200_ABI_VERSION 11\b", hdr)
+    assert _lib.ABI_VERSION == 11 == _lib.load().agb200_abi_version()
 
 
 @pytest.mark.parametrize("entry,max_b", [("decode_attention_fp8", 2), ("decode_attention_rows_fp8", 8)])

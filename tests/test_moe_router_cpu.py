@@ -210,7 +210,7 @@ def test_exports_declared_and_bound():
     assert "agb200_moe_router" in _lib.declared_symbols()
     m = re.search(r"#define AGB200_MOE_ROUTER_MAX_TOP_K (\d+)", hdr)
     assert m and int(m.group(1)) == _lib.MOE_ROUTER_MAX_TOP_K == 8
-    assert _lib.ABI_VERSION == 10
+    assert _lib.ABI_VERSION == 11
 
 
 def test_router_validates_arguments():

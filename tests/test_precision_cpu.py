@@ -59,8 +59,6 @@ def _rejected(y, d, x, path, dt, what):
 @pytest.mark.parametrize("path", sorted(P.PATHS))
 def test_correctly_rounded_result_is_accepted(dt, path):
     pth = P.PATHS[path]
-    if pth.o(dt) == 1024 and dt == "bfloat16":
-        pytest.skip("the biased unpack is fp16 only")
     d = _layer(dt, act_order=True)
     for kind in P.acts_for(dt):
         x = P.activations(kind, 4, K, dt, seed=1)

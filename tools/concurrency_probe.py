@@ -46,7 +46,7 @@ def run(K, N, nbr, groups, tune, parallel):
 
 for (K, N, nbr) in ((4096, 4096, 3), (4096, 11008, 2)):
     groups = 12 if N == 4096 else 8
-    for tune in ((0, 0, 0), (8, 1, 0), (8, 2, 0), (16, 1, 0), (16, 2, 0), (32, 1, 0), (32, 2, 0), (32, 4, 0)):
+    for tune in ((0, 0), (8, 1), (8, 2), (16, 1), (16, 2), (32, 1), (32, 2), (32, 4)):
         try:
             s = run(K, N, nbr, groups, tune, False); p = run(K, N, nbr, groups, tune, True)
             print(json.dumps({"K": K, "N": N, "siblings": nbr, "tune": tune, "serial_us_per_group": s, "parallel_us_per_group": p}), flush=True)

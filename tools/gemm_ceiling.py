@@ -11,6 +11,5 @@ for (K, N) in ((4096, 4096), (11008, 4096)):
     L = Layers(K, N, 128, 8, "cuda")
     for M in (4096, 16384):
         for dbg, name in ((0, "full"), (1, "no weight loads"), (2, "no x loads"), (3, "expansion + MMA + epilogue only")):
-            for mc in (1, 2):
-                med, _ = time_config(lib, L, M, 2, (256, 1 | (mc << 8) | (dbg << 12), 0))
-                print(json.dumps({"K": K, "N": N, "M": M, "mode": name, "mcast": mc == 2, "us": round(med, 1), "TFLOPs": round(2.0 * M * K * N / med / 1e6, 1)}), flush=True)
+            med, _ = time_config(lib, L, M, 2, (128, 1 | (dbg << 12)))
+            print(json.dumps({"K": K, "N": N, "M": M, "mode": name, "us": round(med, 1), "TFLOPs": round(2.0 * M * K * N / med / 1e6, 1)}), flush=True)

@@ -21,7 +21,7 @@ def main():
             for mt in ((32, 64) if M <= 32 else (64, 128) if M <= 64 else (128,)):
                 for split in (0, 1, 2, 4, 8):
                     try:
-                        med, mn = time_config(lib, L, M, 2, (mt, split, 0))
+                        med, mn = time_config(lib, L, M, 2, (mt, split))
                         rec = {"K": K, "N": N, "M": M, "mt": mt, "split": split, "us": round(med, 2)}
                     except Exception as e:
                         rec = {"K": K, "N": N, "M": M, "mt": mt, "split": split, "error": str(e)[:80]}

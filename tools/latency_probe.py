@@ -45,7 +45,7 @@ def chain(K, N, M, kernel, tune, copies, dependent, iters=5):
 
 pdl = "off" if os.environ.get("AGB200_NO_PDL") == "1" else "on"
 for (K, N, copies) in ((512, 512, 64), (4096, 4096, 48), (4096, 11008, 18)):
-    for name, kernel, tune in (("gemv", 1, (8, 1, 0)), ("skinny", 3, (0, 1, 0))):
+    for name, kernel, tune in (("gemv", 1, (8, 1)), ("skinny", 3, (0, 1))):
         for dep in (False, True):
             try:
                 g, e = chain(K, N, 1, kernel, tune, copies, dep)

@@ -14,8 +14,17 @@ import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 from autogptq_b200 import _lib  # noqa: E402
 
-HBM_PEAK = 6573.2   # GB/s, MEASURED_PEAKS.json (read below if present)
-TF_PEAK = 1722.5
+# NVIDIA's data-sheet figures for the H100 SXM at 700 W: HBM3 GB/s and dense fp16 / bf16 TFLOP/s
+H100_SXM_PEAKS = {"hbm_gbs": 3350.0, "bf16_tflops": 989.0}
+
+
+def peaks():
+    """(GB/s, TFLOP/s) that the fractions of peak divide by: MEASURED_PEAKS.json when present, else the data sheet."""
+    try:
+        pk = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))
+    except (OSError, ValueError):
+        pk = H100_SXM_PEAKS
+    return pk["hbm_gbs"], pk["bf16_tflops"]
 
 
 def alg_bytes(M, K, N, g):
@@ -55,7 +64,7 @@ def time_config(lib, L, M, kernel, tune, iters=5, dev="cuda"):
         for c in range(L.copies):
             rc = lib.agb200_w4a16_forward_ex(x.data_ptr(), L.qw[c].data_ptr(), L.qw_tc[c].data_ptr(), L.qz[c].data_ptr(), L.sc[c].data_ptr(),
                                              None, None, y.data_ptr(), M, L.K, L.N, L.g, 0, None, 0, s,
-                                             kernel, tune[0], tune[1], tune[2])
+                                             kernel, tune[0], tune[1])
             if rc != 0:
                 raise RuntimeError(lib.agb200_last_error().decode())
 
@@ -97,12 +106,7 @@ def main():
     ap.add_argument("--out", default="gpurun_out/micro.jsonl")
     ap.add_argument("--what", default="auto,imma,gemv,skinny,gemm,ref")
     args = ap.parse_args()
-    global HBM_PEAK, TF_PEAK
-    try:
-        pk = json.load(open(os.path.join(os.path.dirname(__file__), "..", "MEASURED_PEAKS.json")))
-        HBM_PEAK, TF_PEAK = pk["hbm_gbs"], pk["bf16_tflops"]
-    except Exception:
-        pass
+    hbm_peak, tf_peak = peaks()
     lib = _lib.load()
     os.makedirs(os.path.dirname(args.out) or ".", exist_ok=True)
     out = open(args.out, "a")
@@ -133,19 +137,19 @@ def main():
         if "auto" in args.what:
             for M in (sweep_ms or (1, 2, 3, 4, 5, 8, 16)):
                 try:
-                    med, mn = time_config(lib, L, M, 0, (0, 0, 0))
+                    med, mn = time_config(lib, L, M, 0, (0, 0))
                 except Exception as e:
                     emit({"kernel": "auto", "K": K, "N": N, "g": g, "M": M, "error": str(e)[:200]})
                     continue
                 ab = alg_bytes(M, K, N, g)
                 emit({"kernel": "auto", "K": K, "N": N, "g": g, "M": M, "us": round(med, 3), "us_min": round(mn, 3),
-                      "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / HBM_PEAK, 3),
+                      "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / hbm_peak, 3),
                       "TFLOPs": round(2.0 * M * K * N / med / 1e6, 1)})
         if "imma" in args.what:
             for M in (1, 2, 3, 4, 5, 8):
-                variants = [(0, 0, 0)]
+                variants = [(0, 0)]
                 if M in (1, 2, 4):
-                    variants += [(2, 0, 0)]
+                    variants += [(2, 0)]
                 for tune in variants:
                     try:
                         med, mn = time_config(lib, L, M, 6, tune)
@@ -154,12 +158,12 @@ def main():
                         continue
                     ab = alg_bytes(M, K, N, g)
                     emit({"kernel": "imma", "K": K, "N": N, "g": g, "M": M, "tune": tune, "us": round(med, 3), "us_min": round(mn, 3),
-                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / HBM_PEAK, 3)})
+                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / hbm_peak, 3)})
         if "gemv" in args.what:
             for M in (1, 2, 4):
-                variants = [(0, 0, 0)]
+                variants = [(0, 0)]
                 if M == 1 and not args.quick or (K, N, g) == (4096, 4096, 128):
-                    variants += [(ln, sp, b) for ln in (8, 16, 32) for sp in (1, 2, 4, 8) for b in (0, 1)]
+                    variants += [(ln, sp) for ln in (8, 16, 32) for sp in (1, 2, 4, 8)]
                 for tune in variants:
                     try:
                         med, mn = time_config(lib, L, M, 1, tune)
@@ -168,12 +172,12 @@ def main():
                         continue
                     ab = alg_bytes(M, K, N, g)
                     emit({"kernel": "gemv", "K": K, "N": N, "g": g, "M": M, "tune": tune, "us": round(med, 3), "us_min": round(mn, 3),
-                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / HBM_PEAK, 3)})
+                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / hbm_peak, 3)})
         if "skinny" in args.what:
             for M in (1, 2, 4, 8):
-                variants = [(0, 0, 0)]
+                variants = [(0, 0)]
                 if (K, N, g) == (4096, 4096, 128) and M in (1, 8):
-                    variants += [(0, sp, b) for sp in (1, 2, 4, 8) for b in (0, 1)]
+                    variants += [(0, sp) for sp in (1, 2, 4, 8)]
                 for tune in variants:
                     try:
                         med, mn = time_config(lib, L, M, 3, tune)
@@ -182,12 +186,12 @@ def main():
                         continue
                     ab = alg_bytes(M, K, N, g)
                     emit({"kernel": "skinny", "K": K, "N": N, "g": g, "M": M, "tune": tune, "us": round(med, 3), "us_min": round(mn, 3),
-                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / HBM_PEAK, 3)})
+                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / hbm_peak, 3)})
         if "gemm" in args.what:
             for M in ((16, 64, 128, 512, 2048, 16384) if not args.quick else (16, 64, 512, 4096)):
-                variants = [(0, 0, 0)]
+                variants = [(0, 0)]
                 if (K, N, g) == (4096, 4096, 128) and M >= 512:
-                    variants += [(256, 1 | (1 << 8), 0), (256, 1 | (2 << 8), 0), (128, 1 | (1 << 8), 0), (128, 1 | (2 << 8), 0)]
+                    variants += [(128, 1)]
                 for tune in variants:
                     try:
                         med, mn = time_config(lib, L, M, 2, tune)
@@ -197,8 +201,8 @@ def main():
                     ab = alg_bytes(M, K, N, g)
                     fl = 2.0 * M * K * N
                     emit({"kernel": "gemm", "K": K, "N": N, "g": g, "M": M, "tune": tune, "us": round(med, 3), "us_min": round(mn, 3),
-                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / HBM_PEAK, 3),
-                          "TFLOPs": round(fl / med / 1e6, 1), "tensor_frac": round(fl / med / 1e6 / TF_PEAK, 3)})
+                          "GBps": round(ab / med / 1e3, 1), "hbm_frac": round(ab / med / 1e3 / hbm_peak, 3),
+                          "TFLOPs": round(fl / med / 1e6, 1), "tensor_frac": round(fl / med / 1e6 / tf_peak, 3)})
         if "ref" in args.what:
             time_reference(emit, K, N, g, L, args.quick)
         del L

@@ -1,4 +1,4 @@
-"""Launch one configuration a few times (for ncu).  usage: profile_one.py {gemv|gemm|skinny|imma} K N M [tune0 tune1 tune2]"""
+"""Launch one configuration a few times (for ncu).  usage: profile_one.py {gemv|gemm|skinny|imma} K N M [tune0 tune1]"""
 import sys, os
 import torch
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -6,7 +6,7 @@ from autogptq_b200 import _lib
 from tools.microbench import Layers
 
 kind, K, N, M = sys.argv[1], int(sys.argv[2]), int(sys.argv[3]), int(sys.argv[4])
-tune = [int(v) for v in sys.argv[5:8]] + [0] * (3 - len(sys.argv[5:8]))
+tune = [int(v) for v in sys.argv[5:7]] + [0] * (2 - len(sys.argv[5:7]))
 lib = _lib.load()
 L = Layers(K, N, 128, 6, "cuda")
 x = torch.randn(M, K, dtype=torch.float16, device="cuda")
