@@ -1,6 +1,6 @@
 """The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules,
-the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, and the warm-up,
-capture and replay of a step's CUDA graph."""
+the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, the extend of
+cache rows on the project's kernels (DESIGN §3.20), and the warm-up, capture and replay of a step's CUDA graph."""
 from __future__ import annotations
 
 import torch
@@ -189,6 +189,31 @@ class StaticCacheDecoder:
         for i, lay in enumerate(cache.layers):
             self._store_kv(i, (rows, slice(None), slice(0, ids.shape[1])), lay.keys, lay.values)
         return out.logits
+
+    def _extend(self, ids: torch.Tensor, rows: slice, starts) -> torch.Tensor:
+        """Append ``ids`` [n, T] to cache rows ``rows`` (n of them) at positions ``starts`` (n host ints) .. + T - 1
+        on the project's kernels, and return the logits of the last new position [n, vocab].  The model's own modules
+        run every layer (its QuantLinear projections at M = n·T, its norms and MLP), so every rounding outside the
+        attention is HF's; ``prefill_attention`` writes k̂ and v into the static caches and attends causally over them.
+        No DynamicCache is built and only the last position reaches model.norm and lm_head."""
+        from .attention import prefill_attention
+
+        inner = self.model.model
+        if not hasattr(self, "_inv_freq"):
+            self._inv_freq, self._attn_scaling = _rotary_params(inner.rotary_emb, self.head_dim, self._who)
+        n, T = ids.shape
+        start = torch.tensor(list(starts), dtype=torch.int64, device=self.device)
+        h = inner.embed_tokens(ids)
+        out = torch.empty((n, T, self.n_heads * self.head_dim), dtype=self.dtype, device=self.device)
+        for i, layer in enumerate(inner.layers):
+            attn = self._plans[i][0]
+            x = layer.input_layernorm(h)
+            kw = {} if self.k_scale is None else dict(k_scale=self.k_scale[i][rows], v_scale=self.v_scale[i][rows])
+            prefill_attention(attn.q_proj(x), attn.k_proj(x), attn.v_proj(x), self.k_cache[i][rows],
+                              self.v_cache[i][rows], start, self._inv_freq, self._attn_scaling, self.scaling, out, **kw)
+            h = h + attn.o_proj(out)
+            h = h + layer.mlp(layer.post_attention_layernorm(h))
+        return self.model.lm_head(inner.norm(h[:, -1:]))[:, 0]
 
     # ------------------------------------------------------------------ one step
     def _run_step(self, ids: torch.Tensor, use_graph: bool) -> torch.Tensor:

@@ -107,6 +107,9 @@ def _declare(lib):
                                              P]),
         "agb200_decode_attention_rows_fp8": (I, [P, P, P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, P,
                                                   S, P]),
+        "agb200_prefill_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, I, P]),
+        "agb200_prefill_attention_fp8": (I, [P, P, P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, I,
+                                              P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
         "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
     }

@@ -17,6 +17,11 @@ FP8 cache (``agb200_decode_attention_fp8`` / ``agb200_decode_attention_rows_fp8`
 [B, n_kv, max_length], one power-of-two scale per cached row, select the FP8 entries.  The step quantises the new k̂ and v with
 ``quantize_kv``'s rule, writes codes and scales at the position and attends through them.  q, k, v and out stay in
 the activation dtype.  Half the cache bytes (hd + 4 per row instead of 2·hd).
+
+``prefill_attention`` (``agb200_prefill_attention`` / ``agb200_prefill_attention_fp8``, DESIGN §3.20) appends T new
+tokens to each of up to eight rows at their own ``start`` positions and attends them causally over the cache: the
+cache rows it writes are bit-equal to the decode step's for the same token, whatever T, and the attention runs on the
+tensor cores (mma.sync, fp32 softmax).  Feeding a prompt in chunks gives the same cache bytes as one call.
 """
 from __future__ import annotations
 
@@ -108,10 +113,54 @@ def decode_attention_rows(q, k, v, k_cache, v_cache, pos, inv_freq, attention_sc
                    attention_scaling, scaling, out, workspace, k_scale, v_scale)
 
 
+def prefill_attention_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, max_length: int,
+                                dtype) -> str | None:
+    """None when ``prefill_attention`` takes this shape, else the reason it does not (the per-row decode limits)."""
+    return attention_rows_supported(n_heads, n_kv, head_dim, batch, max_length, dtype)
+
+
+def prefill_attention(q, k, v, k_cache, v_cache, start, inv_freq, attention_scaling: float, scaling: float, out, *,
+                      k_scale=None, v_scale=None):
+    """Causal attention of T new tokens per row over the static caches (``agb200_prefill_attention``, DESIGN §3.20):
+    q [B, T, n_heads·hd], k / v [B, T, n_kv·hd], caches [B, n_kv, max_length, hd], start int64 [B] (device), inv_freq
+    fp32 [hd/2], out [B, T, n_heads·hd] written in place and returned.  Row b's tokens are written to the caches at
+    positions start[b] .. start[b] + T - 1 (k̂ with the rotary embedding, as ``decode_attention`` writes one token), then
+    token t attends positions 0 .. start[b] + t.  A row whose tokens do not fit gets NaN and no cache write.
+    float8_e4m3fn caches with ``k_scale`` / ``v_scale``: the FP8 cache, as ``decode_attention``.  Raises
+    NotImplementedError outside the kernel's limits.  No workspace, no host synchronisation."""
+    if q.dim() != 3:
+        raise ValueError(f"q must be [B, T, n_heads·head_dim], got {tuple(q.shape)}")
+    T = q.shape[1]
+    if T < 1:
+        raise ValueError("prefill_attention: T must be at least 1")
+    entry, caches, n_heads, dt = _checked("prefill_attention", prefill_attention_supported, None, q, k, v, k_cache,
+                                          v_cache, start, inv_freq, out, k_scale, v_scale, T=T, pos_name="start")
+    B, n_kv, L, hd = k_cache.shape
+    dev = k_cache.device
+    lib = _lib.load()
+    with torch.cuda.device(dev):
+        rc = getattr(lib, f"agb200_{entry}")(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, start.data_ptr(), inv_freq.data_ptr(),
+            float(attention_scaling), float(scaling), out.data_ptr(), B, T, n_heads, n_kv, hd, L, _DT[dt],
+            torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, f"agb200_{entry}")
+    return out
+
+
 def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out,
             workspace, k_scale=None, v_scale=None):
     """Checks and the call of agb200_<entry> (agb200_<entry>_fp8 for a float8_e4m3fn cache); ``n_pos`` elements of pos
     (None: one per row).  The activation dtype is the 16-bit cache's, or q's for an FP8 cache."""
+    entry, caches, n_heads, dt = _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, out,
+                                          k_scale, v_scale)
+    return _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace,
+                 n_heads, dt)
+
+
+def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, out, k_scale, v_scale, T=None,
+             pos_name="pos"):
+    """``_launch``'s checks: (entry with _fp8 for an FP8 cache, the cache pointers after v, n_heads, dtype).  With
+    ``T`` the activations are [B, T, features] instead of [B, features]."""
     if k_cache.dim() != 4:
         raise ValueError(f"k_cache must be [B, n_kv, max_length, head_dim], got {tuple(k_cache.shape)}")
     B, n_kv, L, hd = k_cache.shape
@@ -124,14 +173,16 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
     if fp8 and (k_scale is None or v_scale is None):
         raise ValueError(f"{entry}: a {FP8} cache needs k_scale and v_scale (fp32 [B, n_kv, max_length])")
     dt = q.dtype if fp8 else k_cache.dtype
-    if q.dim() != 2 or q.shape[0] != B or q.shape[1] % hd != 0:
-        raise ValueError(f"q must be [{B}, n_heads·{hd}], got {tuple(q.shape)}")
-    n_heads = q.shape[1] // hd
+    lead = (B,) if T is None else (B, T)
+    if q.dim() != len(lead) + 1 or tuple(q.shape[:-1]) != lead or q.shape[-1] % hd != 0:
+        raise ValueError(f"q must be [{', '.join(map(str, lead))}, n_heads·{hd}], got {tuple(q.shape)}")
+    n_heads = q.shape[-1] // hd
     why = supported(n_heads, n_kv, hd, B, L, dt)
     if why is not None:
         raise NotImplementedError(f"{entry}: {why}")
-    checks = [("q", q, (B, n_heads * hd), dt), ("k", k, (B, n_kv * hd), dt), ("v", v, (B, n_kv * hd), dt),
-              ("v_cache", v_cache, (B, n_kv, L, hd), k_cache.dtype), ("out", out, (B, n_heads * hd), dt)]
+    checks = [("q", q, lead + (n_heads * hd,), dt), ("k", k, lead + (n_kv * hd,), dt),
+              ("v", v, lead + (n_kv * hd,), dt), ("v_cache", v_cache, (B, n_kv, L, hd), k_cache.dtype),
+              ("out", out, lead + (n_heads * hd,), dt)]
     if fp8:
         checks += [("k_scale", k_scale, (B, n_kv, L), torch.float32), ("v_scale", v_scale, (B, n_kv, L), torch.float32)]
     for name, t, shape, want in checks:
@@ -142,8 +193,8 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
                 raise ValueError(f"{name} is {t.dtype}, the cache {dt}")
             raise ValueError(f"{name} is {t.dtype}, the activations (q) {dt}" if want == dt else
                              f"{name} is {t.dtype}, not {want}")
-    tensors = [("q", q), ("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out), ("pos", pos),
-               ("inv_freq", inv_freq)] + ([("k_scale", k_scale), ("v_scale", v_scale)] if fp8 else [])
+    tensors = [("q", q), ("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out),
+               (pos_name, pos), ("inv_freq", inv_freq)] + ([("k_scale", k_scale), ("v_scale", v_scale)] if fp8 else [])
     for name, t in tensors:
         if t.device != dev:
             raise ValueError(f"{name} is on {t.device}, the cache on {dev}")
@@ -151,14 +202,13 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
             raise ValueError(f"{name} must be contiguous")
     n_pos = B if n_pos is None else n_pos
     if pos.dtype != torch.int64 or pos.numel() != n_pos:
-        raise ValueError(f"pos must be {n_pos} int64 element(s), got {pos.dtype} with {pos.numel()} elements")
+        raise ValueError(f"{pos_name} must be {n_pos} int64 element(s), got {pos.dtype} with {pos.numel()} elements")
     if inv_freq.dtype != torch.float32 or tuple(inv_freq.shape) != (hd // 2,):
         raise ValueError(f"inv_freq must be float32 [{hd // 2}], got {inv_freq.dtype} {list(inv_freq.shape)}")
     caches = (k_cache.data_ptr(), v_cache.data_ptr())
     if fp8:
         entry, caches = entry + "_fp8", caches + (k_scale.data_ptr(), v_scale.data_ptr())
-    return _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace,
-                 n_heads, dt)
+    return entry, caches, n_heads, dt
 
 
 def _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace, n_heads,
@@ -183,4 +233,5 @@ def _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scali
 
 
 __all__ = ["decode_attention", "decode_attention_rows", "decode_attention_workspace", "attention_supported",
-           "attention_rows_supported", "quantize_kv", "dequantize_kv"]
+           "attention_rows_supported", "prefill_attention", "prefill_attention_supported", "quantize_kv",
+           "dequantize_kv"]

@@ -2,6 +2,7 @@
 
     dec = BatchDecoder(model, max_batch=8, max_length=4096)   # model: transformers *ForCausalLM with QuantLinear projections
     logits = dec.prefill(slot, input_ids)      # [T] prompt -> [vocab] logits of its last position; the slot becomes active
+    logits = dec.extend(slot, input_ids)       # [T] more tokens at the slot's position (0 when idle) -> [vocab]
     logits = dec.step(ids)                     # ids [max_batch] -> logits [max_batch, vocab]; active slots advance by one
     dec.release(slot)                          # the slot becomes idle
     outs = dec.generate(prompts, max_new_tokens, eos_token_id=None)    # continuous batching over a list of prompts
@@ -22,7 +23,11 @@ writes the row's cache entry and attends over the row's positions only; an idle 
 Every kernel computes a row from that row's inputs alone, so what one slot holds never changes another slot's logits.
 
 ``prefill`` runs the HF model at batch 1 and stores its keys and values in the slot's row of the static caches; with
-``kv_cache_dtype=torch.float8_e4m3fn`` they are FP8 (DESIGN §3.19), half the cache bytes.  Scope: Llama, Mistral and
+``kv_cache_dtype=torch.float8_e4m3fn`` they are FP8 (DESIGN §3.19), half the cache bytes.  ``extend(slot, ids)``
+appends T tokens at the slot's position on the project's kernels instead (DESIGN §3.20): the model's own modules for
+everything but attention, and ``prefill_attention`` writing the static cache and attending causally over it, with no
+second cache and lm_head on the last position only.  On an idle slot it is a prompt prefill; on an active one it
+continues the sequence (a new conversation turn, or the next chunk of a long prompt).  Scope: Llama, Mistral and
 Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too), greedy; mixture-of-experts blocks are
 refused.  The model checks, the caches, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
 ``ChainDecoder``, which runs each block of batch <= 2 sequences in lockstep as one decode-chain launch.
@@ -120,6 +125,27 @@ class BatchDecoder(StaticCacheDecoder):
         self._pos[slot] = T
         self._host_pos[slot] = T
         return logits[0, -1]
+
+    @torch.no_grad()
+    def extend(self, slot: int, input_ids: torch.Tensor) -> torch.Tensor:
+        """Append the tokens ``input_ids`` [T] to the slot at its position p (0 for an idle slot, so this is a prompt
+        prefill) on the project's kernels (DESIGN §3.20) and make the slot active at p + T.  Other slots' cache rows
+        and positions are not touched.  Returns the logits of the last new position [vocab].  Calling it several times
+        feeds a prompt in chunks, or continues a conversation without re-reading its history."""
+        slot = self._check_slot(slot)
+        if input_ids.dim() != 1:
+            raise ValueError(f"{_WHO}.extend: input_ids must be 1-D [T] (one slot), got {tuple(input_ids.shape)}")
+        T = input_ids.numel()
+        if T < 1:
+            raise ValueError(f"{_WHO}.extend: input_ids is empty")
+        p = max(self._host_pos[slot], 0)
+        if p + T >= self.max_length:
+            raise ValueError(f"{_WHO}.extend: slot {slot} at position {p} + {T} tokens must stay below "
+                             f"max_length={self.max_length}")
+        logits = self._extend(input_ids.to(self.device).view(1, T), slice(slot, slot + 1), [p])
+        self._pos[slot] = p + T
+        self._host_pos[slot] = p + T
+        return logits[0]
 
     def release(self, slot: int):
         """Make the slot idle: its row is skipped by the attention and its cache row is left as it is."""

@@ -27,7 +27,7 @@ NVCC_FLAGS = [
     "-DAGB200_NO_FAST_MATH",
 ]
 # translation units of the library (compiled in parallel, then linked)
-UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu", "attention.cu", "moe_router.cu"]
+UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu", "attention.cu", "moe_router.cu", "prefill_attention.cu"]
 
 
 def _nvcc() -> str:

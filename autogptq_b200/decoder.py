@@ -2,6 +2,7 @@
 
     dec = ChainDecoder(model, batch=1, max_length=2048)    # model: transformers *ForCausalLM with QuantLinear projections
     tokens = dec.generate(input_ids, max_new_tokens=128)   # prefill on the HF model, then one CUDA graph per token
+    logits = dec.extend(input_ids)                         # or: append [batch, T] tokens on the project's kernels
 
 Between two attentions a decoder layer is QuantLinears, elementwise work and one row reduction:
 
@@ -36,6 +37,10 @@ plans and their workspaces are allocated when the decoder is built.  ``prefill``
 than 8 tokens (``MOE_DECODE_MAX_T``) makes each ``QuantExperts`` build its tensor-core weight copies on first use, K·N/2
 bytes per layer, about 22 GB more for Mixtral-8x7B.  Router variants other than Mixtral's (Qwen2-MoE's shared expert,
 DeepSeek, no renormalisation), experts that are not grouped, and models that mix dense and MoE layers are refused.
+
+``extend`` appends tokens at ``position`` without the HF model's cache: the model's own modules with the project's
+``prefill_attention`` writing the static cache (DESIGN §3.20).  It continues a sequence (a new turn, a prompt in chunks)
+or, from position 0, prefills one; Mixtral keeps the HF ``prefill``.
 
 Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  The front end is
 ``autogptq_b200._decoding``'s, shared with ``autogptq_b200.batch_decoder.BatchDecoder``: up to eight independent
@@ -263,6 +268,29 @@ class ChainDecoder(StaticCacheDecoder):
         logits = self._prefill_cache(ids, slice(None))
         self.position = T
         return logits[:, -1]
+
+    @torch.no_grad()
+    def extend(self, input_ids: torch.Tensor) -> torch.Tensor:
+        """Append ``input_ids`` [batch, T] in lockstep at ``position`` on the project's kernels (DESIGN §3.20) and
+        return the logits of the last new position [batch, vocab]; ``position`` advances by T.  The cache layout is
+        the same for both ``fused_attention`` settings, so steps of either kind follow.  Mixture-of-experts models
+        are refused: use ``prefill``."""
+        if self.moe:
+            raise NotImplementedError("ChainDecoder.extend: mixture-of-experts blocks are not supported (the router "
+                                      f"kernel takes at most {_lib.MOE_DECODE_MAX_T} rows); use prefill")
+        if input_ids.dim() != 2 or input_ids.shape[0] != self.batch:
+            raise ValueError(f"ChainDecoder.extend: input_ids must be [{self.batch}, T] (sequences in lockstep), got "
+                             f"{tuple(input_ids.shape)}")
+        T = input_ids.shape[1]
+        if T < 1:
+            raise ValueError("ChainDecoder.extend: input_ids is empty")
+        p = self._length
+        if p + T >= self.max_length:
+            raise ValueError(f"ChainDecoder.extend: position {p} + {T} tokens must stay below "
+                             f"max_length={self.max_length}")
+        logits = self._extend(input_ids.to(self.device), slice(None), [p] * self.batch)
+        self.position = p + T
+        return logits
 
     # ------------------------------------------------------------------ one token
     def _attention(self, i: int, cos, sin, mask):

@@ -634,6 +634,47 @@ int agb200_decode_attention_rows_fp8(const void* q, const void* k, const void* v
                                      void* stream);
 
 /*
+ * Causal attention of T new tokens for each of B <= AGB200_ATTN_ROWS_MAX_B independent sequences, written into the
+ * static cache first (addition to ABI v11), two launches on `stream`, all pointers DEVICE memory:
+ *   q [B, T, n_heads*head_dim], k and v [B, T, n_kv*head_dim]   the projections' outputs (bias included), dtype
+ *   k_cache, v_cache [B, n_kv, max_length, head_dim]             contiguous static caches, dtype
+ *   start                                                         int64 [B]: row b's tokens take positions
+ *                                                                 start[b] .. start[b] + T - 1
+ *   inv_freq [head_dim/2] (fp32), attention_scaling, scaling     as agb200_decode_attention
+ *   out [B, T, n_heads*head_dim]                                  attention output (before o_proj), dtype
+ * The first launch writes k-hat (the rotary embedding at the token's position, transformers' roundings as in
+ * agb200_decode_attention) and v of every new token to its cache row; the bytes of a row depend only on (k, v,
+ * position): they equal what agb200_decode_attention_rows writes for the same token, whatever T or chunking.  The second
+ * reads only the cache: query head h of token t (kv head h / (n_heads/n_kv)) attends positions 0 .. start[b] + t with
+ * fp32 scores from the tensor cores (16-bit inputs, fp32 accumulation), an fp32 running-max softmax whose weights are
+ * rounded to dtype for the P*V product (fp32 accumulation), and the output rounded once.  A row with start[b] < 0 or
+ * start[b] + T > max_length writes NaN to its output rows and leaves its cache rows untouched.  Rows are independent,
+ * bit for bit; two calls on the same input are bit-identical (no atomics).  No workspace; no host synchronisation.
+ * Constraints (else AGB200_ENOSUP): dtype AGB200_F16 / AGB200_BF16, head_dim 64 or 128, n_heads/n_kv <= 8,
+ * B <= AGB200_ATTN_ROWS_MAX_B, B*n_kv*max_length*head_dim < 2^31.  T >= 1 (else AGB200_EINVAL).  q, k, v, the caches
+ * and out 16-byte aligned, start 8-byte aligned (else AGB200_EINVAL).
+ */
+int agb200_prefill_attention(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                             const int64_t* start, const float* inv_freq, float attention_scaling, float scaling,
+                             void* out, int B, int T, int n_heads, int n_kv, int head_dim, int max_length, int dtype,
+                             void* stream);
+
+/*
+ * The same over an FP8 cache (addition to ABI v11): k_cache and v_cache hold E4M3 codes and k_scale, v_scale
+ * [B, n_kv, max_length] (fp32) the power-of-two scale of each row, in the format of agb200_decode_attention_fp8; each new
+ * row is quantised on its own by that rule, so its codes and scale are bit-equal to the decode step's.  The attention
+ * reads every row through its codes and scale: q-hat times the codes on the tensor cores, each score then multiplied by
+ * its row's k scale (exact); the softmax weight of position t is multiplied by vs_t / R before its rounding to dtype,
+ * R the largest v scale of the tiles read so far (a power of two, so the factor is exact unless it underflows), and the
+ * output by R.  Constraints as agb200_prefill_attention; in addition k_scale and v_scale non-null and 4-byte aligned
+ * (else AGB200_EINVAL).
+ */
+int agb200_prefill_attention_fp8(const void* q, const void* k, const void* v, void* k_cache, void* v_cache,
+                                 float* k_scale, float* v_scale, const int64_t* start, const float* inv_freq,
+                                 float attention_scaling, float scaling, void* out, int B, int T, int n_heads, int n_kv,
+                                 int head_dim, int max_length, int dtype, void* stream);
+
+/*
  * Router of a Mixtral-style block for T decode rows (addition to ABI v10), one launch on `stream`, all pointers DEVICE
  * memory of `dtype` unless stated:
  *   x [T, H], x2 [T, H] or NULL   h = x + x2 (the residual add; x2 NULL: h = x)
