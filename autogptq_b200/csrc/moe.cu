@@ -416,6 +416,7 @@ struct BwdLayout {
 };
 
 int bwd_tile(int P, int E) {
+  if (P <= 0) return 32;                       // T = 0: no rows (workspace_bytes still answers)
   const int avg = (P + std::min(E, P) - 1) / std::min(E, P);
   return avg <= 32 ? 32 : avg <= 64 ? 64 : 128;
 }

@@ -105,7 +105,9 @@ class Path:
 # Hopper's tensor-core accumulation is calibrated, not derived.  Measured on an H100 80GB HBM3 (700 W power limit) over
 # the whole matrix of tests/test_gpu_17_precision.py, the largest share of the fp32 γ = λ·√n·u·A a result needed beyond
 # its half-ulp output rounding was 0.40 (wgmma dgrad, fp16), 0.22 (mma.sync skinny, fp16), 0.18 (wgmma GEMM, fp16) against
-# 0.22 / 0.10 for the CUDA-core dgrad / GEMV.  TC_GAMMA = 2 leaves a factor 5 above the largest.
+# 0.22 / 0.10 for the CUDA-core dgrad / GEMV.  TC_GAMMA = 2 leaves a factor 5 above the largest.  The fused backwards'
+# stages (tests/test_gpu_28_backward_stages.py) needed up to 0.60 (dense dx, n = 2I) and, on the experts' fp32 dx_pair
+# that no 16-bit rounding hides, 1.01: there TC_GAMMA = 2 leaves a factor 2.
 TC_GAMMA = 2.0
 _BF = {"bfloat16": 128}
 # Mismatch-rate limits (fraction of well-conditioned elements with y != round(y*)).  Largest rates measured on the H100
