@@ -11,9 +11,11 @@ Only what the path needs lives here:
                    add and RMSNorm alone
   mlp.py           forward_gate_up / FusedQuantMLP / inject_fused_mlp: a dense MLP's gate, up and silu * mul in one launch
   chain.py         DecodeChain: dependent QuantLinear stages (with residual adds and RMSNorms) in one persistent launch
-  decoder.py       ChainDecoder: greedy decoding of a Llama / Mistral / Qwen2 / Mixtral model, one CUDA graph per token
+  decoder.py       ChainDecoder: greedy or sampled decoding of a Llama / Mistral / Qwen2 / Mixtral model, one CUDA graph
+                   per token
   batch_decoder.py BatchDecoder: up to eight independent sequences of a Llama / Mistral / Qwen2 model, admitted and
-                   retired between steps, one CUDA graph per step
+                   retired between steps, greedy or sampled, one CUDA graph per step
+  sampling.py      SamplingParams / sample: temperature, top-k, top-p and min-p sampling in one seeded kernel per step
   attention.py     decode_attention: rotary embedding, KV-cache write and split-KV attention of one layer in one launch;
                    decode_attention_rows: the same with one position per row; both over a 16-bit or an FP8 cache
                    (quantize_kv: E4M3 codes with a power-of-two scale per row)
@@ -29,3 +31,4 @@ from .moe import QuantExperts, add_rmsnorm, group_experts  # noqa: E402,F401
 from .mlp import FusedQuantMLP, forward_gate_up, inject_fused_mlp  # noqa: E402,F401
 from .gptq import GPTQ, patch_auto_gptq_quantizer, quantize_linear  # noqa: E402,F401
 from .batch_decoder import BatchDecoder  # noqa: E402,F401
+from .sampling import SamplingParams, sample, sample_supported  # noqa: E402,F401

@@ -1,6 +1,7 @@
 """The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules,
 the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, the extend of
-cache rows on the project's kernels (DESIGN §3.20), and the warm-up, capture and replay of a step's CUDA graph."""
+cache rows on the project's kernels (DESIGN §3.20), each row's sampling parameters (DESIGN §3.21), and the warm-up,
+capture and replay of a step's CUDA graphs (the step, and the step followed by the sampling kernel)."""
 from __future__ import annotations
 
 import torch
@@ -8,6 +9,7 @@ import torch
 from .attention import FP8, quantize_kv
 from .mlp import FusedQuantMLP, _is_silu
 from .qlinear import QuantLinear
+from .sampling import SamplingState
 
 _RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm", "MixtralRMSNorm")
 _MOE_BLOCKS = ("MixtralSparseMoeBlock",)
@@ -96,7 +98,7 @@ def _plan_common(i: int, layer, dtype, who: str):
 
 
 class StaticCacheDecoder:
-    """Base of a greedy decoder over a static KV cache whose step is one captured CUDA graph.  A subclass sets ``_who``
+    """Base of a decoder over a static KV cache whose step is one captured CUDA graph.  A subclass sets ``_who``
     (the prefix of its refusals) and ``_plan`` (a layer's plan, starting from ``_plan_common``).  Its constructor calls
     ``_read_model``, checks its kernels' limits on the geometry, calls ``_read_layers``, checks what spans the layers
     and calls ``_allocate`` last, so every refusal comes before the device is needed.  It then sets ``_pos``, the device
@@ -161,8 +163,8 @@ class StaticCacheDecoder:
             self.k_scale = [torch.ones(shape[:-1], dtype=torch.float32, device=dev) for _ in range(n)]
             self.v_scale = [torch.ones_like(s) for s in self.k_scale]
         self._ids = torch.zeros(rows, dtype=torch.int64, device=dev)
-        self._graph = None
-        self._logits = None
+        self._graphs = {}                               # step body name -> (CUDA graph, its output buffers)
+        self._sampling = SamplingState(rows, dev)       # each row's sampling parameters, greedy until set
 
     def _store_kv(self, i: int, index, keys, values):
         """Keys and values [.., n_kv, T, hd] into layer i's caches at ``index`` (quantised for FP8)."""
@@ -216,26 +218,30 @@ class StaticCacheDecoder:
         return self.model.lm_head(inner.norm(h[:, -1:]))[:, 0]
 
     # ------------------------------------------------------------------ one step
-    def _run_step(self, ids: torch.Tensor, use_graph: bool) -> torch.Tensor:
-        """The subclass's ``_step_body`` (one step on ``_ids`` at the device positions ``_pos``, which it advances:
-        the logits) on ``ids``, eagerly or through the step's CUDA graph.  The first graph step warms up outside
-        the graph (library workspaces) and captures; both restore ``_pos`` after.  Later steps replay, and the logits
-        are a buffer the next step overwrites."""
+    def _run_step(self, ids: torch.Tensor, use_graph: bool, body=None):
+        """A step body on ``ids``, eagerly or through that body's CUDA graph: the subclass's ``_step_body`` (one step
+        on ``_ids`` at the device positions ``_pos``, which it advances: the logits) by default, or another that runs
+        it and more (the sampled step).  Each body has its own graph, captured on its first graph step after a warm-up
+        outside the graph (library workspaces); both restore ``_pos`` after.  Later steps replay, and the result is a
+        buffer the next replay of that graph overwrites."""
+        body = self._step_body if body is None else body
         self._ids.copy_(ids.reshape(-1).to(self._ids.device))
         if not use_graph:
-            return self._step_body()
-        if self._graph is None:
+            return body()
+        name = body.__name__
+        if name not in self._graphs:
             saved = self._pos.clone()
             side = torch.cuda.Stream(self.device)
             side.wait_stream(torch.cuda.current_stream(self.device))
             with torch.cuda.stream(side):
-                self._step_body()
+                body()
             torch.cuda.current_stream(self.device).wait_stream(side)
             self._pos.copy_(saved)
             g = torch.cuda.CUDAGraph()
             with torch.cuda.graph(g):
-                self._logits = self._step_body()
-            self._graph = g
+                out = body()
+            self._graphs[name] = (g, out)
             self._pos.copy_(saved)
-        self._graph.replay()
-        return self._logits
+        g, out = self._graphs[name]
+        g.replay()
+        return out

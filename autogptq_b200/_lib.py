@@ -7,13 +7,13 @@ from __future__ import annotations
 
 import ctypes
 import os
-from ctypes import c_char_p, c_float, c_int, c_size_t, c_void_p
+from ctypes import c_char_p, c_float, c_int, c_int64, c_size_t, c_void_p
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.path.join(_HERE, "_C", "libautogptq_b200.so")
 
 ABI_VERSION = 11
-F16, BF16 = 0, 1
+F16, BF16, F32 = 0, 1, 2
 ENOSUP = -3                     # AGB200_ENOSUP: a valid layer this build does not handle
 CHAIN_MAX_M = 2
 CHAIN_X_PLAIN, CHAIN_X_SILU_MUL, CHAIN_X_SUM_PARTS, CHAIN_X_RMSNORM, CHAIN_X_ADD_RMSNORM = 0, 1, 2, 3, 4
@@ -34,6 +34,7 @@ ATTN_HEAD_DIMS = (64, 128)
 ATTN_MAX_G = 8
 ATTN_MAX_B = 2
 ATTN_ROWS_MAX_B = 8            # AGB200_ATTN_ROWS_MAX_B
+SAMPLE_MAX_V = 262144          # AGB200_SAMPLE_MAX_V
 
 _lib = None
 
@@ -112,6 +113,7 @@ def _declare(lib):
                                               P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
         "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
+        "agb200_sample": (I, [P, c_int64, I, I, I, P, P, P, P, P, P, P, P]),
     }
     for name, (res, args) in sigs.items():
         fn = getattr(lib, name)

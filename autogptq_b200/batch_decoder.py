@@ -1,4 +1,4 @@
-"""Greedy decoding of up to eight independent sequences of a GPTQ Llama / Mistral / Qwen2 model, one CUDA graph per step.
+"""Decoding of up to eight independent sequences of a GPTQ Llama / Mistral / Qwen2 model, one CUDA graph per step.
 
     dec = BatchDecoder(model, max_batch=8, max_length=4096)   # model: transformers *ForCausalLM with QuantLinear projections
     logits = dec.prefill(slot, input_ids)      # [T] prompt -> [vocab] logits of its last position; the slot becomes active
@@ -6,6 +6,10 @@
     logits = dec.step(ids)                     # ids [max_batch] -> logits [max_batch, vocab]; active slots advance by one
     dec.release(slot)                          # the slot becomes idle
     outs = dec.generate(prompts, max_new_tokens, eos_token_id=None)    # continuous batching over a list of prompts
+    dec.set_sampling(slot, SamplingParams(temperature=0.7, top_p=0.9))  # the slot's sampling parameters (None: greedy)
+    token = dec.sample(slot, logits)           # sample prefill's / extend's logits with them
+    tokens, logits = dec.step_sample(ids)      # the step and the sampling kernel in one CUDA graph
+    outs = dec.generate(prompts, max_new_tokens, sampling=SamplingParams(...))     # sampled continuous batching
 
 Each of the ``max_batch`` slots holds one sequence at its own position, or none.  Positions live in a device tensor
 ``pos`` [max_batch], -1 for an idle slot, so a step is the same launches whatever the slots hold: it is captured once in
@@ -27,9 +31,13 @@ Every kernel computes a row from that row's inputs alone, so what one slot holds
 appends T tokens at the slot's position on the project's kernels instead (DESIGN §3.20): the model's own modules for
 everything but attention, and ``prefill_attention`` writing the static cache and attending causally over it, with no
 second cache and lm_head on the last position only.  On an idle slot it is a prompt prefill; on an active one it
-continues the sequence (a new conversation turn, or the next chunk of a long prompt).  Scope: Llama, Mistral and
-Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too), greedy; mixture-of-experts blocks are
-refused.  The model checks, the caches, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
+continues the sequence (a new conversation turn, or the next chunk of a long prompt).
+
+Tokens are greedy, or sampled (temperature, top-k, top-p, min-p; DESIGN §3.21) by ``autogptq_b200.sampling``'s kernel,
+which runs in the step's graph: each slot's parameters and seed live in device tensors [max_batch], so one graph serves
+any mix of greedy and sampled slots, and a slot's token depends only on its own logits, parameters, seed and position.
+Scope: Llama, Mistral and Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too); mixture-of-experts
+blocks are refused.  The model checks, the caches, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
 ``ChainDecoder``, which runs each block of batch <= 2 sequences in lockstep as one decode-chain launch.
 """
 from __future__ import annotations
@@ -44,12 +52,13 @@ from .attention import attention_rows_supported, decode_attention_rows, decode_a
 from .mlp import forward_gate_up
 from .moe import add_rmsnorm, add_rmsnorm_supported
 from .qlinear import forward_group
+from .sampling import SamplingParams, sampling_list
 
 _WHO = "BatchDecoder"
 
 
 class BatchDecoder(StaticCacheDecoder):
-    """Greedy decoder of up to ``max_batch`` <= 8 independent sequences over a transformers ``LlamaForCausalLM`` /
+    """Greedy or sampling decoder of up to ``max_batch`` <= 8 independent sequences over a transformers ``LlamaForCausalLM`` /
     ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose projections are ``autogptq_b200.QuantLinear``.
     ``kv_cache_dtype``: None (the activation dtype) or ``torch.float8_e4m3fn``."""
 
@@ -147,6 +156,25 @@ class BatchDecoder(StaticCacheDecoder):
         self._host_pos[slot] = p + T
         return logits[0]
 
+    def set_sampling(self, slot: int, params: SamplingParams | None):
+        """The slot's sampling parameters for ``sample`` and ``step_sample`` (None: greedy); a ``seed=None`` draws its
+        seed from torch's default CPU generator now.  They stay until set again, across release and prefill."""
+        slot = self._check_slot(slot)
+        if params is not None and not isinstance(params, SamplingParams):
+            raise TypeError(f"{_WHO}.set_sampling: params must be a SamplingParams or None, got {type(params).__name__}")
+        self._sampling.set(slot, params)
+
+    @torch.no_grad()
+    def sample(self, slot: int, logits: torch.Tensor) -> int:
+        """Sample the [vocab] logits ``prefill`` / ``extend`` returned for an active slot with the slot's parameters,
+        at counter = the slot's position (where the token will go).  One device-to-host read."""
+        slot = self._check_slot(slot)
+        p = self._host_pos[slot]
+        if p < 0:
+            raise RuntimeError(f"{_WHO}.sample: slot {slot} is idle")
+        counter = torch.full((1,), p, dtype=torch.int64, device=self.device)
+        return int(self._sampling.sample(logits.reshape(1, -1), counter, slice(slot, slot + 1))[0])
+
     def release(self, slot: int):
         """Make the slot idle: its row is skipped by the attention and its cache row is left as it is."""
         slot = self._check_slot(slot)
@@ -175,27 +203,50 @@ class BatchDecoder(StaticCacheDecoder):
         self._pos.add_(self._pos >= 0)                  # active slots advance; idle ones stay at -1
         return logits
 
+    def _sampled_step_body(self):
+        """The step, then every slot's token sampled at its advanced position (idle slots: -1, token 0)."""
+        logits = self._step_body()
+        return self._sampling.sample(logits, self._pos), logits
+
+    def _check_step(self, what: str):
+        active = [p for p in self._host_pos if p >= 0]
+        if not active:
+            raise RuntimeError(f"{_WHO}.{what}: no slot is active (prefill one first)")
+        if max(active) >= self.max_length:
+            raise RuntimeError(f"{_WHO}.{what}: a slot's static cache is full ({self.max_length} tokens)")
+
     @torch.no_grad()
     def step(self, ids: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
         """Decode one token for every active slot: ``ids`` [max_batch] (entries of idle slots are ignored) -> logits
         [max_batch, vocab]; rows of idle slots carry no meaning.  With ``use_graph`` the result is a buffer the next
         step overwrites: the first graph step captures the whole step in one CUDA graph, later steps replay it."""
-        active = [p for p in self._host_pos if p >= 0]
-        if not active:
-            raise RuntimeError(f"{_WHO}.step: no slot is active (prefill one first)")
-        if max(active) >= self.max_length:
-            raise RuntimeError(f"{_WHO}.step: a slot's static cache is full ({self.max_length} tokens)")
+        self._check_step("step")
         logits = self._run_step(ids, use_graph)
         self._host_pos = [p + 1 if p >= 0 else p for p in self._host_pos]
         return logits
 
+    @torch.no_grad()
+    def step_sample(self, ids: torch.Tensor, use_graph: bool = True):
+        """``step`` followed by the sampling kernel with each slot's parameters (``set_sampling``) at counter = the
+        slot's advanced position: ``ids`` [max_batch] -> (tokens int64 [max_batch], logits [max_batch, vocab]); idle
+        slots get token 0.  With ``use_graph`` both run in one CUDA graph, captured apart from ``step``'s, and the
+        results are buffers the next sampled step overwrites."""
+        self._check_step("step_sample")
+        out = self._run_step(ids, use_graph, self._sampled_step_body)
+        self._host_pos = [p + 1 if p >= 0 else p for p in self._host_pos]
+        return out
+
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
-    def generate(self, prompts, max_new_tokens: int, eos_token_id=None) -> list:
-        """Greedy decoding of every prompt (1-D, any lengths) -> a list of 1-D tensors, prompt followed by its new
-        tokens: at most ``max_new_tokens``, fewer when ``eos_token_id`` comes first (it is kept).  Prompts fill free
-        slots in order; a sequence retires at EOS or after ``max_new_tokens`` and the next prompt takes its slot.  One
-        small device-to-host read per step (the greedy tokens)."""
+    def generate(self, prompts, max_new_tokens: int, eos_token_id=None, sampling=None) -> list:
+        """Decoding of every prompt (1-D, any lengths) -> a list of 1-D tensors, prompt followed by its new tokens: at
+        most ``max_new_tokens``, fewer when ``eos_token_id`` comes first (it is kept).  Prompts fill free slots in
+        order; a sequence retires at EOS or after ``max_new_tokens`` and the next prompt takes its slot.  One small
+        device-to-host read per step (the tokens).  ``sampling``: None is greedy (the argmax of the logits); a
+        ``SamplingParams``, or a list of one per prompt, samples: each admitted prompt's parameters go to its slot, the
+        first token comes from ``sample`` and the later ones from ``step_sample``."""
+        prompts = list(prompts)
+        params = None if sampling is None else sampling_list(sampling, len(prompts), f"{_WHO}.generate")
         prompts = [p.reshape(-1) for p in prompts]
         if max_new_tokens < 1:
             raise ValueError(f"max_new_tokens must be >= 1, got {max_new_tokens}")
@@ -223,14 +274,21 @@ class BatchDecoder(StaticCacheDecoder):
                 while owner[s] is None and queue:
                     j = queue.popleft()
                     owner[s] = j
-                    take(s, int(self.prefill(s, prompts[j]).argmax()))
+                    if params is None:
+                        take(s, int(self.prefill(s, prompts[j]).argmax()))
+                    else:
+                        self.set_sampling(s, params[j])
+                        take(s, self.sample(s, self.prefill(s, prompts[j])))
             live = [s for s in range(self.max_batch) if owner[s] is not None]
             if not live:
                 break
             ids = torch.zeros(self.max_batch, dtype=torch.int64)
             for s in live:
                 ids[s] = new[owner[s]][-1]
-            toks = self.step(ids.to(self.device)).argmax(-1).tolist()
+            if params is None:
+                toks = self.step(ids.to(self.device)).argmax(-1).tolist()
+            else:
+                toks = self.step_sample(ids.to(self.device))[0].tolist()
             for s in live:
                 take(s, toks[s])
         return [torch.cat([p.to(self.device), torch.tensor(t, dtype=p.dtype, device=self.device)])

@@ -27,7 +27,8 @@ NVCC_FLAGS = [
     "-DAGB200_NO_FAST_MATH",
 ]
 # translation units of the library (compiled in parallel, then linked)
-UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu", "attention.cu", "moe_router.cu", "prefill_attention.cu"]
+UNITS = ["abi.cu", "chain.cu", "moe.cu", "gptq.cu", "attention.cu", "moe_router.cu", "prefill_attention.cu",
+         "sample.cu"]
 
 
 def _nvcc() -> str:

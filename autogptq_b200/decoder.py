@@ -1,7 +1,8 @@
-"""Greedy decoding of a GPTQ Llama / Mistral / Qwen2 model with one decode-chain launch per decoder block.
+"""Decoding of a GPTQ Llama / Mistral / Qwen2 model with one decode-chain launch per decoder block.
 
     dec = ChainDecoder(model, batch=1, max_length=2048)    # model: transformers *ForCausalLM with QuantLinear projections
     tokens = dec.generate(input_ids, max_new_tokens=128)   # prefill on the HF model, then one CUDA graph per token
+    tokens = dec.generate(input_ids, 128, sampling=SamplingParams(temperature=0.7, top_p=0.9))   # sampled
     logits = dec.extend(input_ids)                         # or: append [batch, T] tokens on the project's kernels
 
 Between two attentions a decoder layer is QuantLinears, elementwise work and one row reduction:
@@ -42,7 +43,11 @@ DeepSeek, no renormalisation), experts that are not grouped, and models that mix
 ``prefill_attention`` writing the static cache (DESIGN §3.20).  It continues a sequence (a new turn, a prompt in chunks)
 or, from position 0, prefills one; Mixtral keeps the HF ``prefill``.
 
-Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy.  The front end is
+``generate(..., sampling=...)`` samples each token (temperature, top-k, top-p, min-p; DESIGN §3.21) with
+``autogptq_b200.sampling``'s kernel inside a second graph of the step; it only reads the logits, so dense and Mixtral
+blocks alike take it.
+
+Scope: batch <= 2 (the chain's M), sequences in lockstep (one prompt length), greedy or sampled.  The front end is
 ``autogptq_b200._decoding``'s, shared with ``autogptq_b200.batch_decoder.BatchDecoder``: up to eight independent
 sequences of any lengths, admitted and retired between steps.
 """
@@ -57,6 +62,7 @@ from ._decoding import _RMSNORMS, _check_window, _norm_of  # noqa: F401 - the ch
 from .attention import FP8, attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
 from .moe import QuantExperts, moe_router, router_supported
+from .sampling import sampling_list
 
 _ROUTERS = ("MixtralTopKRouter",)
 
@@ -128,7 +134,7 @@ def _is_moe(plans) -> bool:
 
 
 class ChainDecoder(StaticCacheDecoder):
-    """Greedy decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
+    """Greedy or sampling decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
     projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too), or a
     ``MixtralForCausalLM`` whose experts are ``autogptq_b200.QuantExperts``.  ``fused_attention``:
     run each layer's attention as one CUDA launch (``autogptq_b200.attention.decode_attention``) instead of torch.
@@ -158,6 +164,7 @@ class ChainDecoder(StaticCacheDecoder):
         plans, attn0, H = self._plans, self._plans[0][0], self.hidden_size
         B, dev, dt = batch, self.device, self.dtype
         self._pos = torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
+        self._counter = torch.zeros(B, dtype=torch.int64, device=dev)      # its copy per row, the sampler's counter
         self._arange = torch.arange(self.max_length, device=dev)
         self._length = 0                                                    # host copy of the position
         if self.fused_attention:                                            # shared by the layers (one stream)
@@ -333,6 +340,12 @@ class ChainDecoder(StaticCacheDecoder):
         self._pos.add_(1)
         return logits
 
+    def _sampled_step_body(self):
+        """The step, then every row's token sampled at the advanced position."""
+        logits = self._step_body()
+        self._counter.copy_(self._pos.expand(self.batch))
+        return self._sampling.sample(logits, self._counter), logits
+
     @torch.no_grad()
     def step(self, ids: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
         """Decode one token per sequence: ``ids`` [batch] -> logits [batch, vocab] (a buffer the next step overwrites
@@ -344,10 +357,15 @@ class ChainDecoder(StaticCacheDecoder):
         return logits
 
     @torch.no_grad()
-    def generate(self, input_ids: torch.Tensor, max_new_tokens: int) -> torch.Tensor:
-        """Greedy decoding: prompt [batch, T] -> [batch, T + max_new_tokens]."""
+    def generate(self, input_ids: torch.Tensor, max_new_tokens: int, sampling=None) -> torch.Tensor:
+        """Decoding: prompt [batch, T] -> [batch, T + max_new_tokens].  ``sampling``: None is greedy (the argmax of the
+        logits); a ``SamplingParams``, or a list of ``batch`` of them, samples row b with its parameters at counter =
+        the token's position: the first token from the prefill's logits, the later ones in the step's sampled graph."""
+        params = None if sampling is None else sampling_list(sampling, self.batch, "ChainDecoder.generate")
         if input_ids.shape[1] + max_new_tokens > self.max_length:
             raise ValueError(f"prompt + {max_new_tokens} new tokens exceed max_length={self.max_length}")
+        if params is not None:
+            return self._generate_sampled(input_ids, max_new_tokens, params)
         logits = self.prefill(input_ids)
         out = [input_ids.to(self.device)]
         for t in range(max_new_tokens):
@@ -355,6 +373,21 @@ class ChainDecoder(StaticCacheDecoder):
             out.append(tok.view(-1, 1))
             if t + 1 < max_new_tokens:
                 logits = self.step(tok)
+        return torch.cat(out, dim=1)
+
+    def _generate_sampled(self, input_ids: torch.Tensor, max_new_tokens: int, params: list) -> torch.Tensor:
+        for b, sp in enumerate(params):
+            self._sampling.set(b, sp)
+        logits = self.prefill(input_ids)
+        out = [input_ids.to(self.device)]
+        for t in range(max_new_tokens):
+            if t == 0:                                  # the prefill's logits, sampled at the first new position
+                self._counter.fill_(self._length)
+                tok = self._sampling.sample(logits, self._counter).clone()
+            else:                                       # the step and the sampler in one graph
+                tok = self._run_step(tok, True, self._sampled_step_body)[0].clone()
+                self._length += 1
+            out.append(tok.view(-1, 1))
         return torch.cat(out, dim=1)
 
 

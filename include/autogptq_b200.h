@@ -41,6 +41,7 @@ extern "C" {
 /* element types of x / y / scales / bias */
 #define AGB200_F16 0
 #define AGB200_BF16 1
+#define AGB200_F32 2   /* agb200_sample's logits only */
 
 /* error codes */
 #define AGB200_OK 0
@@ -713,6 +714,40 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
  */
 int agb200_add_rmsnorm(const void* x, const void* x2, const void* norm_weight, float eps, int T, int H, int dtype,
                        void* h, void* n, void* stream);
+
+/*
+ * Next-token sampling of B rows of logits (addition to ABI v11), one launch on `stream`; every pointer is DEVICE memory
+ * with one entry per row unless stated:
+ *   logits [B, row_stride] of `dtype` (AGB200_F16, AGB200_BF16 or AGB200_F32)   row b is logits[b, :V]
+ *   temperature fp32, top_k int32, top_p fp32, min_p fp32, seed uint64          the row's parameters
+ *   counter int64    the position the sampled token will occupy in its sequence; < 0: an idle row, which writes 0
+ *   tokens int64     the sampled token of each row
+ * The semantics are transformers' TemperatureLogitsWarper, TopKLogitsWarper, TopPLogitsWarper and MinPLogitsWarper in
+ * that order (min_tokens_to_keep = 1), made exact so a float64 replay can check every draw.  For one row:
+ *   temperature <= 0 (or NaN): greedy, the argmax of the logits with the lower index on ties (a NaN above everything):
+ *     bit-equal to torch.argmax.
+ *   Otherwise s_j = fl32(float(l_j) / temperature) (IEEE division) and the kept set K is the intersection of
+ *     top-k   s_j >= the k-th largest s (ties at the k-th value kept); top_k == 0 or top_k >= V turns it off;
+ *     top-p   the softmax mass, over the top-k set, of the tokens with strictly larger s than s_j is < top_p; ties at the
+ *             boundary are all kept and the largest token always is; top_p >= 1 turns it off.  The masses are
+ *             expf(s - s_max) in units of 2^-40 (integer sums) and the bound is ceil(top_p · Z) of those units;
+ *     min-p   expf(s_j - s_max) >= min_p (transformers' probs >= min_p · max_prob); min_p <= 0 turns it off.
+ *   The token is the Gumbel-max argmax over K of fl32(s_j + g_j), the lower index on ties, with g_j = -log(-log(u_j))
+ *   in fp32 (the accurate logf), u_j = ((r_j >> 9) + 0.5) · 2^-23 (exact, in (0, 1)) and r_j word j & 3 of
+ *   Philox4x32-10 under key (seed lo, seed hi) at counter (j >> 2, counter lo, counter hi, 0).  This samples exactly
+ *   the renormalised softmax over K, in one pass, with no sort and no prefix sum.
+ * The token is always in 0 .. V-1, even for NaN or all -inf logits (where it is unspecified); a -inf logit is never
+ * drawn while a finite one is in K.  A row's token depends only on its logits, parameters, seed and counter, not on
+ * its index or on other rows, and two calls are bit-identical: every reduction runs in a fixed order and there are no
+ * floating-point atomics.  No workspace and no host synchronisation, so the call can be captured in a CUDA graph.
+ * Constraints: B >= 1, 1 <= V, row_stride >= V (else AGB200_EINVAL); V <= AGB200_SAMPLE_MAX_V, B <= 65535 (else
+ * AGB200_ENOSUP).  logits aligned to its element, the 32-bit arrays to 4 bytes, seed, counter and tokens to 8 (else
+ * AGB200_EINVAL).
+ */
+#define AGB200_SAMPLE_MAX_V 262144
+int agb200_sample(const void* logits, int64_t row_stride, int dtype, int B, int V, const float* temperature,
+                  const int32_t* top_k, const float* top_p, const float* min_p, const uint64_t* seed,
+                  const int64_t* counter, int64_t* tokens, void* stream);
 
 /* Static facts about the build, for logs: returns e.g. "autogptq_b200 sm_90a: ... gemm=wgmma ...". */
 const char* agb200_build_info(void);
