@@ -101,8 +101,9 @@ class StaticCacheDecoder:
     """Base of a decoder over a static KV cache whose step is one captured CUDA graph.  A subclass sets ``_who``
     (the prefix of its refusals) and ``_plan`` (a layer's plan, starting from ``_plan_common``).  Its constructor calls
     ``_read_model``, checks its kernels' limits on the geometry, calls ``_read_layers``, checks what spans the layers
-    and calls ``_allocate`` last, so every refusal comes before the device is needed.  It then sets ``_pos``, the device
-    positions its ``_step_body`` reads and advances."""
+    and calls ``_allocate`` last, so every refusal comes before the caches are allocated (a refusal that asks the device,
+    such as a decode chain's shared memory, takes ``_cuda_device`` first).  It then sets ``_pos``, the device positions
+    its ``_step_body`` reads and advances."""
 
     # ------------------------------------------------------------------ reading the model
     def _read_model(self, model, max_length: int, kv_cache_dtype):
@@ -148,13 +149,18 @@ class StaticCacheDecoder:
         self._final = _norm_of(inner.norm, "model.norm", self._who)
 
     # ------------------------------------------------------------------ the KV cache
+    def _cuda_device(self) -> torch.device:
+        """``device``: the model's, which must be a CUDA device."""
+        self.device = self.model.model.embed_tokens.weight.device
+        if self.device.type != "cuda":
+            raise RuntimeError(f"{self._who} needs the model on a CUDA device")
+        return self.device
+
     def _allocate(self, rows: int):
         """After every refusal: the CUDA device, the static caches of ``rows`` rows and the step's token ids.  The
         caches are per layer [rows, n_kv, max_length, head_dim] in the activation dtype, or E4M3 codes with fp32
         scales ``k_scale`` / ``v_scale`` [rows, n_kv, max_length] for FP8 (else the scales are None)."""
-        self.device = self.model.model.embed_tokens.weight.device
-        if self.device.type != "cuda":
-            raise RuntimeError(f"{self._who} needs the model on a CUDA device")
+        self._cuda_device()
         shape, n, dev = (rows, self.n_kv, self.max_length, self.head_dim), len(self._plans), self.device
         self.k_cache = [torch.zeros(shape, dtype=FP8 if self._fp8 else self.dtype, device=dev) for _ in range(n)]
         self.v_cache = [torch.zeros_like(c) for c in self.k_cache]

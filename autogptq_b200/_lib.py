@@ -40,7 +40,12 @@ _lib = None
 
 
 class B200KernelError(RuntimeError):
-    """Raised when a C-ABI call returns a non-zero status (mirrors the reference's TORCH_CHECK -> RuntimeError)."""
+    """Raised when a C-ABI call returns a non-zero status (mirrors the reference's TORCH_CHECK -> RuntimeError).
+    ``code`` is that status (``ENOSUP``: a valid input this build does not handle)."""
+
+    def __init__(self, msg: str = "", code: int = 0):
+        super().__init__(msg)
+        self.code = code
 
 
 def _declare(lib):
@@ -141,7 +146,7 @@ def load():
 def check(rc: int, what: str = ""):
     if rc != 0:
         msg = load().agb200_last_error().decode(errors="replace")
-        raise B200KernelError(f"{what or 'autogptq_b200'} failed (code {rc}): {msg}")
+        raise B200KernelError(f"{what or 'autogptq_b200'} failed (code {rc}): {msg}", rc)
 
 
 def declared_symbols():

@@ -296,7 +296,8 @@ int agb200_chain_create_norm(const agb200_chain_stage* stages, const agb200_chai
   const size_t fixed = M == 1 ? agb::ChainSmem<1>::fixed(rows_pad_max, xs_bytes) : agb::ChainSmem<2>::fixed(rows_pad_max, xs_bytes);
   if (fixed + 4 * size_t(agb::kChSlotBytes) > static_cast<size_t>(smem_cap)) smem_cap = smem_optin;      // wide x: take it all
   if (fixed + 3 * size_t(agb::kChSlotBytes) > static_cast<size_t>(smem_cap))
-    return failf(AGB200_ENOSUP, "chain: K up to %d with M=%d needs %zu B of shared memory besides the ring (> %d)", rows_pad_max * 8, M, fixed, smem_cap);
+    return failf(AGB200_ENOSUP, "chain: K up to %d with M=%d needs %zu B of shared memory (%zu B besides the smallest ring of 3 slots), "
+                 "more than the %d B a block may opt in to", rows_pad_max * 8, M, fixed + 3 * size_t(agb::kChSlotBytes), fixed, smem_cap);
   int slots = static_cast<int>((static_cast<size_t>(smem_cap) - fixed) / agb::kChSlotBytes);
   if (slots > agb::kChMaxSlots) slots = agb::kChMaxSlots;
   if (const char* e = getenv("AGB200_CHAIN_SLOTS")) { const int v = atoi(e); if (v >= agb::kChGroups && v < slots) slots = v; }

@@ -159,10 +159,11 @@ class ChainDecoder(StaticCacheDecoder):
                                                                 "ChainDecoder(fused_attention=True)")
         self._read_layers()
         self.moe = _is_moe(self._plans)
-        self._allocate(batch)
 
+        # the chains are built before the caches: whether a block's chain fits the device's shared memory is the
+        # library's decision (DESIGN §3.5), and a block that does not fit is refused before the caches are allocated
         plans, attn0, H = self._plans, self._plans[0][0], self.hidden_size
-        B, dev, dt = batch, self.device, self.dtype
+        B, dev, dt = batch, self._cuda_device(), self.dtype
         self._pos = torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
         self._counter = torch.zeros(B, dtype=torch.int64, device=dev)      # its copy per row, the sampler's counter
         self._arange = torch.arange(self.max_length, device=dev)
@@ -176,16 +177,28 @@ class ChainDecoder(StaticCacheDecoder):
         self._x0 = ch.input(H)
         w, eps = plans[0][2]
         qkv = ch.stage([attn0.q_proj, attn0.k_proj, attn0.v_proj], self._x0, x_mode="rmsnorm", norm_weight=w, norm_eps=eps)
-        self.chains.append(ch.build())
+        self.chains.append(self._build(ch, 0))
         self._qkv = [qkv]              # q, k, v of block i
         self._attn_in = []             # o_proj input of block i (written by the attention)
         if self.moe:
             self._build_moe(plans, H)
         else:
             self._build_dense(plans)
+        self._allocate(batch)
 
     def _plan(self, i: int, layer):
         return _plan_layer(i, layer, self.batch, self.dtype)
+
+    def _build(self, ch: DecodeChain, i: int) -> DecodeChain:
+        """``ch.build()`` of a chain that starts in block i; a chain the device cannot hold (ENOSUP: the digits of its
+        widest x leave no room for the smallest ring) is a refusal."""
+        try:
+            return ch.build()
+        except _lib.B200KernelError as e:
+            if e.code != _lib.ENOSUP:
+                raise
+            raise NotImplementedError(f"ChainDecoder: model.layers.{i} at batch {self.batch} does not fit in one decode "
+                                      f"chain launch: {e}") from None
 
     def _build_dense(self, plans):
         """chain_i = [o_i, add_rmsnorm -> gate|up_i, silu_mul -> down_i, add_rmsnorm(input_layernorm_i+1) -> q|k|v_i+1]"""
@@ -207,7 +220,7 @@ class ChainDecoder(StaticCacheDecoder):
             else:
                 self._last = (h1, down)
             self._attn_in.append(a_in)
-            self.chains.append(ch.build())
+            self.chains.append(self._build(ch, i))
 
     def _build_moe(self, plans, H: int):
         """Per block i: chain [o_i]; the router (h1 = x + o, n2 = post_attention_layernorm(h1), top-k); the grouped
@@ -220,7 +233,7 @@ class ChainDecoder(StaticCacheDecoder):
             ch = DecodeChain(M=B, dtype=dt, device=dev)
             a_in = ch.input(attn.o_proj.infeatures)
             (o,) = ch.stage([attn.o_proj], a_in)
-            self._o_chains.append(ch.build())
+            self._o_chains.append(self._build(ch, i))
             self._attn_in.append(a_in)
             h1, n2, out = (torch.zeros((B, H), dtype=dt, device=dev) for _ in range(3))
             idx = torch.zeros((B, k), dtype=torch.int32, device=dev)
@@ -235,7 +248,7 @@ class ChainDecoder(StaticCacheDecoder):
                 q, kk, v, resid = ch.stage([na.q_proj, na.k_proj, na.v_proj], out, x2=h1, x_mode="add_rmsnorm",
                                            norm_weight=w1, norm_eps=eps1)
                 self._qkv.append((q, kk, v))
-                self._qkv_chains.append(ch.build())
+                self._qkv_chains.append(self._build(ch, i + 1))
             else:
                 self._last = (h1, out)
 

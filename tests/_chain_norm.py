@@ -76,6 +76,28 @@ def check_n(n, h, w, eps, dtype, what="") -> float:
     return float((ok1 & ~ok0).sum()) / n.size
 
 
+def reference_y(d, h, w, eps, dtype, cols=None) -> P.Ref:
+    """The chain's reference of a normed stage's output on the host-side n0 of the h the stage read, widened by
+    Σ|n1 − n0|·|W| over the elements whose n has two candidates (the digit block maximum may be n1's).  ``cols``:
+    (c0, c1) or None for every column."""
+    pc = P.PATHS["chain"]
+    n0, n1, amb = n_candidates(h, w, eps, dtype)
+    ref = P.reference(d, n0, pc, dtype, cols=cols)
+    if amb.any():
+        q, z, s, gi, _ = P.layer_parts(d, dtype, cols)
+        W = np.abs(s[gi] * (q - z[gi]))
+        extra = (np.where(amb, np.abs(n1 - n0), 0.0) @ W) * (1 + 2.0 ** -7)
+        hx = np.where(amb & (np.abs(n1) > np.abs(n0)), n1, n0)
+        ref.F = np.maximum(ref.F, P.reference(d, hx, pc, dtype, cols=cols).F) + extra
+    return ref
+
+
+def check_y(y, d, h, w, eps, dtype, cols, what):
+    """A normed stage's output y [M, N] (float64) on ``cols`` against ``reference_y``; the ``P.check`` measurement."""
+    c0, c1 = cols or (0, d["N"])
+    return P.check(y[:, c0:c1], reference_y(d, h, w, eps, dtype, cols), P.PATHS["chain"], dtype, what=what)
+
+
 def kernel_model(x, x2, w, eps, dtype, threads: int = 384):
     """NumPy restatement of ch_norm_prepass for one launch: (h, n) with the kernel's fp32 order of Σh² (each thread
     sums its k8-rows ctid, ctid + threads, ... with fused multiply-adds, then a xor-shuffle tree per warp of 32 and the

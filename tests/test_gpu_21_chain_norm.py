@@ -8,7 +8,7 @@ Stage level (Llama-2-7B shapes, one H = 8192 stage; fp16 / bf16; M = 1, 2; plain
 
 * h1 and h2 are bit-equal to rnd(a + b) of what the stage read;
 * each y is within the chain's DESIGN §3.12 bound (``tests/_precision.py``) against float64 on the host-side n,
-  widened by Σ|n_alt − n|·|W| where n has two candidates (``tests/_chain_norm.py``);
+  widened by Σ|n_alt − n|·|W| where n has two candidates (``tests/_chain_norm.py``, ``check_y``);
 * three consecutive launches (tags are never reset) each pass, and two launches on one input are bit-identical.
 
 Model level: a small random Llama and a Qwen2 with q/k/v biases, 32 teacher-forced ChainDecoder steps against the HF
@@ -49,22 +49,6 @@ def _weight(K, dtype, seed):
     return P.round_dt(rng.uniform(0.05, 3.0, size=K) * np.where(rng.random(K) < 0.3, -1, 1), P.dt_name(dtype))
 
 
-def _check_y(y, d, h, w, eps, dtype, cols, what):
-    """y against the chain's bound on the host-side n0 of the h the stage read, widened by Σ|n1 − n0|·|W| over the
-    elements whose n has two candidates (the digit block maximum may be n1's)."""
-    pc = P.PATHS["chain"]
-    n0, n1, amb = N.n_candidates(h, w, eps, dtype)
-    ref = P.reference(d, n0, pc, dtype, cols=cols)
-    if amb.any():
-        q, z, s, gi, _ = P.layer_parts(d, dtype, cols)
-        W = np.abs(s[gi] * (q - z[gi]))
-        extra = (np.where(amb, np.abs(n1 - n0), 0.0) @ W) * (1 + 2.0 ** -7)
-        hx = np.where(amb & (np.abs(n1) > np.abs(n0)), n1, n0)
-        ref.F = np.maximum(ref.F, P.reference(d, hx, pc, dtype, cols=cols).F) + extra
-    c0, c1 = cols or (0, d["N"])
-    return P.check(y[:, c0:c1], ref, pc, dtype, what=what)
-
-
 @pytest.mark.parametrize("dtype", DTS, ids=["f16", "bf16"])
 @pytest.mark.parametrize("M", [1, 2])
 @pytest.mark.parametrize("H,I,act", [(4096, 11008, False), (4096, 11008, True), (8192, 1024, False)],
@@ -103,9 +87,9 @@ def test_norm_stages(dtype, M, H, I, act):
         assert np.array_equal(h1n, N.add_rounded(yan, rn, dtype)), f"h1 != rnd(y_a + r) ({kind})"
         assert np.array_equal(h2n, N.add_rounded(ybn, h1n, dtype)), f"h2 != rnd(y_b + h1) ({kind})"
         tag = f"{dt} M={M} H={H} act={act} {kind} launch {launch}"
-        _check_y(yan, da, xs, wa, eps, dtype, cols_h, f"rmsnorm stage {tag}")
-        _check_y(ybn, db, h1n, wb, eps, dtype, cols_h, f"add_rmsnorm stage (external residual) {tag}")
-        _check_y(_np(yc), dc, h2n, wc, eps, dtype, cols_i, f"add_rmsnorm stage (chain residual) {tag}")
+        N.check_y(yan, da, xs, wa, eps, dtype, cols_h, f"rmsnorm stage {tag}")
+        N.check_y(ybn, db, h1n, wb, eps, dtype, cols_h, f"add_rmsnorm stage (external residual) {tag}")
+        N.check_y(_np(yc), dc, h2n, wc, eps, dtype, cols_i, f"add_rmsnorm stage (chain residual) {tag}")
 
 
 def test_chain_without_norm_stages_keeps_its_shape():

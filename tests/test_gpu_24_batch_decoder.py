@@ -1,7 +1,7 @@
 """Independent decode rows on the GPU: the per-row decode attention (``agb200_decode_attention_rows``), the residual add
 + RMSNorm kernel (``agb200_add_rmsnorm``) and BatchDecoder against the transformers model it runs.
 
-Attention, B ∈ {1, 2, 3, 5, 8} × fp16 / bf16 × hd {64, 128} × G {1, 4, 8}, rows at positions 0, 31, 32, 33 (tile
+Attention, B ∈ {1, 2, 3, 5, 8} × fp16 / bf16 × hd {64, 128} × G {1, 4, 6, 7, 8}, rows at positions 0, 31, 32, 33 (tile
 edges), max_length - 1 and idle (-1):
 * each active row's new cache entries are bit-equal to apply_rotary_pos_emb at that row's position; every other cache
   byte is unchanged (rows above each position hold NaN, so a read past it would show);
@@ -117,7 +117,7 @@ def _positions(B, shift):
     return [POS[(b + shift) % len(POS)] for b in range(B)]
 
 
-@pytest.mark.parametrize("G", [1, 4, 8])
+@pytest.mark.parametrize("G", [1, 4, 6, 7, 8])
 @pytest.mark.parametrize("hd", [64, 128])
 @pytest.mark.parametrize("dtype", DTS, ids=["f16", "bf16"])
 @pytest.mark.parametrize("B", [1, 2, 3, 5, 8])

@@ -2,7 +2,7 @@
 on CUDA, and BatchDecoder / ChainDecoder with ``kv_cache_dtype=torch.float8_e4m3fn`` against transformers attending
 over the decoder's dequantised cache (see the comment above ``_qdq`` for why the decoder's rows, not HF's own).
 
-Attention, B ∈ {1, 2, 3, 5, 8} × fp16 / bf16 × hd {64, 128} × G {1, 4, 8}, rows at positions 0, 31, 32, 33, L - 1 and
+Attention, B ∈ {1, 2, 3, 5, 8} × fp16 / bf16 × hd {64, 128} × G {1, 4, 6, 7, 8}, rows at positions 0, 31, 32, 33, L - 1 and
 idle, as ``tests/test_gpu_24_batch_decoder.py``:
 * each active row's new codes and scales are bit-equal to ``quantize_kv`` of apply_rotary_pos_emb(k) and of v; every
   other code and scale byte is unchanged (positions above each row hold code 0x7F and NaN scales, so a read past the
@@ -138,7 +138,7 @@ def _report(what):
         print(f"[kv-fp8] {what} {dn}: largest err/bound so far {w:.3f}, mismatch rate {m}/{n}")
 
 
-@pytest.mark.parametrize("G", [1, 4, 8])
+@pytest.mark.parametrize("G", [1, 4, 6, 7, 8])
 @pytest.mark.parametrize("hd", [64, 128])
 @pytest.mark.parametrize("dtype", DTS, ids=["f16", "bf16"])
 @pytest.mark.parametrize("B", [1, 2, 3, 5, 8])
