@@ -156,12 +156,14 @@ class StaticCacheDecoder:
             raise RuntimeError(f"{self._who} needs the model on a CUDA device")
         return self.device
 
-    def _allocate(self, rows: int):
+    def _allocate(self, rows: int, cache_shape=None):
         """After every refusal: the CUDA device, the static caches of ``rows`` rows and the step's token ids.  The
         caches are per layer [rows, n_kv, max_length, head_dim] in the activation dtype, or E4M3 codes with fp32
-        scales ``k_scale`` / ``v_scale`` [rows, n_kv, max_length] for FP8 (else the scales are None)."""
+        scales ``k_scale`` / ``v_scale`` [rows, n_kv, max_length] for FP8 (else the scales are None).  ``cache_shape``
+        replaces [rows, n_kv, max_length, head_dim] (a paged cache's pools)."""
         self._cuda_device()
-        shape, n, dev = (rows, self.n_kv, self.max_length, self.head_dim), len(self._plans), self.device
+        shape = (rows, self.n_kv, self.max_length, self.head_dim) if cache_shape is None else tuple(cache_shape)
+        n, dev = len(self._plans), self.device
         self.k_cache = [torch.zeros(shape, dtype=FP8 if self._fp8 else self.dtype, device=dev) for _ in range(n)]
         self.v_cache = [torch.zeros_like(c) for c in self.k_cache]
         self.k_scale = self.v_scale = None
@@ -204,8 +206,6 @@ class StaticCacheDecoder:
         run every layer (its QuantLinear projections at M = n·T, its norms and MLP), so every rounding outside the
         attention is HF's; ``prefill_attention`` writes k̂ and v into the static caches and attends causally over them.
         No DynamicCache is built and only the last position reaches model.norm and lm_head."""
-        from .attention import prefill_attention
-
         inner = self.model.model
         if not hasattr(self, "_inv_freq"):
             self._inv_freq, self._attn_scaling = _rotary_params(inner.rotary_emb, self.head_dim, self._who)
@@ -216,12 +216,18 @@ class StaticCacheDecoder:
         for i, layer in enumerate(inner.layers):
             attn = self._plans[i][0]
             x = layer.input_layernorm(h)
-            kw = {} if self.k_scale is None else dict(k_scale=self.k_scale[i][rows], v_scale=self.v_scale[i][rows])
-            prefill_attention(attn.q_proj(x), attn.k_proj(x), attn.v_proj(x), self.k_cache[i][rows],
-                              self.v_cache[i][rows], start, self._inv_freq, self._attn_scaling, self.scaling, out, **kw)
+            self._extend_attention(i, rows, attn.q_proj(x), attn.k_proj(x), attn.v_proj(x), start, out)
             h = h + attn.o_proj(out)
             h = h + layer.mlp(layer.post_attention_layernorm(h))
         return self.model.lm_head(inner.norm(h[:, -1:]))[:, 0]
+
+    def _extend_attention(self, i: int, rows: slice, q, k, v, start, out):
+        """``prefill_attention`` of layer i on cache rows ``rows``: writes the new rows and attends causally."""
+        from .attention import prefill_attention
+
+        kw = {} if self.k_scale is None else dict(k_scale=self.k_scale[i][rows], v_scale=self.v_scale[i][rows])
+        prefill_attention(q, k, v, self.k_cache[i][rows], self.v_cache[i][rows], start, self._inv_freq,
+                          self._attn_scaling, self.scaling, out, **kw)
 
     # ------------------------------------------------------------------ one step
     def _run_step(self, ids: torch.Tensor, use_graph: bool, body=None):

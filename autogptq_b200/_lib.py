@@ -34,6 +34,7 @@ ATTN_HEAD_DIMS = (64, 128)
 ATTN_MAX_G = 8
 ATTN_MAX_B = 2
 ATTN_ROWS_MAX_B = 8            # AGB200_ATTN_ROWS_MAX_B
+KV_BLOCK_SIZES = (16, 32, 64, 128, 256)   # block sizes of a paged KV cache
 SAMPLE_MAX_V = 262144          # AGB200_SAMPLE_MAX_V
 
 _lib = None
@@ -116,6 +117,14 @@ def _declare(lib):
         "agb200_prefill_attention": (I, [P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, I, P]),
         "agb200_prefill_attention_fp8": (I, [P, P, P, P, P, P, P, P, P, c_float, c_float, P, I, I, I, I, I, I, I,
                                               P]),
+        "agb200_decode_attention_rows_paged": (I, [P, P, P, P, P, P, I, I, I, P, P, c_float, c_float, P, I, I, I, I, I,
+                                                    P, S, P]),
+        "agb200_decode_attention_rows_paged_fp8": (I, [P, P, P, P, P, P, P, P, I, I, I, P, P, c_float, c_float, P, I,
+                                                        I, I, I, I, P, S, P]),
+        "agb200_prefill_attention_paged": (I, [P, P, P, P, P, P, I, I, I, P, P, c_float, c_float, P, I, I, I, I, I, I,
+                                                P]),
+        "agb200_prefill_attention_paged_fp8": (I, [P, P, P, P, P, P, P, P, I, I, I, P, P, c_float, c_float, P, I, I, I,
+                                                    I, I, I, P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
         "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
         "agb200_sample": (I, [P, c_int64, I, I, I, P, P, P, P, P, P, P, P]),

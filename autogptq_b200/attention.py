@@ -22,6 +22,14 @@ the activation dtype.  Half the cache bytes (hd + 4 per row instead of 2·hd).
 tokens to each of up to eight rows at their own ``start`` positions and attends them causally over the cache: the
 cache rows it writes are bit-equal to the decode step's for the same token, whatever T, and the attention runs on the
 tensor cores (mma.sync, fp32 softmax).  Feeding a prompt in chunks gives the same cache bytes as one call.
+
+Paged cache (``decode_attention_rows_paged`` / ``prefill_attention_paged``, DESIGN §3.22): per layer, pools
+[num_blocks, n_kv, block_size, hd] (and for FP8 scale pools [num_blocks, n_kv, block_size]) and an int32 block table
+[B, max_blocks]; position t of row b is row t % block_size of block table[b, t // block_size].  block_size is a power of
+two in 16..256.  For the same contents the outputs and every cache byte written are bit-equal to the static entries'
+with max_length = max_blocks·block_size.  A table entry outside [0, num_blocks) is no block: it is never dereferenced,
+and the row it belongs to gets NaN (decode: if it holds pos, or any position below it; prefill: any position of
+0 .. start + T - 1), with no write to the pools at pos (decode) or at all (prefill).
 """
 from __future__ import annotations
 
@@ -80,6 +88,20 @@ def attention_rows_supported(n_heads: int, n_kv: int, head_dim: int, batch: int,
         why = f"batch {batch}; the kernel takes 1..{_lib.ATTN_ROWS_MAX_B} independent rows"
     if why is None and batch * n_kv * max_length * head_dim >= 2 ** 31:
         why = "the cache has 2^31 elements or more"
+    return why
+
+
+def paged_attention_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, block_size: int, num_blocks: int,
+                              dtype) -> str | None:
+    """None when the paged entries take this shape (pools of ``num_blocks`` blocks of ``block_size`` rows), else the
+    reason they do not: the per-row decode limits, with the pool in place of the static cache."""
+    if block_size not in _lib.KV_BLOCK_SIZES:
+        return f"block_size {block_size}; a power of two in {_lib.KV_BLOCK_SIZES[0]}..{_lib.KV_BLOCK_SIZES[-1]}"
+    if num_blocks < 1:
+        return f"num_blocks {num_blocks}; at least 1"
+    why = attention_rows_supported(n_heads, n_kv, head_dim, batch, 1, dtype)
+    if why is None and num_blocks * n_kv * block_size * head_dim >= 2 ** 31:
+        why = "the pool has 2^31 elements or more"
     return why
 
 
@@ -147,6 +169,76 @@ def prefill_attention(q, k, v, k_cache, v_cache, start, inv_freq, attention_scal
     return out
 
 
+def _paged(entry, q, k_pool, block_table, n_lead):
+    """The paged entries' own checks: (B, block_size, max_blocks, the checks of ``_checked``)."""
+    if k_pool.dim() != 4:
+        raise ValueError(f"k_pool must be [num_blocks, n_kv, block_size, head_dim], got {tuple(k_pool.shape)}")
+    num_blocks, n_kv, bs, hd = k_pool.shape
+    if block_table.dtype != torch.int32 or block_table.dim() != 2:
+        raise ValueError(f"{entry}: block_table must be int32 [B, max_blocks], got {block_table.dtype} "
+                         f"{list(block_table.shape)}")
+    B, max_blocks = block_table.shape
+    if q.dim() != n_lead + 1 or q.shape[0] != B:
+        raise ValueError(f"{entry}: q must have {B} rows (block_table's), got {tuple(q.shape)}")
+    if max_blocks < 1 or max_blocks * bs > 2 ** 30:
+        raise ValueError(f"{entry}: block_table has {max_blocks} blocks per row of {bs}; need 1..2^30 positions")
+    if block_table.device != k_pool.device or not block_table.is_contiguous():
+        raise ValueError(f"{entry}: block_table must be contiguous on {k_pool.device}")
+
+    def supported(n_heads, n_kv_, hd_, batch, block_size, dt):
+        return paged_attention_supported(n_heads, n_kv_, hd_, batch, block_size, num_blocks, dt)
+    return B, bs, max_blocks, supported
+
+
+def decode_attention_rows_paged(q, k, v, k_pool, v_pool, block_table, pos, inv_freq, attention_scaling: float,
+                                scaling: float, out, workspace=None, *, k_scale=None, v_scale=None):
+    """``decode_attention_rows`` over a paged cache (module docstring): pools [num_blocks, n_kv, block_size, hd] (the
+    block size is the pools'), block_table int32 [B, max_blocks] (device), pos int64 [B].  float8_e4m3fn pools with
+    ``k_scale`` / ``v_scale`` fp32 [num_blocks, n_kv, block_size]: the FP8 cache.  The workspace is
+    ``decode_attention_workspace(B, n_heads, n_kv, hd, max_blocks·block_size)``.  Raises NotImplementedError outside
+    the kernel's limits."""
+    B, bs, max_blocks, supported = _paged("decode_attention_rows_paged", q, k_pool, block_table, 1)
+    entry, caches, n_heads, dt = _checked("decode_attention_rows_paged", supported, None, q, k, v, k_pool, v_pool, pos,
+                                          inv_freq, out, k_scale, v_scale, rows=B)
+    num_blocks, n_kv, _, hd = k_pool.shape
+    L, dev, lib = max_blocks * bs, k_pool.device, _lib.load()
+    with torch.cuda.device(dev):
+        need = int(lib.agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, hd, L))
+        if workspace is None:
+            workspace = decode_attention_workspace(B, n_heads, n_kv, hd, L, dev)
+        elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
+            raise ValueError(f"workspace must hold {need} bytes on {dev}")
+        rc = getattr(lib, f"agb200_{entry}")(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, block_table.data_ptr(), bs, num_blocks, max_blocks,
+            pos.data_ptr(), inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads,
+            n_kv, hd, _DT[dt], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
+            torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, f"agb200_{entry}")
+    return out
+
+
+def prefill_attention_paged(q, k, v, k_pool, v_pool, block_table, start, inv_freq, attention_scaling: float,
+                            scaling: float, out, *, k_scale=None, v_scale=None):
+    """``prefill_attention`` over a paged cache (module docstring): q [B, T, n_heads·hd], pools and block_table as
+    ``decode_attention_rows_paged``, start int64 [B].  A row with a position 0 .. start + T - 1 outside the table or
+    without a block gets NaN and no write.  Raises NotImplementedError outside the kernel's limits."""
+    B, bs, max_blocks, supported = _paged("prefill_attention_paged", q, k_pool, block_table, 2)
+    T = q.shape[1]
+    if T < 1:
+        raise ValueError("prefill_attention_paged: T must be at least 1")
+    entry, caches, n_heads, dt = _checked("prefill_attention_paged", supported, None, q, k, v, k_pool, v_pool, start,
+                                          inv_freq, out, k_scale, v_scale, T=T, pos_name="start", rows=B)
+    num_blocks, n_kv, _, hd = k_pool.shape
+    dev, lib = k_pool.device, _lib.load()
+    with torch.cuda.device(dev):
+        rc = getattr(lib, f"agb200_{entry}")(
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, block_table.data_ptr(), bs, num_blocks, max_blocks,
+            start.data_ptr(), inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, T,
+            n_heads, n_kv, hd, _DT[dt], torch.cuda.current_stream(dev).cuda_stream)
+    _lib.check(rc, f"agb200_{entry}")
+    return out
+
+
 def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out,
             workspace, k_scale=None, v_scale=None):
     """Checks and the call of agb200_<entry> (agb200_<entry>_fp8 for a float8_e4m3fn cache); ``n_pos`` elements of pos
@@ -158,12 +250,14 @@ def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, a
 
 
 def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, out, k_scale, v_scale, T=None,
-             pos_name="pos"):
+             pos_name="pos", rows=None):
     """``_launch``'s checks: (entry with _fp8 for an FP8 cache, the cache pointers after v, n_heads, dtype).  With
-    ``T`` the activations are [B, T, features] instead of [B, features]."""
+    ``T`` the activations are [B, T, features] instead of [B, features].  ``rows``: B when the caches are a paged
+    cache's pools [num_blocks, n_kv, block_size, head_dim] (else B is the caches' first dimension)."""
     if k_cache.dim() != 4:
         raise ValueError(f"k_cache must be [B, n_kv, max_length, head_dim], got {tuple(k_cache.shape)}")
-    B, n_kv, L, hd = k_cache.shape
+    nb, n_kv, L, hd = k_cache.shape
+    B = nb if rows is None else rows
     dev = k_cache.device
     if dev.type != "cuda":
         raise RuntimeError(f"{entry} needs CUDA tensors (there is no CPU fallback)")
@@ -181,10 +275,11 @@ def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, 
     if why is not None:
         raise NotImplementedError(f"{entry}: {why}")
     checks = [("q", q, lead + (n_heads * hd,), dt), ("k", k, lead + (n_kv * hd,), dt),
-              ("v", v, lead + (n_kv * hd,), dt), ("v_cache", v_cache, (B, n_kv, L, hd), k_cache.dtype),
+              ("v", v, lead + (n_kv * hd,), dt), ("v_cache", v_cache, (nb, n_kv, L, hd), k_cache.dtype),
               ("out", out, lead + (n_heads * hd,), dt)]
     if fp8:
-        checks += [("k_scale", k_scale, (B, n_kv, L), torch.float32), ("v_scale", v_scale, (B, n_kv, L), torch.float32)]
+        checks += [("k_scale", k_scale, (nb, n_kv, L), torch.float32),
+                   ("v_scale", v_scale, (nb, n_kv, L), torch.float32)]
     for name, t, shape, want in checks:
         if tuple(t.shape) != shape:
             raise ValueError(f"{name} must be {list(shape)}, got {list(t.shape)}")
@@ -234,4 +329,4 @@ def _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scali
 
 __all__ = ["decode_attention", "decode_attention_rows", "decode_attention_workspace", "attention_supported",
            "attention_rows_supported", "prefill_attention", "prefill_attention_supported", "quantize_kv",
-           "dequantize_kv"]
+           "dequantize_kv", "decode_attention_rows_paged", "prefill_attention_paged", "paged_attention_supported"]

@@ -36,19 +36,28 @@ continues the sequence (a new conversation turn, or the next chunk of a long pro
 Tokens are greedy, or sampled (temperature, top-k, top-p, min-p; DESIGN §3.21) by ``autogptq_b200.sampling``'s kernel,
 which runs in the step's graph: each slot's parameters and seed live in device tensors [max_batch], so one graph serves
 any mix of greedy and sampled slots, and a slot's token depends only on its own logits, parameters, seed and position.
+With ``kv_block_size`` the KV cache is paged (DESIGN §3.22): one pool of ``kv_blocks`` blocks per layer, a block table
+per slot, and blocks shared by reference.  The memory then follows the tokens held, not ``max_batch × max_length``;
+``fork(src, dst)`` gives an idle slot another slot's prefix without recomputing or copying its full blocks, and
+``generate(..., n=k)`` prefills each prompt once and samples k continuations from it.  The step, its graph and its
+results are the static cache's, bit for bit; only where a cache row lives changes.
+
 Scope: Llama, Mistral and Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too); mixture-of-experts
 blocks are refused.  The model checks, the caches, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
 ``ChainDecoder``, which runs each block of batch <= 2 sequences in lockstep as one decode-chain launch.
 """
 from __future__ import annotations
 
+import dataclasses
 from collections import deque
 
 import torch
 
 from . import _lib
 from ._decoding import StaticCacheDecoder, _is_moe_block, _plan_common, _rotary_params
-from .attention import attention_rows_supported, decode_attention_rows, decode_attention_workspace
+from .attention import (attention_rows_supported, decode_attention_rows, decode_attention_rows_paged,
+                        decode_attention_workspace, paged_attention_supported, prefill_attention_paged, quantize_kv)
+from .paged_kv import BlockAllocator, blocks_for, worst_case_blocks
 from .mlp import forward_gate_up
 from .moe import add_rmsnorm, add_rmsnorm_supported
 from .qlinear import forward_group
@@ -60,18 +69,31 @@ _WHO = "BatchDecoder"
 class BatchDecoder(StaticCacheDecoder):
     """Greedy or sampling decoder of up to ``max_batch`` <= 8 independent sequences over a transformers ``LlamaForCausalLM`` /
     ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose projections are ``autogptq_b200.QuantLinear``.
-    ``kv_cache_dtype``: None (the activation dtype) or ``torch.float8_e4m3fn``."""
+    ``kv_cache_dtype``: None (the activation dtype) or ``torch.float8_e4m3fn``.  ``kv_block_size``: None (a static
+    cache, ``k_cache[i]`` [max_batch, n_kv, max_length, head_dim]) or a power of two in 16..256: a paged cache of
+    ``kv_blocks`` blocks per layer (default max_batch·ceil(max_length / kv_block_size), the static capacity), whose
+    pools are ``k_cache[i]`` [kv_blocks, n_kv, kv_block_size, head_dim] (FP8 scales ``k_scale[i]``
+    [kv_blocks, n_kv, kv_block_size])."""
 
     _who = _WHO
 
-    def __init__(self, model, max_batch: int = 8, max_length: int = 4096, kv_cache_dtype=None):
+    def __init__(self, model, max_batch: int = 8, max_length: int = 4096, kv_cache_dtype=None, kv_block_size=None,
+                 kv_blocks=None):
         if not 1 <= max_batch <= _lib.ATTN_ROWS_MAX_B:
             raise NotImplementedError(f"{_WHO}: max_batch {max_batch}; the decode kernels run 1..{_lib.ATTN_ROWS_MAX_B} "
                                       "rows")
         self.max_batch = int(max_batch)
         self._read_model(model, max_length, kv_cache_dtype)
         B, H, hd, dt = self.max_batch, self.hidden_size, self.head_dim, self.dtype
-        why = attention_rows_supported(self.n_heads, self.n_kv, hd, B, self.max_length, dt)
+        self.kv_block_size = None if kv_block_size is None else int(kv_block_size)
+        if self.kv_block_size is None:
+            if kv_blocks is not None:
+                raise ValueError(f"{_WHO}: kv_blocks goes with kv_block_size (a paged cache)")
+            why = attention_rows_supported(self.n_heads, self.n_kv, hd, B, self.max_length, dt)
+        else:
+            self._max_blocks = blocks_for(self.max_length, self.kv_block_size)
+            self.kv_blocks = B * self._max_blocks if kv_blocks is None else int(kv_blocks)
+            why = paged_attention_supported(self.n_heads, self.n_kv, hd, B, self.kv_block_size, self.kv_blocks, dt)
         if why is not None:
             raise NotImplementedError(f"{_WHO}: model.layers.*.self_attn: {why}")
         self._inv_freq, self._attn_scaling = _rotary_params(model.model.rotary_emb, hd, _WHO)
@@ -92,7 +114,39 @@ class BatchDecoder(StaticCacheDecoder):
         self._n1 = torch.zeros((B, H), dtype=dt, device=dev)
         self._n2 = torch.zeros((B, H), dtype=dt, device=dev)
         self._attn_out = torch.zeros((B, self.n_heads * hd), dtype=dt, device=dev)
-        self._attn_ws = decode_attention_workspace(B, self.n_heads, self.n_kv, hd, self.max_length, dev)
+        L = self.max_length if self.kv_block_size is None else self._max_blocks * self.kv_block_size
+        self._attn_ws = decode_attention_workspace(B, self.n_heads, self.n_kv, hd, L, dev)
+
+    def _allocate(self, rows: int):
+        """The static caches, or the pools, block table and allocator of a paged cache (``k_cache`` etc. are then the
+        pools; the table is -1, no block, wherever a slot holds none)."""
+        if self.kv_block_size is None:
+            return super()._allocate(rows)
+        nb, bs = self.kv_blocks, self.kv_block_size
+        super()._allocate(rows, (nb, self.n_kv, bs, self.head_dim))
+        self._table = torch.full((rows, self._max_blocks), -1, dtype=torch.int32, device=self.device)
+        self._blocks = BlockAllocator(nb, bs, rows, self._max_blocks)
+
+    @property
+    def kv_cache_bytes(self) -> int:
+        """Bytes of the KV cache: every layer's caches (static) or pools (paged), scales included."""
+        ts = self.k_cache + self.v_cache + (self.k_scale + self.v_scale if self.k_scale is not None else [])
+        return sum(t.numel() * t.element_size() for t in ts)
+
+    @property
+    def kv_blocks_free(self):
+        """Free blocks of the paged cache's pool (None for a static cache)."""
+        return None if self.kv_block_size is None else self._blocks.free
+
+    def _need_paged(self, what: str):
+        if self.kv_block_size is None:
+            raise NotImplementedError(f"{_WHO}.{what} needs the paged KV cache (BatchDecoder(..., kv_block_size=...))")
+
+    def _map(self, need: dict):
+        """Blocks for positions 0 .. need[s] - 1 of each slot s, mirrored into the device table; raises RuntimeError
+        before any change when the pool cannot supply them."""
+        for s, j, b in self._blocks.map(need):
+            self._table[s, j] = b
 
     def _plan(self, i: int, layer):
         mlp = getattr(layer, "mlp", None)
@@ -109,6 +163,9 @@ class BatchDecoder(StaticCacheDecoder):
 
     @positions.setter
     def positions(self, ps):
+        if self.kv_block_size is not None:
+            raise RuntimeError(f"{_WHO}: positions cannot be set with a paged KV cache (a position needs its blocks); "
+                               "use release, prefill or extend")
         ps = [int(p) for p in ps]
         if len(ps) != self.max_batch or any(not -1 <= p <= self.max_length for p in ps):
             raise ValueError(f"positions must be {self.max_batch} values in -1..{self.max_length}, got {ps}")
@@ -130,6 +187,13 @@ class BatchDecoder(StaticCacheDecoder):
         T = ids.shape[1]
         if not 1 <= T < self.max_length:
             raise ValueError(f"prompt length {T} must be in 1..{self.max_length - 1}")
+        if self.kv_block_size is not None:
+            own = sum(self._blocks.ref[b] == 1 for b in self._blocks.blocks[slot])     # freed by the release
+            if blocks_for(T, self.kv_block_size) > self._blocks.free + own:
+                raise RuntimeError(f"{_WHO}.prefill: the KV cache pool cannot hold {T} tokens ({self._blocks.free} "
+                                   "blocks free)")
+            self.release(slot)
+            self._map({slot: T})
         logits = self._prefill_cache(ids, slice(slot, slot + 1))
         self._pos[slot] = T
         self._host_pos[slot] = T
@@ -151,6 +215,8 @@ class BatchDecoder(StaticCacheDecoder):
         if p + T >= self.max_length:
             raise ValueError(f"{_WHO}.extend: slot {slot} at position {p} + {T} tokens must stay below "
                              f"max_length={self.max_length}")
+        if self.kv_block_size is not None:
+            self._map({slot: p + T})
         logits = self._extend(input_ids.to(self.device).view(1, T), slice(slot, slot + 1), [p])
         self._pos[slot] = p + T
         self._host_pos[slot] = p + T
@@ -176,10 +242,61 @@ class BatchDecoder(StaticCacheDecoder):
         return int(self._sampling.sample(logits.reshape(1, -1), counter, slice(slot, slot + 1))[0])
 
     def release(self, slot: int):
-        """Make the slot idle: its row is skipped by the attention and its cache row is left as it is."""
+        """Make the slot idle: its row is skipped by the attention and its cache row is left as it is (paged: the slot
+        drops its blocks; a block no slot holds is free)."""
         slot = self._check_slot(slot)
         self._pos[slot] = -1
         self._host_pos[slot] = -1
+        if self.kv_block_size is not None:
+            self._blocks.release(slot)
+            self._table[slot].fill_(-1)
+
+    @torch.no_grad()
+    def fork(self, src: int, dst: int):
+        """Make the idle slot ``dst`` continue the active slot ``src``'s sequence (paged cache only): ``dst`` takes
+        ``src``'s position and its full blocks by reference, and a copy of its partially filled last block (every
+        layer, FP8 scales included).  Sampling parameters are not copied.  Raises RuntimeError, with nothing changed,
+        when no block is free for the copy."""
+        self._need_paged("fork")
+        src, dst = self._check_slot(src), self._check_slot(dst)
+        p = self._host_pos[src]
+        if p < 0:
+            raise RuntimeError(f"{_WHO}.fork: slot {src} is idle")
+        if self._host_pos[dst] >= 0 or src == dst:
+            raise RuntimeError(f"{_WHO}.fork: slot {dst} must be idle")
+        blocks, copy = self._blocks.fork(src, dst, p)
+        if copy is not None:
+            a, b = copy
+            for ts in (self.k_cache, self.v_cache, self.k_scale or [], self.v_scale or []):
+                for t in ts:
+                    t[b].copy_(t[a])
+        self._table[dst, :len(blocks)] = torch.tensor(blocks, dtype=torch.int32)
+        self._pos[dst] = p
+        self._host_pos[dst] = p
+
+    def _store_kv(self, i: int, index, keys, values):
+        """Keys and values [1, n_kv, T, hd] of the slot ``index[0]`` at positions ``index[2]`` (0 .. T - 1) into its
+        blocks (paged); the static caches' ``_store_kv`` otherwise."""
+        if self.kv_block_size is None:
+            return super()._store_kv(i, index, keys, values)
+        slot, T = index[0].start, index[2].stop
+        t = torch.arange(T)
+        blk = torch.tensor(self._blocks.blocks[slot], dtype=torch.int64)[t // self.kv_block_size].to(self.device)
+        off = (t % self.kv_block_size).to(self.device)
+        if self.k_scale is None:
+            self.k_cache[i][blk, :, off] = keys[0].transpose(0, 1)
+            self.v_cache[i][blk, :, off] = values[0].transpose(0, 1)
+            return
+        for pool, scale, x in ((self.k_cache[i], self.k_scale[i], keys), (self.v_cache[i], self.v_scale[i], values)):
+            codes, sc = quantize_kv(x)
+            pool.view(torch.uint8)[blk, :, off] = codes.view(torch.uint8)[0].transpose(0, 1)
+            scale[blk, :, off] = sc[0].transpose(0, 1)
+
+    def _extend_attention(self, i: int, rows: slice, q, k, v, start, out):
+        if self.kv_block_size is None:
+            return super()._extend_attention(i, rows, q, k, v, start, out)
+        prefill_attention_paged(q, k, v, self.k_cache[i], self.v_cache[i], self._table[rows], start, self._inv_freq,
+                                self._attn_scaling, self.scaling, out, **self._cache_kwargs(i))
 
     # ------------------------------------------------------------------ one step
     def _step_body(self) -> torch.Tensor:
@@ -190,9 +307,14 @@ class BatchDecoder(StaticCacheDecoder):
         resid = self._x
         for i, (attn, mlp, _, (w2, eps2)) in enumerate(self._plans):
             q, k, v = forward_group([attn.q_proj, attn.k_proj, attn.v_proj], self._n1)
-            decode_attention_rows(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq,
-                                  self._attn_scaling, self.scaling, self._attn_out, self._attn_ws,
-                                  **self._cache_kwargs(i))
+            if self.kv_block_size is None:
+                decode_attention_rows(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq,
+                                      self._attn_scaling, self.scaling, self._attn_out, self._attn_ws,
+                                      **self._cache_kwargs(i))
+            else:
+                decode_attention_rows_paged(q, k, v, self.k_cache[i], self.v_cache[i], self._table, self._pos,
+                                            self._inv_freq, self._attn_scaling, self.scaling, self._attn_out,
+                                            self._attn_ws, **self._cache_kwargs(i))
             o = attn.o_proj(self._attn_out)
             add_rmsnorm(o, resid, w2, eps2, h=self._h1, n=self._n2)
             down = mlp.down_proj(forward_gate_up(mlp.gate_proj, mlp.up_proj, self._n2))
@@ -214,6 +336,8 @@ class BatchDecoder(StaticCacheDecoder):
             raise RuntimeError(f"{_WHO}.{what}: no slot is active (prefill one first)")
         if max(active) >= self.max_length:
             raise RuntimeError(f"{_WHO}.{what}: a slot's static cache is full ({self.max_length} tokens)")
+        if self.kv_block_size is not None:               # the block of each position the step writes
+            self._map({s: p + 1 for s, p in enumerate(self._host_pos) if p >= 0})
 
     @torch.no_grad()
     def step(self, ids: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
@@ -238,14 +362,27 @@ class BatchDecoder(StaticCacheDecoder):
 
     # ------------------------------------------------------------------ continuous batching
     @torch.no_grad()
-    def generate(self, prompts, max_new_tokens: int, eos_token_id=None, sampling=None) -> list:
+    def generate(self, prompts, max_new_tokens: int, eos_token_id=None, sampling=None, n: int = 1) -> list:
         """Decoding of every prompt (1-D, any lengths) -> a list of 1-D tensors, prompt followed by its new tokens: at
         most ``max_new_tokens``, fewer when ``eos_token_id`` comes first (it is kept).  Prompts fill free slots in
         order; a sequence retires at EOS or after ``max_new_tokens`` and the next prompt takes its slot.  One small
         device-to-host read per step (the tokens).  ``sampling``: None is greedy (the argmax of the logits); a
         ``SamplingParams``, or a list of one per prompt, samples: each admitted prompt's parameters go to its slot, the
-        first token comes from ``sample`` and the later ones from ``step_sample``."""
+        first token comes from ``sample`` and the later ones from ``step_sample``.
+
+        ``n`` > 1 (paged cache and ``sampling`` only): each prompt is prefilled once and forked into ``n`` slots, and the
+        result lists its ``n`` samples prompt-major (prompt j's copy i at j·n + i).  Copy i of a prompt whose seed is s
+        samples with seed (s + i) mod 2^64, so it equals an ``n=1`` run with that seed; ``seed=None`` draws a seed per
+        copy.  With a paged cache a prompt is admitted only when the pool's uncommitted blocks cover its worst case
+        (``paged_kv.worst_case_blocks``), so no step runs out of blocks; one that could never fit is a ValueError."""
         prompts = list(prompts)
+        n = int(n)
+        if n != 1:
+            self._need_paged("generate(n > 1)")
+            if not 1 <= n <= self.max_batch:
+                raise ValueError(f"{_WHO}.generate: n={n} samples per prompt; 1..max_batch={self.max_batch}")
+            if sampling is None:
+                raise ValueError(f"{_WHO}.generate: n > 1 needs sampling (greedy copies would be identical)")
         params = None if sampling is None else sampling_list(sampling, len(prompts), f"{_WHO}.generate")
         prompts = [p.reshape(-1) for p in prompts]
         if max_new_tokens < 1:
@@ -254,45 +391,73 @@ class BatchDecoder(StaticCacheDecoder):
             if p.numel() + max_new_tokens > self.max_length:
                 raise ValueError(f"prompt {j}: {p.numel()} tokens + {max_new_tokens} new tokens exceed "
                                  f"max_length={self.max_length}")
+        paged = self.kv_block_size is not None
+        worst = [0] * len(prompts)
+        if paged:
+            worst = [worst_case_blocks(p.numel(), max_new_tokens, n, self.kv_block_size) for p in prompts]
+            for j, w in enumerate(worst):
+                if w > self.kv_blocks:
+                    raise ValueError(f"prompt {j}: {prompts[j].numel()} tokens + {max_new_tokens} new tokens, {n} "
+                                     f"sample(s), may need {w} blocks; the pool has {self.kv_blocks}")
         for s in range(self.max_batch):
             if self._host_pos[s] >= 0:
                 self.release(s)
         queue = deque(range(len(prompts)))
-        new = [[] for _ in prompts]
-        owner = [None] * self.max_batch              # prompt index held by each slot
+        new = [[] for _ in range(len(prompts) * n)]
+        owner = [None] * self.max_batch              # output index (prompt j's copy i: j·n + i) held by each slot
+        live = [0] * len(prompts)                    # copies of each prompt still decoding
+        committed = 0                                # worst-case blocks of the prompts with live copies
 
         def take(s, tok):
             """Record slot s's next token; retire the sequence when it is done."""
-            j = owner[s]
-            new[j].append(tok)
-            if tok == eos_token_id or len(new[j]) >= max_new_tokens:
+            nonlocal committed
+            o = owner[s]
+            new[o].append(tok)
+            if tok == eos_token_id or len(new[o]) >= max_new_tokens:
                 self.release(s)
                 owner[s] = None
+                live[o // n] -= 1
+                if live[o // n] == 0:
+                    committed -= worst[o // n]
+
+        def admit(j, slots):
+            nonlocal committed
+            committed += worst[j]
+            live[j] = n
+            for i, s in enumerate(slots):
+                owner[s] = j * n + i
+                if params is not None:
+                    seed = params[j].seed
+                    self.set_sampling(s, params[j] if seed is None or i == 0 else
+                                      dataclasses.replace(params[j], seed=(seed + i) % 2 ** 64))
+            logits = self.prefill(slots[0], prompts[j])
+            for s in slots[1:]:
+                self.fork(slots[0], s)
+            for s in slots:
+                take(s, int(logits.argmax()) if params is None else self.sample(s, logits))
 
         while True:
-            for s in range(self.max_batch):
-                while owner[s] is None and queue:
-                    j = queue.popleft()
-                    owner[s] = j
-                    if params is None:
-                        take(s, int(self.prefill(s, prompts[j]).argmax()))
-                    else:
-                        self.set_sampling(s, params[j])
-                        take(s, self.sample(s, self.prefill(s, prompts[j])))
-            live = [s for s in range(self.max_batch) if owner[s] is not None]
-            if not live:
+            while queue:
+                free = [s for s in range(self.max_batch) if owner[s] is None]
+                j = queue[0]
+                if len(free) < n or (paged and committed + worst[j] > self.kv_blocks):
+                    break
+                queue.popleft()
+                admit(j, free[:n])
+            active = [s for s in range(self.max_batch) if owner[s] is not None]
+            if not active:
                 break
             ids = torch.zeros(self.max_batch, dtype=torch.int64)
-            for s in live:
+            for s in active:
                 ids[s] = new[owner[s]][-1]
             if params is None:
                 toks = self.step(ids.to(self.device)).argmax(-1).tolist()
             else:
                 toks = self.step_sample(ids.to(self.device))[0].tolist()
-            for s in live:
+            for s in active:
                 take(s, toks[s])
-        return [torch.cat([p.to(self.device), torch.tensor(t, dtype=p.dtype, device=self.device)])
-                for p, t in zip(prompts, new)]
-
+        return [torch.cat([prompts[o // n].to(self.device), torch.tensor(t, dtype=prompts[o // n].dtype,
+                                                                         device=self.device)])
+                for o, t in enumerate(new)]
 
 __all__ = ["BatchDecoder"]

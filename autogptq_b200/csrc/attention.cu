@@ -1,5 +1,6 @@
-// Host side of the decode attention (include/autogptq_b200.h: agb200_decode_attention*, 16-bit and FP8 caches): argument
-// checking, the split count, workspace layout and the launch on the caller's stream.  Kernel: attention.cuh.
+// Host side of the decode attention (include/autogptq_b200.h: agb200_decode_attention*, 16-bit and FP8 caches, static
+// or paged): argument checking, the split count, workspace layout and the launch on the caller's stream.  Kernel:
+// attention.cuh.
 #include <cuda_runtime.h>
 
 #include "attention.cuh"
@@ -40,20 +41,30 @@ size_t agb200_decode_attention_workspace_bytes(int B, int n_heads, int n_kv, int
 namespace {
 
 template <bool kBf16, int kHd>
-void launch_attention(bool fp8, dim3 grid, cudaStream_t s, const agb::DecodeAttnParams& p) {
-  if (fp8) agb::decode_attention_kernel<kBf16, kHd, true><<<grid, agb::kAttnThreads, 0, s>>>(p);
-  else agb::decode_attention_kernel<kBf16, kHd><<<grid, agb::kAttnThreads, 0, s>>>(p);
+void launch_attention(bool fp8, const agb::KvPaging* paging, dim3 grid, cudaStream_t s,
+                      const agb::DecodeAttnParams& p) {
+  if (paging) {
+    agb::DecodeAttnPagedParams pp{};
+    static_cast<agb::DecodeAttnParams&>(pp) = p;
+    pp.paging = *paging;
+    if (fp8) agb::decode_attention_kernel<kBf16, kHd, true, true><<<grid, agb::kAttnThreads, 0, s>>>(pp);
+    else agb::decode_attention_kernel<kBf16, kHd, false, true><<<grid, agb::kAttnThreads, 0, s>>>(pp);
+  } else {
+    if (fp8) agb::decode_attention_kernel<kBf16, kHd, true><<<grid, agb::kAttnThreads, 0, s>>>(p);
+    else agb::decode_attention_kernel<kBf16, kHd><<<grid, agb::kAttnThreads, 0, s>>>(p);
+  }
 }
 
 // Every entry: `what` names the entry in errors, `pos_stride` 0 (one position) or 1 (a position per row); k_scale and
-// v_scale are given exactly for an FP8 cache (E4M3 codes in k_cache / v_cache) and null for a 16-bit one.
+// v_scale are given exactly for an FP8 cache (E4M3 codes in k_cache / v_cache) and null for a 16-bit one.  A paged
+// cache (`paging` non-null, DESIGN §3.22) has num_blocks blocks and max_length = max_blocks·block_size.
 int decode_attention(const char* what, int max_b, int pos_stride, const void* q, const void* k, const void* v,
                      void* k_cache, void* v_cache, float* k_scale, float* v_scale, bool fp8, const int64_t* pos,
                      const float* inv_freq, float attention_scaling, float scaling, void* out, int B, int n_heads,
                      int n_kv, int head_dim, int max_length, int dtype, void* workspace, size_t workspace_bytes,
-                     void* stream) {
+                     void* stream, const agb::KvPaging* paging = nullptr) {
   if (!q || !k || !v || !k_cache || !v_cache || !pos || !inv_freq || !out || !workspace ||
-      (fp8 && (!k_scale || !v_scale)))
+      (fp8 && (!k_scale || !v_scale)) || (paging && !paging->table))
     return failf(AGB200_EINVAL, "%s: null pointer argument", what);
   if (B <= 0 || n_heads <= 0 || n_kv <= 0 || head_dim <= 0 || max_length <= 0 || n_heads % n_kv != 0)
     return failf(AGB200_EINVAL, "%s: need positive B, n_heads, n_kv, head_dim, max_length and "
@@ -66,9 +77,10 @@ int decode_attention(const char* what, int max_b, int pos_stride, const void* q,
   if (n_heads / n_kv > agb::kAttnMaxG)
     return failf(AGB200_ENOSUP, "%s: %d query heads per kv head; at most %d", what, n_heads / n_kv, agb::kAttnMaxG);
   if (B > max_b) return failf(AGB200_ENOSUP, "%s: batch %d; at most %d", what, B, max_b);
-  if (static_cast<long long>(B) * n_kv * max_length * head_dim >= (1ll << 31))
-    return failf(AGB200_ENOSUP, "%s: the cache holds %lld elements; at most 2^31 - 1", what,
-                 static_cast<long long>(B) * n_kv * max_length * head_dim);
+  const long long rows = paging ? static_cast<long long>(paging->num_blocks) << paging->block_shift
+                                : static_cast<long long>(B) * max_length;
+  if (rows * n_kv * head_dim >= (1ll << 31))
+    return failf(AGB200_ENOSUP, "%s: the cache holds %lld elements; at most 2^31 - 1", what, rows * n_kv * head_dim);
   if (!aligned(q, 16) || !aligned(k, 16) || !aligned(v, 16) || !aligned(k_cache, 16) || !aligned(v_cache, 16) ||
       !aligned(out, 16) || !aligned(pos, 8) || !aligned(inv_freq, 4) || !aligned(workspace, 256))
     return failf(AGB200_EINVAL, "%s: q, k, v, the caches and out must be 16-byte aligned, the workspace "
@@ -103,17 +115,33 @@ int decode_attention(const char* what, int max_b, int pos_stride, const void* q,
   cudaStream_t s = static_cast<cudaStream_t>(stream);
   const bool bf16 = dtype == AGB200_BF16;
   if (head_dim == 128) {
-    if (bf16) launch_attention<true, 128>(fp8, grid, s, p);
-    else launch_attention<false, 128>(fp8, grid, s, p);
+    if (bf16) launch_attention<true, 128>(fp8, paging, grid, s, p);
+    else launch_attention<false, 128>(fp8, paging, grid, s, p);
   } else {
-    if (bf16) launch_attention<true, 64>(fp8, grid, s, p);
-    else launch_attention<false, 64>(fp8, grid, s, p);
+    if (bf16) launch_attention<true, 64>(fp8, paging, grid, s, p);
+    else launch_attention<false, 64>(fp8, paging, grid, s, p);
   }
   AGB_CUDA(cudaGetLastError());
   return 0;
 }
 
 }  // namespace
+
+int paging_of(const char* what, const int32_t* table, int block_size, int num_blocks, int max_blocks,
+              agb::KvPaging& pg) {
+  if (block_size < 16 || block_size > 256 || (block_size & (block_size - 1)) != 0)
+    return failf(AGB200_ENOSUP, "%s: block_size %d; a power of two in 16..256", what, block_size);
+  if (num_blocks <= 0 || max_blocks <= 0 || static_cast<long long>(max_blocks) * block_size > (1ll << 30))
+    return failf(AGB200_EINVAL, "%s: need positive num_blocks and max_blocks, max_blocks * block_size <= 2^30 "
+                 "(got num_blocks=%d, max_blocks=%d, block_size=%d)", what, num_blocks, max_blocks, block_size);
+  if (!aligned(table, 4)) return failf(AGB200_EINVAL, "%s: the block table must be 4-byte aligned", what);
+  pg.table = table;
+  pg.max_blocks = max_blocks;
+  pg.num_blocks = num_blocks;
+  pg.block_shift = 0;
+  while ((1 << pg.block_shift) < block_size) ++pg.block_shift;
+  return 0;
+}
 
 extern "C" {
 
@@ -153,6 +181,33 @@ int agb200_decode_attention_rows_fp8(const void* q, const void* k, const void* v
   return decode_attention("decode_attention_rows_fp8", agb::kAttnRowsMaxB, 1, q, k, v, k_cache, v_cache, k_scale,
                           v_scale, true, pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim,
                           max_length, dtype, workspace, workspace_bytes, stream);
+}
+
+int agb200_decode_attention_rows_paged(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                       const int32_t* block_table, int block_size, int num_blocks, int max_blocks,
+                                       const int64_t* pos, const float* inv_freq, float attention_scaling,
+                                       float scaling, void* out, int B, int n_heads, int n_kv, int head_dim, int dtype,
+                                       void* workspace, size_t workspace_bytes, void* stream) {
+  agb::KvPaging pg{};
+  if (const int rc = paging_of("decode_attention_rows_paged", block_table, block_size, num_blocks, max_blocks, pg))
+    return rc;
+  return decode_attention("decode_attention_rows_paged", agb::kAttnRowsMaxB, 1, q, k, v, k_pool, v_pool, nullptr,
+                          nullptr, false, pos, inv_freq, attention_scaling, scaling, out, B, n_heads, n_kv, head_dim,
+                          max_blocks * block_size, dtype, workspace, workspace_bytes, stream, &pg);
+}
+
+int agb200_decode_attention_rows_paged_fp8(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                           float* k_scale_pool, float* v_scale_pool, const int32_t* block_table,
+                                           int block_size, int num_blocks, int max_blocks, const int64_t* pos,
+                                           const float* inv_freq, float attention_scaling, float scaling, void* out,
+                                           int B, int n_heads, int n_kv, int head_dim, int dtype, void* workspace,
+                                           size_t workspace_bytes, void* stream) {
+  agb::KvPaging pg{};
+  if (const int rc = paging_of("decode_attention_rows_paged_fp8", block_table, block_size, num_blocks, max_blocks, pg))
+    return rc;
+  return decode_attention("decode_attention_rows_paged_fp8", agb::kAttnRowsMaxB, 1, q, k, v, k_pool, v_pool,
+                          k_scale_pool, v_scale_pool, true, pos, inv_freq, attention_scaling, scaling, out, B, n_heads,
+                          n_kv, head_dim, max_blocks * block_size, dtype, workspace, workspace_bytes, stream, &pg);
 }
 
 }  // extern "C"

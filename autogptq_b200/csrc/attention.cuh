@@ -1,7 +1,8 @@
 // Decode attention of one layer in one launch: rotary embedding of q and k, the KV-cache write at a device-side
 // position, and split-KV attention over positions [0, pos] with a last-arriving-CTA combine (DESIGN §3.16).  The
 // position is one for every row (sequences in lockstep) or one per row (independent sequences, DESIGN §3.18).  The
-// cache holds the activation dtype, or E4M3 codes with a power-of-two fp32 scale per row (DESIGN §3.19).
+// cache holds the activation dtype, or E4M3 codes with a power-of-two fp32 scale per row (DESIGN §3.19).  It is static
+// ([B, n_kv, max_length] rows) or paged (blocks of rows in one pool found through a block table, DESIGN §3.22).
 #pragma once
 #include <math.h>
 
@@ -22,11 +23,18 @@ constexpr int kAttnFp8Stages = 3;       // FP8 cache: tiles in the ring (measure
 // Floats of one split's partials: acc[G][hd], then m and l of up to kAttnMaxG heads (keeps every split 16-byte aligned)
 __host__ __device__ constexpr int attn_part_floats(int G, int hd) { return G * hd + 2 * kAttnMaxG; }
 
+// A paged cache (DESIGN §3.22): K / V pools [num_blocks, n_kv, block_size, hd], scale pools [num_blocks, n_kv,
+// block_size]; position t of row b lives in block table[b·max_blocks + t / block_size] at offset t % block_size.
+struct KvPaging {
+  const int* table;         // [B, max_blocks]; an entry outside [0, num_blocks) is no block
+  int max_blocks, block_shift, num_blocks;   // block_size = 1 << block_shift
+};
+
 struct DecodeAttnParams {
   const uint16_t* q;        // [B, n_heads·hd]
   const uint16_t* k;        // [B, n_kv·hd]
   const uint16_t* v;        // [B, n_kv·hd]
-  uint16_t* k_cache;        // [B, n_kv, max_length, hd]
+  uint16_t* k_cache;        // [B, n_kv, max_length, hd], or paged: [num_blocks, n_kv, block_size, hd]
   uint16_t* v_cache;
   const long long* pos;     // row b reads pos[b * pos_stride]
   int pos_stride;           // 0: one position for every row; 1: one per row, and -1 marks an idle row
@@ -39,6 +47,46 @@ struct DecodeAttnParams {
   int n_heads, n_kv, max_length, splits;
   float* k_scale;           // FP8 cache only: [B, n_kv, max_length] power-of-two scale of each cached row
   float* v_scale;           //   (k_cache / v_cache then hold E4M3 codes, one byte per element)
+};
+// The paged kernel's parameters (max_length = max_blocks·block_size); the static kernels keep DecodeAttnParams alone.
+struct DecodeAttnPagedParams : DecodeAttnParams {
+  KvPaging paging;
+};
+
+// Where the cache rows of (row b, kv head) live: row(t) is the index of position t's row (the index of its scale; times
+// hd, of its first element), ok(r) whether that row exists, elt(r, t) the offset of its first element and scale(s, r, t)
+// the address of its scale in the scale array s.  Static caches hold every position of every row; all offsets stay
+// below 2^31 (host checks).
+template <int kHd, bool kPaged>
+struct KvRows {
+  unsigned cache0, row0;
+  template <class P>
+  __device__ __forceinline__ KvRows(const P& p, int b, int kvh)
+      : cache0(unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) * kHd),
+        row0(unsigned(b * p.n_kv + kvh) * unsigned(p.max_length)) {}
+  __device__ __forceinline__ unsigned row(int t) const { return row0 + unsigned(t); }
+  static __device__ __forceinline__ bool ok(unsigned) { return true; }
+  __device__ __forceinline__ unsigned elt(unsigned, int t) const { return cache0 + unsigned(t) * kHd; }
+  __device__ __forceinline__ const float* scale(const float* s, unsigned, int t) const { return s + row0 + t; }
+};
+
+template <int kHd>
+struct KvRows<kHd, true> {
+  const int* table;
+  unsigned kvh, n_kv;
+  int shift, num_blocks;
+  template <class P>
+  __device__ __forceinline__ KvRows(const P& p, int b, int kvh_)
+      : table(p.paging.table + size_t(b) * p.paging.max_blocks), kvh(kvh_), n_kv(p.n_kv), shift(p.paging.block_shift),
+        num_blocks(p.paging.num_blocks) {}
+  __device__ __forceinline__ unsigned row(int t) const {
+    const int blk = __ldg(table + (t >> shift));
+    return unsigned(blk) < unsigned(num_blocks) ? ((unsigned(blk) * n_kv + kvh) << shift) + unsigned(t & ((1 << shift) - 1))
+                                                : ~0u;
+  }
+  static __device__ __forceinline__ bool ok(unsigned r) { return r != ~0u; }
+  __device__ __forceinline__ unsigned elt(unsigned r, int) const { return r * kHd; }
+  __device__ __forceinline__ const float* scale(const float* s, unsigned r, int) const { return s + r; }
 };
 
 template <int kHd>
@@ -149,9 +197,12 @@ __device__ __forceinline__ float warp_sum(float x) {
 // Grid (splits, n_kv, B), kAttnThreads threads.  CTA (b, kv head, split i) owns positions [i·C, min((i+1)·C, pos+1)),
 // C = ceil((pos+1) / splits) with pos row b's position, for the G query heads of its kv head.  Rows share nothing but
 // the launch: every CTA of row b reads only row b's q, k, v, position, cache rows, partials and counter words.
-// kFp8: the caches hold E4M3 codes and p.k_scale / p.v_scale a power-of-two scale per row (DESIGN §3.19).
-template <bool kBf16, int kHd, bool kFp8 = false>
-__global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const DecodeAttnParams p) {
+// kFp8: the caches hold E4M3 codes and p.k_scale / p.v_scale a power-of-two scale per row (DESIGN §3.19).  kPaged: the
+// rows live in blocks (KvRows); a row whose position pos has no block gets NaN and writes nothing, and a position of
+// 0..pos - 1 without a block reads as NaN.
+template <bool kBf16, int kHd, bool kFp8 = false, bool kPaged = false>
+__global__ void __launch_bounds__(kAttnThreads)
+    decode_attention_kernel(const std::conditional_t<kPaged, DecodeAttnPagedParams, DecodeAttnParams> p) {
   using Smem = std::conditional_t<kFp8, AttnSmemFp8<kHd>, AttnSmem<kHd>>;
   constexpr int kKRow = Smem::kKRow;
   constexpr int kChunks = kHd / 8;                     // 16-byte chunks of a row
@@ -176,7 +227,12 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
   const int n = pos + 1;
   const int C = (n + S - 1) / S;
   const int t0 = min(split * C, n), t1 = min(t0 + C, n);
-  const unsigned cache0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) * kHd;   // < 2^31 (host check)
+  const KvRows<kHd, kPaged> kv(p, b, kvh);
+  const unsigned prow = kv.row(pos);
+  if (!kv.ok(prow)) {                                  // paged: no block at pos
+    for (int i = tid; i < G * kHd; i += kAttnThreads) out[i] = float_to_elt<kBf16>(__int_as_float(0x7fffffff));
+    return;
+  }
   const float fpos = __int2float_rn(pos);
 
   const uint16_t* qrow = p.q + (size_t(b) * p.n_heads + head0) * kHd;
@@ -214,13 +270,12 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
         const uint16_t vc = av == 0.f ? uint16_t(0) : e4m3x2_rn(vq, vq1);
         *reinterpret_cast<uint16_t*>(&sm.knew[tid]) = kc;
         *reinterpret_cast<uint16_t*>(&sm.vnew[tid]) = vc;
-        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.k_cache) + cache0 + unsigned(pos) * kHd + tid) = kc;
-        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.v_cache) + cache0 + unsigned(pos) * kHd + tid) = vc;
+        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.k_cache) + kv.elt(prow, pos) + tid) = kc;
+        *reinterpret_cast<uint16_t*>(reinterpret_cast<uint8_t*>(p.v_cache) + kv.elt(prow, pos) + tid) = vc;
       }
       if (tid == 0) {
-        const unsigned srow = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) + unsigned(pos);
-        sm.ksnew = p.k_scale[srow] = exp2_int(ek);
-        sm.vsnew = p.v_scale[srow] = exp2_int(ev);
+        sm.ksnew = p.k_scale[prow] = exp2_int(ek);
+        sm.vsnew = p.v_scale[prow] = exp2_int(ev);
       }
     }
   } else {
@@ -231,18 +286,17 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
         const uint16_t kn = float_to_elt<kBf16>(rope_elt<kBf16, kHd>(krow, j, p.inv_freq, fpos, p.attn_scaling));
         sm.knew[j] = kn;
         sm.vnew[j] = vrow[j];
-        p.k_cache[cache0 + unsigned(pos) * kHd + j] = kn;
-        p.v_cache[cache0 + unsigned(pos) * kHd + j] = vrow[j];
+        p.k_cache[kv.elt(prow, pos) + j] = kn;
+        p.v_cache[kv.elt(prow, pos) + j] = vrow[j];
       }
     }
   }
   __syncthreads();
 
   const int n_tiles = (t1 - t0 + kAttnTile - 1) / kAttnTile;
-  [[maybe_unused]] const unsigned srow0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length);   // FP8: row scales
-  // K and V rows of one tile into buffer `buf`; the new token's row comes from knew / vnew, never from the cache.  FP8:
-  // E4M3 codes and the scale of each position, in a ring of kAttnFp8Stages tiles with one cp.async group per tile
-  // index (empty past the last tile).
+  // K and V rows of one tile into buffer `buf`; the new token's row comes from knew / vnew, never from the cache, and a
+  // row without a block is NaN.  FP8: E4M3 codes and the scale of each position, in a ring of kAttnFp8Stages tiles with
+  // one cp.async group per tile index (empty past the last tile).
   auto load_tile = [&](int it, int buf) {
     if constexpr (kFp8) {
       if (it < n_tiles) {
@@ -255,10 +309,13 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
           if (t == pos) {
             *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 16]);
             *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 16]);
-          } else {
-            const unsigned g = cache0 + unsigned(t) * kHd + c * 16;
+          } else if (const unsigned row = kv.row(t); kv.ok(row)) {
+            const unsigned g = kv.elt(row, t) + c * 16;
             cp_async16(ks, reinterpret_cast<const uint8_t*>(p.k_cache) + g);
             cp_async16(vs, reinterpret_cast<const uint8_t*>(p.v_cache) + g);
+          } else {
+            *reinterpret_cast<uint4*>(ks) = make_uint4(~0u, ~0u, ~0u, ~0u);   // E4M3 0xff: NaN
+            *reinterpret_cast<uint4*>(vs) = make_uint4(~0u, ~0u, ~0u, ~0u);
           }
         }
         const int r = tid - (kAttnThreads - kAttnTile);   // the last warp: one scale pair per position
@@ -267,9 +324,11 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
           if (t == pos) {
             sm.ks[buf][r] = sm.ksnew;
             sm.vs[buf][r] = sm.vsnew;
+          } else if (const unsigned row = kv.row(t); kv.ok(row)) {
+            cp_async4(&sm.ks[buf][r], kv.scale(p.k_scale, row, t));
+            cp_async4(&sm.vs[buf][r], kv.scale(p.v_scale, row, t));
           } else {
-            cp_async4(&sm.ks[buf][r], p.k_scale + srow0 + t);
-            cp_async4(&sm.vs[buf][r], p.v_scale + srow0 + t);
+            sm.ks[buf][r] = sm.vs[buf][r] = __int_as_float(0x7fffffff);
           }
         }
       }
@@ -283,10 +342,13 @@ __global__ void __launch_bounds__(kAttnThreads) decode_attention_kernel(const De
         if (t == pos) {
           *reinterpret_cast<uint4*>(ks) = *reinterpret_cast<const uint4*>(&sm.knew[c * 8]);
           *reinterpret_cast<uint4*>(vs) = *reinterpret_cast<const uint4*>(&sm.vnew[c * 8]);
-        } else {
-          const unsigned g = cache0 + unsigned(t) * kHd + c * 8;
+        } else if (const unsigned row = kv.row(t); kv.ok(row)) {
+          const unsigned g = kv.elt(row, t) + c * 8;
           cp_async16(ks, p.k_cache + g);
           cp_async16(vs, p.v_cache + g);
+        } else {
+          *reinterpret_cast<uint4*>(ks) = make_uint4(~0u, ~0u, ~0u, ~0u);   // 0xffff: NaN in fp16 and bf16
+          *reinterpret_cast<uint4*>(vs) = make_uint4(~0u, ~0u, ~0u, ~0u);
         }
       }
       cp_async_commit();

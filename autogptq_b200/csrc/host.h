@@ -36,6 +36,12 @@ int device_info(DeviceInfo& out);
 // row must fit in shared memory.  Returns 0 or the failure code (recorded as above).  Defined in abi.cu.
 int agb_internal_unpermute_columns(const void* in, const int* perm, void* out, int M, int K, void* stream);
 
+// Checks the paging arguments of a paged attention entry (DESIGN §3.22): block_size a power of two in 16..256,
+// num_blocks and max_blocks positive, max_blocks·block_size <= 2^30, the table 4-byte aligned; fills `pg`.  Returns 0
+// or the failure code (recorded as above).  Defined in attention.cu.
+namespace agb { struct KvPaging; }
+int paging_of(const char* what, const int32_t* table, int block_size, int num_blocks, int max_blocks, agb::KvPaging& pg);
+
 // Index into the per-device "already set" tables of opt_in_smem.
 inline int current_device_index() {
   int d = 0;

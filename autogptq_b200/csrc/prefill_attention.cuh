@@ -1,4 +1,5 @@
-// Causal attention of T new tokens per row over the static KV cache, in two launches (DESIGN §3.20): an append pass
+// Causal attention of T new tokens per row over the KV cache, static or paged (DESIGN §3.22), in two launches (DESIGN
+// §3.20): an append pass
 // that writes k̂ (rotary embedding) and v of every new token to its cache row, 16-bit or E4M3 codes with a power-of-two
 // scale, by exactly the decode kernel's rules; then an attention pass that reads only the cache.  Row b's tokens take
 // positions start[b] .. start[b] + T - 1; token t attends positions 0 .. start[b] + t.  The attention is FA2-style on
@@ -28,10 +29,32 @@ struct PrefillAttnParams {
   uint16_t* out;            // [B, T, n_heads·hd]
   int T, n_heads, n_kv, max_length;
 };
+// The paged kernels' parameters (max_length = max_blocks·block_size); the static kernels keep PrefillAttnParams alone.
+struct PrefillAttnPagedParams : PrefillAttnParams {
+  KvPaging paging;
+};
+template <bool kPaged>
+using PfParams = std::conditional_t<kPaged, PrefillAttnPagedParams, PrefillAttnParams>;
 
 // Whether row b's tokens fit in the cache: start >= 0 and start + T <= max_length.
 __device__ __forceinline__ bool pf_row_fits(long long s, int T, int max_length) {
   return s >= 0 && s + T <= max_length;
+}
+
+// Paged: whether the blocks of positions 0 .. n - 1 of row b that thread i of n_threads checks all exist (the caller
+// combines the threads).  Static: true.
+template <bool kPaged>
+__device__ __forceinline__ bool pf_blocks_exist(const PfParams<kPaged>& p, int b, int n, int i, int n_threads) {
+  if constexpr (!kPaged) {
+    return true;
+  } else {
+    const KvPaging& pg = p.paging;
+    const int* table = pg.table + size_t(b) * pg.max_blocks;
+    bool ok = true;
+    for (int j = i; j < ((n - 1) >> pg.block_shift) + 1; j += n_threads)
+      ok &= unsigned(__ldg(table + j)) < unsigned(pg.num_blocks);
+    return ok;
+  }
 }
 
 template <int kHd, bool kFp8>
@@ -83,22 +106,24 @@ __device__ __forceinline__ uint32_t pf_e4m3x2(uint16_t c) {
 // Append: grid (ceil(T·n_kv / kPfAppendRows), B), kPfThreads threads; warp w of CTA x writes the cache row of token
 // t = r / n_kv, kv head r % n_kv, r = x·kPfAppendRows + w.  Lane l holds elements 2l + 64i and 2l + 64i + 1.  The
 // values, the scale rule and the code conversion are the decode kernel's, so a row's bytes depend on (k, v, position)
-// only.  A row that does not fit writes nothing.
-template <bool kBf16, int kHd, bool kFp8>
-__global__ void __launch_bounds__(kPfThreads) prefill_append_kernel(const PrefillAttnParams p) {
+// only.  A row that does not fit, or (paged) one with a position 0 .. start + T - 1 without a block, writes nothing.
+template <bool kBf16, int kHd, bool kFp8, bool kPaged = false>
+__global__ void __launch_bounds__(kPfThreads) prefill_append_kernel(const PfParams<kPaged> p) {
   constexpr int kPairs = kHd / 64;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int r = blockIdx.x * kPfAppendRows + warp, b = blockIdx.y;
   if (r >= p.T * p.n_kv) return;
   const long long s64 = p.start[b];
   if (!pf_row_fits(s64, p.T, p.max_length)) return;
+  if (kPaged && !__all_sync(0xffffffffu, pf_blocks_exist<kPaged>(p, b, static_cast<int>(s64) + p.T, lane, 32)))
+    return;
   const int t = r / p.n_kv, kvh = r % p.n_kv;
   const int pos = static_cast<int>(s64) + t;
   const float fpos = __int2float_rn(pos);
   const size_t src = (size_t(b) * p.T + t) * p.n_kv * kHd + size_t(kvh) * kHd;
   const uint16_t* krow = p.k + src;
   const uint16_t* vrow = p.v + src;
-  const unsigned srow = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) + unsigned(pos);   // < 2^31 (host check)
+  const unsigned srow = KvRows<kHd, kPaged>(p, b, kvh).row(pos);   // < 2^31 (host check)
   const unsigned dst = srow * kHd;
   float kx[2 * kPairs], vx[2 * kPairs];
 #pragma unroll
@@ -149,9 +174,10 @@ __global__ void __launch_bounds__(kPfThreads) prefill_append_kernel(const Prefil
 // (FP8: on the codes, then times the row's k scale) times σ, masked above start + t; m = running max; e = expf(s - m);
 // l = l·expf(m_old - m) + Σ e; P = rnd(e) (FP8: rnd(e · vs / R), R the largest v scale seen so far) into the P·V MMA.
 // The output rnd(acc / l) (FP8: rnd(acc / l · R)) is rounded once.  CTAs are issued last token first: they have the
-// most positions to walk.
-template <bool kBf16, int kHd, bool kFp8>
-__global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const PrefillAttnParams p) {
+// most positions to walk.  Paged: a row with a position 0 .. start + T - 1 without a block gets NaN, as one that does
+// not fit.
+template <bool kBf16, int kHd, bool kFp8, bool kPaged = false>
+__global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const PfParams<kPaged> p) {
   using Smem = PfSmem<kHd, kFp8>;
   constexpr int kRow = Smem::kRow, kKvRow = Smem::kKvRow;
   constexpr int kKc = kHd / 16;                 // k-steps of q̂·k
@@ -169,7 +195,9 @@ __global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const Pre
   const size_t tok_stride = size_t(p.n_heads) * kHd;
   uint16_t* outb = p.out + size_t(b) * T * tok_stride + size_t(kvh) * G * kHd;
   const long long s64 = p.start[b];
-  if (!pf_row_fits(s64, T, p.max_length)) {      // nothing fits: NaN out, the cache untouched
+  const bool fits = pf_row_fits(s64, T, p.max_length);
+  if (!fits || (kPaged && !__syncthreads_and(pf_blocks_exist<kPaged>(p, b, static_cast<int>(s64) + T, tid, kPfThreads)))) {
+    // nothing fits: NaN out, the cache untouched
     for (int i = tid; i < nrows * kHd; i += kPfThreads) {
       const int r = r0 + i / kHd;
       outb[size_t(r / G) * tok_stride + (r % G) * kHd + i % kHd] = float_to_elt<kBf16>(__int_as_float(0x7fffffff));
@@ -179,8 +207,7 @@ __global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const Pre
   const int start = static_cast<int>(s64);
   const int n_end = start + (r0 + nrows - 1) / G + 1;     // positions the CTA reads: [0, n_end)
   const int n_tiles = (n_end + kPfTile - 1) / kPfTile;
-  const unsigned cache0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length) * kHd;   // < 2^31 (host check)
-  [[maybe_unused]] const unsigned srow0 = unsigned(b * p.n_kv + kvh) * unsigned(p.max_length);
+  const KvRows<kHd, kPaged> kv(p, b, kvh);   // offsets < 2^31 (host check)
 
   // K and V rows of tile `it` into buffer `buf`, one cp.async group; rows at or past n_end are zero (never NaN).
   auto load_tile = [&](int it, int buf) {
@@ -190,7 +217,7 @@ __global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const Pre
       auto* kd = &sm.k[buf][r * kKvRow + c * kChunkB];
       auto* vd = &sm.v[buf][r * kKvRow + c * kChunkB];
       if (t < n_end) {
-        const unsigned gofs = cache0 + unsigned(t) * kHd + c * kChunkB;
+        const unsigned gofs = kv.elt(kv.row(t), t) + c * kChunkB;
         if constexpr (kFp8) {
           cp_async16(kd, reinterpret_cast<const uint8_t*>(p.k_cache) + gofs);
           cp_async16(vd, reinterpret_cast<const uint8_t*>(p.v_cache) + gofs);
@@ -207,8 +234,9 @@ __global__ void __launch_bounds__(kPfThreads) prefill_attention_kernel(const Pre
       if (tid < kPfTile) {
         const int t = ts + tid;
         if (t < n_end) {
-          cp_async4(&sm.ks[buf][tid], p.k_scale + srow0 + t);
-          cp_async4(&sm.vs[buf][tid], p.v_scale + srow0 + t);
+          const unsigned row = kv.row(t);
+          cp_async4(&sm.ks[buf][tid], kv.scale(p.k_scale, row, t));
+          cp_async4(&sm.vs[buf][tid], kv.scale(p.v_scale, row, t));
         } else {
           sm.ks[buf][tid] = 0.f;
           sm.vs[buf][tid] = 0.f;

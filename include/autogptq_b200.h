@@ -676,6 +676,47 @@ int agb200_prefill_attention_fp8(const void* q, const void* k, const void* v, vo
                                  int head_dim, int max_length, int dtype, void* stream);
 
 /*
+ * The per-row decode step and the prefill over a paged cache (additions to ABI v11, DESIGN §3.22).  Per layer, in place of
+ * the static caches [B, n_kv, max_length, head_dim]:
+ *   k_pool, v_pool [num_blocks, n_kv, block_size, head_dim]       contiguous pools, dtype (FP8: E4M3 codes)
+ *   k_scale_pool, v_scale_pool [num_blocks, n_kv, block_size]     FP8 only: fp32 scale of each row
+ *   block_table int32 [B, max_blocks]                             position t of row b lives in block
+ *                                                                 block_table[b][t / block_size], row t % block_size
+ * block_size is a power of two in 16..256.  Everything else, the results and the cache bytes written are those of
+ * agb200_decode_attention_rows(_fp8) / agb200_prefill_attention(_fp8) on a static cache of max_length =
+ * max_blocks*block_size that holds the same rows, bit for bit: the split count and the tiles are the static ones, and a
+ * tile may straddle blocks.  No table entry outside [0, num_blocks) is dereferenced.  Decode: a row whose position pos[b]
+ * has no valid block writes NaN to its output row and nothing to the pools; any other position 0..pos[b]-1 without a
+ * valid block reads as NaN (that row's output is NaN).  Prefill: a row with any position 0 .. start[b]+T-1 without a
+ * valid block is a row that does not fit (NaN out, pools untouched).  The workspace of the decode step is
+ * agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, head_dim, max_blocks*block_size).  Constraints as the static
+ * entries, with the pool in place of the cache: num_blocks*n_kv*block_size*head_dim < 2^31 (else AGB200_ENOSUP), a
+ * block_size outside the above AGB200_ENOSUP, num_blocks, max_blocks <= 0 or max_blocks*block_size > 2^30
+ * AGB200_EINVAL, block_table 4-byte aligned.
+ */
+int agb200_decode_attention_rows_paged(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                       const int32_t* block_table, int block_size, int num_blocks, int max_blocks,
+                                       const int64_t* pos, const float* inv_freq, float attention_scaling,
+                                       float scaling, void* out, int B, int n_heads, int n_kv, int head_dim, int dtype,
+                                       void* workspace, size_t workspace_bytes, void* stream);
+int agb200_decode_attention_rows_paged_fp8(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                           float* k_scale_pool, float* v_scale_pool, const int32_t* block_table,
+                                           int block_size, int num_blocks, int max_blocks, const int64_t* pos,
+                                           const float* inv_freq, float attention_scaling, float scaling, void* out,
+                                           int B, int n_heads, int n_kv, int head_dim, int dtype, void* workspace,
+                                           size_t workspace_bytes, void* stream);
+int agb200_prefill_attention_paged(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                   const int32_t* block_table, int block_size, int num_blocks, int max_blocks,
+                                   const int64_t* start, const float* inv_freq, float attention_scaling, float scaling,
+                                   void* out, int B, int T, int n_heads, int n_kv, int head_dim, int dtype,
+                                   void* stream);
+int agb200_prefill_attention_paged_fp8(const void* q, const void* k, const void* v, void* k_pool, void* v_pool,
+                                       float* k_scale_pool, float* v_scale_pool, const int32_t* block_table,
+                                       int block_size, int num_blocks, int max_blocks, const int64_t* start,
+                                       const float* inv_freq, float attention_scaling, float scaling, void* out, int B,
+                                       int T, int n_heads, int n_kv, int head_dim, int dtype, void* stream);
+
+/*
  * Router of a Mixtral-style block for T decode rows (addition to ABI v10), one launch on `stream`, all pointers DEVICE
  * memory of `dtype` unless stated:
  *   x [T, H], x2 [T, H] or NULL   h = x + x2 (the residual add; x2 NULL: h = x)
