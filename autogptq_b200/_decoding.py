@@ -1,5 +1,5 @@
-"""The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules,
-the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, the extend of
+"""The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules and
+the Mixtral block's (router, grouped experts, no mixed dense and MoE layers), the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, the extend of
 cache rows on the project's kernels (DESIGN §3.20), each row's sampling parameters (DESIGN §3.21), and the warm-up,
 capture and replay of a step's CUDA graphs (the step, and the step followed by the sampling kernel)."""
 from __future__ import annotations
@@ -8,11 +8,13 @@ import torch
 
 from .attention import FP8, quantize_kv
 from .mlp import FusedQuantMLP, _is_silu
+from .moe import QuantExperts, router_supported
 from .qlinear import QuantLinear
 from .sampling import SamplingState
 
 _RMSNORMS = ("LlamaRMSNorm", "MistralRMSNorm", "Qwen2RMSNorm", "MixtralRMSNorm")
 _MOE_BLOCKS = ("MixtralSparseMoeBlock",)
+_ROUTERS = ("MixtralTopKRouter",)
 
 
 def _is_moe_block(mlp) -> bool:
@@ -95,6 +97,51 @@ def _plan_common(i: int, layer, dtype, who: str):
         if w.dtype != dtype:
             raise NotImplementedError(f"{who}: {where}.{n}.weight is {w.dtype}, the activations {dtype}")
     return attn, mlp, norms[0][1], norms[1][1]
+
+
+def _plan_moe(i: int, mlp, H: int, batch: int, dtype, who: str = "ChainDecoder"):
+    """(router weight [E, H], top_k, QuantExperts) of a Mixtral sparse MoE block (``_is_moe_block``), after checking
+    that they fit the router kernel at ``batch`` rows and the grouped experts."""
+    where = f"model.layers.{i}.mlp"
+    if type(mlp).__name__ not in _MOE_BLOCKS:
+        raise NotImplementedError(f"{who}: {where} is {type(mlp).__name__}; the only mixture-of-experts block {who} "
+                                  f"runs is {', '.join(_MOE_BLOCKS)}")
+    gate, experts = getattr(mlp, "gate", None), getattr(mlp, "experts", None)
+    if type(gate).__name__ not in _ROUTERS:
+        raise NotImplementedError(f"{who}: {where}.gate is {type(gate).__name__}; only {', '.join(_ROUTERS)} "
+                                  "(softmax, top-k, renormalised weights) runs in the router kernel")
+    w = getattr(gate, "weight", None)
+    if getattr(gate, "bias", None) is not None:
+        raise NotImplementedError(f"{who}: {where}.gate has a bias; the router kernel is bias-free")
+    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[1] != H:
+        raise NotImplementedError(f"{who}: {where}.gate.weight has shape "
+                                  f"{None if w is None else tuple(w.shape)}, not [num_experts, {H}]")
+    if w.dtype != dtype:
+        raise NotImplementedError(f"{who}: {where}.gate.weight is {w.dtype}, the activations {dtype}")
+    if not isinstance(experts, QuantExperts):
+        raise NotImplementedError(f"{who}: {where}.experts is {type(experts).__name__}, not "
+                                  "autogptq_b200.QuantExperts (build one from the experts' QuantLinear layers with "
+                                  "autogptq_b200.group_experts)")
+    E, k = w.shape[0], int(getattr(gate, "top_k", 0))
+    if experts.hidden_size != H or experts.num_experts != E:
+        raise NotImplementedError(f"{who}: {where}.experts has {experts.num_experts} experts of hidden size "
+                                  f"{experts.hidden_size}; the router has {E} of {H}")
+    why = router_supported(batch, H, E, k, dtype)
+    if why is not None:
+        raise NotImplementedError(f"{who}: {where}.gate: {why}")
+    return w.detach().contiguous(), k, experts
+
+
+def _is_moe(plans, who: str = "ChainDecoder") -> bool:
+    """Whether the layer plans (attn, mlp, ln1, ln2, moe) are all mixture-of-experts blocks (moe not None), else all
+    dense; a model that mixes the two is refused."""
+    moe = plans[0][4] is not None
+    for i, p in enumerate(plans):
+        if (p[4] is not None) != moe:
+            raise NotImplementedError(f"{who}: model.layers.{i}.mlp is {type(p[1]).__name__} but "
+                                      f"model.layers.0.mlp is {type(plans[0][1]).__name__}; a model that mixes dense "
+                                      "and mixture-of-experts layers is not supported")
+    return moe
 
 
 class StaticCacheDecoder:

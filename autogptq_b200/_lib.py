@@ -126,6 +126,7 @@ def _declare(lib):
         "agb200_prefill_attention_paged_fp8": (I, [P, P, P, P, P, P, P, P, I, I, I, P, P, c_float, c_float, P, I, I, I,
                                                     I, I, I, P]),
         "agb200_moe_router": (I, [P, P, P, c_float, P, I, I, I, I, I, P, P, P, P, P, P]),
+        "agb200_moe_router_rows": (I, [P, P, P, c_float, P, P, I, I, I, I, I, P, P, P, P, P, P]),
         "agb200_add_rmsnorm": (I, [P, P, P, c_float, I, I, I, P, P, P]),
         "agb200_sample": (I, [P, c_int64, I, I, I, P, P, P, P, P, P, P, P]),
     }

@@ -1,5 +1,5 @@
-// Host side of the MoE router and of its residual add + RMSNorm alone (include/autogptq_b200.h: agb200_moe_router,
-// agb200_add_rmsnorm): argument checking and the launch on the caller's stream.  Kernels: moe_router.cuh.
+// Host side of the MoE router, with and without idle rows, and of its residual add + RMSNorm alone
+// (include/autogptq_b200.h: agb200_moe_router, agb200_moe_router_rows, agb200_add_rmsnorm): argument checking and the launch on the caller's stream.  Kernels: moe_router.cuh.
 #include <cuda_runtime.h>
 
 #include "host.h"
@@ -9,12 +9,13 @@ static_assert(agb::kRouterMaxH == AGB200_CHAIN_NORM_MAX_K, "router and chain nor
 static_assert(agb::kRouterMaxE == AGB200_MOE_MAX_EXPERTS, "router and grouped experts share the expert limit");
 static_assert(agb::kRouterMaxTopK == AGB200_MOE_ROUTER_MAX_TOP_K, "router top-k limit");
 
-extern "C" {
+namespace {
 
-int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, int T,
-                      int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
-                      void* logits, void* stream) {
-  if (!x || !norm_weight || !gate_weight || !n || !top_k_index || !top_k_weights)
+// Both router entries: `rows` selects agb200_moe_router_rows (pos marks idle rows), else pos is unused.
+int router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, const int64_t* pos,
+           bool rows, int T, int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
+           void* logits, void* stream) {
+  if (!x || !norm_weight || !gate_weight || !n || !top_k_index || !top_k_weights || (rows && !pos))
     return failf(AGB200_EINVAL, "moe_router: null pointer argument");
   if ((x2 == nullptr) != (h == nullptr)) return failf(AGB200_EINVAL, "moe_router: h is written exactly when x2 is given");
   if (T < 0 || H <= 0 || E <= 0 || k <= 0)
@@ -31,6 +32,7 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
       (h && !aligned(h, 16)) || !aligned(n, 16) || !aligned(top_k_index, 4) || !aligned(top_k_weights, 4) ||
       (logits && !aligned(logits, 2)))
     return failf(AGB200_EINVAL, "moe_router: x, x2, norm_weight, gate_weight, h and n must be 16-byte aligned");
+  if (rows && !aligned(pos, 8)) return failf(AGB200_EINVAL, "moe_router_rows: pos must be 8-byte aligned");
   if (T == 0) return 0;
   agb::MoeRouterParams p{};
   p.x = static_cast<const uint16_t*>(x);
@@ -46,11 +48,36 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
   p.H = H;
   p.E = E;
   p.k = k;
+  p.pos = pos;
   cudaStream_t s = static_cast<cudaStream_t>(stream);
-  if (dtype == AGB200_BF16) agb::moe_router_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
-  else agb::moe_router_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
+  const bool bf = dtype == AGB200_BF16;
+  if (rows) {
+    if (bf) agb::moe_router_kernel<true, true><<<T, agb::kRouterThreads, 0, s>>>(p);
+    else agb::moe_router_kernel<false, true><<<T, agb::kRouterThreads, 0, s>>>(p);
+  } else {
+    if (bf) agb::moe_router_kernel<true><<<T, agb::kRouterThreads, 0, s>>>(p);
+    else agb::moe_router_kernel<false><<<T, agb::kRouterThreads, 0, s>>>(p);
+  }
   AGB_CUDA(cudaGetLastError());
   return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight, int T,
+                      int H, int E, int k, int dtype, void* h, void* n, int32_t* top_k_index, float* top_k_weights,
+                      void* logits, void* stream) {
+  return router(x, x2, norm_weight, eps, gate_weight, nullptr, false, T, H, E, k, dtype, h, n, top_k_index,
+                top_k_weights, logits, stream);
+}
+
+int agb200_moe_router_rows(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight,
+                           const int64_t* pos, int T, int H, int E, int k, int dtype, void* h, void* n,
+                           int32_t* top_k_index, float* top_k_weights, void* logits, void* stream) {
+  return router(x, x2, norm_weight, eps, gate_weight, pos, true, T, H, E, k, dtype, h, n, top_k_index, top_k_weights,
+                logits, stream);
 }
 
 int agb200_add_rmsnorm(const void* x, const void* x2, const void* norm_weight, float eps, int T, int H, int dtype,

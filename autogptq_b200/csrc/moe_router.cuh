@@ -27,6 +27,7 @@ struct MoeRouterParams {
   uint16_t* logits;         // [T, E] or null
   float eps;
   int H, E, k;
+  const int64_t* pos;       // [T] (kRows only): a row with pos < 0 is idle
 };
 
 struct RouterSmem {
@@ -124,7 +125,9 @@ __device__ __forceinline__ void add_rmsnorm_row(const uint16_t* x, const uint16_
 //   top-k of p, largest first, an exact tie to the lower expert index;  w_j = p_j / Σ_j p_j  (fp32, j in order)
 // Every sum runs in a fixed order (per thread in index order, a xor-shuffle tree per warp, the warps in order), so two
 // launches on the same input are bit-identical.  Σh² is summed exactly as ch_norm_prepass sums it for one row.
-template <bool kBf16>
+// kRows: p.pos marks idle rows (pos < 0), which still write h and n but route to no expert (idx -1, weight 0) and skip
+// the logits; every other row runs the code of kRows = false unchanged.
+template <bool kBf16, bool kRows = false>
 __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRouterParams p) {
   __shared__ __align__(16) RouterSmem sm;
   const int ctid = threadIdx.x, lane = ctid & 31, warp = ctid >> 5;
@@ -132,6 +135,15 @@ __global__ void __launch_bounds__(kRouterThreads) moe_router_kernel(const MoeRou
 
   // h, n (into sm.xs, each thread over its own rows: no barrier is needed before the logit loop reads them)
   add_rmsnorm_row<kBf16>(p.x, p.x2, p.norm_w, p.h, p.n, p.eps, H, blockIdx.x, sm.xs, sm.red);
+  if constexpr (kRows) {
+    if (p.pos[blockIdx.x] < 0) {            // uniform over the CTA: the whole row leaves here
+      if (ctid < p.k) {
+        p.idx[static_cast<size_t>(blockIdx.x) * p.k + ctid] = -1;
+        p.wts[static_cast<size_t>(blockIdx.x) * p.k + ctid] = 0.f;
+      }
+      return;
+    }
+  }
 
   // logits: thread ctid owns the same 8-element rows of every expert's G row; per-warp partials, then the warps in order
   for (int eb = 0; eb < E; eb += kRouterEB) {

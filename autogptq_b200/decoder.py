@@ -57,44 +57,12 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from ._decoding import _MOE_BLOCKS, StaticCacheDecoder, _is_moe_block, _plan_common, _rotary_params
-from ._decoding import _RMSNORMS, _check_window, _norm_of  # noqa: F401 - the chain's checks, also importable from here
+from ._decoding import StaticCacheDecoder, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
+from ._decoding import _MOE_BLOCKS, _RMSNORMS, _ROUTERS, _check_window, _norm_of  # noqa: F401 - also importable here
 from .attention import FP8, attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
-from .moe import QuantExperts, moe_router, router_supported
+from .moe import moe_router
 from .sampling import sampling_list
-
-_ROUTERS = ("MixtralTopKRouter",)
-
-
-def _plan_moe(i: int, mlp, H: int, batch: int, dtype):
-    """(router weight [E, H], top_k, QuantExperts) of a Mixtral sparse MoE block, after checking that they fit."""
-    where = f"model.layers.{i}.mlp"
-    gate, experts = getattr(mlp, "gate", None), getattr(mlp, "experts", None)
-    if type(gate).__name__ not in _ROUTERS:
-        raise NotImplementedError(f"ChainDecoder: {where}.gate is {type(gate).__name__}; only {', '.join(_ROUTERS)} "
-                                  "(softmax, top-k, renormalised weights) runs in the router kernel")
-    w = getattr(gate, "weight", None)
-    if getattr(gate, "bias", None) is not None:
-        raise NotImplementedError(f"ChainDecoder: {where}.gate has a bias; the router kernel is bias-free")
-    if not isinstance(w, torch.Tensor) or w.dim() != 2 or w.shape[1] != H:
-        raise NotImplementedError(f"ChainDecoder: {where}.gate.weight has shape "
-                                  f"{None if w is None else tuple(w.shape)}, not [num_experts, {H}]")
-    if w.dtype != dtype:
-        raise NotImplementedError(f"ChainDecoder: {where}.gate.weight is {w.dtype}, the activations {dtype}")
-    if not isinstance(experts, QuantExperts):
-        raise NotImplementedError(f"ChainDecoder: {where}.experts is {type(experts).__name__}, not "
-                                  "autogptq_b200.QuantExperts (build one from the experts' QuantLinear layers with "
-                                  "autogptq_b200.group_experts)")
-    E, k = w.shape[0], int(getattr(gate, "top_k", 0))
-    if experts.hidden_size != H or experts.num_experts != E:
-        raise NotImplementedError(f"ChainDecoder: {where}.experts has {experts.num_experts} experts of hidden size "
-                                  f"{experts.hidden_size}; the router has {E} of {H}")
-    why = router_supported(batch, H, E, k, dtype)
-    if why is not None:
-        raise NotImplementedError(f"ChainDecoder: {where}.gate: {why}")
-    return w.detach().contiguous(), k, experts
-
 
 def _plan_layer(i: int, layer, batch: int, dtype):
     """The shared rules, then the chain's: (attn, mlp, ln1, ln2, moe) of decoder layer i with moe = (router weight,
@@ -106,11 +74,8 @@ def _plan_layer(i: int, layer, batch: int, dtype):
     moe = None
     if not _is_moe_block(mlp):
         groups.update({"mlp.gate_proj|up_proj": [mlp.gate_proj, mlp.up_proj], "mlp.down_proj": [mlp.down_proj]})
-    elif type(mlp).__name__ in _MOE_BLOCKS:
-        moe = _plan_moe(i, mlp, H, batch, dtype)
     else:
-        raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp is {type(mlp).__name__}; the only "
-                                  f"mixture-of-experts block ChainDecoder runs is {', '.join(_MOE_BLOCKS)}")
+        moe = _plan_moe(i, mlp, H, batch, dtype, "ChainDecoder")
     for n, ls in groups.items():
         if not chain_supported(ls, batch):
             raise NotImplementedError(f"ChainDecoder: model.layers.{i}.{n} cannot run in a decode chain (needs "
@@ -120,17 +85,6 @@ def _plan_layer(i: int, layer, batch: int, dtype):
         raise NotImplementedError(f"ChainDecoder: model.layers.{i}: hidden size {H} > {_lib.CHAIN_NORM_MAX_K}, the "
                                   "largest a chain norm stage takes")
     return attn, mlp, ln1, ln2, moe
-
-
-def _is_moe(plans) -> bool:
-    """Whether the layers of ``_plan_layer`` are all mixture-of-experts blocks (else all dense)."""
-    moe = plans[0][4] is not None
-    for i, p in enumerate(plans):
-        if (p[4] is not None) != moe:
-            raise NotImplementedError(f"ChainDecoder: model.layers.{i}.mlp is {type(p[1]).__name__} but "
-                                      f"model.layers.0.mlp is {type(plans[0][1]).__name__}; a model that mixes dense "
-                                      "and mixture-of-experts layers is not supported")
-    return moe
 
 
 class ChainDecoder(StaticCacheDecoder):
@@ -158,7 +112,7 @@ class ChainDecoder(StaticCacheDecoder):
             self._inv_freq, self._attn_scaling = _rotary_params(model.model.rotary_emb, self.head_dim,
                                                                 "ChainDecoder(fused_attention=True)")
         self._read_layers()
-        self.moe = _is_moe(self._plans)
+        self.moe = _is_moe(self._plans, "ChainDecoder")
 
         # the chains are built before the caches: whether a block's chain fits the device's shared memory is the
         # library's decision (DESIGN §3.5), and a block that does not fit is refused before the caches are allocated

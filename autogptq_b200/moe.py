@@ -329,7 +329,8 @@ def router_supported(T: int, H: int, E: int, k: int, dtype) -> str | None:
     return None
 
 
-def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n=None, idx=None, w=None, logits=None):
+def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n=None, idx=None, w=None, logits=None,
+               pos=None):
     """The routing of a Mixtral-style block for decode rows in one launch (``agb200_moe_router``, DESIGN §3.17):
 
         h = x + x2 (skipped when x2 is None)   n = RMSNorm(h; norm_weight, eps)   logits = n · gate_weightᵀ
@@ -338,7 +339,11 @@ def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n
     with the roundings of transformers' MixtralDecoderLayer / MixtralRMSNorm / MixtralTopKRouter.  x, x2 [T, H] and
     norm_weight [H], gate_weight [E, H] of one 16-bit dtype.  Returns (h or None, n [T, H], idx int32 [T, k],
     w fp32 [T, k], logits [T, E] or None); ``h``, ``n``, ``idx`` and ``w`` are written in place when given (a decoder
-    preallocates them), ``logits`` only when a buffer is given.  No host synchronisation."""
+    preallocates them), ``logits`` only when a buffer is given.  No host synchronisation.
+
+    ``pos`` (int64 [T], ``agb200_moe_router_rows``): a row with pos < 0 is idle; it still gets h and n, but idx -1 and
+    w 0 (so ``QuantExperts._forward`` gives it a zero row and streams no expert for it), and its logits row is not
+    written.  Rows with pos >= 0 are bit-identical to a call without ``pos``."""
     if x.dim() != 2:
         raise ValueError(f"x must be [T, H], got {tuple(x.shape)}")
     T, H = x.shape
@@ -364,6 +369,8 @@ def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n
         raise ValueError("h is the residual x + x2; pass x2 or leave h out")
     if logits is not None:
         checks.append(("logits", logits, (T, E), dt))
+    if pos is not None:
+        checks.append(("pos", pos, (T,), torch.int64))
     for name, t, shape, tdt in checks:
         if tuple(t.shape) != shape or t.dtype != tdt:
             raise ValueError(f"{name} must be {tdt} {list(shape)}, got {t.dtype} {list(t.shape)}")
@@ -371,14 +378,20 @@ def moe_router(x, x2, norm_weight, eps: float, gate_weight, k: int, *, h=None, n
             raise ValueError(f"{name} is on {t.device}, x on {dev}")
         if not t.is_contiguous():
             raise ValueError(f"{name} must be contiguous")
-        if t.dtype != torch.float32 and t.dtype != torch.int32 and name != "logits" and t.data_ptr() % 16:
+        if t.dtype not in (torch.float32, torch.int32, torch.int64) and name != "logits" and t.data_ptr() % 16:
             raise ValueError(f"{name} must be 16-byte aligned")
     lib = _lib.load()
     with torch.cuda.device(dev):
-        rc = lib.agb200_moe_router(x.data_ptr(), _ptr(x2), norm_weight.data_ptr(), float(eps), gate_weight.data_ptr(),
-                                   T, H, E, k, _DTYPE_CODE[dt], _ptr(h), n.data_ptr(), idx.data_ptr(), w.data_ptr(),
-                                   _ptr(logits), torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(rc, "agb200_moe_router")
+        stream = torch.cuda.current_stream(dev).cuda_stream
+        if pos is None:
+            rc = lib.agb200_moe_router(x.data_ptr(), _ptr(x2), norm_weight.data_ptr(), float(eps),
+                                       gate_weight.data_ptr(), T, H, E, k, _DTYPE_CODE[dt], _ptr(h), n.data_ptr(),
+                                       idx.data_ptr(), w.data_ptr(), _ptr(logits), stream)
+        else:
+            rc = lib.agb200_moe_router_rows(x.data_ptr(), _ptr(x2), norm_weight.data_ptr(), float(eps),
+                                            gate_weight.data_ptr(), pos.data_ptr(), T, H, E, k, _DTYPE_CODE[dt],
+                                            _ptr(h), n.data_ptr(), idx.data_ptr(), w.data_ptr(), _ptr(logits), stream)
+    _lib.check(rc, "agb200_moe_router" if pos is None else "agb200_moe_router_rows")
     return h, n, idx, w, logits
 
 

@@ -742,6 +742,18 @@ int agb200_moe_router(const void* x, const void* x2, const void* norm_weight, fl
                       void* logits, void* stream);
 
 /*
+ * agb200_moe_router with idle rows (addition to ABI v11), for a decoder whose step runs every slot of a batch:
+ *   pos int64 [T] (DEVICE)        a row with pos[r] < 0 is idle
+ * An idle row writes h and n as agb200_moe_router does, top_k_index = -1 and top_k_weights = 0 for all k (so
+ * agb200_moe_forward gives it a zero output row and streams no expert for it), and leaves its logits row unwritten.
+ * Every row with pos[r] >= 0 is bit-identical to agb200_moe_router on the same inputs.  Same constraints and errors as
+ * agb200_moe_router, and pos non-null and 8-byte aligned (else AGB200_EINVAL).
+ */
+int agb200_moe_router_rows(const void* x, const void* x2, const void* norm_weight, float eps, const void* gate_weight,
+                           const int64_t* pos, int T, int H, int E, int k, int dtype, void* h, void* n,
+                           int32_t* top_k_index, float* top_k_weights, void* logits, void* stream);
+
+/*
  * The residual add and RMSNorm of agb200_moe_router without the router (addition to ABI v10): for T decode rows of a
  * dense block, one launch on `stream`, all pointers DEVICE memory of `dtype`:
  *   x [T, H], x2 [T, H] or NULL   h = x + x2 (x2 NULL: h = x)

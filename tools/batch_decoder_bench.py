@@ -76,7 +76,7 @@ def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
     plans = dec._plans
 
     def linears():
-        for attn, mlp, _, _ in plans:
+        for attn, mlp, *_ in plans:
             forward_group([attn.q_proj, attn.k_proj, attn.v_proj], dec._n1)
             attn.o_proj(dec._attn_out)
             mlp.down_proj(forward_gate_up(mlp.gate_proj, mlp.up_proj, dec._n2))
@@ -91,7 +91,7 @@ def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
     def norms():
         w, eps = plans[0][2]
         add_rmsnorm(dec._x, None, w, eps, n=dec._n1)
-        for _, _, _, (w2, eps2) in plans:
+        for _, _, _, (w2, eps2), _ in plans:
             add_rmsnorm(dec._x, dec._resid, w2, eps2, h=dec._h1, n=dec._n2)
             add_rmsnorm(dec._x, dec._h1, w2, eps2, h=dec._resid, n=dec._n1)
 
