@@ -1,12 +1,13 @@
 """The front end ``ChainDecoder`` and ``BatchDecoder`` share (DESIGN §3.18): reading the model, the dense-layer rules and
-the Mixtral block's (router, grouped experts, no mixed dense and MoE layers), the static KV cache (16-bit, or E4M3 codes with a power-of-two scale per row), the HF prefill into it, the extend of
-cache rows on the project's kernels (DESIGN §3.20), each row's sampling parameters (DESIGN §3.21), and the warm-up,
-capture and replay of a step's CUDA graphs (the step, and the step followed by the sampling kernel)."""
+the Mixtral block's (router, grouped experts, no mixed dense and MoE layers), allocating the KV cache the decoder chose
+(``autogptq_b200.kv_cache``), the HF prefill into it, the extend of cache rows on the project's kernels (DESIGN §3.20),
+each row's sampling parameters (DESIGN §3.21), and the warm-up, capture and replay of a step's CUDA graphs (the step,
+and the step followed by the sampling kernel)."""
 from __future__ import annotations
 
 import torch
 
-from .attention import FP8, quantize_kv
+from .attention import FP8
 from .mlp import FusedQuantMLP, _is_silu
 from .moe import QuantExperts, router_supported
 from .qlinear import QuantLinear
@@ -144,13 +145,13 @@ def _is_moe(plans, who: str = "ChainDecoder") -> bool:
     return moe
 
 
-class StaticCacheDecoder:
-    """Base of a decoder over a static KV cache whose step is one captured CUDA graph.  A subclass sets ``_who``
-    (the prefix of its refusals) and ``_plan`` (a layer's plan, starting from ``_plan_common``).  Its constructor calls
-    ``_read_model``, checks its kernels' limits on the geometry, calls ``_read_layers``, checks what spans the layers
-    and calls ``_allocate`` last, so every refusal comes before the caches are allocated (a refusal that asks the device,
-    such as a decode chain's shared memory, takes ``_cuda_device`` first).  It then sets ``_pos``, the device positions
-    its ``_step_body`` reads and advances."""
+class DecoderBase:
+    """Base of a decoder over a KV cache whose step is one captured CUDA graph.  A subclass sets ``_who`` (the prefix
+    of its refusals) and ``_plan`` (a layer's plan, starting from ``_plan_common``).  Its constructor calls
+    ``_read_model``, sets ``_cache`` (a ``KVCache`` or ``PagedKVCache``, not yet allocated), checks its kernels' limits
+    on the geometry, calls ``_read_layers``, checks what spans the layers and calls ``_allocate`` last, so every refusal
+    comes before the cache is allocated (a refusal that asks the device, such as a decode chain's shared memory, takes
+    ``_cuda_device`` first).  It then sets ``_pos``, the device positions its ``_step_body`` reads and advances."""
 
     # ------------------------------------------------------------------ reading the model
     def _read_model(self, model, max_length: int, kv_cache_dtype):
@@ -203,55 +204,33 @@ class StaticCacheDecoder:
             raise RuntimeError(f"{self._who} needs the model on a CUDA device")
         return self.device
 
-    def _allocate(self, rows: int, cache_shape=None):
-        """After every refusal: the CUDA device, the static caches of ``rows`` rows and the step's token ids.  The
-        caches are per layer [rows, n_kv, max_length, head_dim] in the activation dtype, or E4M3 codes with fp32
-        scales ``k_scale`` / ``v_scale`` [rows, n_kv, max_length] for FP8 (else the scales are None).  ``cache_shape``
-        replaces [rows, n_kv, max_length, head_dim] (a paged cache's pools)."""
+    def _allocate(self, rows: int):
+        """After every refusal: the CUDA device, the KV cache ``_cache`` the subclass chose (``k_cache`` / ``v_cache`` /
+        ``k_scale`` / ``v_scale`` are its tensors) and the step's token ids of ``rows`` rows."""
         self._cuda_device()
-        shape = (rows, self.n_kv, self.max_length, self.head_dim) if cache_shape is None else tuple(cache_shape)
-        n, dev = len(self._plans), self.device
-        self.k_cache = [torch.zeros(shape, dtype=FP8 if self._fp8 else self.dtype, device=dev) for _ in range(n)]
-        self.v_cache = [torch.zeros_like(c) for c in self.k_cache]
-        self.k_scale = self.v_scale = None
-        if self._fp8:
-            self.k_scale = [torch.ones(shape[:-1], dtype=torch.float32, device=dev) for _ in range(n)]
-            self.v_scale = [torch.ones_like(s) for s in self.k_scale]
-        self._ids = torch.zeros(rows, dtype=torch.int64, device=dev)
+        c = self._cache
+        c.allocate(len(self._plans), self.device)
+        self.k_cache, self.v_cache, self.k_scale, self.v_scale = c.k, c.v, c.k_scale, c.v_scale
+        self._ids = torch.zeros(rows, dtype=torch.int64, device=self.device)
         self._graphs = {}                               # step body name -> (CUDA graph, its output buffers)
-        self._sampling = SamplingState(rows, dev)       # each row's sampling parameters, greedy until set
-
-    def _store_kv(self, i: int, index, keys, values):
-        """Keys and values [.., n_kv, T, hd] into layer i's caches at ``index`` (quantised for FP8)."""
-        if self.k_scale is None:
-            self.k_cache[i][index].copy_(keys)
-            self.v_cache[i][index].copy_(values)
-            return
-        for cache, scale, x in ((self.k_cache[i], self.k_scale[i], keys), (self.v_cache[i], self.v_scale[i], values)):
-            codes, sc = quantize_kv(x)
-            cache.view(torch.uint8)[index].copy_(codes.view(torch.uint8))
-            scale[index].copy_(sc)
-
-    def _cache_kwargs(self, i: int) -> dict:
-        """Layer i's cache keyword arguments of ``decode_attention`` / ``decode_attention_rows`` beyond the caches."""
-        return {} if self.k_scale is None else dict(k_scale=self.k_scale[i], v_scale=self.v_scale[i])
+        self._sampling = SamplingState(rows, self.device)   # each row's sampling parameters, greedy until set
 
     def _prefill_cache(self, ids: torch.Tensor, rows: slice) -> torch.Tensor:
         """Run ``ids`` [len(rows), T] through the HF model (its own prefill kernels) and store every layer's keys and
-        values into the static caches at ``rows``, positions :T.  Returns the model's logits [len(rows), T, vocab]."""
+        values into the cache at ``rows``, positions :T.  Returns the model's logits [len(rows), T, vocab]."""
         from transformers import DynamicCache
 
         cache = DynamicCache(config=self.model.config)
         out = self.model(input_ids=ids, past_key_values=cache, use_cache=True)
         for i, lay in enumerate(cache.layers):
-            self._store_kv(i, (rows, slice(None), slice(0, ids.shape[1])), lay.keys, lay.values)
+            self._cache.store(i, rows, lay.keys, lay.values)
         return out.logits
 
     def _extend(self, ids: torch.Tensor, rows: slice, starts) -> torch.Tensor:
         """Append ``ids`` [n, T] to cache rows ``rows`` (n of them) at positions ``starts`` (n host ints) .. + T - 1
         on the project's kernels, and return the logits of the last new position [n, vocab].  The model's own modules
         run every layer (its QuantLinear projections at M = n·T, its norms and MLP), so every rounding outside the
-        attention is HF's; ``prefill_attention`` writes k̂ and v into the static caches and attends causally over them.
+        attention is HF's; the cache's prefill attention writes k̂ and v into it and attends causally over it.
         No DynamicCache is built and only the last position reaches model.norm and lm_head."""
         inner = self.model.model
         if not hasattr(self, "_inv_freq"):
@@ -263,18 +242,11 @@ class StaticCacheDecoder:
         for i, layer in enumerate(inner.layers):
             attn = self._plans[i][0]
             x = layer.input_layernorm(h)
-            self._extend_attention(i, rows, attn.q_proj(x), attn.k_proj(x), attn.v_proj(x), start, out)
+            self._cache.prefill(i, rows, attn.q_proj(x), attn.k_proj(x), attn.v_proj(x), start, self._inv_freq,
+                                self._attn_scaling, self.scaling, out)
             h = h + attn.o_proj(out)
             h = h + layer.mlp(layer.post_attention_layernorm(h))
         return self.model.lm_head(inner.norm(h[:, -1:]))[:, 0]
-
-    def _extend_attention(self, i: int, rows: slice, q, k, v, start, out):
-        """``prefill_attention`` of layer i on cache rows ``rows``: writes the new rows and attends causally."""
-        from .attention import prefill_attention
-
-        kw = {} if self.k_scale is None else dict(k_scale=self.k_scale[i][rows], v_scale=self.v_scale[i][rows])
-        prefill_attention(q, k, v, self.k_cache[i][rows], self.v_cache[i][rows], start, self._inv_freq,
-                          self._attn_scaling, self.scaling, out, **kw)
 
     # ------------------------------------------------------------------ one step
     def _run_step(self, ids: torch.Tensor, use_graph: bool, body=None):

@@ -33,6 +33,8 @@ and the row it belongs to gets NaN (decode: if it holds pos, or any position bel
 """
 from __future__ import annotations
 
+import functools
+
 import torch
 
 from . import _lib
@@ -123,16 +125,16 @@ def decode_attention(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling
     """q [B, n_heads·hd], k / v [B, n_kv·hd], caches [B, n_kv, max_length, hd], pos int64 [1] (device), inv_freq fp32
     [hd/2], out [B, n_heads·hd] written in place and returned.  Raises NotImplementedError outside the kernel's limits.
     float8_e4m3fn caches with ``k_scale`` / ``v_scale`` fp32 [B, n_kv, max_length]: the FP8 cache (module docstring)."""
-    return _launch("decode_attention", attention_supported, 1, q, k, v, k_cache, v_cache, pos, inv_freq,
-                   attention_scaling, scaling, out, workspace, k_scale, v_scale)
+    return _launch("decode_attention", attention_supported, q, k, v, k_cache, v_cache, pos, inv_freq,
+                   attention_scaling, scaling, out, k_scale, v_scale, workspace=workspace, n_pos=1)
 
 
 def decode_attention_rows(q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling: float, scaling: float, out,
                           workspace=None, *, k_scale=None, v_scale=None):
     """``decode_attention`` for independent sequences: pos int64 [B] (device), one position per row, -1 for an idle
     row (zeros out, cache row untouched).  B <= ``ATTN_ROWS_MAX_B``.  FP8 caches as ``decode_attention``."""
-    return _launch("decode_attention_rows", attention_rows_supported, None, q, k, v, k_cache, v_cache, pos, inv_freq,
-                   attention_scaling, scaling, out, workspace, k_scale, v_scale)
+    return _launch("decode_attention_rows", attention_rows_supported, q, k, v, k_cache, v_cache, pos, inv_freq,
+                   attention_scaling, scaling, out, k_scale, v_scale, workspace=workspace)
 
 
 def prefill_attention_supported(n_heads: int, n_kv: int, head_dim: int, batch: int, max_length: int,
@@ -150,44 +152,8 @@ def prefill_attention(q, k, v, k_cache, v_cache, start, inv_freq, attention_scal
     token t attends positions 0 .. start[b] + t.  A row whose tokens do not fit gets NaN and no cache write.
     float8_e4m3fn caches with ``k_scale`` / ``v_scale``: the FP8 cache, as ``decode_attention``.  Raises
     NotImplementedError outside the kernel's limits.  No workspace, no host synchronisation."""
-    if q.dim() != 3:
-        raise ValueError(f"q must be [B, T, n_heads·head_dim], got {tuple(q.shape)}")
-    T = q.shape[1]
-    if T < 1:
-        raise ValueError("prefill_attention: T must be at least 1")
-    entry, caches, n_heads, dt = _checked("prefill_attention", prefill_attention_supported, None, q, k, v, k_cache,
-                                          v_cache, start, inv_freq, out, k_scale, v_scale, T=T, pos_name="start")
-    B, n_kv, L, hd = k_cache.shape
-    dev = k_cache.device
-    lib = _lib.load()
-    with torch.cuda.device(dev):
-        rc = getattr(lib, f"agb200_{entry}")(
-            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, start.data_ptr(), inv_freq.data_ptr(),
-            float(attention_scaling), float(scaling), out.data_ptr(), B, T, n_heads, n_kv, hd, L, _DT[dt],
-            torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(rc, f"agb200_{entry}")
-    return out
-
-
-def _paged(entry, q, k_pool, block_table, n_lead):
-    """The paged entries' own checks: (B, block_size, max_blocks, the checks of ``_checked``)."""
-    if k_pool.dim() != 4:
-        raise ValueError(f"k_pool must be [num_blocks, n_kv, block_size, head_dim], got {tuple(k_pool.shape)}")
-    num_blocks, n_kv, bs, hd = k_pool.shape
-    if block_table.dtype != torch.int32 or block_table.dim() != 2:
-        raise ValueError(f"{entry}: block_table must be int32 [B, max_blocks], got {block_table.dtype} "
-                         f"{list(block_table.shape)}")
-    B, max_blocks = block_table.shape
-    if q.dim() != n_lead + 1 or q.shape[0] != B:
-        raise ValueError(f"{entry}: q must have {B} rows (block_table's), got {tuple(q.shape)}")
-    if max_blocks < 1 or max_blocks * bs > 2 ** 30:
-        raise ValueError(f"{entry}: block_table has {max_blocks} blocks per row of {bs}; need 1..2^30 positions")
-    if block_table.device != k_pool.device or not block_table.is_contiguous():
-        raise ValueError(f"{entry}: block_table must be contiguous on {k_pool.device}")
-
-    def supported(n_heads, n_kv_, hd_, batch, block_size, dt):
-        return paged_attention_supported(n_heads, n_kv_, hd_, batch, block_size, num_blocks, dt)
-    return B, bs, max_blocks, supported
+    return _launch("prefill_attention", prefill_attention_supported, q, k, v, k_cache, v_cache, start, inv_freq,
+                   attention_scaling, scaling, out, k_scale, v_scale, prefill=True)
 
 
 def decode_attention_rows_paged(q, k, v, k_pool, v_pool, block_table, pos, inv_freq, attention_scaling: float,
@@ -197,24 +163,8 @@ def decode_attention_rows_paged(q, k, v, k_pool, v_pool, block_table, pos, inv_f
     ``k_scale`` / ``v_scale`` fp32 [num_blocks, n_kv, block_size]: the FP8 cache.  The workspace is
     ``decode_attention_workspace(B, n_heads, n_kv, hd, max_blocks·block_size)``.  Raises NotImplementedError outside
     the kernel's limits."""
-    B, bs, max_blocks, supported = _paged("decode_attention_rows_paged", q, k_pool, block_table, 1)
-    entry, caches, n_heads, dt = _checked("decode_attention_rows_paged", supported, None, q, k, v, k_pool, v_pool, pos,
-                                          inv_freq, out, k_scale, v_scale, rows=B)
-    num_blocks, n_kv, _, hd = k_pool.shape
-    L, dev, lib = max_blocks * bs, k_pool.device, _lib.load()
-    with torch.cuda.device(dev):
-        need = int(lib.agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, hd, L))
-        if workspace is None:
-            workspace = decode_attention_workspace(B, n_heads, n_kv, hd, L, dev)
-        elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
-            raise ValueError(f"workspace must hold {need} bytes on {dev}")
-        rc = getattr(lib, f"agb200_{entry}")(
-            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, block_table.data_ptr(), bs, num_blocks, max_blocks,
-            pos.data_ptr(), inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads,
-            n_kv, hd, _DT[dt], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
-            torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(rc, f"agb200_{entry}")
-    return out
+    return _launch("decode_attention_rows_paged", paged_attention_supported, q, k, v, k_pool, v_pool, pos, inv_freq,
+                   attention_scaling, scaling, out, k_scale, v_scale, workspace=workspace, table=block_table)
 
 
 def prefill_attention_paged(q, k, v, k_pool, v_pool, block_table, start, inv_freq, attention_scaling: float,
@@ -222,42 +172,43 @@ def prefill_attention_paged(q, k, v, k_pool, v_pool, block_table, start, inv_fre
     """``prefill_attention`` over a paged cache (module docstring): q [B, T, n_heads·hd], pools and block_table as
     ``decode_attention_rows_paged``, start int64 [B].  A row with a position 0 .. start + T - 1 outside the table or
     without a block gets NaN and no write.  Raises NotImplementedError outside the kernel's limits."""
-    B, bs, max_blocks, supported = _paged("prefill_attention_paged", q, k_pool, block_table, 2)
-    T = q.shape[1]
-    if T < 1:
-        raise ValueError("prefill_attention_paged: T must be at least 1")
-    entry, caches, n_heads, dt = _checked("prefill_attention_paged", supported, None, q, k, v, k_pool, v_pool, start,
-                                          inv_freq, out, k_scale, v_scale, T=T, pos_name="start", rows=B)
-    num_blocks, n_kv, _, hd = k_pool.shape
-    dev, lib = k_pool.device, _lib.load()
-    with torch.cuda.device(dev):
-        rc = getattr(lib, f"agb200_{entry}")(
-            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, block_table.data_ptr(), bs, num_blocks, max_blocks,
-            start.data_ptr(), inv_freq.data_ptr(), float(attention_scaling), float(scaling), out.data_ptr(), B, T,
-            n_heads, n_kv, hd, _DT[dt], torch.cuda.current_stream(dev).cuda_stream)
-    _lib.check(rc, f"agb200_{entry}")
-    return out
+    return _launch("prefill_attention_paged", paged_attention_supported, q, k, v, k_pool, v_pool, start, inv_freq,
+                   attention_scaling, scaling, out, k_scale, v_scale, prefill=True, table=block_table)
 
 
-def _launch(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out,
-            workspace, k_scale=None, v_scale=None):
-    """Checks and the call of agb200_<entry> (agb200_<entry>_fp8 for a float8_e4m3fn cache); ``n_pos`` elements of pos
-    (None: one per row).  The activation dtype is the 16-bit cache's, or q's for an FP8 cache."""
-    entry, caches, n_heads, dt = _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, out,
-                                          k_scale, v_scale)
-    return _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace,
-                 n_heads, dt)
-
-
-def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, out, k_scale, v_scale, T=None,
-             pos_name="pos", rows=None):
-    """``_launch``'s checks: (entry with _fp8 for an FP8 cache, the cache pointers after v, n_heads, dtype).  With
-    ``T`` the activations are [B, T, features] instead of [B, features].  ``rows``: B when the caches are a paged
-    cache's pools [num_blocks, n_kv, block_size, head_dim] (else B is the caches' first dimension)."""
+def _launch(entry, supported, q, k, v, k_cache, v_cache, pos, inv_freq, attention_scaling, scaling, out, k_scale,
+            v_scale, *, workspace=None, n_pos=None, prefill=False, table=None):
+    """Checks, the workspace (decode) and the call of agb200_<entry>[_fp8]: ``n_pos`` elements of pos (None: one per
+    row); ``prefill``: activations [B, T, features] from start positions; ``table``: the caches are pools read through
+    this block table.  The activation dtype is the 16-bit cache's, or q's for an FP8 cache."""
+    paging = ()
+    if table is not None:
+        if k_cache.dim() != 4:
+            raise ValueError(f"k_pool must be [num_blocks, n_kv, block_size, head_dim], got {tuple(k_cache.shape)}")
+        num_blocks, _, bs, _ = k_cache.shape
+        if table.dtype != torch.int32 or table.dim() != 2:
+            raise ValueError(f"{entry}: block_table must be int32 [B, max_blocks], got {table.dtype} "
+                             f"{list(table.shape)}")
+        rows, max_blocks = table.shape
+        if q.dim() != (3 if prefill else 2) or q.shape[0] != rows:
+            raise ValueError(f"{entry}: q must have {rows} rows (block_table's), got {tuple(q.shape)}")
+        if max_blocks < 1 or max_blocks * bs > 2 ** 30:
+            raise ValueError(f"{entry}: block_table has {max_blocks} blocks per row of {bs}; need 1..2^30 positions")
+        if table.device != k_cache.device or not table.is_contiguous():
+            raise ValueError(f"{entry}: block_table must be contiguous on {k_cache.device}")
+        supported = functools.partial(supported, num_blocks=num_blocks)
+        paging = (table.data_ptr(), bs, num_blocks, max_blocks)
+    lead = ()
+    if prefill:
+        if q.dim() != 3:
+            raise ValueError(f"q must be [B, T, n_heads·head_dim], got {tuple(q.shape)}")
+        lead = (q.shape[1],)
+        if lead[0] < 1:
+            raise ValueError(f"{entry}: T must be at least 1")
     if k_cache.dim() != 4:
         raise ValueError(f"k_cache must be [B, n_kv, max_length, head_dim], got {tuple(k_cache.shape)}")
     nb, n_kv, L, hd = k_cache.shape
-    B = nb if rows is None else rows
+    B = rows if paging else nb
     dev = k_cache.device
     if dev.type != "cuda":
         raise RuntimeError(f"{entry} needs CUDA tensors (there is no CPU fallback)")
@@ -267,11 +218,11 @@ def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, 
     if fp8 and (k_scale is None or v_scale is None):
         raise ValueError(f"{entry}: a {FP8} cache needs k_scale and v_scale (fp32 [B, n_kv, max_length])")
     dt = q.dtype if fp8 else k_cache.dtype
-    lead = (B,) if T is None else (B, T)
+    lead = (B,) + lead                              # [B, features], or [B, T, features] for prefill
     if q.dim() != len(lead) + 1 or tuple(q.shape[:-1]) != lead or q.shape[-1] % hd != 0:
         raise ValueError(f"q must be [{', '.join(map(str, lead))}, n_heads·{hd}], got {tuple(q.shape)}")
     n_heads = q.shape[-1] // hd
-    why = supported(n_heads, n_kv, hd, B, L, dt)
+    why = supported(n_heads, n_kv, hd, B, L, dtype=dt)
     if why is not None:
         raise NotImplementedError(f"{entry}: {why}")
     checks = [("q", q, lead + (n_heads * hd,), dt), ("k", k, lead + (n_kv * hd,), dt),
@@ -288,6 +239,7 @@ def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, 
                 raise ValueError(f"{name} is {t.dtype}, the cache {dt}")
             raise ValueError(f"{name} is {t.dtype}, the activations (q) {dt}" if want == dt else
                              f"{name} is {t.dtype}, not {want}")
+    pos_name = "start" if prefill else "pos"
     tensors = [("q", q), ("k", k), ("v", v), ("k_cache", k_cache), ("v_cache", v_cache), ("out", out),
                (pos_name, pos), ("inv_freq", inv_freq)] + ([("k_scale", k_scale), ("v_scale", v_scale)] if fp8 else [])
     for name, t in tensors:
@@ -303,26 +255,22 @@ def _checked(entry, supported, n_pos, q, k, v, k_cache, v_cache, pos, inv_freq, 
     caches = (k_cache.data_ptr(), v_cache.data_ptr())
     if fp8:
         entry, caches = entry + "_fp8", caches + (k_scale.data_ptr(), v_scale.data_ptr())
-    return entry, caches, n_heads, dt
-
-
-def _call(entry, caches, n_pos, q, k, v, k_cache, pos, inv_freq, attention_scaling, scaling, out, workspace, n_heads,
-          dt):
-    """agb200_<entry> after the checks: ``caches`` the cache pointers the entry takes after v."""
-    B, n_kv, L, hd = k_cache.shape
-    dev = k_cache.device
+    if paging:
+        L = max_blocks * bs                         # the positions a row can address
     lib = _lib.load()
     with torch.cuda.device(dev):
-        need = int(lib.agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, hd, L))
-        if workspace is None:
-            workspace = decode_attention_workspace(B, n_heads, n_kv, hd, L, dev)
-        elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
-            raise ValueError(f"workspace must hold {need} bytes on {dev}")
+        ws = ()
+        if not prefill:
+            need = int(lib.agb200_decode_attention_workspace_bytes(B, n_heads, n_kv, hd, L))
+            if workspace is None:
+                workspace = decode_attention_workspace(B, n_heads, n_kv, hd, L, dev)
+            elif workspace.device != dev or workspace.numel() * workspace.element_size() < need:
+                raise ValueError(f"workspace must hold {need} bytes on {dev}")
+            ws = (workspace.data_ptr(), workspace.numel() * workspace.element_size())
         rc = getattr(lib, f"agb200_{entry}")(
-            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, pos.data_ptr(), inv_freq.data_ptr(),
-            float(attention_scaling), float(scaling), out.data_ptr(), B, n_heads, n_kv, hd, L,
-            _DT[dt], workspace.data_ptr(), workspace.numel() * workspace.element_size(),
-            torch.cuda.current_stream(dev).cuda_stream)
+            q.data_ptr(), k.data_ptr(), v.data_ptr(), *caches, *paging, pos.data_ptr(), inv_freq.data_ptr(),
+            float(attention_scaling), float(scaling), out.data_ptr(), *lead, n_heads, n_kv, hd,
+            *(() if paging else (L,)), _DT[dt], *ws, torch.cuda.current_stream(dev).cuda_stream)
     _lib.check(rc, f"agb200_{entry}")
     return out
 

@@ -38,10 +38,10 @@ model's ``lm_head`` (torch) give the logits.  The attention applies each row's r
 writes the row's cache entry and attends over the row's positions only; an idle row writes zeros and touches no cache.
 Every kernel computes a row from that row's inputs alone, so what one slot holds never changes another slot's logits.
 
-``prefill`` runs the HF model at batch 1 and stores its keys and values in the slot's row of the static caches; with
+``prefill`` runs the HF model at batch 1 and stores its keys and values in the slot's cache rows; with
 ``kv_cache_dtype=torch.float8_e4m3fn`` they are FP8 (DESIGN §3.19), half the cache bytes.  ``extend(slot, ids)``
 appends T tokens at the slot's position on the project's kernels instead (DESIGN §3.20): the model's own modules for
-everything but attention, and ``prefill_attention`` writing the static cache and attending causally over it, with no
+everything but attention, and ``prefill_attention`` writing the cache and attending causally over it, with no
 second cache and lm_head on the last position only.  On an idle slot it is a prompt prefill; on an active one it
 continues the sequence (a new conversation turn, or the next chunk of a long prompt).  For Mixtral both run the model's
 own MoE blocks, so a prompt of more than 8 tokens (``MOE_DECODE_MAX_T``) makes each ``QuantExperts`` build its
@@ -54,12 +54,13 @@ With ``kv_block_size`` the KV cache is paged (DESIGN §3.22): one pool of ``kv_b
 per slot, and blocks shared by reference.  The memory then follows the tokens held, not ``max_batch × max_length``;
 ``fork(src, dst)`` gives an idle slot another slot's prefix without recomputing or copying its full blocks, and
 ``generate(..., n=k)`` prefills each prompt once and samples k continuations from it.  The step, its graph and its
-results are the static cache's, bit for bit; only where a cache row lives changes.
+results are the static cache's, bit for bit; only where a cache row lives changes.  Both layouts are
+``autogptq_b200.kv_cache``'s ``KVCache`` and ``PagedKVCache``.
 
 Scope: Llama, Mistral and Qwen2 blocks with ``QuantLinear`` projections (``FusedQuantMLP`` MLPs too), and Mixtral blocks
 with ``QuantLinear`` attention projections and ``QuantExperts``.  Router variants other than Mixtral's (Qwen2-MoE's
 shared expert, DeepSeek, a router bias), experts that are not grouped, and models that mix dense and MoE layers are
-refused.  The model checks, the caches, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
+refused.  The model checks, the prefill and the graph capture are ``autogptq_b200._decoding``'s, shared with
 ``ChainDecoder``, which runs each block of batch <= 2 sequences in lockstep as one decode-chain launch.
 """
 from __future__ import annotations
@@ -70,11 +71,9 @@ from collections import deque
 import torch
 
 from . import _lib
-from ._decoding import (_MOE_BLOCKS, StaticCacheDecoder, _is_moe, _is_moe_block, _plan_common, _plan_moe,
-                        _rotary_params)
-from .attention import (attention_rows_supported, decode_attention_rows, decode_attention_rows_paged,
-                        decode_attention_workspace, paged_attention_supported, prefill_attention_paged, quantize_kv)
-from .paged_kv import BlockAllocator, blocks_for, worst_case_blocks
+from ._decoding import _MOE_BLOCKS, DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
+from .attention import decode_attention_workspace
+from .kv_cache import KVCache, PagedKVCache
 from .mlp import forward_gate_up
 from .moe import QuantExperts, add_rmsnorm, add_rmsnorm_supported, moe_router
 from .qlinear import forward_group
@@ -83,7 +82,7 @@ from .sampling import SamplingParams, sampling_list
 _WHO = "BatchDecoder"
 
 
-class BatchDecoder(StaticCacheDecoder):
+class BatchDecoder(DecoderBase):
     """Greedy or sampling decoder of up to ``max_batch`` <= 8 independent sequences over a transformers ``LlamaForCausalLM`` /
     ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose projections are ``autogptq_b200.QuantLinear``, or a
     ``MixtralForCausalLM`` whose attention projections are ``QuantLinear`` and whose experts are
@@ -108,11 +107,11 @@ class BatchDecoder(StaticCacheDecoder):
         if self.kv_block_size is None:
             if kv_blocks is not None:
                 raise ValueError(f"{_WHO}: kv_blocks goes with kv_block_size (a paged cache)")
-            why = attention_rows_supported(self.n_heads, self.n_kv, hd, B, self.max_length, dt)
+            self._cache = KVCache(B, self.n_kv, self.max_length, hd, dt, self._fp8)
         else:
-            self._max_blocks = blocks_for(self.max_length, self.kv_block_size)
-            self.kv_blocks = B * self._max_blocks if kv_blocks is None else int(kv_blocks)
-            why = paged_attention_supported(self.n_heads, self.n_kv, hd, B, self.kv_block_size, self.kv_blocks, dt)
+            self._cache = PagedKVCache(B, self.n_kv, self.max_length, hd, dt, self._fp8, self.kv_block_size, kv_blocks)
+            self.kv_blocks = self._cache.num_blocks
+        why = self._cache.unsupported(self.n_heads)
         if why is not None:
             raise NotImplementedError(f"{_WHO}: model.layers.*.self_attn: {why}")
         self._inv_freq, self._attn_scaling = _rotary_params(model.model.rotary_emb, hd, _WHO)
@@ -134,8 +133,7 @@ class BatchDecoder(StaticCacheDecoder):
         self._n1 = torch.zeros((B, H), dtype=dt, device=dev)
         self._n2 = torch.zeros((B, H), dtype=dt, device=dev)
         self._attn_out = torch.zeros((B, self.n_heads * hd), dtype=dt, device=dev)
-        L = self.max_length if self.kv_block_size is None else self._max_blocks * self.kv_block_size
-        self._attn_ws = decode_attention_workspace(B, self.n_heads, self.n_kv, hd, L, dev)
+        self._attn_ws = decode_attention_workspace(B, self.n_heads, self.n_kv, hd, self._cache.length, dev)
         self._moe_layers = []                       # per Mixtral block: the router's outputs and the experts' buffers
         for *_, (w2, eps2), moe in (self._plans if self.moe else []):
             gate, k, experts = moe
@@ -147,36 +145,20 @@ class BatchDecoder(StaticCacheDecoder):
                 w=torch.zeros((B, k), dtype=torch.float32, device=dev),
                 out=torch.zeros((B, H), dtype=dt, device=dev)))
 
-    def _allocate(self, rows: int):
-        """The static caches, or the pools, block table and allocator of a paged cache (``k_cache`` etc. are then the
-        pools; the table is -1, no block, wherever a slot holds none)."""
-        if self.kv_block_size is None:
-            return super()._allocate(rows)
-        nb, bs = self.kv_blocks, self.kv_block_size
-        super()._allocate(rows, (nb, self.n_kv, bs, self.head_dim))
-        self._table = torch.full((rows, self._max_blocks), -1, dtype=torch.int32, device=self.device)
-        self._blocks = BlockAllocator(nb, bs, rows, self._max_blocks)
-
     @property
     def kv_cache_bytes(self) -> int:
         """Bytes of the KV cache: every layer's caches (static) or pools (paged), scales included."""
-        ts = self.k_cache + self.v_cache + (self.k_scale + self.v_scale if self.k_scale is not None else [])
-        return sum(t.numel() * t.element_size() for t in ts)
+        return self._cache.nbytes
 
     @property
     def kv_blocks_free(self):
         """Free blocks of the paged cache's pool (None for a static cache)."""
-        return None if self.kv_block_size is None else self._blocks.free
+        return self._cache.blocks_free
 
     def _need_paged(self, what: str):
+        """The refusal of ``fork`` and ``generate(n > 1)`` on a static cache, before their arguments are checked."""
         if self.kv_block_size is None:
             raise NotImplementedError(f"{_WHO}.{what} needs the paged KV cache (BatchDecoder(..., kv_block_size=...))")
-
-    def _map(self, need: dict):
-        """Blocks for positions 0 .. need[s] - 1 of each slot s, mirrored into the device table; raises RuntimeError
-        before any change when the pool cannot supply them."""
-        for s, j, b in self._blocks.map(need):
-            self._table[s, j] = b
 
     def _plan(self, i: int, layer):
         """(attn, mlp, ln1, ln2, moe): ``_plan_common``'s, with moe = (router weight, top_k, QuantExperts) of a
@@ -218,20 +200,18 @@ class BatchDecoder(StaticCacheDecoder):
     @torch.no_grad()
     def prefill(self, slot: int, input_ids: torch.Tensor) -> torch.Tensor:
         """Run the prompt [T] through the HF model at batch 1 (its own prefill kernels), copy its keys and values into
-        the slot's row of the static caches and make the slot active at position T.  Other slots are not touched.
+        the slot's cache rows and make the slot active at position T.  Other slots are not touched.
         Returns the logits of the last prompt position [vocab]."""
         slot = self._check_slot(slot)
         ids = input_ids.to(self.device).reshape(1, -1)
         T = ids.shape[1]
         if not 1 <= T < self.max_length:
             raise ValueError(f"prompt length {T} must be in 1..{self.max_length - 1}")
-        if self.kv_block_size is not None:
-            own = sum(self._blocks.ref[b] == 1 for b in self._blocks.blocks[slot])     # freed by the release
-            if blocks_for(T, self.kv_block_size) > self._blocks.free + own:
-                raise RuntimeError(f"{_WHO}.prefill: the KV cache pool cannot hold {T} tokens ({self._blocks.free} "
-                                   "blocks free)")
-            self.release(slot)
-            self._map({slot: T})
+        if not self._cache.fits(slot, T):
+            raise RuntimeError(f"{_WHO}.prefill: the KV cache pool cannot hold {T} tokens ({self.kv_blocks_free} "
+                               "blocks free)")
+        self.release(slot)
+        self._cache.reserve({slot: T})
         logits = self._prefill_cache(ids, slice(slot, slot + 1))
         self._pos[slot] = T
         self._host_pos[slot] = T
@@ -253,8 +233,7 @@ class BatchDecoder(StaticCacheDecoder):
         if p + T >= self.max_length:
             raise ValueError(f"{_WHO}.extend: slot {slot} at position {p} + {T} tokens must stay below "
                              f"max_length={self.max_length}")
-        if self.kv_block_size is not None:
-            self._map({slot: p + T})
+        self._cache.reserve({slot: p + T})
         logits = self._extend(input_ids.to(self.device).view(1, T), slice(slot, slot + 1), [p])
         self._pos[slot] = p + T
         self._host_pos[slot] = p + T
@@ -285,9 +264,7 @@ class BatchDecoder(StaticCacheDecoder):
         slot = self._check_slot(slot)
         self._pos[slot] = -1
         self._host_pos[slot] = -1
-        if self.kv_block_size is not None:
-            self._blocks.release(slot)
-            self._table[slot].fill_(-1)
+        self._cache.release(slot)
 
     @torch.no_grad()
     def fork(self, src: int, dst: int):
@@ -302,39 +279,9 @@ class BatchDecoder(StaticCacheDecoder):
             raise RuntimeError(f"{_WHO}.fork: slot {src} is idle")
         if self._host_pos[dst] >= 0 or src == dst:
             raise RuntimeError(f"{_WHO}.fork: slot {dst} must be idle")
-        blocks, copy = self._blocks.fork(src, dst, p)
-        if copy is not None:
-            a, b = copy
-            for ts in (self.k_cache, self.v_cache, self.k_scale or [], self.v_scale or []):
-                for t in ts:
-                    t[b].copy_(t[a])
-        self._table[dst, :len(blocks)] = torch.tensor(blocks, dtype=torch.int32)
+        self._cache.fork(src, dst, p)
         self._pos[dst] = p
         self._host_pos[dst] = p
-
-    def _store_kv(self, i: int, index, keys, values):
-        """Keys and values [1, n_kv, T, hd] of the slot ``index[0]`` at positions ``index[2]`` (0 .. T - 1) into its
-        blocks (paged); the static caches' ``_store_kv`` otherwise."""
-        if self.kv_block_size is None:
-            return super()._store_kv(i, index, keys, values)
-        slot, T = index[0].start, index[2].stop
-        t = torch.arange(T)
-        blk = torch.tensor(self._blocks.blocks[slot], dtype=torch.int64)[t // self.kv_block_size].to(self.device)
-        off = (t % self.kv_block_size).to(self.device)
-        if self.k_scale is None:
-            self.k_cache[i][blk, :, off] = keys[0].transpose(0, 1)
-            self.v_cache[i][blk, :, off] = values[0].transpose(0, 1)
-            return
-        for pool, scale, x in ((self.k_cache[i], self.k_scale[i], keys), (self.v_cache[i], self.v_scale[i], values)):
-            codes, sc = quantize_kv(x)
-            pool.view(torch.uint8)[blk, :, off] = codes.view(torch.uint8)[0].transpose(0, 1)
-            scale[blk, :, off] = sc[0].transpose(0, 1)
-
-    def _extend_attention(self, i: int, rows: slice, q, k, v, start, out):
-        if self.kv_block_size is None:
-            return super()._extend_attention(i, rows, q, k, v, start, out)
-        prefill_attention_paged(q, k, v, self.k_cache[i], self.v_cache[i], self._table[rows], start, self._inv_freq,
-                                self._attn_scaling, self.scaling, out, **self._cache_kwargs(i))
 
     # ------------------------------------------------------------------ one step
     def _step_body(self) -> torch.Tensor:
@@ -345,14 +292,8 @@ class BatchDecoder(StaticCacheDecoder):
         resid = self._x
         for i, (attn, mlp, _, (w2, eps2), moe) in enumerate(self._plans):
             q, k, v = forward_group([attn.q_proj, attn.k_proj, attn.v_proj], self._n1)
-            if self.kv_block_size is None:
-                decode_attention_rows(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq,
-                                      self._attn_scaling, self.scaling, self._attn_out, self._attn_ws,
-                                      **self._cache_kwargs(i))
-            else:
-                decode_attention_rows_paged(q, k, v, self.k_cache[i], self.v_cache[i], self._table, self._pos,
-                                            self._inv_freq, self._attn_scaling, self.scaling, self._attn_out,
-                                            self._attn_ws, **self._cache_kwargs(i))
+            self._cache.decode(i, q, k, v, self._pos, self._inv_freq, self._attn_scaling, self.scaling, self._attn_out,
+                               self._attn_ws)
             o = attn.o_proj(self._attn_out)
             w1, eps1 = self._plans[i + 1][2] if i + 1 < len(self._plans) else self._final
             if moe is None:
@@ -381,8 +322,7 @@ class BatchDecoder(StaticCacheDecoder):
             raise RuntimeError(f"{_WHO}.{what}: no slot is active (prefill one first)")
         if max(active) >= self.max_length:
             raise RuntimeError(f"{_WHO}.{what}: a slot's static cache is full ({self.max_length} tokens)")
-        if self.kv_block_size is not None:               # the block of each position the step writes
-            self._map({s: p + 1 for s, p in enumerate(self._host_pos) if p >= 0})
+        self._cache.reserve({s: p + 1 for s, p in enumerate(self._host_pos) if p >= 0})   # the blocks the step writes
 
     @torch.no_grad()
     def step(self, ids: torch.Tensor, use_graph: bool = True) -> torch.Tensor:
@@ -436,14 +376,12 @@ class BatchDecoder(StaticCacheDecoder):
             if p.numel() + max_new_tokens > self.max_length:
                 raise ValueError(f"prompt {j}: {p.numel()} tokens + {max_new_tokens} new tokens exceed "
                                  f"max_length={self.max_length}")
-        paged = self.kv_block_size is not None
-        worst = [0] * len(prompts)
-        if paged:
-            worst = [worst_case_blocks(p.numel(), max_new_tokens, n, self.kv_block_size) for p in prompts]
-            for j, w in enumerate(worst):
-                if w > self.kv_blocks:
-                    raise ValueError(f"prompt {j}: {prompts[j].numel()} tokens + {max_new_tokens} new tokens, {n} "
-                                     f"sample(s), may need {w} blocks; the pool has {self.kv_blocks}")
+        pool = self._cache.num_blocks                # 0 for a static cache, whose prompts need no blocks
+        worst = [self._cache.worst_case_blocks(p.numel(), max_new_tokens, n) for p in prompts]
+        for j, w in enumerate(worst):
+            if w > pool:
+                raise ValueError(f"prompt {j}: {prompts[j].numel()} tokens + {max_new_tokens} new tokens, {n} "
+                                 f"sample(s), may need {w} blocks; the pool has {pool}")
         for s in range(self.max_batch):
             if self._host_pos[s] >= 0:
                 self.release(s)
@@ -485,7 +423,7 @@ class BatchDecoder(StaticCacheDecoder):
             while queue:
                 free = [s for s in range(self.max_batch) if owner[s] is None]
                 j = queue[0]
-                if len(free) < n or (paged and committed + worst[j] > self.kv_blocks):
+                if len(free) < n or committed + worst[j] > pool:
                     break
                 queue.popleft()
                 admit(j, free[:n])

@@ -16,10 +16,11 @@ The decode chain's norm stage inputs (``x_mode="add_rmsnorm"``) cover the adds a
     chain_i = [o_i, add_rmsnorm -> gate|up_i, silu_mul -> down_i, add_rmsnorm(input_layernorm_i+1) -> q|k|v_i+1]
 
 (the last block ends at down_i).  Attention needs the KV cache and runs in torch between two chains: the model's own
-rotary embedding and ``apply_rotary_pos_emb``, a static [batch, kv_heads, max_length, head_dim] cache written at a
-device-side position, and ``F.scaled_dot_product_attention`` with GQA and a length mask; its output goes straight into
-the next chain's o_proj input buffer.  The final add, ``model.model.norm`` and ``lm_head`` run in torch.  One token is
-then n_layers + 1 chain launches and n_layers attentions, captured together in one CUDA graph.
+rotary embedding and ``apply_rotary_pos_emb``, a static [batch, kv_heads, max_length, head_dim] cache
+(``autogptq_b200.kv_cache.KVCache``) written at a device-side position, and ``F.scaled_dot_product_attention`` with
+GQA and a length mask; its output goes straight into the next chain's o_proj input buffer.  The final add,
+``model.model.norm`` and ``lm_head`` run in torch.  One token is then n_layers + 1 chain launches and n_layers
+attentions, captured together in one CUDA graph.
 
 ``fused_attention=True`` runs each attention as one ``agb200_decode_attention`` launch instead (rotary embedding, cache
 write and split-KV attention, ``autogptq_b200.attention``): a token is then 2·n_layers + 1 launches of the project's own
@@ -57,10 +58,11 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from ._decoding import StaticCacheDecoder, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
+from ._decoding import DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
 from ._decoding import _MOE_BLOCKS, _RMSNORMS, _ROUTERS, _check_window, _norm_of  # noqa: F401 - also importable here
 from .attention import FP8, attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
+from .kv_cache import KVCache
 from .moe import moe_router
 from .sampling import sampling_list
 
@@ -87,7 +89,7 @@ def _plan_layer(i: int, layer, batch: int, dtype):
     return attn, mlp, ln1, ln2, moe
 
 
-class ChainDecoder(StaticCacheDecoder):
+class ChainDecoder(DecoderBase):
     """Greedy or sampling decoder over a transformers ``LlamaForCausalLM`` / ``MistralForCausalLM`` / ``Qwen2ForCausalLM`` whose
     projections are ``autogptq_b200.QuantLinear`` (``FusedQuantMLP`` MLPs are accepted too), or a
     ``MixtralForCausalLM`` whose experts are ``autogptq_b200.QuantExperts``.  ``fused_attention``:
@@ -105,6 +107,7 @@ class ChainDecoder(StaticCacheDecoder):
                                       "attention reads a 16-bit cache")
         self.batch, self.fused_attention = batch, bool(fused_attention)
         self._read_model(model, max_length, kv_cache_dtype)
+        self._cache = KVCache(batch, self.n_kv, self.max_length, self.head_dim, self.dtype, self._fp8)
         if self.fused_attention:
             why = attention_supported(self.n_heads, self.n_kv, self.head_dim, batch, self.max_length, self.dtype)
             if why is not None:
@@ -285,7 +288,7 @@ class ChainDecoder(StaticCacheDecoder):
     def _fused_attention(self, i: int):
         q, k, v = self._qkv[i]
         decode_attention(q, k, v, self.k_cache[i], self.v_cache[i], self._pos, self._inv_freq, self._attn_scaling,
-                         self.scaling, self._attn_in[i], self._attn_ws, **self._cache_kwargs(i))
+                         self.scaling, self._attn_in[i], self._attn_ws, **self._cache.scales(i))
 
     def _step_body(self) -> torch.Tensor:
         inner = self.model.model

@@ -5,8 +5,8 @@ A slot's blocks are its block-table row in order: block j holds positions j·blo
 is free (count 0) or held by one or more slots (count = the number of slots whose list has it).  Invariant: the block
 holding the position a slot writes next has count 1, so the kernels never write a block another slot reads.  Full
 blocks are shared by ``fork``; the partially filled last block is never shared (``fork`` hands back a fresh block for a
-copy of it).  Every method that can fail checks first and changes nothing when it raises.  Pure Python: the decoder
-mirrors every change into its device block table.
+copy of it).  Every method that can fail checks first and changes nothing when it raises.  Pure Python:
+``kv_cache.PagedKVCache`` mirrors every change into its device block table.
 """
 from __future__ import annotations
 

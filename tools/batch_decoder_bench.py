@@ -38,12 +38,12 @@ def ragged(B, prompt, spread):
     return [prompt - spread + (2 * spread * s) // (B - 1) for s in range(B)]
 
 
-def _fill(dec, index, T, gen):
-    """Synthetic keys and values N(0, 1) in positions :T of the decoder's caches at ``index`` (quantised for FP8)."""
+def _fill(dec, rows, T, gen):
+    """Synthetic keys and values N(0, 1) in positions :T of the decoder's cache rows ``rows`` (quantised for FP8)."""
+    n = len(range(dec._cache.rows)[rows])
     for i, k in enumerate(dec.k_cache):
-        shape = k[index][..., :T, :].shape
-        x = [torch.randn(shape, generator=gen, device=k.device).half() for _ in range(2)]
-        dec._store_kv(i, index + (slice(0, T),), *x)
+        x = [torch.randn((n, dec.n_kv, T, dec.head_dim), generator=gen, device=k.device).half() for _ in range(2)]
+        dec._cache.store(i, rows, *x)
 
 
 def _kv_dtype(kv):
@@ -53,7 +53,6 @@ def _kv_dtype(kv):
 @torch.no_grad()
 def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
     """One BatchDecoder run with every slot active at the given lengths: ms per step, tokens/s and the split."""
-    from autogptq_b200.attention import decode_attention_rows
     from autogptq_b200.batch_decoder import BatchDecoder
     from autogptq_b200.mlp import forward_gate_up
     from autogptq_b200.moe import add_rmsnorm
@@ -63,7 +62,7 @@ def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
                        kv_cache_dtype=_kv_dtype(kv))
     gen = torch.Generator(device=dev).manual_seed(2)
     for s, T in enumerate(lengths):
-        _fill(dec, (s, slice(None)), T, gen)
+        _fill(dec, slice(s, s + 1), T, gen)
     dec.positions = lengths
     tok = torch.randint(0, 32000, (B,), device=dev, generator=gen)
     for _ in range(3):                                   # capture + warm replays
@@ -85,8 +84,8 @@ def batch_decoder(model, B, lengths, S, dev, kv="dtype", min_length=0):
 
     def attentions():
         for i, (qq, kk, vv) in enumerate(q):
-            decode_attention_rows(qq, kk, vv, dec.k_cache[i], dec.v_cache[i], dec._pos, dec._inv_freq,
-                                  dec._attn_scaling, dec.scaling, dec._attn_out, dec._attn_ws, **dec._cache_kwargs(i))
+            dec._cache.decode(i, qq, kk, vv, dec._pos, dec._inv_freq, dec._attn_scaling, dec.scaling, dec._attn_out,
+                              dec._attn_ws)
 
     def norms():
         w, eps = plans[0][2]
@@ -115,7 +114,7 @@ def chain_decoder(model, B, T, S, dev, kv="dtype", min_length=0):
     dec = ChainDecoder(model, batch=B, max_length=max(min_length, T + S + 8), fused_attention=True,
                        kv_cache_dtype=_kv_dtype(kv))
     gen = torch.Generator(device=dev).manual_seed(2)
-    _fill(dec, (slice(None), slice(None)), T, gen)
+    _fill(dec, slice(None), T, gen)
     dec.position = T
     tok = torch.randint(0, 32000, (B,), device=dev, generator=gen)
     for _ in range(3):

@@ -93,13 +93,12 @@ def attn_part(reps, repeats):
 
 
 def _fill(dec, s, T, gen):
-    """Synthetic N(0, 1) keys and values at positions :T of slot s (blocks mapped first on a paged cache)."""
-    if dec.kv_block_size is not None:
-        dec._map({s: T})
+    """Synthetic N(0, 1) keys and values at positions :T of slot s (blocks reserved first on a paged cache)."""
+    dec._cache.reserve({s: T})
     for i, k in enumerate(dec.k_cache):
         shape = (1, dec.n_kv, T, dec.head_dim)
         x = [torch.randn(shape, generator=gen, device=k.device).half() for _ in range(2)]
-        dec._store_kv(i, (slice(s, s + 1), slice(None), slice(0, T)), *x)
+        dec._cache.store(i, slice(s, s + 1), *x)
     dec._pos[s] = T
     dec._host_pos[s] = T
 
@@ -155,12 +154,12 @@ def gen_part(layers, repeats):
     p = torch.randint(0, 32000, (2048,), generator=torch.Generator().manual_seed(3))
     sp = [SamplingParams(temperature=0.8, top_k=50, seed=10 + i) for i in range(4)]
     peak = [0]
-    mapper = dec._map
+    reserve = dec._cache.reserve
 
     def tracked(need):
-        mapper(need)
+        reserve(need)
         peak[0] = max(peak[0], dec.kv_blocks - dec.kv_blocks_free)
-    dec._map = tracked
+    dec._cache.reserve = tracked
 
     def fork():
         return dec.generate([p], 64, sampling=sp[0], n=4)
