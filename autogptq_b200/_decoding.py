@@ -7,6 +7,7 @@ from __future__ import annotations
 
 import torch
 
+from . import _lib
 from .attention import FP8
 from .mlp import FusedQuantMLP, _is_silu
 from .moe import QuantExperts, router_supported
@@ -131,6 +132,22 @@ def _plan_moe(i: int, mlp, H: int, batch: int, dtype, who: str = "ChainDecoder")
     if why is not None:
         raise NotImplementedError(f"{who}: {where}.gate: {why}")
     return w.detach().contiguous(), k, experts
+
+
+def _plan_experts(plans, dtype, device, who: str):
+    """Create every Mixtral block's expert plan (``QuantExperts._plan``) before the caches exist.  Whether the grouped
+    experts' decode kernels fit the device's shared memory is ``agb200_moe_create``'s decision; a block they do not fit
+    (ENOSUP) is refused here, naming the layer, instead of failing at the first step.  The plans are cached, so the
+    decoder's static buffers reuse them."""
+    for i, p in enumerate(plans):
+        if p[4] is None:
+            continue
+        try:
+            p[4][2]._plan(dtype, device)
+        except _lib.B200KernelError as e:
+            if e.code != _lib.ENOSUP:
+                raise
+            raise NotImplementedError(f"{who}: model.layers.{i}.mlp.experts cannot run on this device: {e}") from None
 
 
 def _is_moe(plans, who: str = "ChainDecoder") -> bool:

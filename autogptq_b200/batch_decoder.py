@@ -71,7 +71,8 @@ from collections import deque
 import torch
 
 from . import _lib
-from ._decoding import _MOE_BLOCKS, DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
+from ._decoding import (_MOE_BLOCKS, DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_experts, _plan_moe,
+                        _rotary_params)
 from .attention import decode_attention_workspace
 from .kv_cache import KVCache, PagedKVCache
 from .mlp import forward_gate_up
@@ -122,6 +123,8 @@ class BatchDecoder(DecoderBase):
             raise NotImplementedError(f"{_WHO}: model.layers.*.input_layernorm: {why}")
         if self._final[0].dtype != dt:                  # the last add_rmsnorm reads it
             raise NotImplementedError(f"{_WHO}: model.norm.weight is {self._final[0].dtype}, the activations {dt}")
+        if self.moe:
+            _plan_experts(self._plans, dt, self._cuda_device(), _WHO)
         self._allocate(B)
 
         dev = self.device

@@ -58,7 +58,7 @@ import torch
 import torch.nn.functional as F
 
 from . import _lib
-from ._decoding import DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_moe, _rotary_params
+from ._decoding import DecoderBase, _is_moe, _is_moe_block, _plan_common, _plan_experts, _plan_moe, _rotary_params
 from ._decoding import _MOE_BLOCKS, _RMSNORMS, _ROUTERS, _check_window, _norm_of  # noqa: F401 - also importable here
 from .attention import FP8, attention_supported, decode_attention, decode_attention_workspace
 from .chain import DecodeChain, chain_supported
@@ -121,7 +121,9 @@ class ChainDecoder(DecoderBase):
         # library's decision (DESIGN §3.5), and a block that does not fit is refused before the caches are allocated
         plans, attn0, H = self._plans, self._plans[0][0], self.hidden_size
         B, dev, dt = batch, self._cuda_device(), self.dtype
-        self._pos = torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
+        if self.moe:
+            _plan_experts(plans, dt, dev, "ChainDecoder")
+        self._pos =torch.zeros(1, dtype=torch.int64, device=dev)          # device-side position of the next token
         self._counter = torch.zeros(B, dtype=torch.int64, device=dev)      # its copy per row, the sampler's counter
         self._arange = torch.arange(self.max_length, device=dev)
         self._length = 0                                                    # host copy of the position
